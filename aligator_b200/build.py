@@ -48,7 +48,8 @@ def build(verbose=False, force=False, ptxas_v=False):
     hdrs = [os.path.join(CSRC, f) for f in ("riccati_group.cuh", "riccati_launch.cuh", "riccati_configs.h")]
     hdrs.append(os.path.join(PKG, "..", "include", "aligator_b200", "gar.h"))
     hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
-                                                          "lq_assemble.h", "kkt_error.h", "linesearch.h")]
+                                                          "lq_assemble.h", "kkt_error.h", "linesearch.h",
+                                                          "proxddp_inner.h")]
     extra = ["-Xptxas", "-v"] if ptxas_v else []
     jobs = []
     for (nx, nu, nc, g) in configs():
@@ -74,7 +75,10 @@ def build(verbose=False, force=False, ptxas_v=False):
     src = os.path.join(CSRC, "linesearch.cu")
     obj = os.path.join(OBJ, "linesearch_%s.o" % _digest([os.path.join(CSRC, "linesearch.h"), src], str(extra)))
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    todo = [(o, c) for (o, c) in jobs if force or not os.path.exists(o)]
+    src = os.path.join(CSRC, "proxddp_inner.cu")
+    obj = os.path.join(OBJ, "inner_%s.o" % _digest([hdrs[-1], os.path.join(CSRC, "proxddp_inner.h"), src], str(extra)))
+    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
+    todo =[(o, c) for (o, c) in jobs if force or not os.path.exists(o)]
     logs = []
     if todo:
         with cf.ThreadPoolExecutor(max_workers=max(1, min(len(todo), os.cpu_count() or 4))) as ex:

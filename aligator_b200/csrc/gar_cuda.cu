@@ -18,6 +18,7 @@
 #include "kkt_error.h"
 #include "linesearch.h"
 #include "lq_assemble.h"
+#include "proxddp_inner.h"
 #include "riccati_block_launch.h"
 #include "riccati_configs.h"
 #include "riccati_launch.cuh"
@@ -238,7 +239,8 @@ struct ab2_gar_solver {
   double *own_stage_sym = nullptr; // triangle-packed stage records as uploaded by ab2_gar_sweep_host_sym
   double *gains_tmp = nullptr, *kkt_tmp = nullptr, *theta_dev = nullptr, *ls_tmp = nullptr;
   double *fddp_slack = nullptr, *fddp_G0 = nullptr, *fddp_g0 = nullptr, *fddp_vx = nullptr;
-  int nth = 0;  // parameter dimension of the value function outputs (= nx in leg mode)
+  double *inner_tmp = nullptr; // [batch][2] per-instance scalars of multipliers / criterion, for host destinations
+  int nth = 0; // parameter dimension of the value function outputs (= nx in leg mode)
   int rec_nth = 0; // parameter blocks carried by the knot records (0 in leg mode)
   int legs = 0;    // >= 2: gar::ParallelRiccatiSolver (leg mode)
   bool dense = false; // gar::RiccatiSolverDense (one CTA per instance, stage-dense KKT): FF/FB have nu+nc+2nx rows
@@ -505,7 +507,7 @@ int ab2_gar_destroy(ab2_gar_solver *s) {
   if (s->pg_done)
     cudaFree(s->pg_done);
   for (double *q : {s->own_stage_sym, s->own_stage, s->own_term, s->own_G0, s->own_g0, s->gains_tmp, s->kkt_tmp, s->theta_dev, s->cond, s->ls_tmp, s->fddp_slack, s->fddp_G0,
-                    s->fddp_g0, s->fddp_vx})
+                    s->fddp_g0, s->fddp_vx, s->inner_tmp})
     if (q)
       cudaFree(q);
   for (int i = 0; i < ab2_gar_solver::kPipeStreams; ++i) {
@@ -1274,6 +1276,89 @@ int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double
   s->launches += 1;
   if (memspace != AB2_DEVICE)
     CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  return AB2_OK;
+}
+
+// ---- multipliers, Lagrangian gradient, criterion (proxddp_inner.cu) ----
+static ab2::InnerDims inner_dims(const ab2_gar_solver *s) {
+  const ab2_gar_dims &d = s->d;
+  return ab2::InnerDims{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0};
+}
+// device destination of a [batch][2] result: the caller's buffer or the handle's scratch (copied out afterwards)
+static int inner_result(ab2_gar_solver *s, double *dst, int memspace, double **dev) {
+  if (memspace == AB2_DEVICE) {
+    *dev = dst;
+    return AB2_OK;
+  }
+  if (!s->inner_tmp)
+    CUDA_TRY(cudaMalloc(&s->inner_tmp, (size_t)s->d.batch * 2 * sizeof(double)));
+  *dev = s->inner_tmp;
+  return AB2_OK;
+}
+int ab2_gar_multipliers(ab2_gar_solver *s, const ab2_mult_inputs *in, const ab2_mult_outputs *out, double *dst,
+                        int memspace, void *stream) {
+  if (!s || !in || !out || !dst)
+    return fail(AB2_ERR_INVALID, "null argument");
+  const ab2_gar_dims &d = s->d;
+  const bool stages = d.horizon > 0;
+  if (stages && (in->xnext != nullptr) == (in->fs != nullptr))
+    return fail(AB2_ERR_INVALID, "multipliers: give exactly one of xnext and fs");
+  const bool ok = (!stages || ((in->fs || in->xs) && in->lams && out->slack && out->lams_plus)) &&
+                  (d.nc0 == 0 || (in->init_value && in->lam0 && out->lam0_plus)) &&
+                  (d.nc == 0 || !stages ||
+                   (in->vs && in->prev_vs && in->cval && in->lo && in->hi && out->vs_plus && out->shifted && out->Lv)) &&
+                  (d.nct == 0 || (in->vsT && in->prev_vsT && in->cval_N && in->loN && in->hiN && out->vsT_plus &&
+                                  out->shifted_N && out->Lv_N));
+  if (!ok)
+    return fail(AB2_ERR_INVALID, "multipliers: a required array is NULL for these dimensions");
+  if (!(in->mu > 0.0) || !(in->mu_dyn > 0.0))
+    return fail(AB2_ERR_INVALID, "multipliers: mu and mu_dyn must be positive");
+  CUDA_TRY(cudaSetDevice(d.device));
+  double *dev = nullptr;
+  if (int rc = inner_result(s, dst, memspace, &dev))
+    return rc;
+  CUDA_TRY(ab2::launch_multipliers(inner_dims(s), *in, *out, dev, (cudaStream_t)stream));
+  s->launches += 1;
+  if (memspace != AB2_DEVICE)
+    CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * 2 * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  return AB2_OK;
+}
+int ab2_gar_lagrangian_gradient(ab2_gar_solver *s, const ab2_lag_inputs *in, const ab2_lag_outputs *out, void *stream) {
+  if (!s || !in || !out)
+    return fail(AB2_ERR_INVALID, "null argument");
+  const ab2_gar_dims &d = s->d;
+  const bool stages = d.horizon > 0;
+  if (!out->Lx && !out->Lx_N && !out->Lu && !out->Lxs && !out->Lus)
+    return fail(AB2_ERR_INVALID, "lagrangian_gradient: no output array given");
+  const bool ok = in->lx_N && (!stages || (in->lx && in->lu && in->Jx && in->Ju && in->lams)) &&
+                  (d.nc == 0 || !stages || (in->cJx && in->cJu && in->vs)) && (d.nct == 0 || (in->cJx_N && in->vsT)) &&
+                  (d.nc0 == 0 || (in->G0 && in->lam0));
+  if (!ok)
+    return fail(AB2_ERR_INVALID, "lagrangian_gradient: a required input array is NULL for these dimensions");
+  CUDA_TRY(cudaSetDevice(d.device));
+  CUDA_TRY(ab2::launch_lagrangian_gradient(inner_dims(s), *in, *out, (cudaStream_t)stream));
+  s->launches += 1;
+  return AB2_OK;
+}
+int ab2_gar_criterion(ab2_gar_solver *s, const double *Lxs, const double *Lus, const double *init_value,
+                      const double *slack, const double *Lv, const double *Lv_N, double *dst, int memspace,
+                      void *stream) {
+  if (!s || !dst)
+    return fail(AB2_ERR_INVALID, "null argument");
+  const ab2_gar_dims &d = s->d;
+  const bool stages = d.horizon > 0;
+  const bool ok = Lxs && (!stages || Lus) && (d.nc0 == 0 || !stages || init_value) && (d.horizon < 2 || slack) &&
+                  (d.nc == 0 || !stages || Lv) && (d.nct == 0 || Lv_N);
+  if (!ok)
+    return fail(AB2_ERR_INVALID, "criterion: a required array is NULL for these dimensions");
+  CUDA_TRY(cudaSetDevice(d.device));
+  double *dev = nullptr;
+  if (int rc = inner_result(s, dst, memspace, &dev))
+    return rc;
+  CUDA_TRY(ab2::launch_criterion(inner_dims(s), Lxs, Lus, init_value, slack, Lv, Lv_N, dev, (cudaStream_t)stream));
+  s->launches += 1;
+  if (memspace != AB2_DEVICE)
+    CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * 2 * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return AB2_OK;
 }
 

@@ -52,6 +52,40 @@ class LsIterate(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _LS_KEYS]
 
 
+_MULT_IN = ("xs", "lam0", "lams", "vs", "vsT", "prev_vs", "prev_vsT", "init_value", "xnext", "fs", "cval", "cval_N",
+            "lo", "hi", "loN", "hiN")
+_MULT_OUT = ("slack", "lam0_plus", "lams_plus", "vs_plus", "vsT_plus", "shifted", "shifted_N", "Lv", "Lv_N")
+
+
+class MultInputs(C.Structure):
+    """``ab2_mult_inputs``: device pointers of computeMultipliers' inputs, then mu, mu_dyn."""
+    _fields_ = [(k, C.c_void_p) for k in _MULT_IN] + [("mu", C.c_double), ("mu_dyn", C.c_double)]
+
+
+class MultOutputs(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in _MULT_OUT]
+
+
+_LAG_IN = ("lx", "lu", "lx_N", "Jx", "Ju", "cJx", "cJu", "cJx_N", "G0", "lam0", "lams", "vs", "vsT")
+_LAG_OUT = ("Lx", "Lx_N", "Lu", "Lxs", "Lus")
+
+
+class LagInputs(C.Structure):
+    """``ab2_lag_inputs``: device pointers of LagrangianDerivatives::compute's inputs."""
+    _fields_ = [(k, C.c_void_p) for k in _LAG_IN] + [("force_initial_condition", C.c_int)]
+
+
+class LagOutputs(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in _LAG_OUT]
+
+
+def _fill(struct, keys, arrays):
+    for k in keys:
+        a = arrays.get(k)
+        setattr(struct, k, None if a is None else _ptr(a).value)
+    return struct
+
+
 class GarTuning(C.Structure):
     _fields_ = [("variant", C.c_int), ("stagger_ns", C.c_int), ("ctas_per_sm", C.c_int)]
 
@@ -117,6 +151,10 @@ def lib():
         L.ab2_gar_linear_step.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
         L.ab2_gar_directional_derivative.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_al_value.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_int, C.c_void_p]
+        L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
+                                          C.c_void_p]
+        L.ab2_gar_lagrangian_gradient.argtypes = [C.c_void_p, C.POINTER(LagInputs), C.POINTER(LagOutputs), C.c_void_p]
+        L.ab2_gar_criterion.argtypes = [C.c_void_p] + [C.c_void_p] * 7 + [C.c_int, C.c_void_p]
         L.ab2_gar_peer_gather_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.ab2_gar_peer_gather_connect.argtypes = [C.c_void_p, C.c_void_p]
         L.ab2_gar_policy_allgather.argtypes = [C.c_void_p, C.c_void_p]
@@ -430,6 +468,47 @@ class CudaRiccatiBatch:
                                       AB2_HOST, C.c_void_p(stream)))
         self.synchronize(stream)
         return out
+
+    # ---- multipliers, Lagrangian gradient, criterion (the rest of the inner iteration) ----
+    def _scalars(self, call, out, stream):
+        """Run `call(dst, memspace)` for a [batch][2] result: into the device tensor `out`, or to the host."""
+        if out is not None:
+            call(_ptr(out), AB2_DEVICE)
+            return out
+        host = np.empty((self.dims.batch, 2), dtype=np.float64)
+        call(_ptr(host), AB2_HOST)
+        self.synchronize(stream)
+        return host
+
+    def multipliers(self, inputs, outputs, mu, mu_dyn, out=None, stream=0):
+        """computeMultipliers on the device (``ab2_gar_multipliers``).  ``inputs``: dict of device tensors keyed like
+        ``ab2_mult_inputs`` (exactly one of xnext, fs); ``outputs``: dict of device tensors keyed like
+        ``ab2_mult_outputs``.  Returns [batch][2] = [prim_infeas, finite (1.0 / 0.0)] as numpy, or writes it into the
+        device tensor ``out`` and returns that."""
+        inp = _fill(MultInputs(), _MULT_IN, inputs)
+        inp.mu, inp.mu_dyn = float(mu), float(mu_dyn)
+        o = _fill(MultOutputs(), _MULT_OUT, outputs)
+        self._keep_inner = (inputs, outputs)
+        return self._scalars(lambda dst, ms: _check(lib().ab2_gar_multipliers(
+            self.h, C.byref(inp), C.byref(o), dst, ms, C.c_void_p(stream))), out, stream)
+
+    def lagrangian_gradient(self, inputs, outputs, force_initial_condition=False, stream=0):
+        """LagrangianDerivatives::compute on the device (``ab2_gar_lagrangian_gradient``).  ``inputs``: dict of
+        device tensors keyed like ``ab2_lag_inputs``; ``outputs``: any of Lx, Lx_N, Lu (assemble layout) and Lxs,
+        Lus (directional-derivative layout)."""
+        inp = _fill(LagInputs(), _LAG_IN, inputs)
+        inp.force_initial_condition = int(bool(force_initial_condition))
+        o = _fill(LagOutputs(), _LAG_OUT, outputs)
+        self._keep_inner = (inputs, outputs)
+        _check(lib().ab2_gar_lagrangian_gradient(self.h, C.byref(inp), C.byref(o), C.c_void_p(stream)))
+
+    def criterion(self, arrays, out=None, stream=0):
+        """computeCriterion on the device (``ab2_gar_criterion``).  ``arrays``: dict of device tensors Lxs, Lus,
+        init_value, slack, Lv, Lv_N.  Returns [batch][2] = [inner_criterion, dual_infeas] (numpy, or into ``out``)."""
+        ptrs = [_ptr(arrays.get(k)) for k in ("Lxs", "Lus", "init_value", "slack", "Lv", "Lv_N")]
+        self._keep_inner = (arrays,)
+        return self._scalars(lambda dst, ms: _check(lib().ab2_gar_criterion(
+            self.h, *ptrs, dst, ms, C.c_void_p(stream))), out, stream)
 
     def fddp_backward_pass(self, arrays, preg, Vx_out=None, Quuks_out=None, stream=0):
         """SolverFDDP::backwardPass on the device (``ab2_fddp_backward_pass``); ``arrays``: dict of device

@@ -318,6 +318,75 @@ int ab2_gar_directional_derivative(ab2_gar_solver *s, const double *Lxs, const d
 int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, double mudyn, double mucstr,
                      double *dst, int memspace, void *stream);
 
+/* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
+ * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
+ * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
+ * All array arguments are DEVICE pointers in the layouts of ab2_lq_inputs / ab2_ls_iterate: stage arrays
+ * [batch][N][.], terminal and initial arrays [batch][.], matrices column-major, xs [batch][N+1][nx],
+ * lam0 [batch][nc0], lams [batch][N][nx] (lams[1..N]), vs [batch][N][nc], vsT [batch][nct].
+ *
+ * Normal-cone projection per row, from the bounds encoding of ab2_lq_inputs (the same rows the active-set rule
+ * above keeps): an equality row (lo = +inf) has NC(z) = z (equality-constraint.hpp:37-40); every other row has
+ * NC(z) = z - max(min(z, hi), lo) (box-constraint.hpp:27-37), i.e. max(z, 0) for the negative orthant
+ * (lo = -inf, hi = 0, negative-orthant.hpp:36-38). */
+typedef struct ab2_mult_inputs {
+  const double *xs, *lam0, *lams, *vs, *vsT; /* the iterate the estimates are computed at                       */
+  const double *prev_vs, *prev_vsT;          /* workspace_.prev_vs, laid out like vs / vsT                      */
+  const double *init_value;                  /* [batch][nc0] init_data value_ (assemble's g0)                   */
+  const double *xnext, *fs;                  /* EXACTLY ONE: xnext [batch][N][nx] (dd.xnext_; vector-space
+                                                difference fs[t+1] = xnext_t - x_{t+1}) or fs [batch][N][nx]
+                                                given by a caller on a manifold                                 */
+  const double *cval, *cval_N;               /* constraint values [batch][N][nc], [batch][nct]                  */
+  const double *lo, *hi, *loN, *hiN;         /* [nc] / [nct] row bounds, shared by all knots and instances      */
+  double mu, mu_dyn;
+} ab2_mult_inputs;
+typedef struct ab2_mult_outputs {
+  double *slack;                                  /* [batch][N][nx] dyn_slacks[1..N] (assemble's slack)      */
+  double *lam0_plus, *lams_plus, *vs_plus, *vsT_plus; /* lams_plus / vs_plus: an ab2_ls_iterate for al_value */
+  double *shifted, *shifted_N;                    /* shifted_constraints                                     */
+  double *Lv, *Lv_N;                              /* Lvs                                                     */
+} ab2_mult_outputs;
+/* Replaces: SolverProxDDP::computeMultipliers, solver-proxddp.hxx:220-318, for every instance (one warp each):
+ *   fs0 = init_value,  lam0_plus = lam0 + fs0 / mu   (mu, not mu_dyn: :246-247),
+ *   fs[t+1] = xnext_t - x_{t+1},  lams_plus[t+1] = lams[t+1] + fs[t+1] / mu_dyn   (:263-264),
+ *   shifted = cval + mu prev_vs,  Lv = NC(shifted) - mu vs,  vs_plus = (1/mu) NC(shifted),
+ *   stage_infeas = mu (vs_plus - prev_vs)   (:277-286; the terminal block likewise when nct > 0, :292-314).
+ * dst [batch][2] (host or device) = [prim_infeas, finite]: prim_infeas = max(|stage_infeas|_inf over all knots,
+ * |fs|_inf over fs0..fs_N) (:315-316); finite = 1.0 if every lams_plus and Lv entry is finite, else 0.0 -- the
+ * reference returns false at the first non-finite one (RET_FALSE_IF_NAN, :248, 265, 289, 313); prim_infeas of
+ * such an instance is unspecified.  Every output array is required (arrays of zero size may be NULL). */
+int ab2_gar_multipliers(ab2_gar_solver *s, const ab2_mult_inputs *in, const ab2_mult_outputs *out, double *dst,
+                        int memspace, void *stream);
+
+typedef struct ab2_lag_inputs {
+  const double *lx, *lu, *lx_N;        /* cost gradients cost_data->Lx_, Lu_: [batch][N][nx], [batch][N][nu], [batch][nx] */
+  const double *Jx, *Ju;               /* dynamics Jacobians [batch][N][nx*nx], [batch][N][nx*nu]                          */
+  const double *cJx, *cJu, *cJx_N;     /* constraint Jacobians [batch][N][nc*nx], [batch][N][nc*nu], [batch][nct*nx]       */
+  const double *G0;                    /* init_data Jx_ [batch][nc0*nx]                                                    */
+  const double *lam0, *lams, *vs, *vsT; /* any multiplier set: the iterate (LQ right-hand side) or the *_plus estimates
+                                           (ALFunction::directionalDerivative, merit-function.hxx:82-84)                  */
+  int force_initial_condition;         /* nonzero: Lx_0 = 0, as innerLoop does after the call (solver-proxddp.hxx:592-594) */
+} ab2_lag_inputs;
+typedef struct ab2_lag_outputs {
+  double *Lx, *Lx_N, *Lu; /* assemble layout: [batch][N][nx], [batch][nx], [batch][N][nu]      */
+  double *Lxs, *Lus;      /* directional-derivative layout: [batch][N+1][nx], [batch][N][nu]   */
+} ab2_lag_outputs;
+/* Replaces: LagrangianDerivatives::compute, core/lagrangian.hpp:29-92, for every instance and knot:
+ *   Lx_t = lx_t + Jx_t^T lam_{t+1} + cJx_t^T v_t - lam_t  (t >= 1; t = 0: + G0^T lam0 instead of - lam_0),
+ *   Lu_t = lu_t + Ju_t^T lam_{t+1} + cJu_t^T v_t,
+ *   Lx_N = lx_N + cJx_N^T v_N - lam_N  (N = 0: Lx_0 = lx_N + cJx_N^T v_N + G0^T lam0).
+ * Writes whichever of the five outputs are non-NULL (at least one). */
+int ab2_gar_lagrangian_gradient(ab2_gar_solver *s, const ab2_lag_inputs *in, const ab2_lag_outputs *out, void *stream);
+
+/* Replaces: SolverProxDDP::computeCriterion, solver-proxddp.hxx:703-732: dst [batch][2] (host or device) =
+ * [inner_criterion, dual_infeas].  Lxs [batch][N+1][nx], Lus [batch][N][nu] (lagrangian_gradient's outputs),
+ * init_value [batch][nc0] = fs0, slack [batch][N][nx] = fs[1..N], Lv [batch][N][nc], Lv_N [batch][nct].
+ * As in the reference, knot i's dynamics residual is dyn_slacks[i]: inner_criterion covers fs0..fs_{N-1} (fs0 only
+ * when N >= 1) and never fs_N; dual_infeas = max(|Lxs|_inf over knots 0..N, |Lus|_inf). */
+int ab2_gar_criterion(ab2_gar_solver *s, const double *Lxs, const double *Lus, const double *init_value,
+                      const double *slack, const double *Lv, const double *Lv_N, double *dst, int memspace,
+                      void *stream);
+
 /* SolverFDDPTpl::backwardPass, solvers/fddp/solver-fddp.hxx:204-277 (SURVEY section 8f rank 4), for a batch: the
  * unconstrained recursion is the sweep's own stage step with A = Jx, B = Ju, f_i = fs[i+1], Q = Lxx + preg I,
  * S = Lxu, R = Luu + preg I, q = Lx, r = Lu (nc = 0; the LLT of Quu (:259-260) is the Bunch-Kaufman factorisation
