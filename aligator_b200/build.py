@@ -45,7 +45,8 @@ def _run(cmd):
 
 def build(verbose=False, force=False, ptxas_v=False):
     os.makedirs(OBJ, exist_ok=True)
-    hdrs = [os.path.join(CSRC, f) for f in ("riccati_group.cuh", "riccati_launch.cuh", "riccati_configs.h")]
+    hdrs = [os.path.join(CSRC, f) for f in ("riccati_group.cuh", "riccati_launch.cuh", "riccati_configs.h",
+                                            "vxx_layout.h")]
     hdrs.append(os.path.join(PKG, "..", "include", "aligator_b200", "gar.h"))
     hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
                                                           "lq_assemble.h", "kkt_error.h", "linesearch.h",

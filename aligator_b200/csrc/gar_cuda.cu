@@ -165,17 +165,42 @@ __global__ void fddp_prep_kernel(const double *__restrict__ fs, double *__restri
   }
 }
 // after: Vx_i = vx_i + sym(Vxx_i) fs[i] (:219-220, 272-276), then Quuks_i = -(Lu_i + Ju_i^T Vx_{i+1}) = Quu_i k_i (:264)
-__global__ void fddp_vx_kernel(const double *__restrict__ Vxx, const double *__restrict__ vx, const double *__restrict__ fs,
-                               double *__restrict__ Vx_out, int batch, int N, int nx) {
+// (Vxx0 != null: Vxx in the packed layout of vxx_layout.h, knot t in factor slot t)
+__global__ void fddp_vx_kernel(const double *__restrict__ Vxx, const double *__restrict__ Vxx0, const double *__restrict__ vx,
+                               const double *__restrict__ fs, double *__restrict__ Vx_out, int batch, int N, int nx) {
   const long total = (long)batch * (N + 1) * nx;
+  const int P = vxx_packed_doubles(nx);
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const long kn = i / nx;
     const int r = (int)(i % nx);
-    const double *V = Vxx + kn * nx * nx, *f = fs + kn * nx;
+    const double *f = fs + kn * nx;
     double acc = 0.0;
-    for (int c = 0; c < nx; ++c) // the lower triangle mirrored (selfadjointView<Lower>, :272)
-      acc += (r >= c ? V[r + (size_t)c * nx] : V[c + (size_t)r * nx]) * f[c];
+    if (Vxx0 && !vxx_slot_is_full((int)(kn % (N + 1)))) {
+      const double *V = Vxx + kn * P;
+      for (int c = 0; c < nx; ++c)
+        acc += V[vxx_packed_index(nx, r, c)] * f[c];
+    } else {
+      const double *V = Vxx0 ? Vxx0 + kn / (N + 1) * nx * nx : Vxx + kn * nx * nx;
+      for (int c = 0; c < nx; ++c) // the lower triangle mirrored (selfadjointView<Lower>, :272)
+        acc += (r >= c ? V[r + (size_t)c * nx] : V[c + (size_t)r * nx]) * f[c];
+    }
     Vx_out[i] = vx[i] + acc;
+  }
+}
+// Knots [t0, t0 + nt) of instances [b0, b0 + nb) of a packed Vxx (vxx_layout.h) as full column-major blocks;
+// stage knot t < N sits in factor slot (t + head) mod N, the terminal knot in slot N.
+__global__ void vxx_expand_kernel(const double *__restrict__ pk, const double *__restrict__ full0, double *__restrict__ dst,
+                                  int N, int nx, int head, int b0, int nb, int t0, int nt) {
+  const long nn = (long)nx * nx, total = (long)nb * nt * nn;
+  const int P = vxx_packed_doubles(nx);
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long kn = i / nn;
+    const int e = (int)(i - kn * nn);
+    const long b = b0 + kn / nt;
+    const int t = t0 + (int)(kn % nt);
+    const int slot = t < N ? (t + head) % N : t;
+    dst[i] = vxx_slot_is_full(slot) ? full0[b * nn + e]
+                                    : pk[(b * (N + 1) + slot) * P + vxx_packed_index(nx, e % nx, e / nx)];
   }
 }
 __global__ void fddp_quuks_kernel(const double *__restrict__ Ju, const double *__restrict__ Lu, const double *__restrict__ Vx,
@@ -268,6 +293,9 @@ struct ab2_gar_solver {
   bool have_problem = false, have_backward = false, have_forward = false;
   long launches = 0;
   int variant = -1;
+  // Layout of out[AB2_OUT_VXX] as the last backward left it: true = packed (warp-per-instance kernel,
+  // vxx_layout.h; p.Vxx0 is the full slot-0 array behind it), false = [batch][N+1][nx*nx] blocks.
+  bool vxx_packed = false;
   int group_doubles[4] = {0, 0, 0, 0};
   // ab2_gar_sweep_host: internal streams, one event per stream + a fork event
   static constexpr int kPipeStreams = 4;
@@ -399,10 +427,15 @@ static int create_impl(const ab2_gar_dims *dims, int nth, int legs, ab2_gar_solv
   setup(AB2_OUT_KKT0FTH, (size_t)(nx + d.nc0) * nth, 1);
   setup(AB2_OUT_THGRAD, nth, 1);
   setup(AB2_OUT_THHESS, (size_t)nth * nth, 1);
+  // warp-per-instance handles: VXX holds either layout (packed + the full slot-0 array, or full blocks for variant 9)
+  const size_t vxx_packed_total = (size_t)B * (N + 1) * ab2::vxx_packed_doubles(nx) + (size_t)B * nx * nx;
   for (int w = 0; w < AB2_OUT_COUNT; ++w) {
     // (+2: the forward pass of the CTA-per-instance kernel fetches odd-sized gain records
     // with 16-byte granularity, up to one double past the end of the array)
-    const size_t bytes = (s->out_doubles[w] > 0 ? s->out_doubles[w] + 2 : 2) * sizeof(double);
+    size_t n = s->out_doubles[w];
+    if (w == AB2_OUT_VXX && s->k && vxx_packed_total > n)
+      n = vxx_packed_total;
+    const size_t bytes = (n > 0 ? n + 2 : 2) * sizeof(double);
     cudaError_t e = cudaMalloc(&s->out[w], bytes);
     if (e == cudaSuccess)
       e = cudaMemset(s->out[w], 0, bytes);
@@ -450,6 +483,8 @@ static int create_impl(const ab2_gar_dims *dims, int nth, int legs, ab2_gar_solv
   p.ff = s->out[AB2_OUT_FF];
   p.fb = s->out[AB2_OUT_FB];
   p.Vxx = s->out[AB2_OUT_VXX];
+  if (s->k)
+    p.Vxx0 = p.Vxx + (size_t)B * (N + 1) * ab2::vxx_packed_doubles(nx);
   p.vx = s->out[AB2_OUT_VX];
   p.ffT = s->out[AB2_OUT_FFT];
   p.fbT = s->out[AB2_OUT_FBT];
@@ -587,7 +622,10 @@ int ab2_gar_set_problem(ab2_gar_solver *s, const double *stage, const double *te
   return AB2_OK;
 }
 
-// SweepParams of the instances [b0, b0 + nb): every array leads with the batch index.
+// The configured backward runs the warp-per-instance kernel, which stores Vxx packed.
+static bool warp_kernel(const ab2_gar_solver *s) { return s->k && s->variant != 9; }
+
+// SweepParams of the instances [b0, b0 + nb) of a backward + forward launch: every array leads with the batch index.
 static ab2::SweepParams slice_params(const ab2_gar_solver *s, int b0, int nb) {
   ab2::SweepParams q = s->p;
   const size_t b = (size_t)b0;
@@ -601,8 +639,13 @@ static ab2::SweepParams slice_params(const ab2_gar_solver *s, int b0, int nb) {
     q.g0 += b * s->d.nc0;
   q.ff += b * s->out_knots[AB2_OUT_FF] * s->out_rec[AB2_OUT_FF];
   q.fb += b * s->out_knots[AB2_OUT_FB] * s->out_rec[AB2_OUT_FB];
-  q.Vxx += b * s->out_knots[AB2_OUT_VXX] * s->out_rec[AB2_OUT_VXX];
-  q.vx += b * s->out_knots[AB2_OUT_VX] * s->out_rec[AB2_OUT_VX];
+  if (warp_kernel(s)) {
+    q.Vxx += b * (N + 1) * ab2::vxx_packed_doubles(nx);
+    q.Vxx0 += b * nx * nx;
+  } else {
+    q.Vxx += b * s->out_knots[AB2_OUT_VXX] * s->out_rec[AB2_OUT_VXX];
+  }
+  q.vx +=b * s->out_knots[AB2_OUT_VX] * s->out_rec[AB2_OUT_VX];
   q.ffT += b * s->out_rec[AB2_OUT_FFT];
   q.fbT += b * s->out_rec[AB2_OUT_FBT];
   q.kkt0 += b * s->out_rec[AB2_OUT_KKT0];
@@ -655,10 +698,12 @@ static int run_kernels(ab2_gar_solver *s, ab2::SweepParams q, int bwd, int fwd, 
   }
   q.do_bwd = bwd;
   q.do_fwd = fwd;
+  // a forward-only launch reads Vxx in the layout the last backward wrote, whatever the tuning says now
+  const bool warp = bwd ? warp_kernel(s) : s->vxx_packed;
   if (s->dense)
     CUDA_TRY(ab2::launch_dense(q, s->d.nx, s->d.nu, s->d.nc, st));
-  else if (s->k && s->variant != 9)
-    CUDA_TRY(s->k->launch(q, s->variant, s->group_doubles, st, nullptr));
+  else if (warp)
+    CUDA_TRY(s->k->launch(q, s->variant == 9 ? -1 : s->variant, s->group_doubles, st, nullptr));
   else
     CUDA_TRY(ab2::launch_block(q, s->d.nx, s->d.nu, s->d.nc, st, nullptr));
   s->launches += 1;
@@ -697,6 +742,7 @@ static int launch(ab2_gar_solver *s, double mueq, int bwd, int fwd, void *stream
   if (bwd) {
     s->have_backward = true;
     s->fac_head = 0; // every factor slot was rewritten in knot order
+    s->vxx_packed = warp_kernel(s);
   }
   s->have_forward = fwd != 0; // a backward-only launch invalidates the previous trajectory
   return AB2_OK;
@@ -767,6 +813,29 @@ int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream) {
 
 static int copy_ring(const double *base, size_t rec, int knots, int nring, int head, int b0, int nb, int t0, int nt,
                      double *dst, cudaMemcpyKind kind, cudaStream_t st);
+
+// Knots [t0, t0 + nt) of instances [b0, b0 + nb) of a packed VXX, expanded to dense column-major blocks
+// [nb][nt][nx*nx] at dst (host: through a stream-ordered device buffer).  head: the factor ring's head.
+static int get_vxx_packed(ab2_gar_solver *s, int head, int b0, int nb, int t0, int nt, double *dst, int memspace,
+                          cudaStream_t st) {
+  const size_t n = (size_t)nb * nt * s->d.nx * s->d.nx;
+  if (n == 0)
+    return AB2_OK;
+  double *out = dst;
+  if (memspace != AB2_DEVICE)
+    CUDA_TRY(cudaMallocAsync(&out, n * sizeof(double), st));
+  long blocks = (long)((n + 255) / 256);
+  if (blocks > s->p.num_sms * 8L)
+    blocks = s->p.num_sms * 8L;
+  ab2::vxx_expand_kernel<<<(int)blocks, 256, 0, st>>>(s->out[AB2_OUT_VXX], s->p.Vxx0, out, s->d.horizon, s->d.nx, head,
+                                                      b0, nb, t0, nt);
+  CUDA_TRY(cudaGetLastError()); // (a copy for the caller, like cudaMemcpy: not in ab2_gar_launch_count)
+  if (memspace != AB2_DEVICE) {
+    CUDA_TRY(cudaMemcpyAsync(dst, out, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaFreeAsync(out, st));
+  }
+  return AB2_OK;
+}
 
 int ab2_gar_problem_ptr(ab2_gar_solver *s, int what, const double **out) {
   if (!s || !out || what < 0 || what > 3)
@@ -998,7 +1067,10 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
     for (int i = 0; i < nwhat; ++i) {
       const int w = whats[i];
       const size_t per_inst = (size_t)s->out_knots[w] * s->out_rec[w];
-      if (per_inst)
+      if (w == AB2_OUT_VXX && warp_kernel(s)) {
+        if ((rc = get_vxx_packed(s, 0, b0, nb, 0, N + 1, dsts[i] + (size_t)b0 * per_inst, AB2_HOST, st)) != AB2_OK)
+          return rc;
+      } else if (per_inst)
         CUDA_TRY(cudaMemcpyAsync(dsts[i] + (size_t)b0 * per_inst, s->out[w] + (size_t)b0 * per_inst,
                                  (size_t)nb * per_inst * sizeof(double), cudaMemcpyDeviceToHost, st));
     }
@@ -1010,6 +1082,7 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
   s->have_backward = true;
   s->have_forward = true;
   s->fac_head = 0;
+  s->vxx_packed = warp_kernel(s);
   return AB2_OK;
 }
 
@@ -1053,6 +1126,8 @@ int ab2_gar_get(ab2_gar_solver *s, int what, double *dst, int memspace, void *st
   CUDA_TRY(cudaSetDevice(s->d.device));
   if (s->out_doubles[what] == 0)
     return AB2_OK;
+  if (what == AB2_OUT_VXX && s->vxx_packed)
+    return get_vxx_packed(s, s->fac_head, 0, s->d.batch, 0, s->d.horizon + 1, dst, memspace, (cudaStream_t)stream);
   if (ring_indexed(s, what)) // between a cycle_append and the next backward: knot order through the ring head
     return copy_ring(s->out[what], s->out_rec[what], s->out_knots[what], s->d.horizon, s->fac_head, 0, s->d.batch, 0,
                      s->out_knots[what], dst, memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
@@ -1074,6 +1149,8 @@ int ab2_gar_get_range(ab2_gar_solver *s, int what, int b0, int nb, int t0, int n
   const size_t rec = s->out_rec[what];
   if (rec == 0 || nb == 0 || nt == 0)
     return AB2_OK;
+  if (what == AB2_OUT_VXX && s->vxx_packed)
+    return get_vxx_packed(s, s->fac_head, b0, nb, t0, nt, dst, memspace, (cudaStream_t)stream);
   if (ring_indexed(s, what))
     return copy_ring(s->out[what], rec, knots, s->d.horizon, s->fac_head, b0, nb, t0, nt, dst,
                      memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, (cudaStream_t)stream);
@@ -1406,7 +1483,8 @@ int ab2_fddp_backward_pass(ab2_gar_solver *s, const ab2_fddp_inputs *in, double 
   if ((rc = ab2_gar_backward(s, 1.0, stream)) != AB2_OK) // (mueq is unused without constraints)
     return rc;
   double *vxo = Vx_out ? Vx_out : s->fddp_vx;
-  ab2::fddp_vx_kernel<<<s->p.num_sms * 4, 256, 0, st>>>(s->out[AB2_OUT_VXX], s->out[AB2_OUT_VX], in->fs, vxo, B, N, nx);
+  ab2::fddp_vx_kernel<<<s->p.num_sms * 4, 256, 0, st>>>(s->out[AB2_OUT_VXX], s->vxx_packed ? s->p.Vxx0 : nullptr,
+                                                      s->out[AB2_OUT_VX], in->fs, vxo, B, N, nx);
   CUDA_TRY(cudaGetLastError());
   s->launches += 1;
   if (Quuks_out) {
@@ -1468,12 +1546,14 @@ int ab2_gar_cycle_append(ab2_gar_solver *s, const double *new_last, int memspace
     s->fac_head = (s->fac_head + 1) % N;
     const int slot = (N - 1 + s->fac_head) % N; // physical slot of the new stage knot N-1 (= the old knot 0's)
     for (int w : {AB2_OUT_FF, AB2_OUT_FB, AB2_OUT_VXX, AB2_OUT_VX}) {
-      const size_t rec = s->out_rec[w];
+      const size_t rec = (w == AB2_OUT_VXX && s->vxx_packed) ? (size_t)ab2::vxx_packed_doubles(s->d.nx) : s->out_rec[w];
       if (rec == 0)
         continue;
       CUDA_TRY(cudaMemset2DAsync(s->out[w] + (size_t)slot * rec, (size_t)s->out_knots[w] * rec * sizeof(double), 0,
                                  rec * sizeof(double), (size_t)B, st));
     }
+    if (s->vxx_packed && ab2::vxx_slot_is_full(slot)) // slot 0's block lives in the full array
+      CUDA_TRY(cudaMemsetAsync(s->p.Vxx0, 0, (size_t)B * s->d.nx * s->d.nx * sizeof(double), st));
   }
   // kkt0 zeroed (:84-86)
   if (s->out_doubles[AB2_OUT_KKT0])

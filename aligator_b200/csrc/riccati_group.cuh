@@ -33,6 +33,8 @@
 #include <cstdint>
 #include <utility>
 
+#include "vxx_layout.h"
+
 #if defined(__CUDACC__)
 #define AB2_HD __host__ __device__ __forceinline__
 #define AB2_D __device__ __forceinline__ // group-program code: device only under nvcc
@@ -63,7 +65,7 @@ struct SweepParams {
   // backward outputs
   double *ff;   // [batch][N][NR]          [k; z; a]
   double *fb;   // [batch][N][NR*NX]       row-major [K; Z; Ahat]
-  double *Vxx;  // [batch][N+1][NX*NX]     column-major
+  double *Vxx;  // [batch][N+1][NX*NX]     column-major (packed-Vxx builds: see Vxx0)
   double *vx;   // [batch][N+1][NX]
   double *ffT;  // [batch][nct]            terminal z
   double *fbT;  // [batch][nct*NX]         terminal Z (row-major)
@@ -109,6 +111,9 @@ struct SweepParams {
   int peer_world;
   double *peer_dst[8]; // receive buffer of rank w (peer-mapped)
   long long peer_off;  // doubles: slot * world * batch * per + rank * batch * per
+  // Packed-Vxx builds (Cfg::VXX_PACKED, vxx_layout.h): Vxx holds [batch][N+1][vxx_packed_doubles(NX)] and this
+  // [batch][NX*NX] array the full block of factor slot 0.  The full-layout build never reads it.
+  double *Vxx0;
 };
 
 // status bits: see ST_*; in leg mode several CTAs report on one instance
@@ -127,9 +132,14 @@ AB2_HD int cond_offset(int b, int nc0, int nx) { return b == 0 ? 0 : nc0 + (b - 
 // ---------------------------------------------------------------------------
 // Compile-time shape of one kernel instantiation.
 // ---------------------------------------------------------------------------
-template <int NX_, int NU_, int NC_, int G_, bool DB_ = false, bool RB_ = true, bool MMA_ = false> struct Cfg {
+template <int NX_, int NU_, int NC_, int G_, bool DB_ = false, bool RB_ = true, bool MMA_ = false, bool PK_ = false>
+struct Cfg {
   static constexpr int NX = NX_, NU = NU_, NC = NC_, G = G_;
   static constexpr bool DB = DB_;          // double-buffered knot records
+  // Vxx stored as packed lower triangles + a full slot-0 array (vxx_layout.h); false: [N+1][NX*NX] blocks
+  static constexpr bool VXX_PACKED = PK_;
+  static constexpr int VP = vxx_packed_doubles(NX);
+  static constexpr int VXX_REC = PK_ ? VP : NX * NX; // doubles per knot of p.Vxx
   static constexpr int NCOL = NX + NU + 1; // columns of M = [A | B | f]
   static constexpr int NXU = NX + NU;      // rows of H
   static constexpr int NK = NU + NC;       // reduced KKT size
@@ -173,7 +183,9 @@ template <int NX_, int NU_, int NC_, int G_, bool DB_ = false, bool RB_ = true, 
 #define AB2_PARK 1
 #endif
   static constexpr bool PARK = MMA_ && DB_ && (AB2_PARK != 0);
-  static constexpr int LUT_INTS = MMA ? 32 * (NT + NT * NT) : 0; // per-CTA table of per-lane constants
+  // packed Vxx_t store of the tensor-core step: lane l writes the packed pairs l, l + 32, ...
+  static constexpr int VPU = (PK_ && MMA_) ? (VP / 2 + 31) / 32 : 0;
+  static constexpr int LUT_INTS = MMA ? 32 * (NT + NT * NT + VPU) : 0; // per-CTA table of per-lane constants
   // stage record offsets (doubles) -- the reference's 11 buffers, concatenated
   static constexpr int OFF_A = 0;
   static constexpr int OFF_B = OFF_A + NX * NX;
@@ -256,12 +268,13 @@ template <int NX_, int NU_, int NC_, int G_, bool DB_ = false, bool RB_ = true, 
   static constexpr bool FWD_FUSED = FB_BULK && (NX % 2 == 0) && (NR + NX <= G);
   static constexpr int FWD_ROWS = FWD_FUSED ? NR + NX : NR;
   static constexpr bool FWD_FF = FWD_FUSED && (NR % 2 == 0); // ff_t rides in the slot too (no LDG in pass 1)
-  static constexpr int FWD_SLOT =
-      FWD_FUSED ? (NR + NX) * NX + NX + (FWD_FF ? NR : 0) : ev(NR * NX); // doubles per ring slot
+  // fused slot: [K; Z; Ahat]_t (NR*NX) | Vxx_t (VXX_REC) | vx_t (NX) | ff_t (NR, FWD_FF)
+  static constexpr int FWD_BIAS = NR * NX + VXX_REC;
+  static constexpr int FWD_SLOT = FWD_FUSED ? FWD_BIAS + NX + (FWD_FF ? NR : 0) : ev(NR * NX); // doubles per ring slot
   static constexpr int FWD_RING_RAW = (S_STAGE_END - 2 * ev(NX)) / FWD_SLOT;
-  // the fused ring may outgrow the stage area: at least 4 slots, 5 when that costs < 12 %
-  static constexpr int FWD_RING_MIN =
-      FWD_FUSED ? ((5 * FWD_SLOT + 2 * ev(NX)) * 100 <= S_STAGE_END * 112 ? 5 : 4) : 1;
+  // the fused ring may outgrow the stage area up to 4 slots.  No more: with packed Vxx a 5th slot
+  // would grow the C2 tensor-core build by 2.5 % and cost it its 8th resident CTA per SM.
+  static constexpr int FWD_RING_MIN = FWD_FUSED ? 4 : 1;
   static constexpr int FWD_RING = FWD_RING_RAW > 8 ? 8 : (FWD_RING_RAW < FWD_RING_MIN ? FWD_RING_MIN : FWD_RING_RAW);
   static constexpr int NXE = ev(NX);
   static constexpr int FWD_END = FWD_RING * FWD_SLOT + 2 * ev(NX);
@@ -1022,6 +1035,21 @@ template <class C> AB2_HD void fill_mma_lut(int *lut, const int lane, const int 
       lut[r * 32 + lane] = (int)(u0 | (u1 << 16));
     }
   }
+  // packed Vxx_t store: offsets in V' of the two entries of packed pair (r - NT - NT*NT) * 32 + lane,
+  // row j of V' for entry (i, j) (contiguous along a packed column); 0xffff = the zero padding entry
+  for (int r = NT + NT * NT + first; r < NT + NT * NT + C::VPU; r += step) {
+    const int e0 = 2 * ((r - NT - NT * NT) * 32 + lane);
+    unsigned u[2];
+    for (int e = 0; e < 2; ++e) {
+      u[e] = 0xffffu;
+      if (e0 + e < C::NX * (C::NX + 1) / 2) {
+        int i, j;
+        vxx_packed_coords(C::NX, e0 + e, i, j);
+        u[e] = (unsigned)(j * C::VS + i);
+      }
+    }
+    lut[r * 32 + lane] = (int)(u[0] | (u[1] << 16));
+  }
 }
 
 // ---------------------------------------------------------------------------
@@ -1055,7 +1083,8 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
 #define AB2_STAGE_B (p.stage + (size_t)inst * N * C::SREC_PAD)
 #define AB2_FF_B (p.ff + (size_t)inst * N * NR)
 #define AB2_FB_B (p.fb + (size_t)inst * N * NR * NX)
-#define AB2_VXX_B (p.Vxx + (size_t)inst * (N + 1) * NX * NX)
+#define AB2_VXX_B (p.Vxx + (size_t)inst * (N + 1) * C::VXX_REC)
+#define AB2_VXX0_B (C::VXX_PACKED ? p.Vxx0 + (size_t)inst * NX * NX : AB2_VXX_B)
 #define AB2_VX_B (p.vx + (size_t)inst * (N + 1) * NX)
   double *Vn = sm + C::S_VN;
   double *vxn = sm + C::S_VXN;
@@ -1363,7 +1392,7 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
               const double v = VV[mt][nt][e];
               if (jj < NX) {
                 if (t == 0)
-                  AB2_VXX_B[i + jj * NX] = v; // datas[0].Vxx is left unsymmetrised (A1)
+                  AB2_VXX0_B[i + jj * NX] = v; // datas[0].Vxx is left unsymmetrised (A1)
                 if (i >= jj) {            // V' = lower triangle mirrored (:216 of the next step)
                   Vn[i * VS + jj] = v;
                   Vn[jj * VS + i] = v;
@@ -1381,8 +1410,18 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
       ctx.async_fence(); // this lane's writes to V' become visible to the TMA store below
     ctx.sync();
     if (t > 0) { // symmetric Vxx_t, as the next step of the reference leaves it
-      double *Vt = AB2_VXX_B + (size_t)t * NX * NX;
-      if (C::VXX_BULK) { // V' is dense in shared memory: one TMA bulk store, no LDS/STG
+      double *Vt = AB2_VXX_B + (size_t)t * C::VXX_REC;
+      if constexpr (C::VXX_PACKED) { // the lower triangle, packed: one 16-byte store per pair of entries
+        AB2_UNROLL
+        for (int u = 0; u < C::VPU; ++u) {
+          const int e = 2 * (u * 32 + lane);
+          if (e < C::VP) {
+            const unsigned o = (unsigned)lut[(NT + NT * NT + u) * 32 + lane];
+            const unsigned o0 = o & 0xffffu, o1 = o >> 16;
+            stg2(Vt + e, o0 == 0xffffu ? 0.0 : Vn[o0], o1 == 0xffffu ? 0.0 : Vn[o1]);
+          }
+        }
+      } else if (C::VXX_BULK) { // V' is dense in shared memory: one TMA bulk store, no LDS/STG
         ctx.bulk_store(Vt, Vn, NX * NX);
       } else if (lane < NX) { // row `lane` of the symmetric V' = column `lane` of Vxx_t
         if (C::EVEN && (VS % 2 == 0)) {
@@ -1408,7 +1447,21 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
 #undef AB2_FF_B
 #undef AB2_FB_B
 #undef AB2_VXX_B
+#undef AB2_VXX0_B
 #undef AB2_VX_B
+
+// Lane j < NX stores packed column j (rows j..NX-1) of the symmetric V' (row j of V' in shared memory);
+// lane 0 also writes the padding entry.
+template <class C> AB2_D void store_packed_column(double *dst, const double *Vn, const int lane) {
+  constexpr int NX = C::NX;
+  double *col = dst + vxx_packed_col(NX, lane) - lane; // col[i] = entry (i, lane)
+  AB2_UNROLL
+  for (int i = 0; i < NX; ++i)
+    if (i >= lane)
+      col[i] = Vn[lane * C::VS + i];
+  if (C::VP > NX * (NX + 1) / 2 && lane == 0)
+    dst[C::VP - 1] = 0.0;
+}
 
 // ---------------------------------------------------------------------------
 // The sweep of one instance by one group.
@@ -1438,7 +1491,8 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
   const double *stage_b = p.stage + (size_t)inst * N * C::SREC_PAD;
   double *ff_b = p.ff + (size_t)inst * N * NR;
   double *fb_b = p.fb + (size_t)inst * N * NR * NX;
-  double *Vxx_b = p.Vxx + (size_t)inst * (N + 1) * NX * NX;
+  double *Vxx_b = p.Vxx + (size_t)inst * (N + 1) * C::VXX_REC;
+  double *Vxx0_b = C::VXX_PACKED ? p.Vxx0 + (size_t)inst * NX * NX : Vxx_b; // the block of slot 0, full
   double *vx_b = p.vx + (size_t)inst * (N + 1) * NX;
   int st = ST_OK;
   int pv = 0; // pivot statistics: +1 per 2x2 pivot, +0x10000 per interchange
@@ -1473,7 +1527,7 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
       const double *qt = tr + NX * NX;
       const double *Ct = qt + NX;            // nct x NX column-major
       const double *dt = Ct + (size_t)nct * NX;
-      double *VN = Vxx_b + (size_t)N * NX * NX;
+      double *VN = N > 0 ? Vxx_b + (size_t)N * C::VXX_REC : Vxx0_b;
       if (colA || colF) {
         // column j of Z = C/mu (or z = d/mu), then column j of Q + C^T Z (q + C^T z)
         double acc[NX];
@@ -1500,7 +1554,8 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
             vx_b[(size_t)N * NX + i] = s;
             vxn[i] = s;
           } else {
-            VN[i + lane * NX] = s; // as computed; re-written symmetric below when N > 0
+            if (!C::VXX_PACKED || N == 0)
+              VN[i + lane * NX] = s; // as computed; re-written symmetric below when N > 0
             if (i >= lane) {       // V' for the next step = lower triangle mirrored (:216)
               Vn[i * C::VS + lane] = s;
               Vn[lane * C::VS + i] = s;
@@ -1510,9 +1565,13 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
       }
       ctx.sync();
       if (colA && N > 0) { // step N-1 of the reference symmetrises datas[N].Vxx in place (A1)
-        AB2_UNROLL
-        for (int i = 0; i < NX; ++i)
-          VN[i + lane * NX] = Vn[lane * C::VS + i];
+        if constexpr (C::VXX_PACKED)
+          store_packed_column<C>(VN, Vn, lane);
+        else {
+          AB2_UNROLL
+          for (int i = 0; i < NX; ++i)
+            VN[i + lane * NX] = Vn[lane * C::VS + i];
+        }
       }
     }
 
@@ -1742,7 +1801,7 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
         }
         if (colA) {
           if (t == 0) { // datas[0].Vxx is left unsymmetrised (A1)
-            double *Vt = Vxx_b;
+            double *Vt = Vxx0_b;
             AB2_UNROLL
             for (int i = 0; i < NX; ++i)
               Vt[i + lane * NX] = h[i];
@@ -1765,10 +1824,14 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
         ctx.proxy_fence_smem(); // buffer the next bulk copy overwrites (issued after the sync below)
       ctx.sync();
       if (t > 0 && colA) { // symmetric Vxx_t, as the next step of the reference leaves it
-        double *Vt = Vxx_b + (size_t)t * NX * NX;
-        AB2_UNROLL
-        for (int i = 0; i < NX; ++i)
-          Vt[i + lane * NX] = Vn[lane * C::VS + i];
+        double *Vt = Vxx_b + (size_t)t * C::VXX_REC;
+        if constexpr (C::VXX_PACKED)
+          store_packed_column<C>(Vt, Vn, lane);
+        else {
+          AB2_UNROLL
+          for (int i = 0; i < NX; ++i)
+            Vt[i + lane * NX] = Vn[lane * C::VS + i];
+        }
       }
     }
 
@@ -1897,15 +1960,17 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
       ctx.proxy_fence();
     ctx.sync();
     auto fill_slot = [&](int d, int t) { // fb record of knot t -> ring slot d
-      if (FUSED) { // [K; Z; Ahat]_t | Vxx_t (symmetric for t >= 1: row i = column i) | vx_t
-        ctx.copy_expect(d, (t < N ? NR * NX + (C::FWD_FF ? NR : 0) : 0) + NX * NX + NX);
+      if (FUSED) { // [K; Z; Ahat]_t | Vxx_t (symmetric for t >= 1; no lambda row reads Vxx_0) | vx_t
+        constexpr int VR = C::VXX_REC;
+        ctx.copy_expect(d, (t < N ? NR * NX + (C::FWD_FF ? NR : 0) : 0) + (t > 0 ? VR : 0) + NX);
         if (t < N) {
           ctx.copy_add(d, ring + d * FS, fb_b + (size_t)t * NR * NX, NR * NX);
           if (C::FWD_FF)
-            ctx.copy_add(d, ring + d * FS + (NR + NX) * NX + NX, ff_b + (size_t)t * NR, NR);
+            ctx.copy_add(d, ring + d * FS + C::FWD_BIAS + NX, ff_b + (size_t)t * NR, NR);
         }
-        ctx.copy_add(d, ring + d * FS + NR * NX, Vxx_b + (size_t)t * NX * NX, NX * NX);
-        ctx.copy_add(d, ring + d * FS + (NR + NX) * NX, vx_b + (size_t)t * NX, NX);
+        if (t > 0)
+          ctx.copy_add(d, ring + d * FS + NR * NX, Vxx_b + (size_t)t * VR, VR);
+        ctx.copy_add(d, ring + d * FS + C::FWD_BIAS, vx_b + (size_t)t * NX, NX);
       } else if (C::FB_BULK) {
         ctx.issue_copy(d, ring + d * FS, fb_b + (size_t)t * NR * NX, NR * NX);
       } else { // odd record size: no 16-byte granularity, plain cooperative copy
@@ -1949,7 +2014,7 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
             if (FUSED ? ((r < NR && t < N) || (r >= NR && r < ROWS && t >= 1)) : (r < NR)) {
               double s0 = gff[d][q], s1 = 0.0; // two chains halve the dependent-FMA latency
               if (FUSED && (C::FWD_FF || r >= NR)) // ff_t sits right behind vx_t: one bias vector
-                s0 = slot[(NR + NX) * NX + (r >= NR ? r - NR : NX + r)];
+                s0 = slot[C::FWD_BIAS + (r >= NR ? r - NR : NX + r)];
               if (EVF) {
                 // Row r starts NX/2 16-byte units into the slot: with NX/2 = 2 mod 4 (nx = 4, 12)
                 // rows r and r+4 of a quarter-warp's 128-bit load fall on the same banks.  Those
@@ -1960,7 +2025,13 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
                 AB2_UNROLL
                 for (int c = 0; c < NX; c += 2) {
                   const int cc = (ROT && c + 2 == NX) ? (rot2 ? 0 : c) : c + rot2;
-                  const D2 gg = lds2(slot + r * NX + cc);
+                  D2 gg;
+                  if (C::VXX_PACKED && FUSED && r >= NR) { // row r - NR of the packed symmetric Vxx_t
+                    gg.x = slot[NR * NX + vxx_packed_index(NX, r - NR, cc)];
+                    gg.y = slot[NR * NX + vxx_packed_index(NX, r - NR, cc + 1)];
+                  } else {
+                    gg = lds2(slot + r * NX + cc);
+                  }
                   const D2 xx = lds2(xc + cc);
                   s0 += gg.x * xx.x;
                   s1 += gg.y * xx.y;
@@ -1998,10 +2069,11 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
     }
     // Pass 2 -- the parallel part: lbda_{t+1} = vx_{t+1} + Vxx_{t+1} x_{t+1} has no
     // dependence between knots: G/NX knots per iteration, two iterations batched so that
-    // all their loads are in flight together; no synchronisation.
+    // all their loads are in flight together; no synchronisation.  A packed row takes one
+    // predicated load per entry, and two batched iterations spill at nx = 14: one there.
     if (!FUSED) {
       constexpr int KPI = (C::G / NX) > 0 ? (C::G / NX) : 1; // knots per iteration
-      constexpr int U = 2;
+      constexpr int U = C::VXX_PACKED ? 1 : 2;
       const int sub = lane / NX, i = lane % NX;
       if (sub < KPI) {
         for (int t = sub; t < N; t += KPI * U) {
@@ -2010,7 +2082,21 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
           for (int u = 0; u < U; ++u) {
             const int tt = t + u * KPI;
             if (tt < N) {
-              load_row<NX, EVF>(Vxx_b + ((size_t)(tt + 1) * NX + i) * NX, vrow[u]); // row i (symmetric)
+              if constexpr (C::VXX_PACKED) { // row i of the packed symmetric Vxx_{tt+1}
+                // two bases, so that every load has a compile-time offset: entries (c, i), c >= i, lie
+                // at lo[c]; entries (i, c), c < i, at up[col(c) - c]
+                const double *V = Vxx_b + (size_t)(tt + 1) * C::VXX_REC;
+                const double *lo = V + vxx_packed_col(NX, i) - i, *up = V + i;
+                AB2_UNROLL
+                for (int c = 0; c < NX; ++c) {
+                  if (c >= i)
+                    vrow[u][c] = lo[c];
+                  else
+                    vrow[u][c] = up[vxx_packed_col(NX, c) - c];
+                }
+              } else {
+                load_row<NX, EVF>(Vxx_b + ((size_t)(tt + 1) * NX + i) * NX, vrow[u]); // row i (symmetric)
+              }
               load_row<NX, EVF>(xs_b + (size_t)(tt + 1) * NX, xr[u]);
               v0[u] = vx_b[(size_t)(tt + 1) * NX + i];
             }

@@ -276,8 +276,9 @@ inline cudaError_t launch_one(const SweepParams &p, int gd, cudaStream_t st, int
 //  10: as 7 with a single record buffer refilled in two parts (smallest shared-memory footprint)
 template <int NX, int NU, int NC, int G>
 inline cudaError_t launch_cfg(const SweepParams &p, int variant, const int gd[4], cudaStream_t st, int *info) {
-  using CS = Cfg<NX, NU, NC, G, false>;
-  using CD = Cfg<NX, NU, NC, G, true>;
+  // every device build stores Vxx packed (vxx_layout.h)
+  using CS = Cfg<NX, NU, NC, G, false, true, false, true>;
+  using CD = Cfg<NX, NU, NC, G, true, true, false, true>;
   if (variant < 0) {
     variant = 6;
     if constexpr (G == 32 && NC == 0 && NX % 2 == 0) {
@@ -286,7 +287,7 @@ inline cudaError_t launch_cfg(const SweepParams &p, int variant, const int gd[4]
       //   8: double-buffered records, 168 registers, no spills (<= 6 CTAs/SM)
       //  10: single record buffer, 128 registers: the smallest footprint (<= 8 CTAs/SM)
       // fewest rounds wins; ties go to 7 when it reaches 8 CTAs/SM, else 8, else 10.
-      using CM = Cfg<NX, NU, NC, G, true, true, true>;
+      using CM = Cfg<NX, NU, NC, G, true, true, true, true>;
       const int sms = p.num_sms > 0 ? p.num_sms : 132;
       const int grid = (p.batch + 1) / 2;
       auto ctas = [&](int gdw, int cap) {
@@ -314,30 +315,30 @@ inline cudaError_t launch_cfg(const SweepParams &p, int variant, const int gd[4]
   if (variant == 3)
     return launch_one<CS, 4, 72, false>(p, gd[0], st, info);
   if (variant == 4)
-    return launch_one<Cfg<NX, NU, NC, G, false, false>, 4, 72, true>(p, gd[0], st, info);
+    return launch_one<Cfg<NX, NU, NC, G, false, false, false, true>, 4, 72, true>(p, gd[0], st, info);
   if (variant == 5)
-    return launch_one<Cfg<NX, NU, NC, G, true, false>, 2, 144, true>(p, gd[1], st, info);
+    return launch_one<Cfg<NX, NU, NC, G, true, false, false, true>, 2, 144, true>(p, gd[1], st, info);
   if (variant == 6) // as 0 capped at 128 registers (8 CTAs/SM)
     return launch_one<CD, 2, 128, true>(p, gd[1], st, info);
   if constexpr (G == 32 && NC == 0 && NX % 2 == 0) {
-    using CM = Cfg<NX, NU, NC, G, true, true, true>;
+    using CM = Cfg<NX, NU, NC, G, true, true, true, true>;
     if (variant == 7) // stage step on the FP64 tensor cores (DMMA), 2 warps/CTA
       return launch_one<CM, 2, 128, true>(p, gd[2], st, info);
     if (variant == 8) // same, 168 registers
       return launch_one<CM, 2, 168, true>(p, gd[2], st, info);
     if (variant == 10) // same as 7 with a single record buffer refilled in two parts
-      return launch_one<Cfg<NX, NU, NC, G, false, true, true>, 2, 128, true>(p, gd[3], st, info);
+      return launch_one<Cfg<NX, NU, NC, G, false, true, true, true>, 2, 128, true>(p, gd[3], st, info);
   }
   return launch_one<CD, 2, 144, true>(p, gd[1], st, info);
 }
 template <int NX, int NU, int NC, int G> inline void group_doubles_cfg(int nc0, int gd[4]) {
-  gd[0] = Cfg<NX, NU, NC, G, false>::group_doubles(nc0);
-  gd[1] = Cfg<NX, NU, NC, G, true>::group_doubles(nc0);
+  gd[0] = Cfg<NX, NU, NC, G, false, true, false, true>::group_doubles(nc0);
+  gd[1] = Cfg<NX, NU, NC, G, true, true, false, true>::group_doubles(nc0);
   gd[2] = gd[1];
   gd[3] = gd[0];
   if constexpr (G == 32 && NC == 0 && NX % 2 == 0) {
-    gd[2] = Cfg<NX, NU, NC, G, true, true, true>::group_doubles(nc0);
-    gd[3] = Cfg<NX, NU, NC, G, false, true, true>::group_doubles(nc0);
+    gd[2] = Cfg<NX, NU, NC, G, true, true, true, true>::group_doubles(nc0);
+    gd[3] = Cfg<NX, NU, NC, G, false, true, true, true>::group_doubles(nc0);
   }
 }
 

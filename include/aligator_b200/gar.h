@@ -259,6 +259,15 @@ int ab2_gar_get_gains(ab2_gar_solver *s, double *dst, int memspace, void *stream
  * initial condition), constraint (C x + D u + d - mu v) and stationarity residuals.  Computed on
  * the device (one warp per (instance, knot)); dst in host or device memory. */
 int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace, void *stream);
+/* The device array behind an output, in its physical layout.  Every output except AB2_OUT_VXX has the layout
+ * ab2_gar_get returns (up to the ring heads of ab2_gar_cycle_append).  AB2_OUT_VXX, after a backward pass of the
+ * warp-per-instance kernel (every tuning variant except 9 on a plain serial handle whose shape has one; the
+ * CTA-per-instance, dense and parallel solvers keep [batch][N+1][nx*nx]):
+ *   [batch][N+1][P] lower triangles, P = nx(nx+1)/2 rounded up to even: knot t's Vxx, which is symmetric, packed
+ *                   column by column (LAPACK 'L': column j holds rows j..nx-1; the padding double is 0);
+ *   then [batch][nx*nx] the full column-major block of factor slot 0 (Vxx_0, which is not symmetric in general,
+ *                   or the terminal block when N = 0); packed slot 0 is unused.
+ * ab2_gar_get / ab2_gar_get_range expand this to full blocks. */
 int ab2_gar_device_ptr(ab2_gar_solver *s, int what, double **out);
 
 /* Multi-GPU (one process per GPU, the batch sharded by instance, SURVEY section 8e): the ONE exchange
@@ -427,7 +436,7 @@ int ab2_gar_synchronize(ab2_gar_solver *s, void *stream);
  * solver-proxddp.hpp:177-178: allocate once, never in the loop).  free(NULL) is a no-op. */
 int ab2_gar_pinned_alloc(size_t bytes, void **out);
 void ab2_gar_pinned_free(void *p);
-/* Kernels launched by this solver since creation (for bench accounting). */
+/* Kernels launched by this solver since creation (for bench accounting); the getters' copies do not count. */
 long ab2_gar_launch_count(const ab2_gar_solver *s);
 /* Shared memory per CTA / registers etc. of the kernel serving this solver
  * (*regs_per_thread: low 16 bits = registers, high 16 bits = resident CTAs per SM). */
