@@ -79,7 +79,8 @@ struct BlockDevCtx {
 
 // MAXREG 128: two or more CTAs per SM for the shapes whose buffers allow it; 255: the
 // large shapes, which own the SM anyway.
-template <int MAXREG, class D>
+// PI: per-instance mu (SweepParams::mueq_b, the *_v launches); false = the scalar p.mueq
+template <int MAXREG, class D, bool PI>
 __global__ void __launch_bounds__(256) __maxnreg__(MAXREG)
     riccati_block_kernel(const SweepParams p, const D d) {
   extern __shared__ __align__(16) double smem[];
@@ -92,7 +93,12 @@ __global__ void __launch_bounds__(256) __maxnreg__(MAXREG)
   ctx.init(reinterpret_cast<uint64_t *>(smem + d.s_end));
   const int legs = p.legs > 1 ? p.legs : 1; // leg mode: a work item is one (instance, leg)
   for (int item = blockIdx.x; item < p.batch * legs; item += gridDim.x) {
-    riccati_block_sweep(ctx, p, d, item / legs, smem, item % legs);
+    if constexpr (PI) {
+      riccati_block_sweep(ctx, p, d, item / legs, smem, item % legs, InstanceMu());
+      flag_bad_mu(p, item / legs, d.nc > 0 || p.nct > 0, ctx.tid == 0);
+    } else {
+      riccati_block_sweep(ctx, p, d, item / legs, smem, item % legs);
+    }
     __syncthreads();
   }
 }
@@ -116,7 +122,7 @@ __global__ void __launch_bounds__(256) condensed_kernel(const SweepParams p, con
 }
 
 // The stage-dense solver (riccati_dense.cuh): one CTA per instance, persistent over the batch.
-__global__ void __launch_bounds__(256) riccati_dense_kernel(const SweepParams p, const DenseDims d) {
+template <bool PI> __global__ void __launch_bounds__(256) riccati_dense_kernel(const SweepParams p, const DenseDims d) {
   extern __shared__ __align__(16) double smem[];
   BlockDevCtx ctx;
   ctx.tid = threadIdx.x;
@@ -127,7 +133,12 @@ __global__ void __launch_bounds__(256) riccati_dense_kernel(const SweepParams p,
   ctx.bar0 = 0;
   ctx.phase = 0;
   for (int inst = blockIdx.x; inst < p.batch; inst += gridDim.x) {
-    riccati_dense_sweep(ctx, p, d, inst, smem);
+    if constexpr (PI) {
+      riccati_dense_sweep(ctx, p, d, inst, smem, InstanceMu());
+      flag_bad_mu(p, inst, d.nc > 0 || p.nct > 0, ctx.tid == 0);
+    } else {
+      riccati_dense_sweep(ctx, p, d, inst, smem);
+    }
     __syncthreads();
   }
 }
@@ -175,7 +186,7 @@ bool block_supported(int nx, int nu, int nc, int nc0, int nth) {
 template <int MAXREG, class D>
 static cudaError_t launch_block_t(const SweepParams &p, const D &d, int threads, size_t smem,
                                   cudaStream_t st, int *info) {
-  auto kern = riccati_block_kernel<MAXREG, D>;
+  auto kern = p.mueq_b ? riccati_block_kernel<MAXREG, D, true> : riccati_block_kernel<MAXREG, D, false>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;
@@ -252,11 +263,12 @@ cudaError_t launch_dense(const SweepParams &p, int nx, int nu, int nc, cudaStrea
   const DenseDims d = make_dense_dims(nx, nu, nc, p.nct, p.nc0);
   const int threads = dense_threads(d);
   const size_t smem = (size_t)d.s_end * sizeof(double);
-  cudaError_t e = cudaFuncSetAttribute(riccati_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  auto kern = p.mueq_b ? riccati_dense_kernel<true> : riccati_dense_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;
   int nb = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, riccati_dense_kernel, threads, smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, threads, smem);
   if (e != cudaSuccess)
     return e;
   int dev = 0, sms = 132;
@@ -265,7 +277,7 @@ cudaError_t launch_dense(const SweepParams &p, int nx, int nu, int nc, cudaStrea
   int grid = sms * (nb > 0 ? nb : 1);
   if (grid > p.batch)
     grid = p.batch;
-  riccati_dense_kernel<<<grid, threads, smem, st>>>(p, d);
+  kern<<<grid, threads, smem, st>>>(p, d);
   return cudaGetLastError();
 }
 

@@ -265,6 +265,7 @@ struct ab2_gar_solver {
   double *gains_tmp = nullptr, *kkt_tmp = nullptr, *theta_dev = nullptr, *ls_tmp = nullptr;
   double *fddp_slack = nullptr, *fddp_G0 = nullptr, *fddp_g0 = nullptr, *fddp_vx = nullptr;
   double *inner_tmp = nullptr; // [batch][2] per-instance scalars of multipliers / criterion, for host destinations
+  double *mu_dev = nullptr;    // [batch] host-given per-instance mu of the *_v sweeps, staged for the kernels
   int nth = 0; // parameter dimension of the value function outputs (= nx in leg mode)
   int rec_nth = 0; // parameter blocks carried by the knot records (0 in leg mode)
   int legs = 0;    // >= 2: gar::ParallelRiccatiSolver (leg mode)
@@ -542,7 +543,7 @@ int ab2_gar_destroy(ab2_gar_solver *s) {
   if (s->pg_done)
     cudaFree(s->pg_done);
   for (double *q : {s->own_stage_sym, s->own_stage, s->own_term, s->own_G0, s->own_g0, s->gains_tmp, s->kkt_tmp, s->theta_dev, s->cond, s->ls_tmp, s->fddp_slack, s->fddp_G0,
-                    s->fddp_g0, s->fddp_vx, s->inner_tmp})
+                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev})
     if (q)
       cudaFree(q);
   for (int i = 0; i < ab2_gar_solver::kPipeStreams; ++i) {
@@ -710,20 +711,24 @@ static int run_kernels(ab2_gar_solver *s, ab2::SweepParams q, int bwd, int fwd, 
   return AB2_OK;
 }
 
-static int launch(ab2_gar_solver *s, double mueq, int bwd, int fwd, void *stream) {
+// mueq_b: per-instance mu ([batch], device) of a *_v call, or null for the scalar mueq.  It lives in this launch's
+// copy of the parameters only, so later scalar and forward-only calls never see it.
+static int launch(ab2_gar_solver *s, double mueq, const double *mueq_b, int bwd, int fwd, void *stream) {
   if (!s)
     return fail(AB2_ERR_INVALID, "null solver");
   if (!s->have_problem)
     return fail(AB2_ERR_STATE, "set_problem has not been called with all four buffers");
   if (fwd && !bwd && !s->have_backward)
     return fail(AB2_ERR_STATE, "forward() before backward()");
-  if (bwd && !(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
+  if (bwd && !mueq_b && !(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
     return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  s->p.mueq = mueq;
+  if (!mueq_b)
+    s->p.mueq = mueq;
   s->p.do_bwd = bwd;
   s->p.do_fwd = fwd;
   ab2::SweepParams q = s->p;
+  q.mueq_b = mueq_b;
   q.peer_world = 0;
   if (bwd && s->pg_in_sweep && s->pg_peer_base[0] && s->k && s->variant != 9 && s->legs <= 1 && !s->dense &&
       s->d.horizon > 0) {
@@ -748,9 +753,49 @@ static int launch(ab2_gar_solver *s, double mueq, int bwd, int fwd, void *stream
   return AB2_OK;
 }
 
-int ab2_gar_backward(ab2_gar_solver *s, double mueq, void *stream) { return launch(s, mueq, 1, 0, stream); }
-int ab2_gar_forward(ab2_gar_solver *s, void *stream) { return launch(s, s ? s->p.mueq : 0.0, 0, 1, stream); }
-int ab2_gar_sweep(ab2_gar_solver *s, double mueq, void *stream) { return launch(s, mueq, 1, 1, stream); }
+int ab2_gar_backward(ab2_gar_solver *s, double mueq, void *stream) { return launch(s, mueq, nullptr, 1, 0, stream); }
+int ab2_gar_forward(ab2_gar_solver *s, void *stream) { return launch(s, s ? s->p.mueq : 0.0, nullptr, 0, 1, stream); }
+int ab2_gar_sweep(ab2_gar_solver *s, double mueq, void *stream) { return launch(s, mueq, nullptr, 1, 1, stream); }
+
+// A per-instance mu array of a *_v sweep as the kernels read it.  Host arrays are checked by the scalar rule (mu > 0
+// when constraints are present) and staged, stream-ordered, into a buffer the handle owns; device arrays are used as
+// they are (the kernels flag an unusable value with status bit ST_BAD_MU).
+static int stage_mueq(ab2_gar_solver *s, const double *mueq, int memspace, cudaStream_t st, const double **dev) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  if (memspace == AB2_DEVICE) {
+    *dev = mueq;
+    return AB2_OK;
+  }
+  if (memspace != AB2_HOST)
+    return fail(AB2_ERR_INVALID, "memspace must be AB2_HOST or AB2_DEVICE");
+  if (s->d.nc > 0 || s->d.nct > 0)
+    for (int b = 0; b < s->d.batch; ++b)
+      if (!(mueq[b] > 0.0))
+        return fail(AB2_ERR_INVALID, "mueq[" + std::to_string(b) + "] must be > 0 when constraints are present");
+  CUDA_TRY(cudaSetDevice(s->d.device));
+  if (!s->mu_dev)
+    CUDA_TRY(cudaMalloc(&s->mu_dev, (size_t)s->d.batch * sizeof(double)));
+  CUDA_TRY(cudaMemcpyAsync(s->mu_dev, mueq, (size_t)s->d.batch * sizeof(double), cudaMemcpyHostToDevice, st));
+  *dev = s->mu_dev;
+  return AB2_OK;
+}
+static int launch_v(ab2_gar_solver *s, const double *mueq, int memspace, int fwd, void *stream) {
+  if (!s)
+    return fail(AB2_ERR_INVALID, "null solver");
+  if (!s->have_problem) // (checked before anything is staged)
+    return fail(AB2_ERR_STATE, "set_problem has not been called with all four buffers");
+  const double *dev = nullptr;
+  if (int rc = stage_mueq(s, mueq, memspace, (cudaStream_t)stream, &dev))
+    return rc;
+  return launch(s, 0.0, dev, 1, fwd, stream);
+}
+int ab2_gar_backward_v(ab2_gar_solver *s, const double *mueq, int memspace, void *stream) {
+  return launch_v(s, mueq, memspace, 0, stream);
+}
+int ab2_gar_sweep_v(ab2_gar_solver *s, const double *mueq, int memspace, void *stream) {
+  return launch_v(s, mueq, memspace, 1, stream);
+}
 int ab2_gar_forward_theta(ab2_gar_solver *s, const double *theta, int memspace, void *stream) {
   if (!s)
     return fail(AB2_ERR_INVALID, "null solver");
@@ -769,12 +814,13 @@ int ab2_gar_forward_theta(ab2_gar_solver *s, const double *theta, int memspace, 
       s->p.theta = s->theta_dev;
     }
   }
-  const int rc = launch(s, s->p.mueq, 0, 1, stream);
+  const int rc = launch(s, s->p.mueq, nullptr, 0, 1, stream);
   s->p.theta = nullptr;
   return rc;
 }
 
-int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream) {
+static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg_b, const double *mu_inv_b,
+                         void *stream) {
   if (!s || !in)
     return fail(AB2_ERR_INVALID, "null argument");
   if (s->rec_nth > 0)
@@ -799,7 +845,7 @@ int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream) {
   if ((rc = own(s->own_stage, stage_total(s))) != AB2_OK || (rc = own(s->own_term, (size_t)d.batch * s->trec)) != AB2_OK ||
       (rc = own(s->own_G0, (size_t)d.batch * d.nc0 * d.nx)) != AB2_OK || (rc = own(s->own_g0, (size_t)d.batch * d.nc0)) != AB2_OK)
     return rc;
-  CUDA_TRY(ab2::launch_lq_assemble(*in, s->own_stage, s->own_term, s->own_G0, s->own_g0, d.batch, d.horizon, d.nx,
+  CUDA_TRY(ab2::launch_lq_assemble(*in, preg_b, mu_inv_b, s->own_stage, s->own_term, s->own_G0, s->own_g0, d.batch, d.horizon, d.nx,
                                    d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec, (cudaStream_t)stream));
   s->launches += d.horizon > 0 ? 2 : 1;
   s->p.stage = s->own_stage;
@@ -809,6 +855,14 @@ int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream) {
   s->p.g0 = s->own_g0;
   s->have_problem = true;
   return AB2_OK;
+}
+int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream) {
+  return assemble_impl(s, in, nullptr, nullptr, stream);
+}
+int ab2_gar_assemble_v(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg, const double *mu_inv, void *stream) {
+  if (!preg || !mu_inv)
+    return fail(AB2_ERR_INVALID, "assemble_v: null preg / mu_inv array");
+  return assemble_impl(s, in, preg, mu_inv, stream);
 }
 
 static int copy_ring(const double *base, size_t rec, int knots, int nring, int head, int b0, int nb, int t0, int nt,
@@ -947,31 +1001,52 @@ int ab2_gar_pack_stage_sym(int nx, int nu, int nc, const double *stage, double *
 }
 
 static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double *term, const double *G0,
-                           const double *g0, double mueq, int nchunks, const int *whats,
+                           const double *g0, double mueq, const double *mueq_b, int nchunks, const int *whats,
                            double *const *dsts, int nwhat, void *stream, bool sym);
 int ab2_gar_sweep_host(ab2_gar_solver *s, const double *stage, const double *term, const double *G0,
                        const double *g0, double mueq, int nchunks, const int *whats,
                        double *const *dsts, int nwhat, void *stream) {
-  return sweep_host_impl(s, stage, term, G0, g0, mueq, nchunks, whats, dsts, nwhat, stream, false);
+  return sweep_host_impl(s, stage, term, G0, g0, mueq, nullptr, nchunks, whats, dsts, nwhat, stream, false);
+}
+int ab2_gar_sweep_host_v(ab2_gar_solver *s, const double *stage, const double *term, const double *G0,
+                         const double *g0, const double *mueq, int nchunks, const int *whats,
+                         double *const *dsts, int nwhat, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return sweep_host_impl(s, stage, term, G0, g0, 0.0, mueq, nchunks, whats, dsts, nwhat, stream, false);
 }
 int ab2_gar_sweep_host_sym(ab2_gar_solver *s, const double *stage_sym, const double *term, const double *G0,
                            const double *g0, double mueq, int nchunks, const int *whats,
                            double *const *dsts, int nwhat, void *stream) {
   if (s && (s->rec_nth > 0 || s->legs > 1 || s->dense))
     return fail(AB2_ERR_UNSUPPORTED, "sweep_host_sym: plain (nth = 0) serial handles only");
-  return sweep_host_impl(s, stage_sym, term, G0, g0, mueq, nchunks, whats, dsts, nwhat, stream, true);
+  return sweep_host_impl(s, stage_sym, term, G0, g0, mueq, nullptr, nchunks, whats, dsts, nwhat, stream, true);
+}
+int ab2_gar_sweep_host_sym_v(ab2_gar_solver *s, const double *stage_sym, const double *term, const double *G0,
+                             const double *g0, const double *mueq, int nchunks, const int *whats,
+                             double *const *dsts, int nwhat, void *stream) {
+  if (s && (s->rec_nth > 0 || s->legs > 1 || s->dense))
+    return fail(AB2_ERR_UNSUPPORTED, "sweep_host_sym: plain (nth = 0) serial handles only");
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return sweep_host_impl(s, stage_sym, term, G0, g0, 0.0, mueq, nchunks, whats, dsts, nwhat, stream, true);
 }
 
+// mueq_b: per-instance mu in HOST memory (the *_v calls) or null for the scalar mueq
 static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double *term, const double *G0,
-                           const double *g0, double mueq, int nchunks, const int *whats,
+                           const double *g0, double mueq, const double *mueq_b, int nchunks, const int *whats,
                            double *const *dsts, int nwhat, void *stream, const bool sym) {
   if (!s || !stage || !term || (s->d.nc0 > 0 && (!G0 || !g0)) || nwhat < 0 || (nwhat > 0 && (!whats || !dsts)))
     return fail(AB2_ERR_INVALID, "bad argument");
   for (int i = 0; i < nwhat; ++i)
     if (whats[i] < 0 || whats[i] >= AB2_OUT_COUNT || !dsts[i])
       return fail(AB2_ERR_INVALID, "bad output selector");
-  if (!(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
+  if (!mueq_b && !(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
     return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  const double *mu_dev = nullptr; // (staged on the caller's stream, before the fork below)
+  if (mueq_b)
+    if (int rc = stage_mueq(s, mueq_b, AB2_HOST, (cudaStream_t)stream, &mu_dev))
+      return rc;
   CUDA_TRY(cudaSetDevice(s->d.device));
   const int B = s->d.batch, N = s->d.horizon, nx = s->d.nx, nc0 = s->d.nc0;
   constexpr int NS = ab2_gar_solver::kPipeStreams;
@@ -1000,7 +1075,8 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
   s->p.G0 = s->own_G0;
   s->p.g0 = s->own_g0;
   s->have_problem = true;
-  s->p.mueq = mueq;
+  if (!mueq_b)
+    s->p.mueq = mueq;
   s->p.do_bwd = 1;
   s->p.do_fwd = 1;
   if (nchunks <= 0) { // enough slices to hide the first upload / last download, each still one full wave
@@ -1061,7 +1137,9 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
       }
     } else if ((rc = up(s->own_stage, stage, (size_t)N * s->srec)) != AB2_OK)
       return rc;
-    const ab2::SweepParams q = slice_params(s, b0, nb);
+    ab2::SweepParams q = slice_params(s, b0, nb);
+    if (mu_dev)
+      q.mueq_b = mu_dev + b0;
     if (int rc2 = run_kernels(s, q, 1, 1, st))
       return rc2;
     for (int i = 0; i < nwhat; ++i) {
@@ -1214,7 +1292,7 @@ int ab2_gar_get_gains(ab2_gar_solver *s, double *dst, int memspace, void *stream
   return AB2_OK;
 }
 
-int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace, void *stream) {
+static int kkt_error_impl(ab2_gar_solver *s, double mueq, const double *mueq_b, double *dst, int memspace, void *stream) {
   if (!s || !dst)
     return fail(AB2_ERR_INVALID, "bad argument");
   if (!s->have_problem || !s->have_backward || !s->have_forward)
@@ -1236,6 +1314,7 @@ int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace,
   a.trec = s->trec;
   a.stage_head = s->p.stage_head;
   a.mueq = mueq;
+  a.mueq_b = mueq_b;
   a.stage = s->p.stage;
   a.term = s->p.term;
   a.G0 = s->p.G0;
@@ -1253,6 +1332,14 @@ int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace,
     CUDA_TRY(cudaMemcpyAsync(dst, s->kkt_tmp, (size_t)s->d.batch * 3 * sizeof(double), cudaMemcpyDeviceToHost,
                              (cudaStream_t)stream));
   return AB2_OK;
+}
+int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace, void *stream) {
+  return kkt_error_impl(s, mueq, nullptr, dst, memspace, stream);
+}
+int ab2_gar_kkt_error_v(ab2_gar_solver *s, const double *mueq, double *dst, int memspace, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return kkt_error_impl(s, 0.0, mueq, dst, memspace, stream);
 }
 
 int ab2_gar_device_ptr(ab2_gar_solver *s, int what, double **out) {
@@ -1301,8 +1388,8 @@ static int ls_result(ab2_gar_solver *s, double *dst, int memspace, cudaStream_t 
   (void)st;
   return AB2_OK;
 }
-int ab2_gar_linear_step(ab2_gar_solver *s, double alpha, const ab2_ls_iterate *cur, const ab2_ls_trial *trial,
-                        void *stream) {
+static int linear_step_impl(ab2_gar_solver *s, double alpha, const double *alpha_b, const ab2_ls_iterate *cur,
+                            const ab2_ls_trial *trial, void *stream) {
   if (!s || !cur || !trial)
     return fail(AB2_ERR_INVALID, "null argument");
   if (!s->have_forward)
@@ -1316,9 +1403,19 @@ int ab2_gar_linear_step(ab2_gar_solver *s, double alpha, const ab2_ls_iterate *c
   CUDA_TRY(cudaSetDevice(d.device));
   ab2::LinearStepIO io{cur->xs, cur->us, cur->vs, cur->vsT, cur->lam0, cur->lams,
                        trial->xs, trial->us, trial->vs, trial->vsT, trial->lam0, trial->lams};
-  CUDA_TRY(ab2::launch_linear_step(ls_args(s), io, alpha, (cudaStream_t)stream));
+  CUDA_TRY(ab2::launch_linear_step(ls_args(s), io, alpha, alpha_b, (cudaStream_t)stream));
   s->launches += 1;
   return AB2_OK;
+}
+int ab2_gar_linear_step(ab2_gar_solver *s, double alpha, const ab2_ls_iterate *cur, const ab2_ls_trial *trial,
+                        void *stream) {
+  return linear_step_impl(s, alpha, nullptr, cur, trial, stream);
+}
+int ab2_gar_linear_step_v(ab2_gar_solver *s, const double *alpha, const ab2_ls_iterate *cur, const ab2_ls_trial *trial,
+                          void *stream) {
+  if (!alpha)
+    return fail(AB2_ERR_INVALID, "null alpha array");
+  return linear_step_impl(s, 0.0, alpha, cur, trial, stream);
 }
 int ab2_gar_directional_derivative(ab2_gar_solver *s, const double *Lxs, const double *Lus, double *dst, int memspace,
                                    void *stream) {
@@ -1336,8 +1433,8 @@ int ab2_gar_directional_derivative(ab2_gar_solver *s, const double *Lxs, const d
     CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)s->d.batch * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return AB2_OK;
 }
-int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, double mudyn, double mucstr,
-                     double *dst, int memspace, void *stream) {
+static int al_value_impl(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, double mudyn, double mucstr,
+                         const double *mudyn_b, const double *mucstr_b, double *dst, int memspace, void *stream) {
   if (!s || !plus || !dst)
     return fail(AB2_ERR_INVALID, "null argument");
   const ab2_gar_dims &d = s->d;
@@ -1349,11 +1446,21 @@ int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double
   if (int rc = ls_result(s, dst, memspace, (cudaStream_t)stream, &dev))
     return rc;
   CUDA_TRY(ab2::launch_al_value(d.batch, d.horizon, d.nx, d.nc, d.nct, d.nc0, plus->lam0, plus->lams, plus->vs, plus->vsT,
-                                cost, mudyn, mucstr, dev, (cudaStream_t)stream));
+                                cost, mudyn, mucstr, mudyn_b, mucstr_b, dev, (cudaStream_t)stream));
   s->launches += 1;
   if (memspace != AB2_DEVICE)
     CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return AB2_OK;
+}
+int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, double mudyn, double mucstr,
+                     double *dst, int memspace, void *stream) {
+  return al_value_impl(s, plus, cost, mudyn, mucstr, nullptr, nullptr, dst, memspace, stream);
+}
+int ab2_gar_al_value_v(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, const double *mudyn,
+                       const double *mucstr, double *dst, int memspace, void *stream) {
+  if (!mudyn || !mucstr)
+    return fail(AB2_ERR_INVALID, "al_value_v: null mudyn / mucstr array");
+  return al_value_impl(s, plus, cost, 0.0, 0.0, mudyn, mucstr, dst, memspace, stream);
 }
 
 // ---- multipliers, Lagrangian gradient, criterion (proxddp_inner.cu) ----
@@ -1372,8 +1479,8 @@ static int inner_result(ab2_gar_solver *s, double *dst, int memspace, double **d
   *dev = s->inner_tmp;
   return AB2_OK;
 }
-int ab2_gar_multipliers(ab2_gar_solver *s, const ab2_mult_inputs *in, const ab2_mult_outputs *out, double *dst,
-                        int memspace, void *stream) {
+static int multipliers_impl(ab2_gar_solver *s, const ab2_mult_inputs *in, const double *mu_b, const double *mu_dyn_b,
+                            const ab2_mult_outputs *out, double *dst, int memspace, void *stream) {
   if (!s || !in || !out || !dst)
     return fail(AB2_ERR_INVALID, "null argument");
   const ab2_gar_dims &d = s->d;
@@ -1388,17 +1495,27 @@ int ab2_gar_multipliers(ab2_gar_solver *s, const ab2_mult_inputs *in, const ab2_
                                   out->shifted_N && out->Lv_N));
   if (!ok)
     return fail(AB2_ERR_INVALID, "multipliers: a required array is NULL for these dimensions");
-  if (!(in->mu > 0.0) || !(in->mu_dyn > 0.0))
+  if (!mu_b && (!(in->mu > 0.0) || !(in->mu_dyn > 0.0)))
     return fail(AB2_ERR_INVALID, "multipliers: mu and mu_dyn must be positive");
   CUDA_TRY(cudaSetDevice(d.device));
   double *dev = nullptr;
   if (int rc = inner_result(s, dst, memspace, &dev))
     return rc;
-  CUDA_TRY(ab2::launch_multipliers(inner_dims(s), *in, *out, dev, (cudaStream_t)stream));
+  CUDA_TRY(ab2::launch_multipliers(inner_dims(s), *in, mu_b, mu_dyn_b, *out, dev, (cudaStream_t)stream));
   s->launches += 1;
   if (memspace != AB2_DEVICE)
     CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * 2 * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return AB2_OK;
+}
+int ab2_gar_multipliers(ab2_gar_solver *s, const ab2_mult_inputs *in, const ab2_mult_outputs *out, double *dst,
+                        int memspace, void *stream) {
+  return multipliers_impl(s, in, nullptr, nullptr, out, dst, memspace, stream);
+}
+int ab2_gar_multipliers_v(ab2_gar_solver *s, const ab2_mult_inputs *in, const double *mu, const double *mu_dyn,
+                          const ab2_mult_outputs *out, double *dst, int memspace, void *stream) {
+  if (!mu || !mu_dyn)
+    return fail(AB2_ERR_INVALID, "multipliers_v: null mu / mu_dyn array");
+  return multipliers_impl(s, in, mu, mu_dyn, out, dst, memspace, stream);
 }
 int ab2_gar_lagrangian_gradient(ab2_gar_solver *s, const ab2_lag_inputs *in, const ab2_lag_outputs *out, void *stream) {
   if (!s || !in || !out)
@@ -1439,7 +1556,8 @@ int ab2_gar_criterion(ab2_gar_solver *s, const double *Lxs, const double *Lus, c
   return AB2_OK;
 }
 
-int ab2_fddp_backward_pass(ab2_gar_solver *s, const ab2_fddp_inputs *in, double *Vx_out, double *Quuks_out, void *stream) {
+static int fddp_backward_impl(ab2_gar_solver *s, const ab2_fddp_inputs *in, const double *preg_b, double *Vx_out,
+                              double *Quuks_out, void *stream) {
   if (!s || !in)
     return fail(AB2_ERR_INVALID, "null argument");
   const ab2_gar_dims &d = s->d;
@@ -1478,7 +1596,7 @@ int ab2_fddp_backward_pass(ab2_gar_solver *s, const ab2_fddp_inputs *in, double 
   lq.g0 = s->fddp_g0;
   lq.preg = in->preg; // Q, R and the terminal Q carry + preg I (:217, :246, :273)
   lq.mu_inv = 1.0;
-  if ((rc = ab2_gar_assemble(s, &lq, stream)) != AB2_OK)
+  if ((rc = assemble_impl(s, &lq, preg_b, nullptr, stream)) != AB2_OK)
     return rc;
   if ((rc = ab2_gar_backward(s, 1.0, stream)) != AB2_OK) // (mueq is unused without constraints)
     return rc;
@@ -1493,6 +1611,15 @@ int ab2_fddp_backward_pass(ab2_gar_solver *s, const ab2_fddp_inputs *in, double 
     s->launches += 1;
   }
   return AB2_OK;
+}
+int ab2_fddp_backward_pass(ab2_gar_solver *s, const ab2_fddp_inputs *in, double *Vx_out, double *Quuks_out, void *stream) {
+  return fddp_backward_impl(s, in, nullptr, Vx_out, Quuks_out, stream);
+}
+int ab2_fddp_backward_pass_v(ab2_gar_solver *s, const ab2_fddp_inputs *in, const double *preg, double *Vx_out,
+                             double *Quuks_out, void *stream) {
+  if (!preg)
+    return fail(AB2_ERR_INVALID, "fddp_backward_pass_v: null preg array");
+  return fddp_backward_impl(s, in, preg, Vx_out, Quuks_out, stream);
 }
 
 int ab2_gar_collapse_feedback(ab2_gar_solver *s, void *stream) {

@@ -55,7 +55,7 @@ __global__ void __launch_bounds__(256) kkt_error_kernel(const KktErrorArgs a) {
         dynE = upd(dynE, s);
       }
     for (int i = lane; i < ncc; i += 32) { // C x + D u + d - mu v (:110-116)
-      double s = d[i] - a.mueq * v[i];
+      double s = d[i] - (a.mueq_b ? a.mueq_b[b] : a.mueq) * v[i];
       for (int c = 0; c < nx; ++c)
         s += C[i + (long)c * ncc] * x[c];
       for (int c = 0; c < nuu; ++c)

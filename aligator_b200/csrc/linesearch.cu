@@ -15,30 +15,33 @@
 
 namespace ab2 {
 
+// PI: per-instance step lengths alpha_b (ab2_gar_linear_step_v); false = the scalar alpha
+template <bool PI>
 __global__ void __launch_bounds__(256)
-    linear_step_kernel(const LineSearchArgs a, const LinearStepIO io, const double alpha) {
+    linear_step_kernel(const LineSearchArgs a, const LinearStepIO io, const double alpha, const double *__restrict__ alpha_b) {
   const long nX = (long)a.batch * (a.N + 1) * a.nx, nU = (long)a.batch * a.N * a.nu, nV = (long)a.batch * a.N * a.nc,
              nVT = (long)a.batch * a.nct, nL0 = (long)a.batch * a.nc0, nL = (long)a.batch * a.N * a.nx;
   const long total = nX + nU + nV + nVT + nL0 + nL;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    long j = i;
+    long j = i, per; // per: elements of one instance in this array
     const double *cur, *stp;
     double *out;
     if (j < nX) {
-      cur = io.xs, stp = a.dxs, out = io.txs;
+      cur = io.xs, stp = a.dxs, out = io.txs, per = (long)(a.N + 1) * a.nx;
     } else if ((j -= nX) < nU) {
-      cur = io.us, stp = a.dus, out = io.tus;
+      cur = io.us, stp = a.dus, out = io.tus, per = (long)a.N * a.nu;
     } else if ((j -= nU) < nV) {
-      cur = io.vs, stp = a.dvs, out = io.tvs;
+      cur = io.vs, stp = a.dvs, out = io.tvs, per = (long)a.N * a.nc;
     } else if ((j -= nV) < nVT) {
-      cur = io.vsT, stp = a.dvsT, out = io.tvsT;
+      cur = io.vsT, stp = a.dvsT, out = io.tvsT, per = a.nct;
     } else if ((j -= nVT) < nL0) {
-      cur = io.lam0, stp = a.dlam0, out = io.tlam0;
+      cur = io.lam0, stp = a.dlam0, out = io.tlam0, per = a.nc0;
     } else {
       j -= nL0;
-      cur = io.lams, stp = a.dlams, out = io.tlams;
+      cur = io.lams, stp = a.dlams, out = io.tlams, per = (long)a.N * a.nx;
     }
-    out[j] = cur[j] + alpha * stp[j]; // results + alpha * step, as vectorMultiplyAdd / integrate write it
+    const double al = PI ? alpha_b[j / per] : alpha; // the alpha of the instance that owns the element
+    out[j] = cur[j] + al * stp[j]; // results + alpha * step, as vectorMultiplyAdd / integrate write it
   }
 }
 
@@ -78,12 +81,14 @@ __global__ void __launch_bounds__(256)
 __global__ void __launch_bounds__(256)
     al_value_kernel(const int batch, const int N, const int nx, const int nc, const int nct, const int nc0,
                     const double *__restrict__ lam0, const double *__restrict__ lams, const double *__restrict__ vs,
-                    const double *__restrict__ vsT, const double *__restrict__ cost, const double mudyn,
-                    const double mucstr, double *__restrict__ out) {
+                    const double *__restrict__ vsT, const double *__restrict__ cost, const double mudyn_s,
+                    const double mucstr_s, const double *__restrict__ mudyn_b, const double *__restrict__ mucstr_b,
+                    double *__restrict__ out) {
   const int lane = threadIdx.x & 31;
   const long warp = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long nwarps = ((long)gridDim.x * blockDim.x) >> 5;
   for (long b = warp; b < batch; b += nwarps) {
+    const double mudyn = mudyn_b ? mudyn_b[b] : mudyn_s, mucstr = mucstr_b ? mucstr_b[b] : mucstr_s;
     double sl0 = 0.0, sl = 0.0, sv = 0.0;
     for (long i = lane; i < nc0; i += 32)
       sl0 += lam0[b * nc0 + i] * lam0[b * nc0 + i];
@@ -109,9 +114,13 @@ static int grid_for(long work_items, int per_cta) {
   return g < 1 ? 1 : (int)g;
 }
 
-cudaError_t launch_linear_step(const LineSearchArgs &a, const LinearStepIO &io, double alpha, cudaStream_t st) {
+cudaError_t launch_linear_step(const LineSearchArgs &a, const LinearStepIO &io, double alpha, const double *alpha_b,
+                               cudaStream_t st) {
   const long total = (long)a.batch * ((long)(a.N + 1) * a.nx + (long)a.N * (a.nu + a.nc + a.nx) + a.nct + a.nc0);
-  linear_step_kernel<<<grid_for(total, 256 * 4), 256, 0, st>>>(a, io, alpha);
+  if (alpha_b)
+    linear_step_kernel<true><<<grid_for(total, 256 * 4), 256, 0, st>>>(a, io, alpha, alpha_b);
+  else
+    linear_step_kernel<false><<<grid_for(total, 256 * 4), 256, 0, st>>>(a, io, alpha, alpha_b);
   return cudaGetLastError();
 }
 cudaError_t launch_directional_derivative(const LineSearchArgs &a, const double *Lxs, const double *Lus, double *out,
@@ -121,9 +130,9 @@ cudaError_t launch_directional_derivative(const LineSearchArgs &a, const double 
 }
 cudaError_t launch_al_value(int batch, int N, int nx, int nc, int nct, int nc0, const double *lam0, const double *lams,
                             const double *vs, const double *vsT, const double *cost, double mudyn, double mucstr,
-                            double *out, cudaStream_t st) {
+                            const double *mudyn_b, const double *mucstr_b, double *out, cudaStream_t st) {
   al_value_kernel<<<grid_for(batch, 8), 256, 0, st>>>(batch, N, nx, nc, nct, nc0, lam0, lams, vs, vsT, cost, mudyn,
-                                                        mucstr, out);
+                                                        mucstr, mudyn_b, mucstr_b, out);
   return cudaGetLastError();
 }
 

@@ -34,8 +34,11 @@ struct StageTables {
 // A warp per record (grid-stride), lanes stride over the record's elements
 // [A | B | f | Q | S | R | q | r | C | D | d | pad], UNR elements per lane in flight:
 // unit-stride reads of every source block and unit-stride writes of the record.
+// PI: per-instance preg (and mu_inv, when given) arrays (ab2_gar_assemble_v); false = the scalars of `in`
+template <bool PI>
 __global__ void __launch_bounds__(256, 4)
-    lq_assemble_stage_kernel(const ab2_lq_inputs in, double *__restrict__ stage, long nrec, int N, int nx,
+    lq_assemble_stage_kernel(const ab2_lq_inputs in, const double *__restrict__ preg_b,
+                             const double *__restrict__ mu_inv_b, double *__restrict__ stage, long nrec, int N, int nx,
                              int nu, int nc, int srec) {
   extern __shared__ int2 tab[]; // [srec]: x = source | flags << 8 | row << 16, y = offset in the source block
   __shared__ StageTables T;
@@ -122,7 +125,7 @@ __global__ void __launch_bounds__(256, 4)
         if (fl & F_ZERO)
           v[u] = 0.0;
         if (fl & F_DIAG)
-          v[u] += in.preg;
+          v[u] += PI ? preg_b[inst] : in.preg;
         if (fl & F_HESS)
           v[u] += h[u];
         if ((fl & F_H0) && t == 0)
@@ -138,7 +141,7 @@ __global__ void __launch_bounds__(256, 4)
           const int jj = ent[u].y;
           double full = 0.0, proj = 0.0;
           for (int i = 0; i < nc; ++i) {
-            const double lv = in.Lv[rec * nc + i] * in.mu_inv;
+            const double lv = in.Lv[rec * nc + i] * (PI && mu_inv_b ? mu_inv_b[inst] : in.mu_inv);
             const double pij = P[i + (long)jj * nc];
             const double a = row_active(in.shifted[rec * nc + i], in.lo[i], in.hi[i]) ? 1.0 : 0.0;
             full += pij * lv;
@@ -159,7 +162,8 @@ __global__ void __launch_bounds__(256, 4)
 
 // Terminal knot (:785-795), initial condition (:797-800): a warp per instance.
 __global__ void __launch_bounds__(256)
-    lq_assemble_term_kernel(const ab2_lq_inputs in, double *__restrict__ term, double *__restrict__ G0,
+    lq_assemble_term_kernel(const ab2_lq_inputs in, const double *__restrict__ preg_b,
+                            const double *__restrict__ mu_inv_b, double *__restrict__ term, double *__restrict__ G0,
                             double *__restrict__ g0, int batch, int N, int nx, int nct, int nc0, int trec) {
   const int lane = threadIdx.x & 31;
   const long warp = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -167,13 +171,14 @@ __global__ void __launch_bounds__(256)
   const int nxx = nx * nx;
   for (long b = warp; b < batch; b += nwarps) {
     double *dst = term + b * trec;
+    const double preg = preg_b ? preg_b[b] : in.preg, mu_inv = mu_inv_b ? mu_inv_b[b] : in.mu_inv;
     for (int e = lane; e < nxx; e += 32) // knot.Q = tcd.Lxx_; diag += preg
-      dst[e] = in.Lxx_N[b * nxx + e] + ((e % (nx + 1) == 0) ? in.preg : 0.0) +
+      dst[e] = in.Lxx_N[b * nxx + e] + ((e % (nx + 1) == 0) ? preg : 0.0) +
                ((N == 0 && in.Hxx0) ? in.Hxx0[b * nxx + e] : 0.0); // stages[0] is the terminal knot when N = 0 (:803-804)
     for (int j = lane; j < nx; j += 32) { // knot.q = Lxs[N] + cstr_lx_corr[N]
       double full = 0.0, proj = 0.0;
       for (int i = 0; i < nct; ++i) {
-        const double lv = in.Lv_N[b * nct + i] * in.mu_inv;
+        const double lv = in.Lv_N[b * nct + i] * mu_inv;
         const double pij = in.cJx_N[b * nct * nx + i + (long)j * nct];
         const double a = row_active(in.shifted_N[b * nct + i], in.loN[i], in.hiN[i]) ? 1.0 : 0.0;
         full += pij * lv;
@@ -195,7 +200,7 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-cudaError_t launch_lq_assemble(const ab2_lq_inputs &in, double *stage, double *term, double *G0, double *g0,
+cudaError_t launch_lq_assemble(const ab2_lq_inputs &in, const double *preg_b, const double *mu_inv_b, double *stage, double *term, double *G0, double *g0,
                                int batch, int N, int nx, int nu, int nc, int nct, int nc0, int srec, int trec,
                                cudaStream_t st) {
   int dev = 0, sms = 132;
@@ -208,11 +213,11 @@ cudaError_t launch_lq_assemble(const ab2_lq_inputs &in, double *stage, double *t
     if (grid > full)
       grid = full;
     const size_t tab_bytes = (size_t)srec * sizeof(int2);
-    cudaError_t e0 = cudaFuncSetAttribute(lq_assemble_stage_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)tab_bytes);
+    auto kern = preg_b ? lq_assemble_stage_kernel<true> : lq_assemble_stage_kernel<false>;
+    cudaError_t e0 = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tab_bytes);
     if (e0 != cudaSuccess)
       return e0;
-    lq_assemble_stage_kernel<<<(int)grid, 256, tab_bytes, st>>>(in, stage, nrec, N, nx, nu, nc, srec);
+    kern<<<(int)grid, 256, tab_bytes, st>>>(in, preg_b, mu_inv_b, stage, nrec, N, nx, nu, nc, srec);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess)
       return e;
@@ -220,7 +225,7 @@ cudaError_t launch_lq_assemble(const ab2_lq_inputs &in, double *stage, double *t
   long grid = ((long)batch + 7) / 8;
   if (grid > full)
     grid = full;
-  lq_assemble_term_kernel<<<(int)grid, 256, 0, st>>>(in, term, G0, g0, batch, N, nx, nct, nc0, trec);
+  lq_assemble_term_kernel<<<(int)grid, 256, 0, st>>>(in, preg_b, mu_inv_b, term, G0, g0, batch, N, nx, nct, nc0, trec);
   return cudaGetLastError();
 }
 

@@ -32,14 +32,19 @@ __device__ __forceinline__ double normal_cone(double z, double lo, double hi) {
   return z - c;
 }
 
+// PI: per-instance mu_b / mu_dyn_b (ab2_gar_multipliers_v); false = the scalars of `in`
+template <bool PI>
 __global__ void __launch_bounds__(256)
-    multipliers_kernel(const InnerDims d, const ab2_mult_inputs in, const ab2_mult_outputs out, double *__restrict__ out2) {
+    multipliers_kernel(const InnerDims d, const ab2_mult_inputs in, const double *__restrict__ mu_b,
+                       const double *__restrict__ mu_dyn_b, const ab2_mult_outputs out, double *__restrict__ out2) {
   const int lane = threadIdx.x & 31;
   const long warp = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long nwarps = ((long)gridDim.x * blockDim.x) >> 5;
-  const double mu = in.mu, mu_dyn = in.mu_dyn, mu_inv = 1.0 / mu; // mu_inv() = 1 / mu()
+  const double mu_s = in.mu, mu_dyn_s = in.mu_dyn, mu_inv_s = 1.0 / mu_s; // mu_inv() = 1 / mu()
   const long nD = (long)d.N * d.nx, nV = (long)d.N * d.nc;
   for (long b = warp; b < d.batch; b += nwarps) {
+    const double mu = PI ? mu_b[b] : mu_s, mu_dyn = PI ? mu_dyn_b[b] : mu_dyn_s;
+    const double mu_inv = PI ? 1.0 / mu : mu_inv_s; // the same quotient, per instance
     double dyn = 0.0, infeas = 0.0; // |fs|_inf, |stage_infeas|_inf
     bool ok = true;
     // initial constraint: fs[0] = value_, lams_plus[0] = lams[0] + fs[0] / mu()   (:244-248)
@@ -266,9 +271,12 @@ static int warp_grid(long warps_needed) { // 8 warps per CTA, at most 8 CTAs per
   return g < 1 ? 1 : (int)g;
 }
 
-cudaError_t launch_multipliers(const InnerDims &d, const ab2_mult_inputs &in, const ab2_mult_outputs &out,
-                               double *out2, cudaStream_t st) {
-  multipliers_kernel<<<warp_grid(d.batch), 256, 0, st>>>(d, in, out, out2);
+cudaError_t launch_multipliers(const InnerDims &d, const ab2_mult_inputs &in, const double *mu_b, const double *mu_dyn_b,
+                               const ab2_mult_outputs &out, double *out2, cudaStream_t st) {
+  if (mu_b)
+    multipliers_kernel<true><<<warp_grid(d.batch), 256, 0, st>>>(d, in, mu_b, mu_dyn_b, out, out2);
+  else
+    multipliers_kernel<false><<<warp_grid(d.batch), 256, 0, st>>>(d, in, mu_b, mu_dyn_b, out, out2);
   return cudaGetLastError();
 }
 

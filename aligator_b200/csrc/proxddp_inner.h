@@ -9,9 +9,10 @@ namespace ab2 {
 struct InnerDims {
   int batch, N, nx, nu, nc, nct, nc0;
 };
-// computeMultipliers (solver-proxddp.hxx:220-318); out2 [batch][2] = [prim_infeas, finite]
-cudaError_t launch_multipliers(const InnerDims &d, const ab2_mult_inputs &in, const ab2_mult_outputs &out,
-                               double *out2, cudaStream_t st);
+// computeMultipliers (solver-proxddp.hxx:220-318); out2 [batch][2] = [prim_infeas, finite];
+// mu_b, mu_dyn_b: [batch] per-instance values (device) replacing in.mu / in.mu_dyn, or null
+cudaError_t launch_multipliers(const InnerDims &d, const ab2_mult_inputs &in, const double *mu_b, const double *mu_dyn_b,
+                               const ab2_mult_outputs &out, double *out2, cudaStream_t st);
 // LagrangianDerivatives::compute (core/lagrangian.hpp:29-92) into the non-NULL outputs
 cudaError_t launch_lagrangian_gradient(const InnerDims &d, const ab2_lag_inputs &in, const ab2_lag_outputs &out,
                                        cudaStream_t st);

@@ -537,14 +537,14 @@ constexpr int BLK_CH = 4; // n-tiles accumulated together by one warp (one work 
 // ---------------------------------------------------------------------------
 // The sweep of one instance by one CTA.
 // ---------------------------------------------------------------------------
-template <class Ctx, class D>
+// mu: where this instance's mu is read (ScalarMu / InstanceMu, riccati_group.cuh).
+template <class Ctx, class D, class Mu = ScalarMu>
 AB2_D void riccati_block_sweep(Ctx &ctx, const SweepParams &p, const D &d, const int inst,
-                               double *__restrict__ sm, const int leg = 0) {
+                               double *__restrict__ sm, const int leg = 0, const Mu &mu = Mu()) {
   const int nx = d.nx, nu = d.nu, nc = d.nc, nk = d.nk, nr = d.nr;
   const int tid = ctx.tid, T = ctx.nthreads, warp = ctx.warp, lane = ctx.lane, NW = ctx.nwarps;
   const int g = lane >> 2, q = lane & 3;
   const int N = p.N, nct = p.nct, nc0 = p.nc0;
-  const double mueq = p.mueq;
   // leg mode: this CTA owns knots [t_lo, t_hi) of the instance (gar/parallel-solver.hxx:150-164)
   const int NLEG = p.legs > 1 ? p.legs : 1;
   const bool legmode = NLEG > 1;
@@ -634,15 +634,15 @@ AB2_D void riccati_block_sweep(Ctx &ctx, const SweepParams &p, const D &d, const
       double *VN = Vxx_b + (size_t)N * nx * nx;
       for (int m = tid; m < nct * nx; m += T) { // Z = C / mu (stored row-major nct x nx)
         const int r = m / nx, j = m % nx;
-        p.fbT[(size_t)inst * nct * nx + m] = Ct[r + (size_t)j * nct] / mueq;
+        p.fbT[(size_t)inst * nct * nx + m] = Ct[r + (size_t)j * nct] / mu(p, inst);
       }
       for (int m = tid; m < nct; m += T)
-        p.ffT[(size_t)inst * nct + m] = dt[m] / mueq;
+        p.ffT[(size_t)inst * nct + m] = dt[m] / mu(p, inst);
       for (int e = tid; e < nx * nx; e += T) { // Vxx = Q + C^T Z
         const int i = e % nx, j = e / nx;
         double acc = 0.0;
         for (int m = 0; m < nct; ++m)
-          acc += Ct[m + (size_t)i * nct] * (Ct[m + (size_t)j * nct] / mueq);
+          acc += Ct[m + (size_t)i * nct] * (Ct[m + (size_t)j * nct] / mu(p, inst));
         const double s = Qt[i + j * nx] + acc;
         VN[i + j * nx] = s;
         if (i >= j) {
@@ -653,7 +653,7 @@ AB2_D void riccati_block_sweep(Ctx &ctx, const SweepParams &p, const D &d, const
       for (int i = tid; i < nx; i += T) { // vx = q + C^T z
         double acc = 0.0;
         for (int m = 0; m < nct; ++m)
-          acc += Ct[m + (size_t)i * nct] * (dt[m] / mueq);
+          acc += Ct[m + (size_t)i * nct] * (dt[m] / mu(p, inst));
         const double s = qt[i] + acc;
         vx_b[(size_t)N * nx + i] = s;
         vxn[i] = s;
@@ -813,7 +813,7 @@ AB2_D void riccati_block_sweep(Ctx &ctx, const SweepParams &p, const D &d, const
         else if (r >= nu && c < nu)
           v = rec[d.off_d + c * nc + (r - nu)];
         else if (r >= nu && c >= nu)
-          v = (r == c) ? -mueq : 0.0;
+          v = (r == c) ? -mu(p, inst) : 0.0;
         kkt[r + c * nk] = v;
       }
       if (nth > 0) {
@@ -1286,7 +1286,6 @@ AB2_D void riccati_block_sweep(Ctx &ctx, const SweepParams &p, const D &d, const
     ctx.sync();
   }
 }
-
 
 // ---------------------------------------------------------------------------
 // Leg mode, step 2: the condensed system of one instance (the "boundary consensus" of the

@@ -54,12 +54,12 @@ AB2_HD constexpr DenseDims make_dense_dims(int nx, int nu, int nc, int nct, int 
   return d;
 }
 
-template <class Ctx>
+// mu: where this instance's mu is read (ScalarMu / InstanceMu, riccati_group.cuh).
+template <class Ctx, class Mu = ScalarMu>
 AB2_D void riccati_dense_sweep(Ctx &ctx, const SweepParams &p, const DenseDims &d, const int inst,
-                               double *__restrict__ sm) {
+                               double *__restrict__ sm, const Mu &mu = Mu()) {
   const int nx = d.nx, nu = d.nu, nc = d.nc, n = d.n, N = p.N, nct = p.nct, nc0 = p.nc0;
   const int tid = ctx.tid, T = ctx.nthreads;
-  const double mueq = p.mueq;
   const int o2 = nu + nc, o3 = o2 + nx; // row offsets of the l / y blocks
   double *kkt = sm + d.s_kkt, *rhs = sm + d.s_rhs, *work = sm + d.s_work;
   const int nmax = n > nx + nc0 ? n : nx + nc0;
@@ -81,15 +81,15 @@ AB2_D void riccati_dense_sweep(Ctx &ctx, const SweepParams &p, const DenseDims &
       const double *Qt = tr, *qt = tr + nx * nx, *Ct = qt + nx, *dt = Ct + (size_t)nct * nx;
       for (int m = tid; m < nct * nx; m += T) {
         const int r = m / nx, j = m % nx;
-        p.fbT[(size_t)inst * nct * nx + m] = Ct[r + (size_t)j * nct] / mueq;
+        p.fbT[(size_t)inst * nct * nx + m] = Ct[r + (size_t)j * nct] / mu(p, inst);
       }
       for (int m = tid; m < nct; m += T)
-        p.ffT[(size_t)inst * nct + m] = dt[m] / mueq;
+        p.ffT[(size_t)inst * nct + m] = dt[m] / mu(p, inst);
       for (int e = tid; e < nx * nx; e += T) { // Pxx = Q + C^T Z
         const int i = e % nx, j = e / nx;
         double acc = 0.0;
         for (int m = 0; m < nct; ++m)
-          acc += Ct[m + (size_t)i * nct] * (Ct[m + (size_t)j * nct] / mueq);
+          acc += Ct[m + (size_t)i * nct] * (Ct[m + (size_t)j * nct] / mu(p, inst));
         const double s = Qt[e] + acc;
         Pn[e] = s;
         Vxx_b[(size_t)N * nx * nx + e] = s;
@@ -97,7 +97,7 @@ AB2_D void riccati_dense_sweep(Ctx &ctx, const SweepParams &p, const DenseDims &
       for (int i = tid; i < nx; i += T) {
         double acc = 0.0;
         for (int m = 0; m < nct; ++m)
-          acc += Ct[m + (size_t)i * nct] * (dt[m] / mueq);
+          acc += Ct[m + (size_t)i * nct] * (dt[m] / mu(p, inst));
         const double s = qt[i] + acc;
         pxn[i] = s;
         vx_b[(size_t)N * nx + i] = s;
@@ -122,7 +122,7 @@ AB2_D void riccati_dense_sweep(Ctx &ctx, const SweepParams &p, const DenseDims &
         else if (bi == 0 && bj == 1)
           v = Dm[jj + ii * nc];
         else if (bi == 1 && bj == 1)
-          v = (ii == jj) ? -mueq : 0.0;
+          v = (ii == jj) ? -mu(p, inst) : 0.0;
         else if (bi == 2 && bj == 0)
           v = Bm[ii + jj * nx];
         else if (bi == 0 && bj == 2)

@@ -114,10 +114,33 @@ struct SweepParams {
   // Packed-Vxx builds (Cfg::VXX_PACKED, vxx_layout.h): Vxx holds [batch][N+1][vxx_packed_doubles(NX)] and this
   // [batch][NX*NX] array the full block of factor slot 0.  The full-layout build never reads it.
   double *Vxx0;
+  // Per-instance mu ([batch], device) of the *_v entry points, or null: every instance uses mueq.  A non-null array
+  // selects the kernels' per-instance instantiation (InstanceMu); the programs themselves never read this field.
+  const double *mueq_b;
 };
 
-// status bits: see ST_*; in leg mode several CTAs report on one instance
-enum : int { ST_CONDENSED_FACTOR_FAILED = 4 };
+// Where a program reads mu: mu(p, inst) at every use.  ScalarMu (the default) is p.mueq, so the scalar launches run
+// the programs exactly as they were; InstanceMu is the per-instance array of the *_v launches, read at the use, which
+// keeps it out of the registers across the knot loop.
+struct ScalarMu {
+  AB2_HD double operator()(const SweepParams &p, int) const { return p.mueq; }
+};
+struct InstanceMu {
+  AB2_HD double operator()(const SweepParams &p, int inst) const { return p.mueq_b[inst]; }
+};
+
+// status bits: see ST_*; in leg mode several CTAs report on one instance.  ST_BAD_MU: the per-instance mu of a
+// *_v backward was not > 0 while constraints are present (set by the kernels, after the program's own status word)
+enum : int { ST_CONDENSED_FACTOR_FAILED = 4, ST_BAD_MU = 8 };
+// After the backward pass of a per-instance launch (the program has written its status word; `writer` is the thread
+// that wrote it): an instance whose mu is unusable -- not > 0, NaN included -- while constraints are present gets
+// ST_BAD_MU.  Kernel code only; atomic because several CTAs report on one instance in leg mode.
+AB2_D void flag_bad_mu(const SweepParams &p, const int inst, const bool constrained, const bool writer) {
+#if defined(__CUDACC__)
+  if (p.do_bwd && writer && constrained && !(p.mueq_b[inst] > 0.0))
+    atomicOr(p.status + inst, (int)ST_BAD_MU);
+#endif
+}
 
 // physical slot of stage knot t in the (ring-indexed) stage-record array
 AB2_HD int stage_slot(const SweepParams &p, int t) {
@@ -1466,15 +1489,15 @@ template <class C> AB2_D void store_packed_column(double *dst, const double *Vn,
 // ---------------------------------------------------------------------------
 // The sweep of one instance by one group.
 // ---------------------------------------------------------------------------
-template <class C, class Ctx>
+// mu: where this instance's mu is read (ScalarMu / InstanceMu above).
+template <class C, class Ctx, class Mu = ScalarMu>
 AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
-                                double *__restrict__ sm) {
+                                double *__restrict__ sm, const Mu &mu = Mu()) {
   constexpr int NX = C::NX, NU = C::NU, NC = C::NC, NK = C::NK, NR = C::NR;
   constexpr int NXU = C::NXU, NCOL = C::NCOL, FCOL = C::FCOL;
   const int lane = ctx.lane;
   const int N = p.N;
   const int nct = p.nct, nc0 = p.nc0;
-  const double mueq = p.mueq;
 
   double *rec = sm + C::S_REC; // current knot record (buffer 0 / alternating when DB)
   double *Vn = sm + C::S_VN;
@@ -1538,7 +1561,7 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
 #pragma unroll 1
 #endif
         for (int m = 0; m < nct; ++m) {
-          const double zm = (colF ? dt[m] : Ct[m + (size_t)lane * nct]) / mueq;
+          const double zm = (colF ? dt[m] : Ct[m + (size_t)lane * nct]) / mu(p, inst);
           if (colF)
             p.ffT[(size_t)inst * nct + m] = zm;
           else
@@ -1655,7 +1678,7 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
       if (lane < NC) { // (1,1) block: -mu on the diagonal, zeros below
         AB2_UNROLL
         for (int m = 0; m < NC; ++m)
-          kkt[NU + m + (NU + lane) * NK] = (m == lane) ? -mueq : 0.0;
+          kkt[NU + m + (NU + lane) * NK] = (m == lane) ? -mu(p, inst) : 0.0;
       }
       if (colA || colF) {
         AB2_UNROLL

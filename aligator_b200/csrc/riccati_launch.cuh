@@ -153,7 +153,8 @@ template <int G, bool TMA> struct DevCtx {
 // The persistent sweep kernel: every group walks the whole horizon of its
 // instance (backward, initial stage, forward) inside one launch.
 // ---------------------------------------------------------------------------
-template <class C, int WARPS, int MAXREG, bool TMA>
+// PI: per-instance mu (SweepParams::mueq_b, the *_v launches); false = the scalar p.mueq
+template <class C, int WARPS, int MAXREG, bool TMA, bool PI>
 __global__ void __launch_bounds__(WARPS * 32) __maxnreg__(MAXREG)
     riccati_sweep_kernel(const SweepParams p, const int group_doubles) {
   extern __shared__ __align__(16) double smem[];
@@ -182,7 +183,12 @@ __global__ void __launch_bounds__(WARPS * 32) __maxnreg__(MAXREG)
     const int slot = (blockIdx.x / p.num_sms) * WARPS + warp;
     __nanosleep((unsigned)(slot * p.stagger_ns));
   }
-  riccati_group_sweep<C>(ctx, p, inst, sm);
+  if constexpr (PI) {
+    riccati_group_sweep<C>(ctx, p, inst, sm, InstanceMu());
+    flag_bad_mu(p, inst, C::NC > 0 || p.nct > 0, ctx.lane == 0);
+  } else {
+    riccati_group_sweep<C>(ctx, p, inst, sm);
+  }
 }
 
 // ---------------------------------------------------------------------------
@@ -200,7 +206,8 @@ inline cudaError_t launch_one(const SweepParams &p, int gd, cudaStream_t st, int
   constexpr int IPW = 32 / C::G;
   const int groups = WARPS * IPW;
   size_t smem = (size_t)groups * gd * sizeof(double) + (size_t)groups * 8 * NBAR + (size_t)C::LUT_INTS * 4;
-  auto kern = riccati_sweep_kernel<C, WARPS, MAXREG, TMA>;
+  // the per-instance instantiation serves the *_v launches; occupancy and launch shape are decided alike
+  auto kern = p.mueq_b ? riccati_sweep_kernel<C, WARPS, MAXREG, TMA, true> : riccati_sweep_kernel<C, WARPS, MAXREG, TMA, false>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;
@@ -217,15 +224,16 @@ inline cudaError_t launch_one(const SweepParams &p, int gd, cudaStream_t st, int
   // (C2 on 132 SMs: 8 CTAs/SM = rounds of 2112 + 1984 instances; 7 would need a third round.)
   // p.ctas_per_sm > 0 overrides, < 0 keeps the maximum.
   {
-    static thread_local size_t cached_smem = 0; // per kernel instantiation
-    static thread_local int cached_cmax = 0;
-    if (cached_smem != smem) {
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cached_cmax, kern, WARPS * 32, smem);
+    static thread_local size_t cached_smem[2] = {0, 0}; // per kernel instantiation
+    static thread_local int cached_cmax[2] = {0, 0};
+    const int ci = p.mueq_b ? 1 : 0;
+    if (cached_smem[ci] != smem) {
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cached_cmax[ci], kern, WARPS * 32, smem);
       if (e != cudaSuccess)
         return e;
-      cached_smem = smem;
+      cached_smem[ci] = smem;
     }
-    const int cmax = cached_cmax;
+    const int cmax = cached_cmax[ci];
     int want = p.ctas_per_sm;
     if (want == 0 && cmax > 1) {
       const int sms = p.num_sms > 0 ? p.num_sms : 132;

@@ -9,6 +9,7 @@ built, and every call fails loudly without a CUDA device.
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import os
 
 import numpy as np
@@ -121,6 +122,8 @@ def lib():
         L.ab2_gar_backward.argtypes = [C.c_void_p, C.c_double, C.c_void_p]
         L.ab2_gar_forward.argtypes = [C.c_void_p, C.c_void_p]
         L.ab2_gar_sweep.argtypes = [C.c_void_p, C.c_double, C.c_void_p]
+        L.ab2_gar_backward_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        L.ab2_gar_sweep_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_create_parametric.argtypes = [C.POINTER(GarDims), C.c_int, C.POINTER(C.c_void_p)]
         L.ab2_gar_create_parallel.argtypes = [C.POINTER(GarDims), C.c_int, C.POINTER(C.c_void_p)]
         L.ab2_gar_create_dense.argtypes = [C.POINTER(GarDims), C.POINTER(C.c_void_p)]
@@ -132,6 +135,8 @@ def lib():
                                          C.c_double, C.c_int, C.POINTER(C.c_int),
                                          C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.ab2_gar_sweep_host_sym.argtypes = L.ab2_gar_sweep_host.argtypes
+        L.ab2_gar_sweep_host_v.argtypes = L.ab2_gar_sweep_host.argtypes[:5] + [C.c_void_p] + L.ab2_gar_sweep_host.argtypes[6:]
+        L.ab2_gar_sweep_host_sym_v.argtypes = L.ab2_gar_sweep_host_v.argtypes
         L.ab2_gar_stage_record_doubles_sym.restype = C.c_size_t
         L.ab2_gar_stage_record_doubles_sym.argtypes = [C.c_int, C.c_int, C.c_int]
         L.ab2_gar_pack_stage_sym.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_long]
@@ -139,20 +144,27 @@ def lib():
         L.ab2_gar_get_range.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                         C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_assemble.argtypes = [C.c_void_p, C.POINTER(LqInputs), C.c_void_p]
+        L.ab2_gar_assemble_v.argtypes = [C.c_void_p, C.POINTER(LqInputs), C.c_void_p, C.c_void_p, C.c_void_p]
         L.ab2_gar_get_problem.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_problem_ptr.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
         L.ab2_gar_kkt_error.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_int, C.c_void_p]
+        L.ab2_gar_kkt_error_v.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_get_gains.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_first_step_policy.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.ab2_gar_device_ptr.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
         L.ab2_gar_status.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_pivot_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_fddp_backward_pass.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.ab2_fddp_backward_pass_v.argtypes = [C.c_void_p] * 6
         L.ab2_gar_linear_step.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.ab2_gar_linear_step_v.argtypes = [C.c_void_p] * 5
         L.ab2_gar_directional_derivative.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_al_value.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_int, C.c_void_p]
+        L.ab2_gar_al_value_v.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
+        L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
+                                            C.POINTER(MultOutputs), C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_lagrangian_gradient.argtypes = [C.c_void_p, C.POINTER(LagInputs), C.POINTER(LagOutputs), C.c_void_p]
         L.ab2_gar_criterion.argtypes = [C.c_void_p] + [C.c_void_p] * 7 + [C.c_int, C.c_void_p]
         L.ab2_gar_peer_gather_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
@@ -224,6 +236,68 @@ class CudaRiccatiBatch:
         self.srec = int(lib().ab2_gar_stage_record_doubles_th(nx, nu, nc, rec_nth))
         self.trec = int(lib().ab2_gar_term_record_doubles_th(nx, nct, rec_nth))
         self._keep = None
+        self._keep_v = {}
+
+    # ---- per-instance scalars (the *_v twins of the C ABI) ----------------------
+    def _per_instance(self, v, name):
+        """None when `v` is a Python number (the scalar call), else `v` itself after checking that it is a 1-D
+        float64 numpy array or torch tensor of length batch (ValueError otherwise)."""
+        if isinstance(v, numbers.Real) or getattr(v, "ndim", None) == 0:  # numbers, numpy scalars, 0-d arrays
+            return None
+        B = self.dims.batch
+        if isinstance(v, np.ndarray):
+            ok = v.dtype == np.float64 and v.ndim == 1 and v.shape[0] == B
+        elif hasattr(v, "data_ptr") and hasattr(v, "is_cuda"):
+            import torch
+            ok = v.dtype == torch.float64 and v.dim() == 1 and v.shape[0] == B
+        else:
+            ok = False
+        if not ok:
+            raise ValueError("%s: expected a number or a 1-D float64 array / tensor of length batch = %d" % (name, B))
+        return v
+
+    def _host_array(self, v, name):
+        """A checked per-instance array as contiguous host memory, kept alive by the handle."""
+        if not isinstance(v, np.ndarray):
+            v = v.detach().cpu().numpy()
+        v = np.ascontiguousarray(v)
+        self._keep_v[name] = v
+        return v
+
+    def _device_array(self, v, name, stream):
+        """A checked per-instance array as contiguous device memory: CUDA tensors as they are, host arrays uploaded.
+        Kept alive by the handle until the next call that passes `name`; with a non-default stream the allocator
+        is told that the stream uses it."""
+        import torch
+        if not (isinstance(v, torch.Tensor) and v.is_cuda):
+            host = v if isinstance(v, np.ndarray) else v.detach().numpy()
+            v = torch.from_numpy(np.ascontiguousarray(host)).to("cuda:%d" % self.dims.device)
+            if stream:
+                v.record_stream(torch.cuda.ExternalStream(stream))
+        else:
+            v = v.contiguous()
+        self._keep_v[name] = v
+        return v
+
+    def _device_pair(self, a, b, names, stream):
+        """Two per-instance scalars of one call: None when both are numbers, else both as device arrays (a number
+        given beside an array applies to every instance)."""
+        va, vb = self._per_instance(a, names[0]), self._per_instance(b, names[1])
+        if va is None and vb is None:
+            return None
+        B = self.dims.batch
+        va = np.full(B, float(a)) if va is None else va
+        vb = np.full(B, float(b)) if vb is None else vb
+        return self._device_array(va, names[0], stream), self._device_array(vb, names[1], stream)
+
+    def _mueq_arg(self, mueq, stream):
+        """(pointer, memspace) of a per-instance mu for backward_v / sweep_v, or None for a number."""
+        v = self._per_instance(mueq, "mueq")
+        if v is None:
+            return None
+        if hasattr(v, "is_cuda") and v.is_cuda:
+            return _ptr(self._device_array(v, "mueq", stream)), AB2_DEVICE
+        return _ptr(self._host_array(v, "mueq")), AB2_HOST
 
     def close(self):
         if getattr(self, "h", None) is not None and self.h.value:
@@ -250,7 +324,13 @@ class CudaRiccatiBatch:
 
     # ---- the hot calls ------------------------------------------------------
     def backward(self, mueq, stream=0):
-        _check(lib().ab2_gar_backward(self.h, float(mueq), C.c_void_p(stream)))
+        """``mueq``: a number, or a [batch] float64 array / tensor of per-instance values (``ab2_gar_backward_v``;
+        CUDA tensors are read on the device, host arrays are staged by the library)."""
+        v = self._mueq_arg(mueq, stream)
+        if v is None:
+            _check(lib().ab2_gar_backward(self.h, float(mueq), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_backward_v(self.h, v[0], v[1], C.c_void_p(stream)))
 
     def forward(self, stream=0, theta=None):
         """forward(); with ``theta`` ([batch][nth] host array) the parametric rollout."""
@@ -267,7 +347,12 @@ class CudaRiccatiBatch:
         _check(lib().ab2_gar_collapse_feedback(self.h, C.c_void_p(stream)))
 
     def sweep(self, mueq, stream=0):
-        _check(lib().ab2_gar_sweep(self.h, float(mueq), C.c_void_p(stream)))
+        """``mueq``: a number or a [batch] array / tensor (``ab2_gar_sweep_v``), as for ``backward``."""
+        v = self._mueq_arg(mueq, stream)
+        if v is None:
+            _check(lib().ab2_gar_sweep(self.h, float(mueq), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_sweep_v(self.h, v[0], v[1], C.c_void_p(stream)))
 
     def synchronize(self, stream=0):
         _check(lib().ab2_gar_synchronize(self.h, C.c_void_p(stream)))
@@ -276,23 +361,37 @@ class CudaRiccatiBatch:
         """Upload + sweep + download in one pipelined call (``ab2_gar_sweep_host``): the batch
         travels in slices on internal streams so uploads, sweeps and downloads overlap.
         ``outputs``: {OUT_*: host array of the full output size}; pinned arrays make the
-        copies asynchronous.  Asynchronous w.r.t. the host: call ``synchronize(stream)``."""
+        copies asynchronous.  Asynchronous w.r.t. the host: call ``synchronize(stream)``.  ``mueq``: a number or a
+        [batch] array / tensor of per-instance values (``ab2_gar_sweep_host_v``)."""
+        v = self._per_instance(mueq, "mueq")
         whats = (C.c_int * len(outputs))(*outputs.keys())
         dsts = (C.c_void_p * len(outputs))(*[_ptr(a).value for a in outputs.values()])
         self._keep = (stage, term, G0, g0, outputs)
-        _check(lib().ab2_gar_sweep_host(self.h, _ptr(stage), _ptr(term), _ptr(G0), _ptr(g0),
-                                        C.c_double(mueq), int(nchunks), whats, dsts, len(outputs),
-                                        C.c_void_p(stream)))
+        if v is None:
+            _check(lib().ab2_gar_sweep_host(self.h, _ptr(stage), _ptr(term), _ptr(G0), _ptr(g0),
+                                            C.c_double(mueq), int(nchunks), whats, dsts, len(outputs),
+                                            C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_sweep_host_v(self.h, _ptr(stage), _ptr(term), _ptr(G0), _ptr(g0),
+                                              _ptr(self._host_array(v, "mueq")), int(nchunks), whats, dsts,
+                                              len(outputs), C.c_void_p(stream)))
 
     def sweep_host_sym(self, stage_sym, term, G0, g0, mueq, outputs, nchunks=0, stream=0):
         """``sweep_host`` with the symmetric blocks Q, R of every stage knot sent as lower triangles
-        (``ab2_gar_sweep_host_sym``; records made by ``pack_stage_sym``): fewer bytes over PCIe."""
+        (``ab2_gar_sweep_host_sym``; records made by ``pack_stage_sym``): fewer bytes over PCIe.  ``mueq``: a number
+        or a [batch] array / tensor (``ab2_gar_sweep_host_sym_v``)."""
+        v = self._per_instance(mueq, "mueq")
         whats = (C.c_int * len(outputs))(*outputs.keys())
         dsts = (C.c_void_p * len(outputs))(*[_ptr(a).value for a in outputs.values()])
         self._keep = (stage_sym, term, G0, g0, outputs)
-        _check(lib().ab2_gar_sweep_host_sym(self.h, _ptr(stage_sym), _ptr(term), _ptr(G0), _ptr(g0),
-                                            C.c_double(mueq), int(nchunks), whats, dsts, len(outputs),
-                                            C.c_void_p(stream)))
+        if v is None:
+            _check(lib().ab2_gar_sweep_host_sym(self.h, _ptr(stage_sym), _ptr(term), _ptr(G0), _ptr(g0),
+                                                C.c_double(mueq), int(nchunks), whats, dsts, len(outputs),
+                                                C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_sweep_host_sym_v(self.h, _ptr(stage_sym), _ptr(term), _ptr(G0), _ptr(g0),
+                                                  _ptr(self._host_array(v, "mueq")), int(nchunks), whats, dsts,
+                                                  len(outputs), C.c_void_p(stream)))
 
     def pack_stage_sym(self, stage, out=None):
         """Full stage records [batch][N][srec] (host) -> triangle-packed records (``ab2_gar_pack_stage_sym``)."""
@@ -349,14 +448,19 @@ class CudaRiccatiBatch:
     def assemble(self, arrays, preg, mu_inv, stream=0):
         """updateLQSubproblem + computeProjectedJacobians on the device (``ab2_gar_assemble``).
         ``arrays``: {field of ab2_lq_inputs: device tensor / device address}; missing fields
-        are NULL.  The assembled problem becomes the solver's current problem."""
+        are NULL.  The assembled problem becomes the solver's current problem.  ``preg``, ``mu_inv``: numbers, or
+        [batch] arrays / tensors of per-instance values (``ab2_gar_assemble_v``)."""
         inp = LqInputs()
         for n in _LQ_PTRS:
             a = arrays.get(n)
             setattr(inp, n, None if a is None else _ptr(a).value)
-        inp.preg, inp.mu_inv = float(preg), float(mu_inv)
+        v = self._device_pair(preg, mu_inv, ("preg", "mu_inv"), stream)
         self._keep = (arrays,)
-        _check(lib().ab2_gar_assemble(self.h, C.byref(inp), C.c_void_p(stream)))
+        if v is None:
+            inp.preg, inp.mu_inv = float(preg), float(mu_inv)
+            _check(lib().ab2_gar_assemble(self.h, C.byref(inp), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_assemble_v(self.h, C.byref(inp), _ptr(v[0]), _ptr(v[1]), C.c_void_p(stream)))
 
     def get_problem(self, what, stream=0):
         """Host copy of the current packed problem: what = 0 stage, 1 term, 2 G0, 3 g0."""
@@ -378,9 +482,15 @@ class CudaRiccatiBatch:
 
     def kkt_error(self, mueq, stream=0):
         """[batch][3] = (dynamics, constraint, stationarity) infinity norms of lqrComputeKktError
-        (gar/utils.hxx:88-182) for the current problem and the last forward pass, computed on the device."""
+        (gar/utils.hxx:88-182) for the current problem and the last forward pass, computed on the device.
+        ``mueq``: a number or a [batch] array / tensor (``ab2_gar_kkt_error_v``)."""
+        v = self._per_instance(mueq, "mueq")
         out = np.empty((self.dims.batch, 3), dtype=np.float64)
-        _check(lib().ab2_gar_kkt_error(self.h, C.c_double(mueq), _ptr(out), AB2_HOST, C.c_void_p(stream)))
+        if v is None:
+            _check(lib().ab2_gar_kkt_error(self.h, C.c_double(mueq), _ptr(out), AB2_HOST, C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_kkt_error_v(self.h, _ptr(self._device_array(v, "mueq", stream)), _ptr(out), AB2_HOST,
+                                             C.c_void_p(stream)))
         self.synchronize(stream)
         return out
 
@@ -449,11 +559,17 @@ class CudaRiccatiBatch:
     # ---- line-search consumers (device tensors in, device tensors / host scalars out) ----
     def linear_step(self, alpha, current, trial, stream=0):
         """trial = current + alpha * step (tryLinearStep's vector part); `current` / `trial`: dicts with keys
-        xs, us, vs, vsT, lam0, lams of device tensors laid out like the solver's outputs."""
+        xs, us, vs, vsT, lam0, lams of device tensors laid out like the solver's outputs.  ``alpha``: a number or a
+        [batch] array / tensor of per-instance step lengths (``ab2_gar_linear_step_v``)."""
+        v = self._per_instance(alpha, "alpha")
         cur = LsIterate(*[_ptr(current.get(k)).value if current.get(k) is not None else None for k in _LS_KEYS])
         tr = LsIterate(*[_ptr(trial.get(k)).value if trial.get(k) is not None else None for k in _LS_KEYS])
         self._keep_ls = (current, trial)
-        _check(lib().ab2_gar_linear_step(self.h, C.c_double(alpha), C.byref(cur), C.byref(tr), C.c_void_p(stream)))
+        if v is None:
+            _check(lib().ab2_gar_linear_step(self.h, C.c_double(alpha), C.byref(cur), C.byref(tr), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_linear_step_v(self.h, _ptr(self._device_array(v, "alpha", stream)), C.byref(cur),
+                                               C.byref(tr), C.c_void_p(stream)))
 
     def directional_derivative(self, Lxs, Lus, stream=0):
         out = np.empty(self.dims.batch, dtype=np.float64)
@@ -462,10 +578,16 @@ class CudaRiccatiBatch:
         return out
 
     def al_value(self, plus, cost, mudyn, mucstr, stream=0):
+        """``mudyn``, ``mucstr``: numbers, or [batch] arrays / tensors of per-instance values (``ab2_gar_al_value_v``)."""
+        v = self._device_pair(mudyn, mucstr, ("mudyn", "mucstr"), stream)
         it = LsIterate(*[_ptr(plus.get(k)).value if plus.get(k) is not None else None for k in _LS_KEYS])
         out = np.empty(self.dims.batch, dtype=np.float64)
-        _check(lib().ab2_gar_al_value(self.h, C.byref(it), _ptr(cost), C.c_double(mudyn), C.c_double(mucstr), _ptr(out),
-                                      AB2_HOST, C.c_void_p(stream)))
+        if v is None:
+            _check(lib().ab2_gar_al_value(self.h, C.byref(it), _ptr(cost), C.c_double(mudyn), C.c_double(mucstr),
+                                          _ptr(out), AB2_HOST, C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_al_value_v(self.h, C.byref(it), _ptr(cost), _ptr(v[0]), _ptr(v[1]), _ptr(out),
+                                            AB2_HOST, C.c_void_p(stream)))
         self.synchronize(stream)
         return out
 
@@ -484,13 +606,18 @@ class CudaRiccatiBatch:
         """computeMultipliers on the device (``ab2_gar_multipliers``).  ``inputs``: dict of device tensors keyed like
         ``ab2_mult_inputs`` (exactly one of xnext, fs); ``outputs``: dict of device tensors keyed like
         ``ab2_mult_outputs``.  Returns [batch][2] = [prim_infeas, finite (1.0 / 0.0)] as numpy, or writes it into the
-        device tensor ``out`` and returns that."""
+        device tensor ``out`` and returns that.  ``mu``, ``mu_dyn``: numbers, or [batch] arrays / tensors of
+        per-instance values (``ab2_gar_multipliers_v``)."""
+        v = self._device_pair(mu, mu_dyn, ("mu", "mu_dyn"), stream)
         inp = _fill(MultInputs(), _MULT_IN, inputs)
-        inp.mu, inp.mu_dyn = float(mu), float(mu_dyn)
         o = _fill(MultOutputs(), _MULT_OUT, outputs)
         self._keep_inner = (inputs, outputs)
-        return self._scalars(lambda dst, ms: _check(lib().ab2_gar_multipliers(
-            self.h, C.byref(inp), C.byref(o), dst, ms, C.c_void_p(stream))), out, stream)
+        if v is None:
+            inp.mu, inp.mu_dyn = float(mu), float(mu_dyn)
+            return self._scalars(lambda dst, ms: _check(lib().ab2_gar_multipliers(
+                self.h, C.byref(inp), C.byref(o), dst, ms, C.c_void_p(stream))), out, stream)
+        return self._scalars(lambda dst, ms: _check(lib().ab2_gar_multipliers_v(
+            self.h, C.byref(inp), _ptr(v[0]), _ptr(v[1]), C.byref(o), dst, ms, C.c_void_p(stream))), out, stream)
 
     def lagrangian_gradient(self, inputs, outputs, force_initial_condition=False, stream=0):
         """LagrangianDerivatives::compute on the device (``ab2_gar_lagrangian_gradient``).  ``inputs``: dict of
@@ -512,10 +639,17 @@ class CudaRiccatiBatch:
 
     def fddp_backward_pass(self, arrays, preg, Vx_out=None, Quuks_out=None, stream=0):
         """SolverFDDP::backwardPass on the device (``ab2_fddp_backward_pass``); ``arrays``: dict of device
-        tensors Jx, Ju, fs, Lxx, Lxu, Luu, Lx, Lu, Lxx_N, Lx_N."""
-        inp = FddpInputs(*[_ptr(arrays[k]).value for k in _FDDP_KEYS], float(preg))
+        tensors Jx, Ju, fs, Lxx, Lxu, Luu, Lx, Lu, Lxx_N, Lx_N.  ``preg``: a number or a [batch] array / tensor of
+        per-instance values (``ab2_fddp_backward_pass_v``)."""
+        v = self._per_instance(preg, "preg")
+        inp = FddpInputs(*[_ptr(arrays[k]).value for k in _FDDP_KEYS], 0.0 if v is not None else float(preg))
         self._keep = (arrays, Vx_out, Quuks_out)
-        _check(lib().ab2_fddp_backward_pass(self.h, C.byref(inp), _ptr(Vx_out), _ptr(Quuks_out), C.c_void_p(stream)))
+        if v is None:
+            _check(lib().ab2_fddp_backward_pass(self.h, C.byref(inp), _ptr(Vx_out), _ptr(Quuks_out),
+                                                C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_fddp_backward_pass_v(self.h, C.byref(inp), _ptr(self._device_array(v, "preg", stream)),
+                                                  _ptr(Vx_out), _ptr(Quuks_out), C.c_void_p(stream)))
 
     def pivot_stats(self, stream=0):
         """(n_2x2, n_interchanges) per instance of the last backward pass (``ab2_gar_pivot_stats``)."""

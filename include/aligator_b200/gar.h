@@ -36,7 +36,21 @@
  *   STATUS [batch] int   0 = ok, bit0 = a stage LDL^T failed (the reference throws
  *                        "Failed stage LDL factorization", riccati-kernel.hxx:239-241),
  *                        bit1 = the initial-stage factorisation failed,
- *                        bit2 = (parallel solver) a block of the condensed system failed to factor.
+ *                        bit2 = (parallel solver) a block of the condensed system failed to factor,
+ *                        bit3 = a per-instance mu given to a *_v backward / sweep in DEVICE memory was not > 0
+ *                               (NaN included) while constraints are present (nc > 0 or nct > 0); that
+ *                               instance's outputs are unspecified, every other instance is unaffected.
+ *
+ * Per-instance scalars (the *_v twins below).  Each scalar a solver keeps per problem -- the penalty mu
+ * (mu_penal_, solver-proxddp.hxx:509-520), mu_dyn, the regularisation preg (:690-698) and the step length
+ * alpha (:648-671) -- has a twin entry point that takes a [batch] array of doubles instead (the handle's own
+ * batch: the local batch on a sharded rank).  Instance b reads element b; nothing else about the computation
+ * changes, so instance b's outputs equal those of the scalar call with the value of element b.  The arrays are
+ * read in stream order: a device-side update may write them on the same stream just before the call, and the
+ * caller keeps them alive until that work has finished.  The twins launch as many kernels as the scalar calls,
+ * and they leave no trace in the handle: a later scalar or forward-only call behaves as if the twin had never
+ * run.  The streaming twins (multipliers, AL value, assembly, linear step) do not check the values, as they
+ * do not check their other device inputs.
  */
 #ifndef ALIGATOR_B200_GAR_H
 #define ALIGATOR_B200_GAR_H
@@ -177,6 +191,12 @@ int ab2_gar_forward(ab2_gar_solver *s, void *stream);
 /* backward + forward in ONE persistent launch: the loop body of
  * bench/gar-riccati.cpp:46-49 and solver-proxddp.hxx:608-611. */
 int ab2_gar_sweep(ab2_gar_solver *s, double mueq, void *stream);
+/* ab2_gar_backward / ab2_gar_sweep with a per-instance mu: mueq [batch] in host or device memory.  Host arrays are
+ * checked like the scalar (mu > 0 when nc > 0 or nct > 0, else AB2_ERR_INVALID and nothing is launched) and staged
+ * into a buffer the handle owns, as ab2_gar_forward_theta does with theta; device arrays are read by the kernels,
+ * which set status bit3 on an instance whose mu is unusable.  Every handle type the scalar calls serve. */
+int ab2_gar_backward_v(ab2_gar_solver *s, const double *mueq, int memspace, void *stream);
+int ab2_gar_sweep_v(ab2_gar_solver *s, const double *mueq, int memspace, void *stream);
 /* Inputs of the batched LQ assembly: the derivative buffers SolverProxDDP::updateLQSubproblem
  * (solvers/proxddp/solver-proxddp.hxx:734-805) and computeProjectedJacobians (:25-69) read.
  * DEVICE pointers; stage arrays are [batch][N][block], terminal / initial arrays [batch][block],
@@ -203,6 +223,9 @@ typedef struct ab2_lq_inputs {
  * HBM: writes the solver-owned packed problem (the same bytes ab2_gar_set_problem uploads) and
  * makes it the current problem.  A device-resident caller never moves the knots over PCIe. */
 int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream);
+/* The same with per-instance preg [batch] and mu_inv [batch] (DEVICE); in->preg and in->mu_inv are ignored. */
+int ab2_gar_assemble_v(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg, const double *mu_inv,
+                       void *stream);
 /* Device address of the current packed problem: what = 0 stage, 1 term, 2 G0, 3 g0
  * (the bytes workspace_.lqr_problem holds after updateLQSubproblem). */
 int ab2_gar_problem_ptr(ab2_gar_solver *s, int what, const double **out);
@@ -233,6 +256,14 @@ int ab2_gar_pack_stage_sym(int nx, int nu, int nc, const double *stage, double *
 int ab2_gar_sweep_host_sym(ab2_gar_solver *s, const double *stage_sym, const double *term, const double *G0,
                            const double *g0, double mueq, int nchunks, const int *whats,
                            double *const *dsts, int nwhat, void *stream);
+/* ab2_gar_sweep_host / ab2_gar_sweep_host_sym with a per-instance mu: mueq [batch] in HOST memory, checked like the
+ * scalar (AB2_ERR_INVALID, nothing launched), staged once on `stream` and sliced together with the batch. */
+int ab2_gar_sweep_host_v(ab2_gar_solver *s, const double *stage, const double *term, const double *G0,
+                         const double *g0, const double *mueq, int nchunks, const int *whats,
+                         double *const *dsts, int nwhat, void *stream);
+int ab2_gar_sweep_host_sym_v(ab2_gar_solver *s, const double *stage_sym, const double *term, const double *G0,
+                             const double *g0, const double *mueq, int nchunks, const int *whats,
+                             double *const *dsts, int nwhat, void *stream);
 
 /* Replaces: getFeedforward(i)/getFeedback(i) (riccati-base.hpp:33-34), the public
  * `datas[i].vm` / `kkt0` members (proximal-riccati.hpp:40-43) and the caller-owned
@@ -259,6 +290,8 @@ int ab2_gar_get_gains(ab2_gar_solver *s, double *dst, int memspace, void *stream
  * initial condition), constraint (C x + D u + d - mu v) and stationarity residuals.  Computed on
  * the device (one warp per (instance, knot)); dst in host or device memory. */
 int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace, void *stream);
+/* The same with a per-instance mu: mueq [batch] in DEVICE memory (dst in host or device memory). */
+int ab2_gar_kkt_error_v(ab2_gar_solver *s, const double *mueq, double *dst, int memspace, void *stream);
 /* The device array behind an output, in its physical layout.  Every output except AB2_OUT_VXX has the layout
  * ab2_gar_get returns (up to the ring heads of ab2_gar_cycle_append).  AB2_OUT_VXX, after a backward pass of the
  * warp-per-instance kernel (every tuning variant except 9 on a plain serial handle whose shape has one; the
@@ -316,6 +349,10 @@ typedef struct ab2_ls_trial {
  * integrate (:139-150); a manifold's integrate and problem.evaluate() stay with the modelling library. */
 int ab2_gar_linear_step(ab2_gar_solver *s, double alpha, const ab2_ls_iterate *current, const ab2_ls_trial *trial,
                         void *stream);
+/* The same with a per-instance step length alpha [batch] (DEVICE): every element uses the alpha of the instance
+ * that owns it; alpha = 0 leaves that instance's trial equal to its current iterate. */
+int ab2_gar_linear_step_v(ab2_gar_solver *s, const double *alpha, const ab2_ls_iterate *current,
+                          const ab2_ls_trial *trial, void *stream);
 /* Replaces: ALFunction::directionalDerivative, merit-function.hxx:68-104 (Lxs [batch][N+1][nx], Lus [batch][N][nu]
  * = the Lagrangian gradients) and costDirectionalDerivative, :13-31 (pass the cost gradients): dst[batch] =
  * sum_t Lxs_t . dxs_t + sum_t Lus_t . dus_t.  dst in host or device memory. */
@@ -326,6 +363,9 @@ int ab2_gar_directional_derivative(ab2_gar_solver *s, const double *Lxs, const d
  * (only lam0, lams, vs, vsT are read). */
 int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, double mudyn, double mucstr,
                      double *dst, int memspace, void *stream);
+/* The same with per-instance mudyn [batch] and mucstr [batch] (DEVICE). */
+int ab2_gar_al_value_v(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, const double *mudyn,
+                       const double *mucstr, double *dst, int memspace, void *stream);
 
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
@@ -366,6 +406,10 @@ typedef struct ab2_mult_outputs {
  * such an instance is unspecified.  Every output array is required (arrays of zero size may be NULL). */
 int ab2_gar_multipliers(ab2_gar_solver *s, const ab2_mult_inputs *in, const ab2_mult_outputs *out, double *dst,
                         int memspace, void *stream);
+/* The same with per-instance mu [batch] and mu_dyn [batch] (DEVICE; in->mu and in->mu_dyn are ignored); each
+ * instance's mu_inv = 1 / mu is computed from its own mu. */
+int ab2_gar_multipliers_v(ab2_gar_solver *s, const ab2_mult_inputs *in, const double *mu, const double *mu_dyn,
+                          const ab2_mult_outputs *out, double *dst, int memspace, void *stream);
 
 typedef struct ab2_lag_inputs {
   const double *lx, *lu, *lx_N;        /* cost gradients cost_data->Lx_, Lu_: [batch][N][nx], [batch][N][nu], [batch][nx] */
@@ -411,6 +455,9 @@ typedef struct ab2_fddp_inputs {
   double preg;
 } ab2_fddp_inputs;
 int ab2_fddp_backward_pass(ab2_gar_solver *s, const ab2_fddp_inputs *in, double *Vx_out, double *Quuks_out, void *stream);
+/* The same with a per-instance preg [batch] (DEVICE; in->preg is ignored). */
+int ab2_fddp_backward_pass_v(ab2_gar_solver *s, const ab2_fddp_inputs *in, const double *preg, double *Vx_out,
+                             double *Quuks_out, void *stream);
 
 /* Replaces: cycleAppend(knot), proximal-riccati.hxx:79-86 + the problem rotation the
  * caller performs (solver-proxddp.hxx:202-209): factors and stage knots of every
