@@ -514,8 +514,6 @@ static int create_impl(const ab2_gar_dims *dims, int nth, int legs, ab2_gar_solv
   }
   if (const char *f = std::getenv("AB2_PEER_IN_SWEEP")) // 0: the exchange always runs as its own pack + store kernel
     s->pg_in_sweep = std::atoi(f) != 0;
-  if (const char *f = std::getenv("AB2_DEBUG_FLAGS")) // experiment switches, see SweepParams::dbg
-    p.dbg = std::atoi(f);
   if (std::getenv("AB2_PHASE_CLOCKS")) { // profiling aid of the CTA-per-instance kernel: 16 phase counters
     cudaMalloc(&p.clk, 16 * sizeof(long long));
     cudaMemset(p.clk, 0, 16 * sizeof(long long));

@@ -84,7 +84,6 @@ struct SweepParams {
   int num_sms;
   int ctas_per_sm; // host-side launch hint: resident CTAs per SM wanted (0 = whatever fits)
   int stage_head;  // ring head of the stage records: knot t lives in slot (t + stage_head) mod N (O(1) cycleAppend)
-  int dbg;         // experiment switches (env AB2_DEBUG_FLAGS): 1 = no register fast path for the initial system, 2 = no proxy fence before the forward ring, 4 = L2 prefetch of the records ahead (8: at distance 2)
   // parametric problems (nth > 0; CTA-per-instance kernel only): riccati-kernel.hxx:185-192, 278-311
   int nth;
   const double *theta; // [batch][nth] or null (forward)
@@ -196,16 +195,10 @@ struct Cfg {
   static constexpr int WROWS = MMA ? 4 * KT : 0;
   static constexpr int SX = MMA ? fstride(8 * NT2) : 0;  // row stride of X / KK
   static constexpr int XROWS = MMA ? 4 * KT2 : 0;
-  // Vxx_t via a TMA bulk store straight from V' in shared memory instead of LDS.128+STG.128: off,
-  // because every lane must first execute a proxy fence, which costs about what the bulk store saves.
-  static constexpr bool VXX_BULK = false;
   // [Qhat | qhat] waits in V''s storage during the factorisation and the solves (frees 16 registers where the
   // pressure peaks).  Pays where the double-buffered build spills; the single-buffer build of wider shapes
   // has the registers and would only pay the round trip through shared memory.
-#ifndef AB2_PARK
-#define AB2_PARK 1
-#endif
-  static constexpr bool PARK = MMA_ && DB_ && (AB2_PARK != 0);
+  static constexpr bool PARK = MMA_ && DB_;
   // packed Vxx_t store of the tensor-core step: lane l writes the packed pairs l, l + 32, ...
   static constexpr int VPU = (PK_ && MMA_) ? (VP / 2 + 31) / 32 : 0;
   static constexpr int LUT_INTS = MMA ? 32 * (NT + NT * NT + VPU) : 0; // per-CTA table of per-lane constants
@@ -336,13 +329,6 @@ AB2_D D2 ldg2(const double *p) {
   return D2{v.x, v.y};
 #else
   return D2{p[0], p[1]};
-#endif
-}
-AB2_D void prefetch_l2(const void *p) {
-#if defined(__CUDA_ARCH__)
-  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-#else
-  (void)p;
 #endif
 }
 // v[0..N) = p[0..N)  (global memory; ALIGNED: p 16-byte aligned and N even)
@@ -1145,16 +1131,6 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
                        AB2_STAGE_B + (size_t)stage_slot(p, t - 1) * C::SREC_PAD, C::SREC_PAD);
       cur ^= 1;
     }
-    // An L2 prefetch of the record 4 knots ahead used to sit here.  Records prefetched that far ahead are
-    // evicted again by the streaming output before their TMA copy comes, so they are fetched twice: on an H100
-    // (700 W) distance 4 makes the sweep 29 % slower at C2 and 30 % slower at C4.  Off by default;
-    // AB2_DEBUG_FLAGS 4 / 12 bring it back at distance 4 / 2.
-    const int pfd = (p.dbg & 8) ? 2 : 4;
-    if (t >= pfd && (p.dbg & 4)) {
-      const char *nxt = reinterpret_cast<const char *>(AB2_STAGE_B + (size_t)stage_slot(p, t - pfd) * C::SREC_PAD);
-      for (int o = lane * 128; o < C::SREC_PAD * 8; o += C::G * 128)
-        prefetch_l2(nxt + o);
-    }
 
     // fragments of M = [A | f | B]: B-operand of (1) and A-operand (M^T) of (2)
     double Mf[NT][KT];
@@ -1382,8 +1358,6 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
         ctx.sync();
         ctx.issue_copy(0, rec, AB2_STAGE_B + (size_t)stage_slot(p, t - 1) * C::SREC_PAD, C::SPLIT);
       }
-      if (C::VXX_BULK && t > 0)
-        ctx.bulk_store_wait_read(); // the previous knot's Vxx store has finished reading V'
       AB2_UNROLL
       for (int mt = 0; mt < MTX; ++mt) {
         const int i = 8 * mt + g;
@@ -1401,8 +1375,6 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
           }
         }
       }
-      if (C::VXX_BULK)
-        ctx.sync(); // (lane 0 waited above) nobody overwrites V' before the store has read it
       AB2_UNROLL
       for (int mt = 0; mt < MTX; ++mt) {
         const int i = 8 * mt + g;
@@ -1429,8 +1401,6 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
         }
       }
     }
-    if (C::VXX_BULK && t > 0)
-      ctx.async_fence(); // this lane's writes to V' become visible to the TMA store below
     ctx.sync();
     if (t > 0) { // symmetric Vxx_t, as the next step of the reference leaves it
       double *Vt = AB2_VXX_B + (size_t)t * C::VXX_REC;
@@ -1444,8 +1414,6 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
             stg2(Vt + e, o0 == 0xffffu ? 0.0 : Vn[o0], o1 == 0xffffu ? 0.0 : Vn[o1]);
           }
         }
-      } else if (C::VXX_BULK) { // V' is dense in shared memory: one TMA bulk store, no LDS/STG
-        ctx.bulk_store(Vt, Vn, NX * NX);
       } else if (lane < NX) { // row `lane` of the symmetric V' = column `lane` of Vxx_t
         if (C::EVEN && (VS % 2 == 0)) {
           AB2_UNROLL
@@ -1460,10 +1428,6 @@ AB2_D void stage_loop_mma(Ctx &ctx, const SweepParams &p, double *__restrict__ s
         }
       }
     }
-  }
-  if (C::VXX_BULK) { // the last store must have read V' before the initial stage reuses the buffers
-    ctx.bulk_store_wait_read();
-    ctx.sync();
   }
 }
 #undef AB2_STAGE_B
@@ -1897,30 +1861,27 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
       const double *g0 = p.g0 + (size_t)inst * nc0;
       // fast path: LDL^T in registers (lane = column), valid when no pivot test asks for an
       // interchange or a 2x2 pivot; otherwise the general algorithm below, from the same sources
-      bool fast_done = false;
-      if (!(p.dbg & 1)) {
-        const int ld0 = n0 | 1; // odd leading dimension: rows and columns both conflict-free
-        if (colA) {
-          AB2_UNROLL
-          for (int i = 0; i < NX; ++i)
-            if (i >= lane)
-              K0[i + lane * ld0] = vcol[i]; // lower triangle of Vxx_0
-          for (int m = 0; m < nc0; ++m)
-            K0[NX + m + lane * ld0] = G0[m + (size_t)lane * nc0];
-        }
-        for (int m = lane; m < nc0; m += C::G)
-          for (int m2 = m; m2 < nc0; ++m2)
-            K0[NX + m2 + (NX + m) * ld0] = 0.0;
-        const double b = (lane < NX) ? -vx0 : ((lane < n0) ? -g0[lane - NX] : 0.0);
-        double x = 0.0;
-        fast_done = kkt0_fast(ctx, K0, ld0, n0, b, x); // (synchronises before reading)
-        if (fast_done && lane < n0)
-          p.kkt0[(size_t)inst * n0 + lane] = x;
-        if (fast_done)
-          pv |= 0x8000; // statistics: the initial system took the fast path
-        else
-          ctx.sync();   // everyone has left the fast path before the matrix is rebuilt
+      const int ld0 = n0 | 1; // odd leading dimension: rows and columns both conflict-free
+      if (colA) {
+        AB2_UNROLL
+        for (int i = 0; i < NX; ++i)
+          if (i >= lane)
+            K0[i + lane * ld0] = vcol[i]; // lower triangle of Vxx_0
+        for (int m = 0; m < nc0; ++m)
+          K0[NX + m + lane * ld0] = G0[m + (size_t)lane * nc0];
       }
+      for (int m = lane; m < nc0; m += C::G)
+        for (int m2 = m; m2 < nc0; ++m2)
+          K0[NX + m2 + (NX + m) * ld0] = 0.0;
+      const double b = (lane < NX) ? -vx0 : ((lane < n0) ? -g0[lane - NX] : 0.0);
+      double x = 0.0;
+      const bool fast_done = kkt0_fast(ctx, K0, ld0, n0, b, x); // (synchronises before reading)
+      if (fast_done && lane < n0)
+        p.kkt0[(size_t)inst * n0 + lane] = x;
+      if (fast_done)
+        pv |= 0x8000; // statistics: the initial system took the fast path
+      else
+        ctx.sync();   // everyone has left the fast path before the matrix is rebuilt
       if (!fast_done) {
         if (colA) {
           AB2_UNROLL
@@ -1979,8 +1940,7 @@ AB2_D void riccati_group_sweep(Ctx &ctx, const SweepParams &p, const int inst,
     // proxy (initial-stage workspace) and, in the fused sweep, read ff / fb / Vxx / vx this
     // group stored to global memory during the backward pass: every lane orders its
     // generic-proxy writes before the async proxy, then the group synchronises.
-    if (!(p.dbg & 2))
-      ctx.proxy_fence();
+    ctx.proxy_fence();
     ctx.sync();
     auto fill_slot = [&](int d, int t) { // fb record of knot t -> ring slot d
       if (FUSED) { // [K; Z; Ahat]_t | Vxx_t (symmetric for t >= 1; no lambda row reads Vxx_0) | vx_t

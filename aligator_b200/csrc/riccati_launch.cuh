@@ -106,28 +106,11 @@ template <int G, bool TMA> struct DevCtx {
     }
   }
 
-  // Every lane that wrote (through the generic proxy) shared memory a bulk store will read
-  // calls this BEFORE the group synchronisation that precedes bulk_store().
-  __device__ __forceinline__ void async_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
   // Generic-proxy writes of this lane (shared AND global) ordered before later async-proxy
   // (TMA) accesses: executed by every writing lane before the synchronisation that precedes
   // the bulk copy which overwrites or reads what it wrote (PTX memory model, proxies).
   __device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async;" ::: "memory"); }
   __device__ __forceinline__ void proxy_fence_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-  // Shared -> global bulk store of `nd` doubles (TMA).  One lane issues.
-  __device__ __forceinline__ void bulk_store(double *gdst, const double *ssrc, int nd) {
-    if (lane == 0) {
-      asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst),
-                   "r"(smem_u32(ssrc)), "r"((uint32_t)nd * 8u)
-                   : "memory");
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    }
-  }
-  // the source of every earlier bulk_store may be overwritten after this + a sync
-  __device__ __forceinline__ void bulk_store_wait_read() {
-    if (lane == 0)
-      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-  }
 
   __device__ __forceinline__ void wait_copy(int part) {
     if (TMA) {

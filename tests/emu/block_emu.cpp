@@ -74,33 +74,27 @@ struct HostBlockCtx {
 };
 } // namespace
 
-extern "C" int emu_block_stage_record(int nx, int nu, int nc) {
-  return ab2::make_block_dims(nx, nu, nc, 0).srec_pad;
+// nth > 0: parametric records
+extern "C" int emu_block_stage_record(int nx, int nu, int nc, int nth) {
+  return ab2::make_block_dims(nx, nu, nc, 0, nth).srec_pad;
 }
 
 template <class D> static int run_block(const D &d, int nwarps, const ab2::SweepParams &p);
 template <class F> static void run_cta(int nwarps, size_t smem_doubles, F body);
 
+// run-time dimensions; parametric problems when p->nth > 0
+extern "C" int emu_block_sweep(int nx, int nu, int nc, int nwarps, const ab2::SweepParams *p) {
+  return run_block(ab2::make_block_dims(nx, nu, nc, p->nc0, p->nth), nwarps, *p);
+}
+
 // the compile-time specialisation (StaticBlockDims) of two small shapes, to execute that
 // instantiation of the code on the CPU
-extern "C" int emu_block_sweep_static(int nx, int nu, int nc, int nwarps, const ab2::SweepParams *pp) {
-  if (nx == 7 && nu == 3 && nc == 0 && pp->nc0 == 7)
-    return run_block(ab2::StaticBlockDims<7, 3, 0, 7>{}, nwarps, *pp);
-  if (nx == 9 && nu == 5 && nc == 3 && pp->nc0 == 9)
-    return run_block(ab2::StaticBlockDims<9, 5, 3, 9>{}, nwarps, *pp);
+extern "C" int emu_block_sweep_static(int nx, int nu, int nc, int nwarps, const ab2::SweepParams *p) {
+  if (nx == 7 && nu == 3 && nc == 0 && p->nc0 == 7)
+    return run_block(ab2::StaticBlockDims<7, 3, 0, 7>{}, nwarps, *p);
+  if (nx == 9 && nu == 5 && nc == 3 && p->nc0 == 9)
+    return run_block(ab2::StaticBlockDims<9, 5, 3, 9>{}, nwarps, *p);
   return 1;
-}
-
-// parametric problems (nth > 0)
-extern "C" int emu_block_stage_record_th(int nx, int nu, int nc, int nth) {
-  return ab2::make_block_dims(nx, nu, nc, 0, nth).srec_pad;
-}
-extern "C" int emu_block_sweep_th(int nx, int nu, int nc, int nth, int nwarps, const ab2::SweepParams *pp) {
-  return run_block(ab2::make_block_dims(nx, nu, nc, pp->nc0, nth), nwarps, *pp);
-}
-
-extern "C" int emu_block_sweep(int nx, int nu, int nc, int nwarps, const ab2::SweepParams *pp) {
-  return run_block(ab2::make_block_dims(nx, nu, nc, pp->nc0), nwarps, *pp);
 }
 
 // one emulated CTA of 32*nwarps threads running body(ctx, smem)
@@ -130,7 +124,7 @@ template <class F> static void run_cta(int nwarps, size_t smem_doubles, F body) 
     t.join();
 }
 
-template <class D> static int run_block(const D &d, int nwarps, const ab2::SweepParams &p) {
+template <class D, class Mu> static int run_block(const D &d, int nwarps, const ab2::SweepParams &p, const Mu &mu) {
   const int nx = d.nx;
   const int T = 32 * nwarps;
   if (nx + 1 > T || d.nk > T || nx + p.nc0 > T || d.nr > T || d.nth > T)
@@ -138,8 +132,13 @@ template <class D> static int run_block(const D &d, int nwarps, const ab2::Sweep
   const int legs = p.legs > 1 ? p.legs : 1;
   for (int item = 0; item < p.batch * legs; ++item)
     run_cta(nwarps, (size_t)d.s_end,
-            [&](HostBlockCtx &ctx, double *sm) { ab2::riccati_block_sweep(ctx, p, d, item / legs, sm, item % legs); });
+            [&](HostBlockCtx &ctx, double *sm) { ab2::riccati_block_sweep(ctx, p, d, item / legs, sm, item % legs, mu); });
   return 0;
+}
+
+// the mu source as the device launchers pick it: the per-instance array when it is set
+template <class D> static int run_block(const D &d, int nwarps, const ab2::SweepParams &p) {
+  return p.mueq_b ? run_block(d, nwarps, p, ab2::InstanceMu()) : run_block(d, nwarps, p, ab2::ScalarMu());
 }
 
 // Leg mode (gar::ParallelRiccatiSolver): legs backward -> condensed solve -> legs forward, as the
@@ -178,12 +177,16 @@ extern "C" int emu_block_legs(int nx, int nu, int nc, int nwarps, int mode, cons
 }
 
 // The stage-dense solver (riccati_dense.cuh) on emulated CTAs.
-extern "C" int emu_dense_sweep(int nx, int nu, int nc, int nwarps, const ab2::SweepParams *pp) {
-  const ab2::DenseDims d = ab2::make_dense_dims(nx, nu, nc, pp->nct, pp->nc0);
+template <class Mu> static int run_dense(int nx, int nu, int nc, int nwarps, const ab2::SweepParams &p, const Mu &mu) {
+  const ab2::DenseDims d = ab2::make_dense_dims(nx, nu, nc, p.nct, p.nc0);
   const int T = 32 * nwarps;
-  if (d.n > T || nx + pp->nc0 > T || nx + 1 > T)
+  if (d.n > T || nx + p.nc0 > T || nx + 1 > T)
     return 2;
-  for (int inst = 0; inst < pp->batch; ++inst)
-    run_cta(nwarps, (size_t)d.s_end, [&](HostBlockCtx &ctx, double *sm) { ab2::riccati_dense_sweep(ctx, *pp, d, inst, sm); });
+  for (int inst = 0; inst < p.batch; ++inst)
+    run_cta(nwarps, (size_t)d.s_end, [&](HostBlockCtx &ctx, double *sm) { ab2::riccati_dense_sweep(ctx, p, d, inst, sm, mu); });
   return 0;
+}
+
+extern "C" int emu_dense_sweep(int nx, int nu, int nc, int nwarps, const ab2::SweepParams *p) {
+  return p->mueq_b ? run_dense(nx, nu, nc, nwarps, *p, ab2::InstanceMu()) : run_dense(nx, nu, nc, nwarps, *p, ab2::ScalarMu());
 }

@@ -60,17 +60,11 @@ struct HostCtx {
       std::memcpy(dst, src, sizeof(double) * (size_t)nd);
   }
   void wait_copy(int) { sync(); }
-  void bulk_store(double *gdst, const double *ssrc, int nd) {
-    if (lane == 0)
-      std::memcpy(gdst, ssrc, sizeof(double) * (size_t)nd);
-  }
-  void bulk_store_wait_read() {}
-  void async_fence() {}
   void proxy_fence() {}
   void proxy_fence_smem() {}
 };
 
-template <class C> int run(const ab2::SweepParams &p) {
+template <class C, class Mu> int run(const ab2::SweepParams &p, const Mu &mu) {
   constexpr int NX = C::NX, G = C::G;
   if (NX + p.nc0 > G)
     return 2;
@@ -87,30 +81,33 @@ template <class C> int run(const ab2::SweepParams &p) {
     for (int l = 0; l < G; ++l)
       th.emplace_back([&, l] {
         HostCtx ctx{l, G, &bar, xa.data(), xb.data(), lutv.data()};
-        ab2::riccati_group_sweep<C>(ctx, p, inst, sm.data());
+        ab2::riccati_group_sweep<C>(ctx, p, inst, sm.data(), mu);
       });
     for (auto &t : th)
       t.join();
   }
   return 0;
 }
-} // namespace
 
-template <int NX, int NU, int NC, int G> int dispatch(int mode, const ab2::SweepParams &p) {
-  if (mode == 2) { // tensor-core formulation
-    if constexpr (G == 32 && NC == 0 && NX % 2 == 0)
-      return run<ab2::Cfg<NX, NU, NC, G, true, true, true>>(p);
-    else
-      return 3;
-  }
-  if (mode == 3) { // tensor-core formulation, single record buffer
-    if constexpr (G == 32 && NC == 0 && NX % 2 == 0)
-      return run<ab2::Cfg<NX, NU, NC, G, false, true, true>>(p);
-    else
-      return 3;
-  }
-  return mode ? run<ab2::Cfg<NX, NU, NC, G, true>>(p) : run<ab2::Cfg<NX, NU, NC, G, false>>(p);
+// the mu source as the device launchers pick it: the per-instance array when it is set
+template <class C> int run(const ab2::SweepParams &p) {
+  return p.mueq_b ? run<C>(p, ab2::InstanceMu()) : run<C>(p, ab2::ScalarMu());
 }
+
+// mode 0/1: lane-per-column step, single / double record buffer; 2/3: tensor-core step, double / single.
+// PK: Vxx stored packed (every device build) instead of full (the reference the packed program is compared with).
+template <int NX, int NU, int NC, int G, bool PK> int dispatch(int mode, const ab2::SweepParams &p) {
+  if (mode >= 2) {
+    if constexpr (G == 32 && NC == 0 && NX % 2 == 0)
+      return mode == 2 ? run<ab2::Cfg<NX, NU, NC, G, true, true, true, PK>>(p)
+                       : run<ab2::Cfg<NX, NU, NC, G, false, true, true, PK>>(p);
+    else
+      return 3;
+  }
+  return mode ? run<ab2::Cfg<NX, NU, NC, G, true, true, false, PK>>(p)
+              : run<ab2::Cfg<NX, NU, NC, G, false, true, false, PK>>(p);
+}
+} // namespace
 
 extern "C" int emu_stage_record(int nx, int nu, int nc) {
 #define X(NX, NU, NC, G)                                                        \
@@ -121,10 +118,12 @@ extern "C" int emu_stage_record(int nx, int nu, int nc) {
   return -1;
 }
 
-extern "C" int emu_sweep(int nx, int nu, int nc, int db, const ab2::SweepParams *p) {
+extern "C" int emu_vxx_packed_doubles(int nx) { return ab2::vxx_packed_doubles(nx); }
+
+extern "C" int emu_sweep(int nx, int nu, int nc, int mode, int packed, const ab2::SweepParams *p) {
 #define X(NX, NU, NC, G)                                                        \
   if (nx == NX && nu == NU && nc == NC)                                         \
-    return dispatch<NX, NU, NC, G>(db, *p);
+    return packed ? dispatch<NX, NU, NC, G, true>(mode, *p) : dispatch<NX, NU, NC, G, false>(mode, *p);
   AB2_FOR_EACH_CONFIG(X)
 #undef X
   return 1;

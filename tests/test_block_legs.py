@@ -1,47 +1,14 @@
 """Leg mode of the CTA-per-instance program = gar::ParallelRiccatiSolver on the device
 (gar/parallel-solver.hxx:51-243, gar/block-tridiagonal.hpp:52-182): the legs of every instance are
 work items of ONE launch, the condensed block-tridiagonal system is solved by a second kernel, the
-legs roll out in a third.  Host emulation (tests/emu/block_emu.cpp) against the oracle's restatement
+legs roll out in a third.  Host emulation (tests/emu_harness.py) against the oracle's restatement
 of the parallel solver (same leg split) and against the serial solution."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import gen
-import test_group_emulation as tg
+from emu_harness import emulate
 from oracle import gar_oracle as orc
-
-
-def run_legs(probs, nx, nu, nc, nct, N, T, mueq, nw=1, collapse=False):
-    lib = tg._block_lib()
-    B = len(probs)
-    nc0 = probs[0].nc0
-    stage, term, G0, g0 = gen.pack_problems(probs)
-    srec = lib.emu_block_stage_record(nx, nu, nc)
-    if N > 0 and stage.shape[-1] != srec:
-        stage = np.concatenate([stage, np.zeros(stage.shape[:-1] + (srec - stage.shape[-1],))], -1)
-    stage = np.ascontiguousarray(stage)
-    nr, nth = nu + nc + nx, nx
-    z = lambda *s: np.full(s if np.prod(s) > 0 else (1,), np.nan)
-    zz = lambda *s: np.zeros(s if np.prod(s) > 0 else (1,))
-    out = dict(ff=z(B, N, nr), fb=z(B, N, nr, nx), Vxx=z(B, N + 1, nx * nx), vx=z(B, N + 1, nx), ffT=z(B, nct),
-               fbT=z(B, nct, nx), kkt0=z(B, nx + nc0), xs=z(B, N + 1, nx), us=z(B, N, nu), vs=z(B, N, nc),
-               vsT=z(B, nct), lbd0=z(B, nc0), lbdas=z(B, N, nx), fth=zz(B, N, nr, nth), Vxt=zz(B, N + 1, nx * nth),
-               Vtt=zz(B, N + 1, nth * nth), vt=zz(B, N + 1, nth), cond=z(B, nc0 + nx * (2 * T - 1)))
-    status = np.full(B, -1, dtype=np.int32)
-    pivstat = np.zeros(B, dtype=np.int32)
-    sp = tg.SweepParams()
-    sp.N, sp.nct, sp.nc0, sp.batch, sp.mueq, sp.do_bwd, sp.do_fwd, sp.nth, sp.legs = N, nct, nc0, B, mueq, 1, 1, nth, T
-    keep = dict(stage=stage, term=term, G0=G0, g0=g0, **out)
-    for k, v in keep.items():
-        setattr(sp, k, v.ctypes.data_as(tg._dp))
-    sp.status = status.ctypes.data_as(C.POINTER(C.c_int))
-    sp.pivstat = pivstat.ctypes.data_as(C.POINTER(C.c_int))
-    rc = lib.emu_block_legs(nx, nu, nc, nw, 3 | (4 if collapse else 0), C.byref(sp))
-    assert rc == 0, rc
-    out["status"] = status
-    return out
 
 
 def oracle_parallel(prob, T, mueq):
@@ -60,7 +27,7 @@ def test_legs_match_oracle_parallel_and_serial(shape):
     nx, nu, nc, nct, N, T, mueq = shape
     B = 2
     probs = gen.generate_batch(40 + nx + T, B, N, nx, nu, nc, nct)
-    got = run_legs(probs, nx, nu, nc, nct, N, T, mueq)
+    got = emulate("legs", probs, (nx, nu, nc, nct, N), mueq, 1, legs=T)
     assert np.all(got["status"] == 0)
     cat = lambda v: np.concatenate([np.ravel(a) for a in v] + [np.zeros(0)])
     tol = 1e-10
@@ -111,7 +78,7 @@ def test_collapse_feedback_matches_the_reference_statement():
     (oracle and device agree on it)."""
     nx, nu, N, T, mueq = 5, 2, 12, 3, 1e-8
     probs = gen.generate_batch(9, 1, N, nx, nu, 0, 0)
-    got = run_legs(probs, nx, nu, 0, 0, N, T, mueq, collapse=True)
+    got = emulate("legs", probs, (nx, nu, 0, 0, N), mueq, 1, legs=T, collapse=True)
     op, s, sol = oracle_parallel(probs[0], T, mueq)
     s.collapseFeedback()
     assert gen.rel_fro(got["fb"][0, 0, :nu], s.factor(0)["fb"][:nu]) <= 1e-10

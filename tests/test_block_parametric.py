@@ -1,15 +1,11 @@
 """Parametric problems (nth > 0: riccati-kernel.hxx:185-192, 278-311; proximal-riccati.hxx:50-59;
 forward with theta) on the CTA-per-instance program, host emulation vs the oracle."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import gen
-import test_group_emulation as tg
+from emu_harness import emulate
 from oracle import gar_oracle as orc
-
-F = lambda a: np.asarray(a, dtype=np.float64).ravel(order="F")
 
 
 def make_problem(seed, N, nx, nu, nc, nct, nth):
@@ -27,45 +23,14 @@ def make_problem(seed, N, nx, nu, nc, nct, nth):
     return p
 
 
-def run(p, nx, nu, nc, nct, nth, N, mueq, theta, nw):
-    lib = tg._block_lib()
-    srec = lib.emu_block_stage_record_th(nx, nu, nc, nth)
-    stage = np.zeros((1, max(N, 1), srec))
-    for t in range(N):
-        k = p.stages[t]
-        rec = np.concatenate([gen.stage_record(k), F(k.Gx), F(k.Gu), F(k.Gv), F(k.Gth), F(k.gamma)])
-        stage[0, t, :rec.size] = rec
-    kt = p.stages[N]
-    term = np.concatenate([gen.term_record(kt), F(kt.Gx), F(kt.Gv), F(kt.Gth), F(kt.gamma)])[None]
-    G0, g0 = F(p.G0)[None], np.asarray(p.g0)[None]
-    nr, nc0 = nu + nc + nx, p.nc0
-    z = lambda *s: np.full(s if np.prod(s) > 0 else (1,), np.nan)
-    out = dict(ff=z(1, N, nr), fb=z(1, N, nr, nx), Vxx=z(1, N + 1, nx * nx), vx=z(1, N + 1, nx), ffT=z(1, nct),
-               fbT=z(1, nct, nx), kkt0=z(1, nx + nc0), xs=z(1, N + 1, nx), us=z(1, N, nu), vs=z(1, N, nc),
-               vsT=z(1, nct), lbd0=z(1, nc0), lbdas=z(1, N, nx), fth=z(1, N, nr, nth), Vxt=z(1, N + 1, nx * nth),
-               Vtt=z(1, N + 1, nth * nth), vt=z(1, N + 1, nth), kkt0fth=z(1, nx + nc0, nth), thGrad=z(1, nth),
-               thHess=z(1, nth * nth))
-    status = np.full(1, -1, dtype=np.int32)
-    sp = tg.SweepParams()
-    sp.N, sp.nct, sp.nc0, sp.batch, sp.mueq, sp.do_bwd, sp.do_fwd, sp.nth = N, nct, nc0, 1, mueq, 1, 1, nth
-    th = np.ascontiguousarray(theta, dtype=np.float64)
-    keep = dict(stage=np.ascontiguousarray(stage), term=np.ascontiguousarray(term), G0=np.ascontiguousarray(G0),
-                g0=np.ascontiguousarray(g0), theta=th, **out)
-    for k, v in keep.items():
-        setattr(sp, k, v.ctypes.data_as(tg._dp))
-    sp.status = status.ctypes.data_as(C.POINTER(C.c_int))
-    assert lib.emu_block_sweep_th(nx, nu, nc, nth, nw, C.byref(sp)) == 0
-    assert status[0] == 0
-    return out
-
-
 @pytest.mark.parametrize("shape", [(5, 2, 0, 0, 3, 6, 1e-8, 1), (4, 3, 2, 0, 2, 5, 1e-3, 1), (7, 3, 0, 2, 7, 4, 1e-2, 2),
                                    (6, 2, 1, 0, 1, 3, 1e-3, 1)])
 def test_parametric_block_sweep(shape):
     nx, nu, nc, nct, nth, N, mueq, nw = shape
     p = make_problem(sum(shape[:6]), N, nx, nu, nc, nct, nth)
     theta = np.random.default_rng(3).standard_normal(nth)
-    got = run(p, nx, nu, nc, nct, nth, N, mueq, theta, nw)
+    got = emulate("parametric", [p], (nx, nu, nc, nct, N), mueq, nw, nth=nth, theta=theta)
+    assert got["status"][0] == 0
     op = orc.OracleProblem(p)
     ref = orc.ProximalRiccatiSolver(op)
     assert ref.backward(mueq)

@@ -7,26 +7,27 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cxx", "host_class_test.cpp")
-EXE = os.path.join(ROOT, "tests", "cxx", "host_class_test")
 
 
-def _build():
+@pytest.fixture(scope="module")
+def exe(tmp_path_factory):
+    """The test program, built outside the source tree (which may be read-only)."""
     import __graft_entry__ as g
     g.build()
     libdir = os.path.join(ROOT, "aligator_b200")
-    subprocess.check_call(["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", SRC, "-o", EXE,
+    path = str(tmp_path_factory.mktemp("cxx") / "host_class_test")
+    subprocess.check_call(["/usr/bin/g++", "-std=c++17", "-O2", "-Wall", SRC, "-o", path,
                            "-L" + libdir, "-laligator_b200_gar", "-Wl,-rpath," + libdir])
+    return path
 
 
-def test_host_class_compiles_and_links():
-    _build()
-    assert os.path.exists(EXE)
+def test_host_class_compiles_and_links(exe):
+    assert os.path.exists(exe)
 
 
 @pytest.mark.gpu
-def test_host_class_parity_on_gpu():
-    _build()
-    r = subprocess.run([EXE], capture_output=True, text=True, timeout=600)
+def test_host_class_parity_on_gpu(exe):
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=600)
     print(r.stdout, r.stderr)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "ALL OK" in r.stdout

@@ -1,38 +1,12 @@
 """The stage-dense solver on the device (aligator_b200/csrc/riccati_dense.cuh = gar::RiccatiSolverDense): host
 emulation against the oracle's restatement of the same algorithm and against the proximal solution."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import gen
-import test_group_emulation as tg
 from aligator_b200.lqr import LqrKnot
+from emu_harness import emulate
 from oracle import gar_oracle as orc
-
-
-def run_dense_emulated(probs, nx, nu, nc, nct, N, mueq, nw):
-    lib = tg._block_lib()
-    B, nc0 = len(probs), probs[0].nc0
-    stage, term, G0, g0 = gen.pack_problems(probs)
-    srec = lib.emu_block_stage_record(nx, nu, nc)
-    if N > 0 and stage.shape[-1] != srec:
-        stage = np.concatenate([stage, np.zeros(stage.shape[:-1] + (srec - stage.shape[-1],))], -1)
-    n = nu + nc + 2 * nx
-    z = lambda *s: np.full(s if np.prod(s) > 0 else (1,), np.nan)
-    out = dict(ff=z(B, N, n), fb=z(B, N, n, nx), Vxx=z(B, N + 1, nx * nx), vx=z(B, N + 1, nx), ffT=z(B, nct), fbT=z(B, nct, nx),
-               kkt0=z(B, nx + nc0), xs=z(B, N + 1, nx), us=z(B, N, nu), vs=z(B, N, nc), vsT=z(B, nct), lbd0=z(B, nc0),
-               lbdas=z(B, N, nx))
-    status = np.full(B, -1, dtype=np.int32)
-    sp = tg.SweepParams()
-    sp.N, sp.nct, sp.nc0, sp.batch, sp.mueq, sp.do_bwd, sp.do_fwd = N, nct, nc0, B, mueq, 1, 1
-    keep = dict(stage=np.ascontiguousarray(stage), term=term, G0=G0, g0=g0, **out)
-    for k, v in keep.items():
-        setattr(sp, k, v.ctypes.data_as(tg._dp))
-    sp.status = status.ctypes.data_as(C.POINTER(C.c_int))
-    assert lib.emu_dense_sweep(nx, nu, nc, nw, C.byref(sp)) == 0
-    assert np.all(status == 0)
-    return out
 
 
 @pytest.mark.parametrize("shape", [(4, 2, 0, 0, 8, 1e-8, 1), (6, 3, 0, 0, 12, 1e-8, 1), (4, 2, 2, 0, 9, 1e-3, 1),
@@ -40,7 +14,8 @@ def run_dense_emulated(probs, nx, nu, nc, nct, N, mueq, nw):
 def test_dense_kernel_matches_oracle_dense_and_proximal(shape):
     nx, nu, nc, nct, N, mueq, nw = shape
     probs = gen.generate_batch(50 + nx, 2, N, nx, nu, nc, nct)
-    got = run_dense_emulated(probs, nx, nu, nc, nct, N, mueq, nw)
+    got = emulate("dense", probs, (nx, nu, nc, nct, N), mueq, nw)
+    assert np.all(got["status"] == 0)
     n = nu + nc + 2 * nx
     for b, p in enumerate(probs):
         q = p.copy()

@@ -1,105 +1,13 @@
 """CPU execution of the CUDA group program (riccati_group.cuh) through the host
-emulation in tests/emu/group_emu.cpp (G threads + a barrier per group), compared
+emulation (tests/emu_harness.py: G threads + a barrier per group), compared
 with the oracle.  This validates the kernel's arithmetic and indexing without a
 GPU; the TMA/mbarrier plumbing is the only part it cannot see."""
-import ctypes as C
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
 import gen
+from emu_harness import emulate
 from oracle import gar_oracle as orc
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU_DIR = os.path.join(HERE, "emu")
-EMU_LIB = os.path.join(EMU_DIR, "libgroup_emu.so")
-_dp = C.POINTER(C.c_double)
-
-
-class SweepParams(C.Structure):
-    _fields_ = [("N", C.c_int), ("nct", C.c_int), ("nc0", C.c_int), ("batch", C.c_int),
-                ("mueq", C.c_double), ("do_bwd", C.c_int), ("do_fwd", C.c_int)] + \
-               [(n, _dp) for n in ("stage", "term", "G0", "g0", "ff", "fb", "Vxx", "vx", "ffT",
-                                   "fbT", "kkt0", "xs", "us", "vs", "vsT", "lbd0", "lbdas")] + \
-               [("status", C.POINTER(C.c_int)), ("pivstat", C.POINTER(C.c_int)), ("stagger_ns", C.c_int),
-                ("num_sms", C.c_int),
-                ("ctas_per_sm", C.c_int), ("stage_head", C.c_int), ("dbg", C.c_int), ("nth", C.c_int)] + \
-               [(n, _dp) for n in ("theta", "fth", "Vxt", "Vtt", "vt", "kkt0fth", "thGrad", "thHess")] + \
-               [("legs", C.c_int), ("clk", C.c_void_p), ("cond", _dp),
-                ("peer_world", C.c_int), ("peer_dst", C.c_void_p * 8), ("peer_off", C.c_longlong)]
-
-
-def _lib():
-    srcs = [os.path.join(EMU_DIR, "group_emu.cpp"),
-            os.path.join(HERE, "..", "aligator_b200", "csrc", "riccati_group.cuh"),
-            os.path.join(HERE, "..", "aligator_b200", "csrc", "riccati_configs.h")]
-    if (not os.path.exists(EMU_LIB)
-            or os.path.getmtime(EMU_LIB) < max(os.path.getmtime(s) for s in srcs)):
-        subprocess.check_call(["/usr/bin/g++", "-O1", "-std=c++20", "-fPIC", "-shared", "-pthread",
-                               "-o", EMU_LIB, srcs[0]])
-    return C.CDLL(EMU_LIB)
-
-
-BLOCK_LIB = os.path.join(EMU_DIR, "libblock_emu.so")
-
-
-def _block_lib():
-    srcs = [os.path.join(EMU_DIR, "block_emu.cpp"),
-            os.path.join(HERE, "..", "aligator_b200", "csrc", "riccati_block.cuh"),
-            os.path.join(HERE, "..", "aligator_b200", "csrc", "riccati_group.cuh")]
-    if (not os.path.exists(BLOCK_LIB)
-            or os.path.getmtime(BLOCK_LIB) < max(os.path.getmtime(s) for s in srcs)):
-        subprocess.check_call(["/usr/bin/g++", "-O1", "-std=c++20", "-fPIC", "-shared", "-pthread",
-                               "-o", BLOCK_LIB, srcs[0]])
-    return C.CDLL(BLOCK_LIB)
-
-
-def run_emulated(nx, nu, nc, nct, N, probs, mueq, db=0, block=0, peers=None):
-    """block = 0: the warp-per-instance group program; block = NW > 0: the
-    CTA-per-instance program of riccati_block.cuh with NW emulated warps."""
-    lib = _block_lib() if block else _lib()
-    B = len(probs)
-    nc0 = probs[0].nc0
-    stage, term, G0, g0 = gen.pack_problems(probs)
-    srec = lib.emu_block_stage_record(nx, nu, nc) if block else lib.emu_stage_record(nx, nu, nc)
-    assert srec > 0, "shape not instantiated"
-    if N > 0 and stage.shape[-1] != srec:
-        stage = np.concatenate([stage, np.zeros(stage.shape[:-1] + (srec - stage.shape[-1],))], -1)
-    stage = np.ascontiguousarray(stage)
-    nr = nu + nc + nx
-    z = lambda *s: np.full(s if np.prod(s) > 0 else (1,), np.nan)
-    out = dict(ff=z(B, N, nr), fb=z(B, N, nr, nx), Vxx=z(B, N + 1, nx * nx), vx=z(B, N + 1, nx),
-               ffT=z(B, nct), fbT=z(B, nct, nx), kkt0=z(B, nx + nc0), xs=z(B, N + 1, nx),
-               us=z(B, N, nu), vs=z(B, N, nc), vsT=z(B, nct), lbd0=z(B, nc0), lbdas=z(B, N, nx))
-    status = np.full(B, -1, dtype=np.int32)
-    p = SweepParams()
-    p.N, p.nct, p.nc0, p.batch, p.mueq, p.do_bwd, p.do_fwd = N, nct, nc0, B, mueq, 1, 1
-    keep = dict(stage=stage, term=term, G0=G0, g0=g0, **out)
-    for k, v in keep.items():
-        setattr(p, k, v.ctypes.data_as(_dp))
-    p.status = status.ctypes.data_as(C.POINTER(C.c_int))
-    pivstat = np.zeros(B, dtype=np.int32)
-    p.pivstat = pivstat.ctypes.data_as(C.POINTER(C.c_int))
-    if peers is not None:  # sharded batch: (receive buffers of every rank, offset in doubles) -- SweepParams::peer_*
-        bufs, off = peers
-        p.peer_world = len(bufs)
-        for w, b in enumerate(bufs):
-            p.peer_dst[w] = b.ctypes.data
-        p.peer_off = off
-    if block < 0:  # compile-time specialisation of the block program (StaticBlockDims)
-        rc = lib.emu_block_sweep_static(nx, nu, nc, int(-block), C.byref(p))
-    elif block:
-        rc = lib.emu_block_sweep(nx, nu, nc, int(block), C.byref(p))
-    else:
-        rc = lib.emu_sweep(nx, nu, nc, int(db), C.byref(p))
-    assert rc == 0
-    out["Vxx"] = out["Vxx"].reshape(B, N + 1, nx, nx).transpose(0, 1, 3, 2)
-    out["status"] = status
-    out["pivots_2x2"], out["interchanges"] = pivstat & 0x7fff, (pivstat >> 16) & 0xffff
-    out["kkt0_fast"] = ((pivstat >> 15) & 1).astype(bool)
-    return out
 
 
 def check_against_oracle(nx, nu, nc, nct, N, B, mueq, seed, tol=1e-10, style="conditioned", db=0,
@@ -107,7 +15,11 @@ def check_against_oracle(nx, nu, nc, nct, N, B, mueq, seed, tol=1e-10, style="co
     probs = gen.generate_batch(seed, B, N, nx, nu, nc, nct, style=style)
     if pivoting:
         gen.make_pivoting(probs)
-    got = run_emulated(nx, nu, nc, nct, N, probs, mueq, db, block)
+    # block = 0: the warp-per-instance group program; block = NW > 0: the CTA-per-instance program of
+    # riccati_block.cuh with NW emulated warps; block = -NW: its compile-time specialisation (StaticBlockDims)
+    kind = "group" if block == 0 else ("block" if block > 0 else "static")
+    got = emulate(kind, probs, (nx, nu, nc, nct, N), mueq, db if block == 0 else abs(block))
+    got["Vxx"] = got["Vxx"].reshape(B, N + 1, nx, nx).transpose(0, 1, 3, 2)
     assert np.all(got["status"] == 0)
     stage, term, G0, g0 = gen.pack_problems(probs)
     bo = orc.BatchedOracle(nx, nu, nc, nct, probs[0].nc0, N, B, stage, term, G0, g0)
@@ -216,14 +128,18 @@ def test_pivot_statistics_and_initial_fast_path():
     of the initial saddle system and no 2x2 pivot; make_2x2_pivots() problems take min(nu,nc) 2x2
     pivots per knot; make_pivoting() problems take one interchange per knot."""
     nx, nu, N, B = 12, 6, 6, 3
-    got = run_emulated(nx, nu, 0, 0, N, gen.generate_batch(3, B, N, nx, nu, 0, 0), 1e-8, db=2)
-    assert np.all(got["kkt0_fast"]) and np.all(got["pivots_2x2"] == 0) and np.all(got["interchanges"] == 0)
-    got = run_emulated(nx, nu, 0, 0, N, gen.make_pivoting(gen.generate_batch(3, B, N, nx, nu, 0, 0)), 1e-8, db=2)
-    assert np.all(got["interchanges"] >= N)
+    pivots_2x2 = lambda o: o["pivstat"] & 0x7fff
+    interchanges = lambda o: (o["pivstat"] >> 16) & 0xffff
+    got = emulate("group", gen.generate_batch(3, B, N, nx, nu, 0, 0), (nx, nu, 0, 0, N), 1e-8, 2)
+    kkt0_fast = ((got["pivstat"] >> 15) & 1).astype(bool)
+    assert np.all(kkt0_fast) and np.all(pivots_2x2(got) == 0) and np.all(interchanges(got) == 0)
+    got = emulate("group", gen.make_pivoting(gen.generate_batch(3, B, N, nx, nu, 0, 0)), (nx, nu, 0, 0, N), 1e-8, 2)
+    assert np.all(interchanges(got) >= N)
     nx, nu, nc = 4, 2, 2
     probs = gen.make_2x2_pivots(gen.generate_batch(4, B, N, nx, nu, nc, 0))
-    got = run_emulated(nx, nu, nc, 0, N, probs, 1e-3, db=1)
-    assert np.all(got["pivots_2x2"] >= N * min(nu, nc))
+    got = emulate("group", probs, (nx, nu, nc, 0, N), 1e-3, 1)
+    assert np.all(pivots_2x2(got) >= N * min(nu, nc))
+    got["Vxx"] = got["Vxx"].reshape(B, N + 1, nx, nx).transpose(0, 1, 3, 2)
     stage, term, G0, g0 = gen.pack_problems(probs)
     bo = orc.BatchedOracle(nx, nu, nc, 0, nx, N, B, stage, term, G0, g0)
     bo.sweep(1e-3)
@@ -245,8 +161,8 @@ def test_in_sweep_exchange_of_the_first_step_policy(shape, db):
     total = B * per
     bufs = [np.full(3 * world * total, -7.0) for _ in range(world)]
     off = slot * world * total + rank * total
-    out = run_emulated(nx, nu, nc, nct, N, probs, 1e-6, db=db, peers=(bufs, off))
-    ref = run_emulated(nx, nu, nc, nct, N, probs, 1e-6, db=db)
+    out = emulate("group", probs, shape, 1e-6, db, peers=(bufs, off))
+    ref = emulate("group", probs, shape, 1e-6, db)
     assert np.array_equal(out["fb"], ref["fb"]) and np.array_equal(out["xs"], ref["xs"])
     want = np.concatenate([out["fb"][:, 0, :nu, :], out["ff"][:, 0, :nu, None]], axis=2).ravel()
     for b in bufs:
