@@ -225,6 +225,46 @@ def make_2x2_pivots(probs):
     return probs
 
 
+def general_initial_condition(probs, nc0, seed):
+    """Replace G0 = -I, g0 = x0 by nc0 Gaussian rows G0 (any nc0 in [0, nx]) and a Gaussian g0, as a state
+    manifold's G0 = -Jdiff would be.  Each problem gets `cond_G0`, the 2-norm condition number of its G0 (1 when
+    nc0 = 0)."""
+    for b, p in enumerate(probs):
+        rng = np.random.default_rng([seed, b, nc0])
+        nx = p.stages[0].nx
+        p.G0 = np.asfortranarray(rng.standard_normal((nc0, nx)))
+        p.g0 = rng.standard_normal(nc0)
+        p.cond_G0 = float(np.linalg.cond(p.G0)) if nc0 else 1.0
+    return probs
+
+
+def make_homogeneous(probs):
+    """q = r = f = d = g0 = 0 with every other input left as it is: the solution is exactly zero."""
+    for p in probs:
+        for k in p.stages:
+            for name in ("q", "r", "f", "d"):
+                getattr(k, name)[:] = 0.0
+        p.g0[:] = 0.0
+    return probs
+
+
+def scale_instances(probs, exponents, mueq):
+    """Instance b times c_b = 2**exponents[b]: Q, S, R, q, r, C, D, d, G0 and g0 scaled (A, B, f kept), and
+    mu_b = c_b * mueq.  Every saddle-point system of instance b is then exactly c_b times the original one.
+    Returns (scaled copies, [batch] per-instance mu)."""
+    out = []
+    for p, s in zip(probs, exponents):
+        q = p.copy()
+        c = 2.0 ** int(s)
+        for k in q.stages:
+            for name in ("Q", "S", "R", "q", "r", "C", "D", "d"):
+                getattr(k, name)[...] *= c
+        q.G0 *= c
+        q.g0 *= c
+        out.append(q)
+    return out, np.array([2.0 ** int(s) * mueq for s in exponents])
+
+
 def kkt_condition(probs, Vxx, mueq, tmax=8):
     """max over (sampled) knots of cond([[Rhat, D^T],[D, -mu I]]) with Rhat = R + B^T V' B: the factor
     by which two correct fp64 solvers may differ on K, k, Z, z (SURVEY Appendix C).
