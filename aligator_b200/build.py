@@ -49,7 +49,7 @@ def build(verbose=False, force=False, ptxas_v=False):
                                             "vxx_layout.h")]
     hdrs.append(os.path.join(PKG, "..", "include", "aligator_b200", "gar.h"))
     hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
-                                                          "lq_assemble.h", "kkt_error.h", "linesearch.h",
+                                                          "lq_assemble.h", "lq_adjoint.h", "kkt_error.h", "linesearch.h",
                                                           "proxddp_inner.h")]
     extra = ["-Xptxas", "-v"] if ptxas_v else []
     jobs = []
@@ -72,6 +72,9 @@ def build(verbose=False, force=False, ptxas_v=False):
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "lq_assemble.cu")
     obj = os.path.join(OBJ, "assemble_%s.o" % _digest([hdrs[-1], os.path.join(CSRC, "lq_assemble.h"), src], str(extra)))
+    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
+    src = os.path.join(CSRC, "lq_adjoint.cu")
+    obj = os.path.join(OBJ, "adjoint_%s.o" % _digest([os.path.join(CSRC, "lq_adjoint.h"), src], str(extra)))
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "linesearch.cu")
     obj = os.path.join(OBJ, "linesearch_%s.o" % _digest([os.path.join(CSRC, "linesearch.h"), src], str(extra)))

@@ -17,6 +17,7 @@
 #include "../../include/aligator_b200/gar.h"
 #include "kkt_error.h"
 #include "linesearch.h"
+#include "lq_adjoint.h"
 #include "lq_assemble.h"
 #include "proxddp_inner.h"
 #include "riccati_block_launch.h"
@@ -266,6 +267,7 @@ struct ab2_gar_solver {
   double *fddp_slack = nullptr, *fddp_G0 = nullptr, *fddp_g0 = nullptr, *fddp_vx = nullptr;
   double *inner_tmp = nullptr; // [batch][2] per-instance scalars of multipliers / criterion, for host destinations
   double *mu_dev = nullptr;    // [batch] host-given per-instance mu of the *_v sweeps, staged for the kernels
+  double *adj_stage = nullptr, *adj_term = nullptr, *adj_g0 = nullptr; // the adjoint problem of ab2_gar_adjoint
   int nth = 0; // parameter dimension of the value function outputs (= nx in leg mode)
   int rec_nth = 0; // parameter blocks carried by the knot records (0 in leg mode)
   int legs = 0;    // >= 2: gar::ParallelRiccatiSolver (leg mode)
@@ -288,6 +290,7 @@ struct ab2_gar_solver {
   bool pg_in_sweep = true;               // env AB2_PEER_IN_SWEEP=0: always use the separate pack + store kernel
   double *out[AB2_OUT_COUNT] = {};
   size_t out_doubles[AB2_OUT_COUNT] = {};
+  size_t out_alloc[AB2_OUT_COUNT] = {}; // doubles allocated behind out[w] (>= out_doubles[w])
   size_t out_rec[AB2_OUT_COUNT] = {};  // doubles per knot (or per instance)
   int out_knots[AB2_OUT_COUNT] = {};   // knots per instance (1 for per-instance arrays)
   int *status = nullptr, *pivstat = nullptr;
@@ -437,6 +440,7 @@ static int create_impl(const ab2_gar_dims *dims, int nth, int legs, ab2_gar_solv
     if (w == AB2_OUT_VXX && s->k && vxx_packed_total > n)
       n = vxx_packed_total;
     const size_t bytes = (n > 0 ? n + 2 : 2) * sizeof(double);
+    s->out_alloc[w] = bytes / sizeof(double);
     cudaError_t e = cudaMalloc(&s->out[w], bytes);
     if (e == cudaSuccess)
       e = cudaMemset(s->out[w], 0, bytes);
@@ -541,7 +545,7 @@ int ab2_gar_destroy(ab2_gar_solver *s) {
   if (s->pg_done)
     cudaFree(s->pg_done);
   for (double *q : {s->own_stage_sym, s->own_stage, s->own_term, s->own_G0, s->own_g0, s->gains_tmp, s->kkt_tmp, s->theta_dev, s->cond, s->ls_tmp, s->fddp_slack, s->fddp_G0,
-                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev})
+                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev, s->adj_stage, s->adj_term, s->adj_g0})
     if (q)
       cudaFree(q);
   for (int i = 0; i < ab2_gar_solver::kPipeStreams; ++i) {
@@ -815,6 +819,93 @@ int ab2_gar_forward_theta(ab2_gar_solver *s, const double *theta, int memspace, 
   const int rc = launch(s, s->p.mueq, nullptr, 0, 1, stream);
   s->p.theta = nullptr;
   return rc;
+}
+
+// ---- adjoint of the LQ solve (lq_adjoint.cu): records kernel, the sweep on the adjoint problem, gradient kernel ----
+// mueq_arr: the per-instance mu of ab2_gar_adjoint_v (memspace), or null for the scalar mueq.
+static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
+                        const ab2_ls_iterate *primal, const ab2_ls_iterate *cot, const ab2_lq_grad *grad, void *stream) {
+  if (!s || !primal || !cot || !grad)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (s->nth > 0 || s->legs > 1)
+    return fail(AB2_ERR_UNSUPPORTED, "adjoint: parametric (nth > 0) and parallel handles are not supported");
+  if (!s->have_problem)
+    return fail(AB2_ERR_STATE, "set_problem has not been called with all four buffers");
+  const ab2_gar_dims &d = s->d;
+  const int B = d.batch, N = d.horizon, nx = d.nx;
+  const double *pz[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
+  const size_t nz[6] = {(size_t)B * (N + 1) * nx, (size_t)B * N * d.nu, (size_t)B * N * d.nc,
+                        (size_t)B * d.nct, (size_t)B * d.nc0, (size_t)B * N * nx};
+  static const char *names[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
+  for (int i = 0; i < 6; ++i) {
+    if (nz[i] == 0)
+      continue;
+    if (!pz[i])
+      return fail(AB2_ERR_INVALID, std::string("adjoint: primal ") + names[i] + " is NULL");
+    // the adjoint sweep overwrites every trajectory output before the gradient kernel reads the primal
+    for (int w = 0; w < AB2_OUT_COUNT; ++w)
+      if (s->out[w] && pz[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pz[i] + nz[i])
+        return fail(AB2_ERR_INVALID, std::string("adjoint: primal ") + names[i] + " overlaps an output array of the handle");
+  }
+  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  auto own = [&](double *&buf, size_t n) -> int {
+    if (!buf)
+      CUDA_TRY(cudaMalloc(&buf, (n > 0 ? n : 1) * sizeof(double)));
+    return AB2_OK;
+  };
+  int rc;
+  if ((rc = own(s->adj_stage, stage_total(s))) != AB2_OK || (rc = own(s->adj_term, (size_t)B * s->trec)) != AB2_OK ||
+      (rc = own(s->adj_g0, (size_t)B * d.nc0)) != AB2_OK)
+    return rc;
+  const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  // 1. the adjoint problem: same matrices, vectors = -cotangent
+  ab2::AdjointRecordArgs ra{ad, s->p.stage_head, s->p.stage, s->p.term, cot->xs, cot->us, cot->vs, cot->vsT,
+                            cot->lam0, cot->lams, s->adj_stage, s->adj_term, s->adj_g0};
+  CUDA_TRY(ab2::launch_adjoint_records(ra, st));
+  s->launches += 1;
+  // 2. backward + forward on it; the problem pointers change in this launch's copy of the parameters only, and a
+  //    sharded handle never publishes the adjoint gains to its peers
+  if (!mueq_arr)
+    s->p.mueq = mueq;
+  ab2::SweepParams q = s->p;
+  q.stage = s->adj_stage;
+  q.stage_head = 0;
+  q.term = s->adj_term;
+  q.g0 = s->adj_g0;
+  q.mueq_b = mu_dev;
+  q.peer_world = 0;
+  if ((rc = run_kernels(s, q, 1, 1, st)) != AB2_OK)
+    return rc;
+  s->have_backward = true;
+  s->have_forward = true;
+  s->fac_head = 0;
+  s->vxx_packed = warp_kernel(s);
+  // 3. gradient records from the primal z and the adjoint w (the trajectory outputs)
+  ab2::AdjointGradArgs ga{ad,
+                          primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
+                          s->out[AB2_OUT_XS], s->out[AB2_OUT_US], s->out[AB2_OUT_VS], s->out[AB2_OUT_VST],
+                          s->out[AB2_OUT_LBD0], s->out[AB2_OUT_LBDAS],
+                          grad->stage, grad->term, grad->G0, grad->g0};
+  CUDA_TRY(ab2::launch_adjoint_grad(ga, st));
+  s->launches += 1;
+  return AB2_OK;
+}
+int ab2_gar_adjoint(ab2_gar_solver *s, double mueq, const ab2_ls_iterate *primal, const ab2_ls_iterate *cotangent,
+                    const ab2_lq_grad *grad, void *stream) {
+  return adjoint_impl(s, mueq, nullptr, AB2_DEVICE, primal, cotangent, grad, stream);
+}
+int ab2_gar_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace, const ab2_ls_iterate *primal,
+                      const ab2_ls_iterate *cotangent, const ab2_lq_grad *grad, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return adjoint_impl(s, 0.0, mueq, memspace, primal, cotangent, grad, stream);
 }
 
 static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg_b, const double *mu_inv_b,

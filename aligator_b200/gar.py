@@ -53,6 +53,14 @@ class LsIterate(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _LS_KEYS]
 
 
+_GRAD_KEYS = ("stage", "term", "G0", "g0")
+
+
+class LqGrad(C.Structure):
+    """``ab2_lq_grad``: device outputs of ``ab2_gar_adjoint`` (NULL = not wanted)."""
+    _fields_ = [(k, C.c_void_p) for k in _GRAD_KEYS]
+
+
 _MULT_IN = ("xs", "lam0", "lams", "vs", "vsT", "prev_vs", "prev_vsT", "init_value", "xnext", "fs", "cval", "cval_N",
             "lo", "hi", "loN", "hiN")
 _MULT_OUT = ("slack", "lam0_plus", "lams_plus", "vs_plus", "vsT_plus", "shifted", "shifted_N", "Lv", "Lv_N")
@@ -161,6 +169,10 @@ def lib():
         L.ab2_gar_directional_derivative.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_al_value.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_al_value_v.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_void_p]
+        L.ab2_gar_adjoint.argtypes = [C.c_void_p, C.c_double, C.POINTER(LsIterate), C.POINTER(LsIterate),
+                                      C.POINTER(LqGrad), C.c_void_p]
+        L.ab2_gar_adjoint_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LsIterate), C.POINTER(LsIterate),
+                                        C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -590,6 +602,26 @@ class CudaRiccatiBatch:
                                             AB2_HOST, C.c_void_p(stream)))
         self.synchronize(stream)
         return out
+
+    # ---- gradients of the solution with respect to the problem data ----
+    def adjoint(self, primal, cotangent, grad, mueq, stream=0):
+        """Adjoint of the LQ solve (``ab2_gar_adjoint``): gradient records of a loss whose cotangents with respect to
+        the solution are ``cotangent``.  ``primal``, ``cotangent``: dicts with keys xs, us, vs, vsT, lam0, lams of
+        device tensors laid out like the solver's outputs (``primal``: the solution of the current problem at this
+        mu; a cotangent key that is missing or None is zero).  ``grad``: dict with any of stage, term, G0, g0 of
+        device tensors in the problem's layouts, overwritten.  ``mueq``: a number or a [batch] array / tensor
+        (``ab2_gar_adjoint_v``).  Afterwards the handle's outputs are those of the adjoint solve."""
+        v = self._mueq_arg(mueq, stream)
+        pr = _fill(LsIterate(), _LS_KEYS, primal)
+        ct = _fill(LsIterate(), _LS_KEYS, cotangent)
+        gr = _fill(LqGrad(), _GRAD_KEYS, grad)
+        self._keep_adj = (primal, cotangent, grad)
+        if v is None:
+            _check(lib().ab2_gar_adjoint(self.h, C.c_double(mueq), C.byref(pr), C.byref(ct), C.byref(gr),
+                                         C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_adjoint_v(self.h, v[0], v[1], C.byref(pr), C.byref(ct), C.byref(gr),
+                                           C.c_void_p(stream)))
 
     # ---- multipliers, Lagrangian gradient, criterion (the rest of the inner iteration) ----
     def _scalars(self, call, out, stream):

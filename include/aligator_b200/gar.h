@@ -367,6 +367,43 @@ int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double
 int ab2_gar_al_value_v(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, const double *mudyn,
                        const double *mucstr, double *dst, int memspace, void *stream);
 
+/* Gradients of the LQ solution with respect to the problem data (no reference counterpart: what learning a cost or a
+ * model through an MPC layer needs).  The solve is the solution z of one symmetric KKT system K z = -h; for a loss
+ * with cotangent zbar = dL/dz, w = K^-1 zbar is the solution of the SAME LQ problem with the vectors replaced by
+ * q_t = -xbar_t, r_t = -ubar_t, d_t = -vbar_t, f_t = -lambdabar_{t+1}, q_N = -xbar_N, d_N = -vbar_N, g0 = -lambdabar_0,
+ * and the gradients are dh = -w, dK = -w z^T read out of K's blocks.  With w = (xt, ut, vt, lt) and z = (x, u, v, l):
+ *   dq = -xt_t, dr = -ut_t, dd = -vt_t, df = -lt_{t+1}, dg0 = -lt_0,
+ *   dA = -(lt_{t+1} x_t^T + l_{t+1} xt_t^T), dB = -(lt_{t+1} u_t^T + l_{t+1} ut_t^T), dS = -(xt u^T + x ut^T),
+ *   dC = -(vt x^T + v xt^T), dD = -(vt u^T + v ut^T), dG0 = -(lt_0 x_0^T + l_0 xt_0^T),
+ *   dQ = -1/2 (xt x^T + x xt^T), dR = -1/2 (ut u^T + u ut^T), and the terminal record's dQ_N, dq_N, dC_N, dd_N alike.
+ * Q and R are symmetric and the kernels may read either triangle, so their gradient is the one with respect to a
+ * symmetric argument (Q_ij and Q_ji perturbed together): the right chain rule for any symmetric parametrisation,
+ * such as (P + P^T) / 2 or L L^T.  mu is not differentiated.
+ *
+ * All arrays are DEVICE arrays.  `primal` is a solution of the handle's CURRENT problem at the same mu (in practice
+ * what the last sweep returned, copied out by the caller); every field of nonzero size is required and none may
+ * overlap an output array of the handle (AB2_ERR_INVALID).  A NULL `cotangent` field is a zero cotangent.  `grad`
+ * arrays have the problem's layouts -- stage [batch][N][stage_record] (pad double = 0), term [batch][term_record],
+ * G0 [batch][nc0*nx], g0 [batch][nc0] -- and are overwritten; a NULL field is not written.
+ * In order on `stream`, without host synchronisation, three launches: a streaming kernel writes the adjoint problem
+ * into a buffer the handle owns (allocated on the first call), the sweep kernel solves it (backward + forward), a
+ * streaming kernel writes the gradients.  Afterwards the handle's problem is unchanged, but its OUTPUTS (FF .. LBDAS,
+ * status, pivot statistics) are those of the adjoint solve: the matrix recursion is the primal one, so FB, VXX and
+ * the pivot statistics equal the primal sweep's, while the vectors and the trajectory are w.  A later backward or
+ * sweep restores the primal outputs.  Plain serial handles (warp, CTA and dense kernels); parametric (nth > 0) and
+ * parallel handles return AB2_ERR_UNSUPPORTED; a call before set_problem returns AB2_ERR_STATE.  Nothing is launched
+ * on an error. */
+typedef struct ab2_lq_grad {
+  double *stage, *term, *G0, *g0;
+} ab2_lq_grad;
+int ab2_gar_adjoint  (ab2_gar_solver *s, double mueq,
+                      const ab2_ls_iterate *primal, const ab2_ls_iterate *cotangent,
+                      const ab2_lq_grad *grad, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace,
+                      const ab2_ls_iterate *primal, const ab2_ls_iterate *cotangent,
+                      const ab2_lq_grad *grad, void *stream);
+
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
  * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
