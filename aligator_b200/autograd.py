@@ -1,5 +1,6 @@
 """``torch.autograd`` entry point of the batched LQ solve: gradients of the solution with respect to the problem
-data, by one adjoint sweep on the device (``ab2_gar_adjoint``, include/aligator_b200/gar.h).
+data, by one adjoint sweep on the device (``ab2_gar_adjoint``, include/aligator_b200/gar.h), and forward-mode
+derivatives along a data tangent, by one tangent sweep (``ab2_gar_tangent``).
 
     xs, us, vs, vsT, lam0, lams = lq_solve(batch, stage, term, G0, g0, mueq)
 
@@ -9,11 +10,15 @@ in the layouts of gar.h.  :func:`stage_records` and :func:`term_records` build t
 
 Q and R are symmetric, and their gradient is the one with respect to a symmetric argument (Q_ij and Q_ji perturbed
 together).  That is the right chain rule when Q and R are built symmetric, e.g. as ``(P + P^T) / 2`` or ``L L^T``.
-The penalty ``mueq`` (a number or a [batch] tensor) is not differentiated.
+Forward mode (``torch.func.jvp``, ``torch.autograd.forward_ad``) is its exact transpose: the tangent of Q and R enters
+through ``sym(Qdot) = (Qdot + Qdot^T) / 2``, so an asymmetric tangent acts as its symmetric part.  ``jacfwd`` and
+``vmap`` are not supported: the function has no vmap rule.  The penalty ``mueq`` (a number or a [batch] tensor) is not
+differentiated.
 """
 from __future__ import annotations
 
 import torch
+from torch._C import _functorch
 
 from . import gar as _gar
 
@@ -41,22 +46,39 @@ def _check_inputs(batch, arrays):
                                 "" if t.is_contiguous() else ", non-contiguous"))
 
 
+def _outputs(batch, device, stream):
+    """The handle's trajectory outputs copied into new tensors."""
+    outs = []
+    for w in _OUTS:
+        t = torch.empty(batch.out_shape(w), dtype=torch.float64, device=device)
+        if t.numel():
+            batch.get_into(w, _plain(t), _gar.AB2_DEVICE, stream=stream)
+        outs.append(t)
+    return tuple(outs)
+
+
+def _plain(t):
+    """The tensor beneath torch.func's transform wrappers (itself when it is not wrapped)."""
+    while _functorch.is_functorch_wrapped_tensor(t):
+        t = _functorch.get_unwrapped(t)
+    return t
+
+
 class _LqSolve(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, batch, stage, term, G0, g0, mueq):
+    def forward(batch, stage, term, G0, g0, mueq):
         stream = torch.cuda.current_stream(stage.device).cuda_stream
         batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
         batch.sweep(mueq, stream=stream)
-        outs = []
-        for w in _OUTS:
-            t = torch.empty(batch.out_shape(w), dtype=torch.float64, device=stage.device)
-            if t.numel():
-                batch.get_into(w, t, _gar.AB2_DEVICE, stream=stream)
-            outs.append(t)
+        return _outputs(batch, stage.device, stream)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        batch, stage, term, G0, g0, mueq = inputs
         ctx.batch, ctx.mueq = batch, mueq
-        ctx.save_for_backward(stage, term, G0, g0, *outs)
+        ctx.save_for_backward(stage, term, G0, g0, *output)
+        ctx.save_for_forward(stage, term, G0, g0, *output)
         ctx.set_materialize_grads(False)
-        return tuple(outs)
 
     @staticmethod
     def backward(ctx, *gouts):
@@ -72,6 +94,20 @@ class _LqSolve(torch.autograd.Function):
         else:
             grads = {}
         return (None,) + tuple(grads.get(k) for k in _INPUTS) + (None,)
+
+    @staticmethod
+    def jvp(ctx, _batch_t, *tangents):
+        # under torch.func.jvp the saved tensors and tangents arrive wrapped; the library needs the storage beneath
+        stage, term, G0, g0, *outs = [_plain(t) for t in ctx.saved_tensors]
+        batch = ctx.batch
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        dot = {k: None if t is None else _plain(t.to(torch.float64).contiguous())
+               for k, t in zip(_INPUTS, tangents[:4])}
+        if all(t is None for t in dot.values()):
+            return tuple(torch.zeros_like(o) for o in outs)
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        batch.tangent(dict(zip(_KEYS, outs)), dot, ctx.mueq, stream=stream)
+        return _outputs(batch, stage.device, stream)
 
 
 def lq_solve(batch, stage, term, G0, g0, mueq):

@@ -49,8 +49,8 @@ def build(verbose=False, force=False, ptxas_v=False):
                                             "vxx_layout.h")]
     hdrs.append(os.path.join(PKG, "..", "include", "aligator_b200", "gar.h"))
     hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
-                                                          "lq_assemble.h", "lq_adjoint.h", "kkt_error.h", "linesearch.h",
-                                                          "proxddp_inner.h")]
+                                                          "lq_assemble.h", "lq_adjoint.h", "lq_tangent.h", "kkt_error.h",
+                                                          "linesearch.h", "proxddp_inner.h")]
     extra = ["-Xptxas", "-v"] if ptxas_v else []
     jobs = []
     for (nx, nu, nc, g) in configs():
@@ -75,6 +75,10 @@ def build(verbose=False, force=False, ptxas_v=False):
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "lq_adjoint.cu")
     obj = os.path.join(OBJ, "adjoint_%s.o" % _digest([os.path.join(CSRC, "lq_adjoint.h"), src], str(extra)))
+    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
+    src = os.path.join(CSRC, "lq_tangent.cu")
+    obj = os.path.join(OBJ, "tangent_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_tangent.h")]
+                                                     + [src], str(extra)))
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "linesearch.cu")
     obj = os.path.join(OBJ, "linesearch_%s.o" % _digest([os.path.join(CSRC, "linesearch.h"), src], str(extra)))

@@ -18,6 +18,7 @@
 #include "kkt_error.h"
 #include "linesearch.h"
 #include "lq_adjoint.h"
+#include "lq_tangent.h"
 #include "lq_assemble.h"
 #include "proxddp_inner.h"
 #include "riccati_block_launch.h"
@@ -268,6 +269,7 @@ struct ab2_gar_solver {
   double *inner_tmp = nullptr; // [batch][2] per-instance scalars of multipliers / criterion, for host destinations
   double *mu_dev = nullptr;    // [batch] host-given per-instance mu of the *_v sweeps, staged for the kernels
   double *adj_stage = nullptr, *adj_term = nullptr, *adj_g0 = nullptr; // the adjoint problem of ab2_gar_adjoint
+  double *tan_rho = nullptr; // -rho of ab2_gar_tangent, in the cotangent layout (xs, us, vs, vsT, lam0, lams)
   int nth = 0; // parameter dimension of the value function outputs (= nx in leg mode)
   int rec_nth = 0; // parameter blocks carried by the knot records (0 in leg mode)
   int legs = 0;    // >= 2: gar::ParallelRiccatiSolver (leg mode)
@@ -545,7 +547,7 @@ int ab2_gar_destroy(ab2_gar_solver *s) {
   if (s->pg_done)
     cudaFree(s->pg_done);
   for (double *q : {s->own_stage_sym, s->own_stage, s->own_term, s->own_G0, s->own_g0, s->gains_tmp, s->kkt_tmp, s->theta_dev, s->cond, s->ls_tmp, s->fddp_slack, s->fddp_G0,
-                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev, s->adj_stage, s->adj_term, s->adj_g0})
+                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev, s->adj_stage, s->adj_term, s->adj_g0, s->tan_rho})
     if (q)
       cudaFree(q);
   for (int i = 0; i < ab2_gar_solver::kPipeStreams; ++i) {
@@ -822,13 +824,13 @@ int ab2_gar_forward_theta(ab2_gar_solver *s, const double *theta, int memspace, 
 }
 
 // ---- adjoint of the LQ solve (lq_adjoint.cu): records kernel, the sweep on the adjoint problem, gradient kernel ----
-// mueq_arr: the per-instance mu of ab2_gar_adjoint_v (memspace), or null for the scalar mueq.
-static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
-                        const ab2_ls_iterate *primal, const ab2_ls_iterate *cot, const ab2_lq_grad *grad, void *stream) {
-  if (!s || !primal || !cot || !grad)
-    return fail(AB2_ERR_INVALID, "null argument");
+// The checks shared by ab2_gar_adjoint and ab2_gar_tangent, in this order: handle kind, problem set, primal fields,
+// mu.  `refuse_overlap`: a primal field that overlaps an output of the handle is refused (the adjoint reads the
+// primal after its sweep has overwritten the outputs).
+static int check_vector_solve(ab2_gar_solver *s, double mueq, const double *mueq_arr, const ab2_ls_iterate *primal,
+                              const char *who, bool refuse_overlap) {
   if (s->nth > 0 || s->legs > 1)
-    return fail(AB2_ERR_UNSUPPORTED, "adjoint: parametric (nth > 0) and parallel handles are not supported");
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": parametric (nth > 0) and parallel handles are not supported");
   if (!s->have_problem)
     return fail(AB2_ERR_STATE, "set_problem has not been called with all four buffers");
   const ab2_gar_dims &d = s->d;
@@ -841,20 +843,23 @@ static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
     if (nz[i] == 0)
       continue;
     if (!pz[i])
-      return fail(AB2_ERR_INVALID, std::string("adjoint: primal ") + names[i] + " is NULL");
-    // the adjoint sweep overwrites every trajectory output before the gradient kernel reads the primal
-    for (int w = 0; w < AB2_OUT_COUNT; ++w)
-      if (s->out[w] && pz[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pz[i] + nz[i])
-        return fail(AB2_ERR_INVALID, std::string("adjoint: primal ") + names[i] + " overlaps an output array of the handle");
+      return fail(AB2_ERR_INVALID, std::string(who) + ": primal " + names[i] + " is NULL");
+    if (refuse_overlap)
+      for (int w = 0; w < AB2_OUT_COUNT; ++w)
+        if (s->out[w] && pz[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pz[i] + nz[i])
+          return fail(AB2_ERR_INVALID, std::string(who) + ": primal " + names[i] + " overlaps an output array of the handle");
   }
   if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
     return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  return AB2_OK;
+}
+
+// The current problem's matrices with the vectors q, r, d, f, q_N, d_N, g0 = -cot, solved by the handle's own sweep
+// (two launches).  mu_dev: the staged per-instance mu, or null for the scalar mueq.
+static int solve_cotangent_problem(ab2_gar_solver *s, double mueq, const double *mu_dev, const ab2_ls_iterate *cot,
+                                   cudaStream_t st) {
+  const ab2_gar_dims &d = s->d;
+  const int B = d.batch, N = d.horizon, nx = d.nx;
   auto own = [&](double *&buf, size_t n) -> int {
     if (!buf)
       CUDA_TRY(cudaMalloc(&buf, (n > 0 ? n : 1) * sizeof(double)));
@@ -865,14 +870,14 @@ static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
       (rc = own(s->adj_g0, (size_t)B * d.nc0)) != AB2_OK)
     return rc;
   const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
-  // 1. the adjoint problem: same matrices, vectors = -cotangent
+  // 1. the problem: same matrices, vectors = -cot
   ab2::AdjointRecordArgs ra{ad, s->p.stage_head, s->p.stage, s->p.term, cot->xs, cot->us, cot->vs, cot->vsT,
                             cot->lam0, cot->lams, s->adj_stage, s->adj_term, s->adj_g0};
   CUDA_TRY(ab2::launch_adjoint_records(ra, st));
   s->launches += 1;
   // 2. backward + forward on it; the problem pointers change in this launch's copy of the parameters only, and a
-  //    sharded handle never publishes the adjoint gains to its peers
-  if (!mueq_arr)
+  //    sharded handle never publishes these gains to its peers
+  if (!mu_dev)
     s->p.mueq = mueq;
   ab2::SweepParams q = s->p;
   q.stage = s->adj_stage;
@@ -887,6 +892,29 @@ static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
   s->have_forward = true;
   s->fac_head = 0;
   s->vxx_packed = warp_kernel(s);
+  return AB2_OK;
+}
+
+// mueq_arr: the per-instance mu of ab2_gar_adjoint_v (memspace), or null for the scalar mueq.
+static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
+                        const ab2_ls_iterate *primal, const ab2_ls_iterate *cot, const ab2_lq_grad *grad, void *stream) {
+  if (!s || !primal || !cot || !grad)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_vector_solve(s, mueq, mueq_arr, primal, "adjoint", true))
+    return rc;
+  const ab2_gar_dims &d = s->d;
+  const int B = d.batch, N = d.horizon, nx = d.nx;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  // 1. + 2. the adjoint problem (vectors = -cotangent) and its solve
+  int rc;
+  if ((rc = solve_cotangent_problem(s, mueq, mu_dev, cot, st)) != AB2_OK)
+    return rc;
+  const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
   // 3. gradient records from the primal z and the adjoint w (the trajectory outputs)
   ab2::AdjointGradArgs ga{ad,
                           primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
@@ -906,6 +934,49 @@ int ab2_gar_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace, const
   if (!mueq)
     return fail(AB2_ERR_INVALID, "null mueq array");
   return adjoint_impl(s, 0.0, mueq, memspace, primal, cotangent, grad, stream);
+}
+
+// ---- tangent of the LQ solve (lq_tangent.cu): right-hand-side kernel, then the adjoint's records kernel and sweep ----
+static int tangent_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
+                        const ab2_ls_iterate *primal, const ab2_lq_tangent *dot, void *stream) {
+  if (!s || !primal || !dot)
+    return fail(AB2_ERR_INVALID, "null argument");
+  // the primal is read completely by the first launch, before the sweep writes any output: it may alias them
+  if (int rc = check_vector_solve(s, mueq, mueq_arr, primal, "tangent", false))
+    return rc;
+  const ab2_gar_dims &d = s->d;
+  const int B = d.batch, N = d.horizon, nx = d.nx;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  const size_t nxs = (size_t)B * (N + 1) * nx, nus = (size_t)B * N * d.nu, nvs = (size_t)B * N * d.nc,
+               nvT = (size_t)B * d.nct, nl0 = (size_t)B * d.nc0, nls = (size_t)B * N * nx;
+  if (!s->tan_rho)
+    CUDA_TRY(cudaMalloc(&s->tan_rho, (nxs + nus + nvs + nvT + nl0 + nls + 1) * sizeof(double)));
+  double *rxs = s->tan_rho, *rus = rxs + nxs, *rvs = rus + nus, *rvT = rvs + nvs, *rl0 = rvT + nvT, *rls = rl0 + nl0;
+  // 1. -rho = -(Kdot z + hdot), in the cotangent layout
+  const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  ab2::TangentRhsArgs ta{ad, dot->stage, dot->term, dot->G0, dot->g0,
+                         primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
+                         rxs, rus, rvs, rvT, rl0, rls};
+  CUDA_TRY(ab2::launch_tangent_rhs(ta, st));
+  s->launches += 1;
+  // 2. + 3. the tangent problem (vectors = rho) and its solve: the trajectory outputs become zdot
+  const ab2_ls_iterate rho{rxs, rus, rvs, rvT, rl0, rls};
+  return solve_cotangent_problem(s, mueq, mu_dev, &rho, st);
+}
+int ab2_gar_tangent(ab2_gar_solver *s, double mueq, const ab2_ls_iterate *primal, const ab2_lq_tangent *dot,
+                    void *stream) {
+  return tangent_impl(s, mueq, nullptr, AB2_DEVICE, primal, dot, stream);
+}
+int ab2_gar_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace, const ab2_ls_iterate *primal,
+                      const ab2_lq_tangent *dot, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return tangent_impl(s, 0.0, mueq, memspace, primal, dot, stream);
 }
 
 static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg_b, const double *mu_inv_b,

@@ -61,6 +61,11 @@ class LqGrad(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _GRAD_KEYS]
 
 
+class LqTangent(C.Structure):
+    """``ab2_lq_tangent``: device tangent records of ``ab2_gar_tangent`` (NULL = zero), keyed like ``LqGrad``."""
+    _fields_ = [(k, C.c_void_p) for k in _GRAD_KEYS]
+
+
 _MULT_IN = ("xs", "lam0", "lams", "vs", "vsT", "prev_vs", "prev_vsT", "init_value", "xnext", "fs", "cval", "cval_N",
             "lo", "hi", "loN", "hiN")
 _MULT_OUT = ("slack", "lam0_plus", "lams_plus", "vs_plus", "vsT_plus", "shifted", "shifted_N", "Lv", "Lv_N")
@@ -173,6 +178,9 @@ def lib():
                                       C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_adjoint_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LsIterate), C.POINTER(LsIterate),
                                         C.POINTER(LqGrad), C.c_void_p]
+        L.ab2_gar_tangent.argtypes = [C.c_void_p, C.c_double, C.POINTER(LsIterate), C.POINTER(LqTangent), C.c_void_p]
+        L.ab2_gar_tangent_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LsIterate), C.POINTER(LqTangent),
+                                        C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -622,6 +630,23 @@ class CudaRiccatiBatch:
         else:
             _check(lib().ab2_gar_adjoint_v(self.h, v[0], v[1], C.byref(pr), C.byref(ct), C.byref(gr),
                                            C.c_void_p(stream)))
+
+    def tangent(self, primal, tangent, mueq, stream=0):
+        """Forward mode of the LQ solve (``ab2_gar_tangent``): afterwards the handle's trajectory outputs (OUT_XS ..
+        OUT_LBDAS) hold the derivative of the solution along the data tangent ``tangent``, a dict with any of stage,
+        term, G0, g0 of device tensors in the problem's layouts (a key that is missing or None is zero).  ``primal``:
+        dict with keys xs, us, vs, vsT, lam0, lams of device tensors or addresses laid out like the solver's outputs,
+        the solution of the current problem at this mu; it may be the handle's own outputs (``device_ptr``).  The
+        tangent of Q and R is taken through sym(.) = (. + .^T) / 2, as ``adjoint``'s gradient is.  ``mueq``: a number
+        or a [batch] array / tensor (``ab2_gar_tangent_v``)."""
+        v = self._mueq_arg(mueq, stream)
+        pr = _fill(LsIterate(), _LS_KEYS, primal)
+        dt = _fill(LqTangent(), _GRAD_KEYS, tangent)
+        self._keep_tan = (primal, tangent)
+        if v is None:
+            _check(lib().ab2_gar_tangent(self.h, C.c_double(mueq), C.byref(pr), C.byref(dt), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_tangent_v(self.h, v[0], v[1], C.byref(pr), C.byref(dt), C.c_void_p(stream)))
 
     # ---- multipliers, Lagrangian gradient, criterion (the rest of the inner iteration) ----
     def _scalars(self, call, out, stream):

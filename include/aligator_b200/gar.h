@@ -404,6 +404,37 @@ int ab2_gar_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace,
                       const ab2_ls_iterate *primal, const ab2_ls_iterate *cotangent,
                       const ab2_lq_grad *grad, void *stream);
 
+/* Forward mode: the derivative zdot of the LQ solution along a tangent pdot of the problem data (a perturbed model
+ * A, B, a shifted reference in q, the initial state through g0, ...), for the whole batch in one call.  K is affine
+ * in the data, so zdot = -K^-1 (Kdot z + hdot): the SAME LQ problem with the vectors replaced by rho = Kdot z + hdot.
+ * With z = (x, u, v, l), l_{t+1} = lams[t], sym(M) = (M + M^T) / 2 and dotted blocks the tangent records, per stage knot
+ *   q_t <- qdot + sym(Qdot) x_t + Sdot u_t + Cdot^T v_t + Adot^T l_{t+1}   (+ G0dot^T l_0 at t = 0)
+ *   r_t <- rdot + Sdot^T x_t + sym(Rdot) u_t + Ddot^T v_t + Bdot^T l_{t+1}
+ *   d_t <- ddot + Cdot x_t + Ddot u_t,       f_t <- fdot + Adot x_t + Bdot u_t
+ * and q_N <- qdot_N + sym(Qdot_N) x_N + C_Ndot^T v_N, d_N <- ddot_N + C_Ndot x_N, g0 <- g0dot + G0dot x_0.
+ * sym(Qdot) and sym(Rdot) make this the exact transpose of ab2_gar_adjoint's symmetric-argument gradient:
+ * <zbar, zdot> = <grad, pdot> for any pdot, including an asymmetric Qdot or Rdot.  mu is not differentiated.
+ *
+ * `dot` holds DEVICE arrays in the problem's layouts (stage [batch][N][stage_record], pad double ignored;
+ * term [batch][term_record]; G0 [batch][nc0*nx]; g0 [batch][nc0]); a NULL field is a zero tangent.  `primal` is a
+ * solution of the handle's CURRENT problem at the same mu; every field of nonzero size is required.  It is read
+ * completely before the sweep writes anything, so it MAY be the handle's own outputs (ab2_gar_device_ptr).
+ * In order on `stream`, without host synchronisation, three launches: a streaming kernel writes -rho into a buffer
+ * the handle owns (allocated on the first call), ab2_gar_adjoint's records kernel builds the tangent problem from it,
+ * the sweep kernel solves it.  Afterwards the handle's problem is unchanged and its trajectory outputs (XS .. LBDAS)
+ * are zdot; as after ab2_gar_adjoint, FB, VXX and the pivot statistics equal the primal sweep's, and a later backward
+ * or sweep restores the primal outputs.  Plain serial handles (warp, CTA and dense kernels); parametric (nth > 0) and
+ * parallel handles return AB2_ERR_UNSUPPORTED; a call before set_problem returns AB2_ERR_STATE; a NULL primal field
+ * of nonzero size, or mueq <= 0 with constraints, returns AB2_ERR_INVALID.  Nothing is launched on an error. */
+typedef struct ab2_lq_tangent {
+  const double *stage, *term, *G0, *g0;
+} ab2_lq_tangent;
+int ab2_gar_tangent  (ab2_gar_solver *s, double mueq, const ab2_ls_iterate *primal,
+                      const ab2_lq_tangent *dot, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace, const ab2_ls_iterate *primal,
+                      const ab2_lq_tangent *dot, void *stream);
+
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
  * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
