@@ -14,6 +14,11 @@ Forward mode (``torch.func.jvp``, ``torch.autograd.forward_ad``) is its exact tr
 through ``sym(Qdot) = (Qdot + Qdot^T) / 2``, so an asymmetric tangent acts as its symmetric part.  ``jacfwd`` and
 ``vmap`` are not supported: the function has no vmap rule.  The penalty ``mueq`` (a number or a [batch] tensor) is not
 differentiated.
+
+:func:`lq_resolve` re-solves the matrices of the handle's last backward for new vectors (``ab2_gar_resolve``), many
+right-hand sides in one call.  It is linear in the vectors and its own transpose, so its ``backward`` and ``jvp`` are
+``lq_resolve`` calls again, and it has a vmap rule: ``torch.func.vmap``, ``jacrev``, ``jacfwd`` and higher orders work
+with respect to the vectors.
 """
 from __future__ import annotations
 
@@ -141,3 +146,88 @@ def term_records(Q, q, C, d):
     """Terminal records [..., term_record] = [Q | q | C | d] from Q [..., nx, nx], q [..., nx], C [..., nct, nx],
     d [..., nct].  Differentiable."""
     return torch.cat([_colmajor(Q), q, _colmajor(C), d], dim=-1)
+
+
+_RHS = ("q", "r", "d", "dN", "g0", "f")
+
+
+def _rhs_shapes(batch):
+    """Per-right-hand-side shape of each vector field, in the layouts of the solution (q like xs, ..., f like lams)."""
+    d = batch.dims
+    B, N = d.batch, d.horizon
+    return dict(q=(B, N + 1, d.nx), r=(B, N, d.nu), d=(B, N, d.nc), dN=(B, d.nct), g0=(B, d.nc0), f=(B, N, d.nx))
+
+
+class _LqResolve(torch.autograd.Function):
+    """z = resolve(h) on [nrhs][batch][...] tensors.  Linear and self-transpose: VJP and JVP are resolve again."""
+
+    @staticmethod
+    def forward(batch, mueq, epoch, *h):
+        if batch.factor_epoch() != epoch:
+            raise RuntimeError("lq_resolve: the handle has been refactored since these derivatives were recorded")
+        h = [None if t is None else _plain(t).to(torch.float64).contiguous() for t in h]
+        given = [t for t in h if t is not None]
+        device = given[0].device if given else torch.device("cuda", batch.dims.device)
+        nrhs = given[0].shape[0] if given else 1
+        outs = [torch.empty((nrhs,) + s, dtype=torch.float64, device=device) for s in _rhs_shapes(batch).values()]
+        if nrhs:
+            stream = torch.cuda.current_stream(device).cuda_stream
+            batch.resolve(dict(zip(_RHS, h)), dict(zip(_KEYS, outs)), mueq, stream=stream)
+        return tuple(outs)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.batch, ctx.mueq, ctx.epoch = inputs[:3]
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *gz):
+        if all(g is None for g in gz):
+            return (None,) * 9
+        gh = _LqResolve.apply(ctx.batch, ctx.mueq, ctx.epoch, *gz)
+        return (None, None, None) + tuple(g if need else None for g, need in zip(gh, ctx.needs_input_grad[3:]))
+
+    @staticmethod
+    def jvp(ctx, _b, _m, _e, *hdot):
+        return _LqResolve.apply(ctx.batch, ctx.mueq, ctx.epoch, *hdot)
+
+    @staticmethod
+    def vmap(info, in_dims, batch, mueq, epoch, *h):
+        V = info.batch_size
+        flat = []
+        for t, bd in zip(h, in_dims[3:]):
+            if t is not None:
+                t = t.movedim(bd, 0) if bd is not None else t.unsqueeze(0).expand(V, *t.shape)
+                t = t.reshape(V * t.shape[1], *t.shape[2:])
+            flat.append(t)
+        outs = _LqResolve.apply(batch, mueq, epoch, *flat)
+        return tuple(o.reshape(V, o.shape[0] // V, *o.shape[1:]) for o in outs), (0,) * len(outs)
+
+
+def lq_resolve(batch, mueq, q=None, r=None, d=None, dN=None, g0=None, f=None):
+    """Solve the LQ problem of ``batch``'s last backward with its vectors replaced by (q, r, d, dN, g0, f); returns
+    ``(xs, us, vs, vsT, lam0, lams)``.  Each vector has the shape of the solution field it pairs with (q like xs
+    [batch][N+1][nx], r like us, d like vs, dN like vsT, g0 like lam0 [batch][nc0], f like lams with f_t in the row of
+    lambda_{t+1}) behind any leading dimensions; the leading dimensions are broadcast, flattened into the right-hand
+    sides of one device call, and lead every output.  None is zero.  ``mueq`` must be the mu of that backward.
+    Differentiable with respect to the vectors in both modes and under ``torch.func`` transforms; calling ``backward``
+    or ``jvp`` after the handle has been refactored (``factor_epoch`` changed) raises RuntimeError."""
+    if not isinstance(batch, _gar.CudaRiccatiBatch):
+        raise ValueError("lq_resolve: `batch` must be a CudaRiccatiBatch")
+    shapes = _rhs_shapes(batch)
+    h = dict(q=q, r=r, d=d, dN=dN, g0=g0, f=f)
+    lead = []
+    for k, t in h.items():
+        if t is None:
+            continue
+        s = shapes[k]
+        if not isinstance(t, torch.Tensor) or t.dim() < len(s) or tuple(t.shape[t.dim() - len(s):]) != s:
+            raise ValueError("lq_resolve: %s must be a tensor of shape [..., %s]" % (k, ", ".join(map(str, s))))
+        lead.append(tuple(t.shape[:t.dim() - len(s)]))
+    lead = tuple(torch.broadcast_shapes(*lead)) if lead else ()
+    nrhs = 1
+    for n in lead:
+        nrhs *= n
+    flat = [None if t is None else t.expand(*lead, *shapes[k]).reshape(nrhs, *shapes[k]) for k, t in h.items()]
+    outs = _LqResolve.apply(batch, mueq, batch.factor_epoch(), *flat)
+    return tuple(o.reshape(*lead, *o.shape[1:]) for o in outs)

@@ -49,7 +49,8 @@ def build(verbose=False, force=False, ptxas_v=False):
                                             "vxx_layout.h")]
     hdrs.append(os.path.join(PKG, "..", "include", "aligator_b200", "gar.h"))
     hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
-                                                          "lq_assemble.h", "lq_adjoint.h", "lq_tangent.h", "kkt_error.h",
+                                                          "lq_assemble.h", "lq_adjoint.h", "lq_tangent.h", "lq_resolve.h",
+                                                          "lq_resolve.cuh", "kkt_error.h",
                                                           "linesearch.h", "proxddp_inner.h")]
     extra = ["-Xptxas", "-v"] if ptxas_v else []
     jobs = []
@@ -78,6 +79,11 @@ def build(verbose=False, force=False, ptxas_v=False):
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "lq_tangent.cu")
     obj = os.path.join(OBJ, "tangent_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_tangent.h")]
+                                                     + [src], str(extra)))
+    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
+    src = os.path.join(CSRC, "lq_resolve.cu")
+    obj = os.path.join(OBJ, "resolve_%s.o" % _digest([os.path.join(CSRC, f) for f in ("vxx_layout.h", "lq_resolve.h",
+                                                                                      "lq_resolve.cuh")]
                                                      + [src], str(extra)))
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "linesearch.cu")

@@ -19,6 +19,7 @@
 #include "linesearch.h"
 #include "lq_adjoint.h"
 #include "lq_tangent.h"
+#include "lq_resolve.h"
 #include "lq_assemble.h"
 #include "proxddp_inner.h"
 #include "riccati_block_launch.h"
@@ -297,6 +298,10 @@ struct ab2_gar_solver {
   int out_knots[AB2_OUT_COUNT] = {};   // knots per instance (1 for per-instance arrays)
   int *status = nullptr, *pivstat = nullptr;
   bool have_problem = false, have_backward = false, have_forward = false;
+  // ab2_gar_resolve: FB / VXX belong to the current problem (a backward ran after the last set_problem, assemble or
+  // cycle_append), and the count of calls that rewrote the factorisation or the records (ab2_gar_factor_epoch)
+  bool factor_current = false;
+  long long epoch = 0;
   long launches = 0;
   int variant = -1;
   // Layout of out[AB2_OUT_VXX] as the last backward left it: true = packed (warp-per-instance kernel,
@@ -624,6 +629,8 @@ int ab2_gar_set_problem(ab2_gar_solver *s, const double *stage, const double *te
   s->have_problem = s->p.stage && s->p.term && (s->p.G0 || s->d.nc0 == 0) && (s->p.g0 || s->d.nc0 == 0);
   if (s->d.horizon == 0 && s->p.term)
     s->have_problem = true;
+  s->factor_current = false;
+  s->epoch += 1;
   return AB2_OK;
 }
 
@@ -752,6 +759,8 @@ static int launch(ab2_gar_solver *s, double mueq, const double *mueq_b, int bwd,
     s->have_backward = true;
     s->fac_head = 0; // every factor slot was rewritten in knot order
     s->vxx_packed = warp_kernel(s);
+    s->factor_current = true;
+    s->epoch += 1;
   }
   s->have_forward = fwd != 0; // a backward-only launch invalidates the previous trajectory
   return AB2_OK;
@@ -892,6 +901,8 @@ static int solve_cotangent_problem(ab2_gar_solver *s, double mueq, const double 
   s->have_forward = true;
   s->fac_head = 0;
   s->vxx_packed = warp_kernel(s);
+  s->factor_current = true;
+  s->epoch += 1;
   return AB2_OK;
 }
 
@@ -979,6 +990,101 @@ int ab2_gar_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace, const
   return tangent_impl(s, 0.0, mueq, memspace, primal, dot, stream);
 }
 
+// ---- re-solve for new vectors (lq_resolve.cu): the vector half of the recursion on the last backward's factorisation ----
+static int resolve_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int nrhs,
+                        const ab2_lq_rhs *rhs, const ab2_ls_trial *out, void *stream) {
+  if (!s || !rhs || !out)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (s->nth > 0 || s->legs > 1 || s->dense)
+    return fail(AB2_ERR_UNSUPPORTED, "resolve: dense, parametric (nth > 0) and parallel handles are not supported");
+  if (!s->have_problem || !s->factor_current)
+    return fail(AB2_ERR_STATE, "resolve: no backward since the last set_problem, assemble or cycle_append");
+  if (nrhs < 0)
+    return fail(AB2_ERR_INVALID, "resolve: nrhs < 0");
+  const ab2_gar_dims &d = s->d;
+  const int N = d.horizon;
+  double *const po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
+  const size_t no[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
+                        (size_t)N * d.nx};
+  static const char *names[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
+  for (int i = 0; i < 6; ++i)
+    if (no[i] && !po[i])
+      return fail(AB2_ERR_INVALID, std::string("resolve: out ") + names[i] + " is NULL");
+  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  // the backward pass parks its per-knot vectors in the out arrays before it has read every rhs entry: an out array
+  // that overlaps an rhs array would be read after it was overwritten
+  const double *pr[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
+  static const char *rnames[6] = {"q", "r", "d", "dN", "g0", "f"};
+  const size_t R = (size_t)nrhs * d.batch;
+  for (int i = 0; i < 6; ++i)
+    for (int o = 0; o < 6; ++o)
+      if (pr[i] && po[o] && no[i] && no[o] && pr[i] < po[o] + R * no[o] && po[o] < pr[i] + R * no[i])
+        return fail(AB2_ERR_INVALID, std::string("resolve: rhs ") + rnames[i] + " overlaps out " + names[o]);
+  if ((size_t)ab2::resolve_item_doubles(d.nx, d.nu, d.nc, d.nc0, 1) * sizeof(double) > ab2::kResolveSmemMax)
+    return fail(AB2_ERR_UNSUPPORTED, "resolve: one right-hand side of this shape does not fit 227 KB of shared memory");
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  ab2::ResolveArgs a{};
+  a.batch = d.batch;
+  a.N = N;
+  a.nx = d.nx;
+  a.nu = d.nu;
+  a.nc = d.nc;
+  a.nct = d.nct;
+  a.nc0 = d.nc0;
+  a.srec = s->srec;
+  a.trec = s->trec;
+  a.stage_head = s->p.stage_head;
+  a.nrhs = nrhs;
+  a.stage = s->p.stage;
+  a.term = s->p.term;
+  a.G0 = s->p.G0;
+  a.fb = s->out[AB2_OUT_FB];
+  a.fbT = s->out[AB2_OUT_FBT];
+  a.Vxx = s->out[AB2_OUT_VXX];
+  a.Vxx0 = s->vxx_packed ? s->p.Vxx0 : nullptr;
+  a.mueq = mueq;
+  a.mueq_b = mu_dev;
+  a.q = rhs->q;
+  a.r = rhs->r;
+  a.d = rhs->d;
+  a.dN = rhs->dN;
+  a.g0 = rhs->g0;
+  a.f = rhs->f;
+  a.xs = out->xs;
+  a.us = out->us;
+  a.vs = out->vs;
+  a.vsT = out->vsT;
+  a.lam0 = out->lam0;
+  a.lams = out->lams;
+  CUDA_TRY(ab2::launch_resolve(a, st));
+  s->launches += 1;
+  return AB2_OK;
+}
+int ab2_gar_resolve(ab2_gar_solver *s, double mueq, int nrhs, const ab2_lq_rhs *rhs, const ab2_ls_trial *out,
+                    void *stream) {
+  return resolve_impl(s, mueq, nullptr, AB2_DEVICE, nrhs, rhs, out, stream);
+}
+int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs, const ab2_lq_rhs *rhs,
+                      const ab2_ls_trial *out, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return resolve_impl(s, 0.0, mueq, memspace, nrhs, rhs, out, stream);
+}
+int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch) {
+  if (!s || !epoch)
+    return fail(AB2_ERR_INVALID, "null argument");
+  *epoch = s->epoch;
+  return AB2_OK;
+}
+
 static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg_b, const double *mu_inv_b,
                          void *stream) {
   if (!s || !in)
@@ -1014,6 +1120,8 @@ static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const doubl
   s->p.G0 = s->own_G0;
   s->p.g0 = s->own_g0;
   s->have_problem = true;
+  s->factor_current = false;
+  s->epoch += 1;
   return AB2_OK;
 }
 int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream) {
@@ -1321,6 +1429,8 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
   s->have_forward = true;
   s->fac_head = 0;
   s->vxx_packed = warp_kernel(s);
+  s->factor_current = true;
+  s->epoch += 1;
   return AB2_OK;
 }
 
@@ -1858,6 +1968,8 @@ int ab2_gar_cycle_append(ab2_gar_solver *s, const double *new_last, int memspace
   CUDA_TRY(cudaGetLastError());
   s->have_backward = false;
   s->have_forward = false;
+  s->factor_current = false;
+  s->epoch += 1;
   return AB2_OK;
 }
 

@@ -66,6 +66,14 @@ class LqTangent(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _GRAD_KEYS]
 
 
+_RHS_KEYS = ("q", "r", "d", "dN", "g0", "f")
+
+
+class LqRhs(C.Structure):
+    """``ab2_lq_rhs``: device right-hand sides of ``ab2_gar_resolve`` (NULL = zero), [nrhs][batch][...]."""
+    _fields_ = [(k, C.c_void_p) for k in _RHS_KEYS]
+
+
 _MULT_IN = ("xs", "lam0", "lams", "vs", "vsT", "prev_vs", "prev_vsT", "init_value", "xnext", "fs", "cval", "cval_N",
             "lo", "hi", "loN", "hiN")
 _MULT_OUT = ("slack", "lam0_plus", "lams_plus", "vs_plus", "vsT_plus", "shifted", "shifted_N", "Lv", "Lv_N")
@@ -181,6 +189,11 @@ def lib():
         L.ab2_gar_tangent.argtypes = [C.c_void_p, C.c_double, C.POINTER(LsIterate), C.POINTER(LqTangent), C.c_void_p]
         L.ab2_gar_tangent_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LsIterate), C.POINTER(LqTangent),
                                         C.c_void_p]
+        L.ab2_gar_resolve.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LqRhs), C.POINTER(LsIterate),
+                                      C.c_void_p]
+        L.ab2_gar_resolve_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LqRhs),
+                                        C.POINTER(LsIterate), C.c_void_p]
+        L.ab2_gar_factor_epoch.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -647,6 +660,32 @@ class CudaRiccatiBatch:
             _check(lib().ab2_gar_tangent(self.h, C.c_double(mueq), C.byref(pr), C.byref(dt), C.c_void_p(stream)))
         else:
             _check(lib().ab2_gar_tangent_v(self.h, v[0], v[1], C.byref(pr), C.byref(dt), C.c_void_p(stream)))
+
+    def resolve(self, rhs, out, mueq, stream=0):
+        """Re-solve the last backward's LQ matrices for new vectors (``ab2_gar_resolve``): ``out`` receives
+        z = -K^-1 h, the solution of the current problem with its vectors replaced by h.  ``rhs``: dict with any of
+        q, r, d, dN, g0, f (a key that is missing or None is zero), ``out``: dict with keys xs, us, vs, vsT, lam0, lams;
+        device tensors [nrhs][batch][...] in the layouts of the solution (q like xs, r like us, d like vs, dN like vsT,
+        g0 like lam0, f like lams).  nrhs is read from ``out["xs"]``.  ``mueq``: the mu of the last backward, a number
+        or a [batch] array / tensor (``ab2_gar_resolve_v``).  The handle's own outputs are not touched."""
+        d = self.dims
+        nrhs = out["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
+        v = self._mueq_arg(mueq, stream)
+        rh = _fill(LqRhs(), _RHS_KEYS, rhs)
+        ot = _fill(LsIterate(), _LS_KEYS, out)
+        self._keep_rs = (rhs, out)
+        if v is None:
+            _check(lib().ab2_gar_resolve(self.h, C.c_double(mueq), int(nrhs), C.byref(rh), C.byref(ot),
+                                         C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_resolve_v(self.h, v[0], v[1], int(nrhs), C.byref(rh), C.byref(ot),
+                                           C.c_void_p(stream)))
+
+    def factor_epoch(self):
+        """``ab2_gar_factor_epoch``: bumped by every call that rewrites the factorisation or the records."""
+        e = C.c_longlong()
+        _check(lib().ab2_gar_factor_epoch(self.h, C.byref(e)))
+        return e.value
 
     # ---- multipliers, Lagrangian gradient, criterion (the rest of the inner iteration) ----
     def _scalars(self, call, out, stream):

@@ -435,6 +435,51 @@ int ab2_gar_tangent  (ab2_gar_solver *s, double mueq, const ab2_ls_iterate *prim
 int ab2_gar_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace, const ab2_ls_iterate *primal,
                       const ab2_lq_tangent *dot, void *stream);
 
+/* Re-solve the last backward's LQ matrices for new vectors, many right-hand sides at once (Jacobians, batched VJPs
+ * and JVPs, linear MPC where only g0 and the references change).  With h = (q_t, r_t, d_t, f_t, q_N, d_N, g0) in the
+ * layouts of the solution (ab2_ls_iterate: q [batch][N+1][nx] with q_N last, r like us, d like vs, dN like vsT, g0 like
+ * lam0, f like lams with f_t in the row of lambda_{t+1}), the call returns z = -K^-1 h: the solution of the handle's
+ * current LQ problem with all its vectors replaced by h, K the symmetric KKT matrix of the whole problem.  The
+ * problem's own vectors give the primal solution, h = -zbar the adjoint's w (ab2_gar_adjoint), h = rho the tangent
+ * (ab2_gar_tangent).  K is symmetric and h and z pair block for block, so the call is its own transpose: the VJP of z
+ * with respect to h is resolve(zbar) and the JVP is resolve(hdot).
+ * Only the vector half of the recursion runs; FB = [K; Z; Ahat] and VXX are read (in the layout the last backward
+ * wrote, ab2_gar_device_ptr), together with the stage records' matrices (through the ring head) and C_N, G0:
+ *   terminal  z_N = d_N / mu,  vx_N = q_N + C_N^T z_N
+ *   stage t   V' = Vxx_{t+1},  v+ = vx_{t+1} + V' f_t,  rhat = r_t + B^T v+,
+ *             [k; z] = -[[R + B^T V' B, D^T], [D, -mu I]]^-1 [rhat; d_t]   (Bunch-Kaufman, once per knot, instance and
+ *             chunk of right-hand sides),  a = f_t + B k,
+ *             vx_t = (qhat + Shat k) + C^T z  with qhat = q_t + A^T v+, Shat k = S k + A^T V' B k (the reference's order)
+ *   initial   [x_0; lam_0] = -[[Vxx_0, G0^T], [G0, 0]]^-1 [vx_0; g0]
+ *   forward   u_t = k + K x_t,  v_t = z + Z x_t,  x_{t+1} = a + Ahat x_t,  lam_{t+1} = vx_{t+1} + Vxx_{t+1} x_{t+1},
+ *             v_N = z_N + Z_N x_N.
+ * Every saddle-point matrix is read from its lower triangle, as the sweep's factorisations read theirs.
+ * Layout: every rhs and out field is [nrhs][batch][...] in DEVICE memory; right-hand side j of instance b is block
+ * j * batch + b.  A NULL rhs field is zero; an out field of nonzero size is required.  The out arrays hold the
+ * backward pass's per-knot vectors before every rhs entry has been read, so no rhs array may overlap an out array
+ * (an in-place re-solve such as q -> xs is refused).  `mueq` must be the mu of the last
+ * backward.  The call writes the out arrays and nothing else: every output of the handle (FF .. LBDAS, status, pivot
+ * statistics) is unchanged.  One launch on `stream`; right-hand side j's result is bit for bit independent of nrhs and
+ * of its position among the right-hand sides (no atomics).
+ * Errors (nothing is launched): AB2_ERR_UNSUPPORTED for dense, parametric (nth > 0) and parallel handles;
+ * AB2_ERR_STATE when no backward (backward, sweep, their *_v twins, sweep_host*, adjoint, tangent, fddp_backward_pass)
+ * has run since the last set_problem, assemble or cycle_append; AB2_ERR_INVALID for nrhs < 0, a NULL required out
+ * field, an rhs array overlapping an out array, or mueq <= 0 with constraints.  Every shape a plain serial handle accepts
+ * fits (one right-hand side needs max(nx^2 + (nu+nc+nx) nx + 2 nx nu + (nu+nc)(nu+nc+1), (nx+nc0)(nx+nc0+1)) +
+ * 4 nx + max(nu+nc, nx+nc0) doubles of shared memory); a shape that did not would return AB2_ERR_UNSUPPORTED.  nrhs == 0 launches nothing. */
+typedef struct ab2_lq_rhs {
+  const double *q, *r, *d, *dN, *g0, *f;
+} ab2_lq_rhs;
+int ab2_gar_resolve  (ab2_gar_solver *s, double mueq, int nrhs, const ab2_lq_rhs *rhs,
+                      const ab2_ls_trial *out, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs,
+                      const ab2_lq_rhs *rhs, const ab2_ls_trial *out, void *stream);
+/* A counter that every call rewriting FB / VXX or the records bumps (set_problem, assemble, cycle_append and every
+ * backward listed above): a caller that keeps derivatives for later re-solves checks that the factorisation they
+ * belong to is still the handle's.  A host-side increment; it changes nothing those calls compute. */
+int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch);
+
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
  * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
