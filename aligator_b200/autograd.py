@@ -11,9 +11,14 @@ in the layouts of gar.h.  :func:`stage_records` and :func:`term_records` build t
 Q and R are symmetric, and their gradient is the one with respect to a symmetric argument (Q_ij and Q_ji perturbed
 together).  That is the right chain rule when Q and R are built symmetric, e.g. as ``(P + P^T) / 2`` or ``L L^T``.
 Forward mode (``torch.func.jvp``, ``torch.autograd.forward_ad``) is its exact transpose: the tangent of Q and R enters
-through ``sym(Qdot) = (Qdot + Qdot^T) / 2``, so an asymmetric tangent acts as its symmetric part.  ``jacfwd`` and
-``vmap`` are not supported: the function has no vmap rule.  The penalty ``mueq`` (a number or a [batch] tensor) is not
-differentiated.
+through ``sym(Qdot) = (Qdot + Qdot^T) / 2``, so an asymmetric tangent acts as its symmetric part.  The penalty
+``mueq`` (a number or a [batch] tensor) is not differentiated, and the gradients and jvps are not differentiable again.
+
+Jacobians: under ``torch.func.jacrev``, ``jacfwd``, ``vmap`` of a vjp function or ``vmap`` over ``torch.func.jvp``
+tangents, the V cotangents or tangents go to the device in one call on one factorisation (``ab2_gar_adjoint_many`` /
+``ab2_gar_tangent_many``, through ``ab2_gar_resolve``; one single call per slice on a dense handle).  Outside vmap the
+gradients and jvps are those of one ``adjoint`` or ``tangent`` call.  vmap over the problem data itself raises
+``NotImplementedError``.
 
 :func:`lq_resolve` re-solves the matrices of the handle's last backward for new vectors (``ab2_gar_resolve``), many
 right-hand sides in one call.  It is linear in the vectors and its own transpose, so its ``backward`` and ``jvp`` are
@@ -24,6 +29,7 @@ from __future__ import annotations
 
 import torch
 from torch._C import _functorch
+from torch.autograd.function import once_differentiable
 
 from . import gar as _gar
 
@@ -88,31 +94,135 @@ class _LqSolve(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *gouts):
         stage, term, G0, g0, *outs = ctx.saved_tensors
-        inputs = dict(zip(_INPUTS, (stage, term, G0, g0)))
-        grads = {k: torch.empty_like(t) for i, (k, t) in enumerate(inputs.items()) if ctx.needs_input_grad[1 + i]}
-        if grads and any(g is not None for g in gouts):
-            batch = ctx.batch
-            stream = torch.cuda.current_stream(stage.device).cuda_stream
-            batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
-            cot = {k: None if g is None else g.to(torch.float64).contiguous() for k, g in zip(_KEYS, gouts)}
-            batch.adjoint(dict(zip(_KEYS, outs)), cot, grads, ctx.mueq, stream=stream)
-        else:
-            grads = {}
-        return (None,) + tuple(grads.get(k) for k in _INPUTS) + (None,)
+        need = tuple(ctx.needs_input_grad[1:5])
+        if not any(need) or all(g is None for g in gouts):
+            return (None,) * 6
+        grads = iter(_LqSolveVjp.apply(ctx.batch, ctx.mueq, need, stage, term, G0, g0, *outs, *gouts))
+        return (None,) + tuple(next(grads) if n else None for n in need) + (None,)
 
     @staticmethod
     def jvp(ctx, _batch_t, *tangents):
-        # under torch.func.jvp the saved tensors and tangents arrive wrapped; the library needs the storage beneath
+        # under torch.func.jvp the saved tensors arrive wrapped; the library needs the storage beneath.  The tangents
+        # are passed on as they are: under vmap (jacfwd) they are batched, and _LqSolveJvp's vmap rule takes them.
         stage, term, G0, g0, *outs = [_plain(t) for t in ctx.saved_tensors]
-        batch = ctx.batch
-        stream = torch.cuda.current_stream(stage.device).cuda_stream
-        dot = {k: None if t is None else _plain(t.to(torch.float64).contiguous())
-               for k, t in zip(_INPUTS, tangents[:4])}
-        if all(t is None for t in dot.values()):
+        dot = tangents[:4]
+        if all(t is None for t in dot):
             return tuple(torch.zeros_like(o) for o in outs)
+        return _LqSolveJvp.apply(ctx.batch, ctx.mueq, stage, term, G0, g0, *outs, *dot)
+
+    @staticmethod
+    def vmap(info, in_dims, batch, stage, term, G0, g0, mueq):
+        # torch runs the forward unbatched when no input is batched (jacfwd, vmap over cotangents); it needs this rule
+        # to exist all the same
+        raise NotImplementedError(_NO_DATA_VMAP)
+
+
+_NO_DATA_VMAP = ("lq_solve: vmap over the problem data (stage, term, G0, g0, mueq) is not supported; vmap over "
+                 "cotangents and tangents is (torch.func.jacrev, jacfwd, vmap of a vjp or jvp function)")
+_NOT_TWICE = "lq_solve is differentiable once: its gradients and jvps have no derivatives"
+
+
+def _stacked(t, bd, V):
+    """A vmapped argument as a [V][...] float64 tensor: its batch dimension first, or broadcast when unbatched."""
+    if t is None:
+        return None
+    t = t.movedim(bd, 0) if bd is not None else t.unsqueeze(0).expand(V, *t.shape)
+    return t.to(torch.float64).contiguous()
+
+
+class _LqSolveVjp(torch.autograd.Function):
+    """Gradient records of ``lq_solve`` for the cotangents ``gouts`` of its outputs: one ``adjoint`` call, or under vmap
+    one ``adjoint_many`` over all the cotangents (one ``adjoint`` per cotangent on a dense handle)."""
+
+    @staticmethod
+    def forward(batch, mueq, need, stage, term, G0, g0, *rest):
+        # saved tensors of a torch.func.vjp arrive as wrappers of a finished transform; the library needs the storage
+        stage, term, G0, g0, *outs = [_plain(t) for t in (stage, term, G0, g0) + rest[:6]]
+        gouts = rest[6:]
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        inputs = dict(zip(_INPUTS, (stage, term, G0, g0)))
+        grads = {k: torch.empty_like(t) for (k, t), n in zip(inputs.items(), need) if n}
         batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
-        batch.tangent(dict(zip(_KEYS, outs)), dot, ctx.mueq, stream=stream)
+        cot = {k: None if g is None else g.to(torch.float64).contiguous() for k, g in zip(_KEYS, gouts)}
+        batch.adjoint(dict(zip(_KEYS, outs)), cot, grads, mueq, stream=stream)
+        return tuple(grads.values())
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *_):
+        raise RuntimeError(_NOT_TWICE)
+
+    @staticmethod
+    def vmap(info, in_dims, batch, mueq, need, stage, term, G0, g0, *rest):
+        if any(d is not None for d in (in_dims[1],) + in_dims[3:13]):  # in_dims[2]: `need`, not a tensor
+            raise NotImplementedError(_NO_DATA_VMAP)
+        V = info.batch_size
+        stage, term, G0, g0, *outs = [_plain(t) for t in (stage, term, G0, g0) + rest[:6]]
+        primal = dict(zip(_KEYS, outs))
+        cot = {k: _stacked(g, bd, V) for k, g, bd in zip(_KEYS, rest[6:], in_dims[13:])}
+        shapes = {k: t.shape for k, t in zip(_INPUTS, (stage, term, G0, g0))}
+        grads = {k: torch.empty((V,) + shapes[k], dtype=torch.float64, device=stage.device)
+                 for k, n in zip(_INPUTS, need) if n}
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        if batch.dense:  # resolve does not serve dense handles: one adjoint per cotangent
+            for j in range(V):
+                batch.adjoint(primal, {k: None if c is None else c[j] for k, c in cot.items()},
+                              {k: g[j] for k, g in grads.items()}, mueq, stream=stream)
+        else:
+            batch.backward(mueq, stream=stream)
+            work = {k: torch.empty((V,) + o.shape, dtype=torch.float64, device=stage.device) for k, o in primal.items()}
+            batch.adjoint_many(primal, cot, work, grads, mueq, stream=stream)
+        return tuple(grads.values()), 0
+
+
+class _LqSolveJvp(torch.autograd.Function):
+    """The derivative of ``lq_solve``'s outputs along the data tangents ``dot``: one ``tangent`` call, or under vmap one
+    ``tangent_many`` over all the tangents (one ``tangent`` per tangent on a dense handle)."""
+
+    @staticmethod
+    def forward(batch, mueq, stage, term, G0, g0, *rest):
+        outs, dot = rest[:6], rest[6:]
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        dot = {k: None if t is None else _plain(t.to(torch.float64).contiguous()) for k, t in zip(_INPUTS, dot)}
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        batch.tangent(dict(zip(_KEYS, outs)), dot, mueq, stream=stream)
         return _outputs(batch, stage.device, stream)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *_):
+        raise RuntimeError(_NOT_TWICE)
+
+    @staticmethod
+    def vmap(info, in_dims, batch, mueq, stage, term, G0, g0, *rest):
+        if any(d is not None for d in in_dims[1:12]):
+            raise NotImplementedError(_NO_DATA_VMAP)
+        V = info.batch_size
+        stage, term, G0, g0, *outs = [_plain(t) for t in (stage, term, G0, g0) + rest[:6]]
+        primal = dict(zip(_KEYS, outs))
+        dot = {k: _stacked(t, bd, V) for k, t, bd in zip(_INPUTS, rest[6:], in_dims[12:])}
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        if batch.dense:  # resolve does not serve dense handles: one tangent per tangent
+            res = []
+            for j in range(V):
+                batch.tangent(primal, {k: None if t is None else t[j] for k, t in dot.items()}, mueq, stream=stream)
+                res.append(_outputs(batch, stage.device, stream))
+            return tuple(torch.stack(r) for r in zip(*res)), 0
+        batch.backward(mueq, stream=stream)
+        work = {k: torch.empty((V,) + o.shape, dtype=torch.float64, device=stage.device) for k, o in primal.items()}
+        res = {k: torch.empty((V,) + o.shape, dtype=torch.float64, device=stage.device) for k, o in primal.items()}
+        batch.tangent_many(primal, dot, work, res, mueq, stream=stream)
+        return tuple(res[k] for k in _KEYS), 0
 
 
 def lq_solve(batch, stage, term, G0, g0, mueq):

@@ -11,7 +11,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/aligator_b200/gar.h"
@@ -20,6 +22,7 @@
 #include "lq_adjoint.h"
 #include "lq_tangent.h"
 #include "lq_resolve.h"
+#include "lq_jacobian.h"
 #include "lq_assemble.h"
 #include "proxddp_inner.h"
 #include "riccati_block_launch.h"
@@ -991,49 +994,30 @@ int ab2_gar_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace, const
 }
 
 // ---- re-solve for new vectors (lq_resolve.cu): the vector half of the recursion on the last backward's factorisation ----
-static int resolve_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int nrhs,
-                        const ab2_lq_rhs *rhs, const ab2_ls_trial *out, void *stream) {
-  if (!s || !rhs || !out)
-    return fail(AB2_ERR_INVALID, "null argument");
+// The first checks of every call that runs resolve's program, in this order: handle kind, factorisation current, nrhs.
+static int check_resolve_handle(const ab2_gar_solver *s, int nrhs, const char *who) {
   if (s->nth > 0 || s->legs > 1 || s->dense)
-    return fail(AB2_ERR_UNSUPPORTED, "resolve: dense, parametric (nth > 0) and parallel handles are not supported");
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": dense, parametric (nth > 0) and parallel handles are not supported");
   if (!s->have_problem || !s->factor_current)
-    return fail(AB2_ERR_STATE, "resolve: no backward since the last set_problem, assemble or cycle_append");
+    return fail(AB2_ERR_STATE, std::string(who) + ": no backward since the last set_problem, assemble or cycle_append");
   if (nrhs < 0)
-    return fail(AB2_ERR_INVALID, "resolve: nrhs < 0");
+    return fail(AB2_ERR_INVALID, std::string(who) + ": nrhs < 0");
+  return AB2_OK;
+}
+static int check_resolve_fits(const ab2_gar_solver *s, const char *who) {
   const ab2_gar_dims &d = s->d;
-  const int N = d.horizon;
-  double *const po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
-  const size_t no[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
-                        (size_t)N * d.nx};
-  static const char *names[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
-  for (int i = 0; i < 6; ++i)
-    if (no[i] && !po[i])
-      return fail(AB2_ERR_INVALID, std::string("resolve: out ") + names[i] + " is NULL");
-  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
-  // the backward pass parks its per-knot vectors in the out arrays before it has read every rhs entry: an out array
-  // that overlaps an rhs array would be read after it was overwritten
-  const double *pr[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
-  static const char *rnames[6] = {"q", "r", "d", "dN", "g0", "f"};
-  const size_t R = (size_t)nrhs * d.batch;
-  for (int i = 0; i < 6; ++i)
-    for (int o = 0; o < 6; ++o)
-      if (pr[i] && po[o] && no[i] && no[o] && pr[i] < po[o] + R * no[o] && po[o] < pr[i] + R * no[i])
-        return fail(AB2_ERR_INVALID, std::string("resolve: rhs ") + rnames[i] + " overlaps out " + names[o]);
   if ((size_t)ab2::resolve_item_doubles(d.nx, d.nu, d.nc, d.nc0, 1) * sizeof(double) > ab2::kResolveSmemMax)
-    return fail(AB2_ERR_UNSUPPORTED, "resolve: one right-hand side of this shape does not fit 227 KB of shared memory");
-  if (nrhs == 0)
-    return AB2_OK;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one right-hand side of this shape does not fit 227 KB of shared memory");
+  return AB2_OK;
+}
+// resolve's program on the handle's current factorisation, rhs -> out (one launch).  mu_dev: the staged per-instance
+// mu, or null for the scalar mueq.
+static int run_resolve(ab2_gar_solver *s, double mueq, const double *mu_dev, int nrhs, const ab2_lq_rhs *rhs,
+                       const ab2_ls_trial *out, cudaStream_t st) {
+  const ab2_gar_dims &d = s->d;
   ab2::ResolveArgs a{};
   a.batch = d.batch;
-  a.N = N;
+  a.N = d.horizon;
   a.nx = d.nx;
   a.nu = d.nu;
   a.nc = d.nc;
@@ -1068,6 +1052,44 @@ static int resolve_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
   s->launches += 1;
   return AB2_OK;
 }
+static int resolve_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int nrhs,
+                        const ab2_lq_rhs *rhs, const ab2_ls_trial *out, void *stream) {
+  if (!s || !rhs || !out)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_resolve_handle(s, nrhs, "resolve"))
+    return rc;
+  const ab2_gar_dims &d = s->d;
+  const int N = d.horizon;
+  double *const po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
+  const size_t no[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
+                        (size_t)N * d.nx};
+  static const char *names[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
+  for (int i = 0; i < 6; ++i)
+    if (no[i] && !po[i])
+      return fail(AB2_ERR_INVALID, std::string("resolve: out ") + names[i] + " is NULL");
+  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  // the backward pass parks its per-knot vectors in the out arrays before it has read every rhs entry: an out array
+  // that overlaps an rhs array would be read after it was overwritten
+  const double *pr[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
+  static const char *rnames[6] = {"q", "r", "d", "dN", "g0", "f"};
+  const size_t R = (size_t)nrhs * d.batch;
+  for (int i = 0; i < 6; ++i)
+    for (int o = 0; o < 6; ++o)
+      if (pr[i] && po[o] && no[i] && no[o] && pr[i] < po[o] + R * no[o] && po[o] < pr[i] + R * no[i])
+        return fail(AB2_ERR_INVALID, std::string("resolve: rhs ") + rnames[i] + " overlaps out " + names[o]);
+  if (int rc = check_resolve_fits(s, "resolve"))
+    return rc;
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  return run_resolve(s, mueq, mu_dev, nrhs, rhs, out, st);
+}
 int ab2_gar_resolve(ab2_gar_solver *s, double mueq, int nrhs, const ab2_lq_rhs *rhs, const ab2_ls_trial *out,
                     void *stream) {
   return resolve_impl(s, mueq, nullptr, AB2_DEVICE, nrhs, rhs, out, stream);
@@ -1083,6 +1105,183 @@ int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch) {
     return fail(AB2_ERR_INVALID, "null argument");
   *epoch = s->epoch;
   return AB2_OK;
+}
+
+// ---- Jacobians (lq_jacobian.cu): many cotangents or tangents on the last backward's factorisation, through resolve ----
+// The fields of one argument, for the NULL and overlap checks: pointers and sizes in doubles.
+struct Fields {
+  const char *what;
+  const char *const *names;
+  const double *p[6];
+  size_t n[6];
+  int count;
+};
+typedef std::pair<const Fields *, const Fields *> FieldPair;
+static const char *const kSolNames[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
+static const char *const kRecNames[4] = {"stage", "term", "G0", "g0"};
+// fields in the solution's layouts, `blocks` instances (batch, or nrhs * batch)
+static Fields sol_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
+  const ab2_gar_dims &d = s->d;
+  const int N = d.horizon;
+  const size_t per[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
+                         (size_t)N * d.nx};
+  Fields f{what, kSolNames, {}, {}, 6};
+  for (int i = 0; i < 6; ++i) {
+    f.p[i] = p[i];
+    f.n[i] = blocks * per[i];
+  }
+  return f;
+}
+// fields in the problem's record layouts (stage, term, G0, g0), `blocks` instances
+static Fields rec_fields(const ab2_gar_solver *s, const char *what, const double *const p[4], size_t blocks) {
+  const ab2_gar_dims &d = s->d;
+  const size_t per[4] = {(size_t)d.horizon * s->srec, (size_t)s->trec, (size_t)d.nc0 * d.nx, (size_t)d.nc0};
+  Fields f{what, kRecNames, {}, {}, 4};
+  for (int i = 0; i < 4; ++i) {
+    f.p[i] = p[i];
+    f.n[i] = blocks * per[i];
+  }
+  return f;
+}
+static int require(const Fields &f, const char *who) {
+  for (int i = 0; i < f.count; ++i)
+    if (f.n[i] && !f.p[i])
+      return fail(AB2_ERR_INVALID, std::string(who) + ": " + f.what + " " + f.names[i] + " is NULL");
+  return AB2_OK;
+}
+// no field of a may overlap a field of b (a and b the same argument: two different fields of it)
+static int refuse_overlap(const Fields &a, const Fields &b, const char *who) {
+  for (int i = 0; i < a.count; ++i)
+    for (int o = &a == &b ? i + 1 : 0; o < b.count; ++o)
+      if (a.p[i] && b.p[o] && a.n[i] && b.n[o] && a.p[i] < b.p[o] + b.n[o] && b.p[o] < a.p[i] + a.n[i])
+        return fail(AB2_ERR_INVALID, std::string(who) + ": " + a.what + " " + a.names[i] + " overlaps " + b.what + " " +
+                                         b.names[o]);
+  return AB2_OK;
+}
+
+static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int nrhs,
+                             const ab2_ls_iterate *primal, const ab2_ls_iterate *cot, const ab2_ls_trial *work,
+                             const ab2_lq_grad *grad, void *stream) {
+  const char *who = "adjoint_many";
+  if (!s || !primal || !cot || !work || !grad)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_resolve_handle(s, nrhs, who))
+    return rc;
+  const ab2_gar_dims &d = s->d;
+  const size_t B = d.batch, R = (size_t)nrhs * B;
+  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
+  const double *pc[6] = {cot->xs, cot->us, cot->vs, cot->vsT, cot->lam0, cot->lams};
+  const double *pw[6] = {work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
+  const double *pg[4] = {grad->stage, grad->term, grad->G0, grad->g0};
+  const Fields P = sol_fields(s, "primal", pp, B), Z = sol_fields(s, "cotangent", pc, R),
+               W = sol_fields(s, "work", pw, R), G = rec_fields(s, "grad", pg, R);
+  if (int rc = require(W, who))
+    return rc;
+  if (int rc = require(P, who))
+    return rc;
+  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  // resolve writes work while it reads the cotangent; the gradient kernel then reads work and the primal
+  for (const FieldPair &ab : {FieldPair{&Z, &W}, FieldPair{&W, &P}, FieldPair{&G, &P}, FieldPair{&G, &W},
+                              FieldPair{&G, &G}})
+    if (int rc = refuse_overlap(*ab.first, *ab.second, who))
+      return rc;
+  if (int rc = check_resolve_fits(s, who))
+    return rc;
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  // 1. y_j = resolve(zbar_j) = -K^-1 zbar_j: the cotangent fields are resolve's rhs fields
+  const ab2_lq_rhs rhs{cot->xs, cot->us, cot->vs, cot->vsT, cot->lam0, cot->lams};
+  if (int rc = run_resolve(s, mueq, mu_dev, nrhs, &rhs, work, st))
+    return rc;
+  // 2. gradient records from y_j and z
+  const ab2::AdjointDims ad{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  ab2::JacobianGradArgs ga{ad, nrhs,
+                           primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
+                           work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams,
+                           grad->stage, grad->term, grad->G0, grad->g0};
+  CUDA_TRY(ab2::launch_jacobian_grad(ga, st));
+  s->launches += 1;
+  return AB2_OK;
+}
+int ab2_gar_adjoint_many(ab2_gar_solver *s, double mueq, int nrhs, const ab2_ls_iterate *primal,
+                         const ab2_ls_iterate *cotangent, const ab2_ls_trial *work, const ab2_lq_grad *grad,
+                         void *stream) {
+  return adjoint_many_impl(s, mueq, nullptr, AB2_DEVICE, nrhs, primal, cotangent, work, grad, stream);
+}
+int ab2_gar_adjoint_many_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs, const ab2_ls_iterate *primal,
+                           const ab2_ls_iterate *cotangent, const ab2_ls_trial *work, const ab2_lq_grad *grad,
+                           void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return adjoint_many_impl(s, 0.0, mueq, memspace, nrhs, primal, cotangent, work, grad, stream);
+}
+
+static int tangent_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int nrhs,
+                             const ab2_ls_iterate *primal, const ab2_lq_tangent *dot, const ab2_ls_trial *work,
+                             const ab2_ls_trial *out, void *stream) {
+  const char *who = "tangent_many";
+  if (!s || !primal || !dot || !work || !out)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_resolve_handle(s, nrhs, who))
+    return rc;
+  const ab2_gar_dims &d = s->d;
+  const size_t B = d.batch, R = (size_t)nrhs * B;
+  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
+  const double *pd[4] = {dot->stage, dot->term, dot->G0, dot->g0};
+  const double *pw[6] = {work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
+  const double *po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
+  const Fields P = sol_fields(s, "primal", pp, B), D = rec_fields(s, "dot", pd, R),
+               W = sol_fields(s, "work", pw, R), O = sol_fields(s, "out", po, R);
+  if (int rc = require(W, who))
+    return rc;
+  if (int rc = require(O, who))
+    return rc;
+  if (int rc = require(P, who))
+    return rc;
+  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  // the rho kernel writes work while it reads the tangent and the primal; resolve then writes out while it reads work
+  for (const FieldPair &ab : {FieldPair{&D, &W}, FieldPair{&P, &W}, FieldPair{&W, &O}, FieldPair{&O, &P},
+                              FieldPair{&O, &O}})
+    if (int rc = refuse_overlap(*ab.first, *ab.second, who))
+      return rc;
+  if (int rc = check_resolve_fits(s, who))
+    return rc;
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  // 1. rho_j = Kdot_j z + hdot_j into work, in resolve's rhs layouts
+  const ab2::AdjointDims ad{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  ab2::JacobianRhsArgs ra{ad, nrhs, dot->stage, dot->term, dot->G0, dot->g0,
+                          primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
+                          work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
+  CUDA_TRY(ab2::launch_jacobian_rhs(ra, st));
+  s->launches += 1;
+  // 2. zdot_j = resolve(rho_j) = -K^-1 rho_j
+  const ab2_lq_rhs rhs{work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
+  return run_resolve(s, mueq, mu_dev, nrhs, &rhs, out, st);
+}
+int ab2_gar_tangent_many(ab2_gar_solver *s, double mueq, int nrhs, const ab2_ls_iterate *primal,
+                         const ab2_lq_tangent *dot, const ab2_ls_trial *work, const ab2_ls_trial *out, void *stream) {
+  return tangent_many_impl(s, mueq, nullptr, AB2_DEVICE, nrhs, primal, dot, work, out, stream);
+}
+int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs, const ab2_ls_iterate *primal,
+                           const ab2_lq_tangent *dot, const ab2_ls_trial *work, const ab2_ls_trial *out, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return tangent_many_impl(s, 0.0, mueq, memspace, nrhs, primal, dot, work, out, stream);
 }
 
 static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg_b, const double *mu_inv_b,

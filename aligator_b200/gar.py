@@ -194,6 +194,15 @@ def lib():
         L.ab2_gar_resolve_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LqRhs),
                                         C.POINTER(LsIterate), C.c_void_p]
         L.ab2_gar_factor_epoch.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
+        L.ab2_gar_adjoint_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LsIterate), C.POINTER(LsIterate),
+                                           C.POINTER(LsIterate), C.POINTER(LqGrad), C.c_void_p]
+        L.ab2_gar_adjoint_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LsIterate),
+                                             C.POINTER(LsIterate), C.POINTER(LsIterate), C.POINTER(LqGrad), C.c_void_p]
+        L.ab2_gar_tangent_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LsIterate), C.POINTER(LqTangent),
+                                           C.POINTER(LsIterate), C.POINTER(LsIterate), C.c_void_p]
+        L.ab2_gar_tangent_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LsIterate),
+                                             C.POINTER(LqTangent), C.POINTER(LsIterate), C.POINTER(LsIterate),
+                                             C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -680,6 +689,54 @@ class CudaRiccatiBatch:
         else:
             _check(lib().ab2_gar_resolve_v(self.h, v[0], v[1], int(nrhs), C.byref(rh), C.byref(ot),
                                            C.c_void_p(stream)))
+
+    def adjoint_many(self, primal, cotangent, work, grad, mueq, stream=0):
+        """Many cotangents on the last backward's factorisation (``ab2_gar_adjoint_many``): ``grad`` receives, for every
+        cotangent j, the gradient records ``adjoint`` would give, and ``work`` receives y_j = -K^-1 zbar_j, the vector
+        gradient in the solution's layouts.  ``primal``: dict with keys xs, us, vs, vsT, lam0, lams of device tensors
+        [batch][...] (the solution of the current problem at this mu).  ``cotangent`` (a key that is missing or None is
+        zero) and ``work``: dicts with the same keys of device tensors [nrhs][batch][...]; nrhs is read from
+        ``work["xs"]``.  ``grad``: dict with any of stage, term, G0, g0 of device tensors [nrhs][batch][...] in the
+        problem's layouts, overwritten (a missing key is not written).  ``mueq``: the mu of the last backward, a number
+        or a [batch] array / tensor (``ab2_gar_adjoint_many_v``).  The handle's own outputs are not touched."""
+        d = self.dims
+        nrhs = work["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
+        v = self._mueq_arg(mueq, stream)
+        pr = _fill(LsIterate(), _LS_KEYS, primal)
+        ct = _fill(LsIterate(), _LS_KEYS, cotangent)
+        wk = _fill(LsIterate(), _LS_KEYS, work)
+        gr = _fill(LqGrad(), _GRAD_KEYS, grad)
+        self._keep_adj_many = (primal, cotangent, work, grad)
+        if v is None:
+            _check(lib().ab2_gar_adjoint_many(self.h, C.c_double(mueq), int(nrhs), C.byref(pr), C.byref(ct),
+                                              C.byref(wk), C.byref(gr), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_adjoint_many_v(self.h, v[0], v[1], int(nrhs), C.byref(pr), C.byref(ct), C.byref(wk),
+                                                C.byref(gr), C.c_void_p(stream)))
+
+    def tangent_many(self, primal, tangent, work, out, mueq, stream=0):
+        """Many tangents on the last backward's factorisation (``ab2_gar_tangent_many``): ``out`` receives, for every
+        tangent j, the derivative zdot_j of the solution that ``tangent`` would give, and ``work`` the right-hand side
+        rho_j = Kdot_j z + hdot_j in resolve's rhs layouts.  ``tangent``: dict with any of stage, term, G0, g0 of device
+        tensors [nrhs][batch][...] in the problem's layouts (a key that is missing or None is zero).  ``primal``,
+        ``work``, ``out``: dicts with keys xs, us, vs, vsT, lam0, lams of device tensors, [batch][...] for ``primal``
+        and [nrhs][batch][...] for the others; nrhs is read from ``out["xs"]``.  ``mueq``: the mu of the last backward,
+        a number or a [batch] array / tensor (``ab2_gar_tangent_many_v``).  The handle's own outputs are not
+        touched."""
+        d = self.dims
+        nrhs = out["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
+        v = self._mueq_arg(mueq, stream)
+        pr = _fill(LsIterate(), _LS_KEYS, primal)
+        dt = _fill(LqTangent(), _GRAD_KEYS, tangent)
+        wk = _fill(LsIterate(), _LS_KEYS, work)
+        ot = _fill(LsIterate(), _LS_KEYS, out)
+        self._keep_tan_many = (primal, tangent, work, out)
+        if v is None:
+            _check(lib().ab2_gar_tangent_many(self.h, C.c_double(mueq), int(nrhs), C.byref(pr), C.byref(dt),
+                                              C.byref(wk), C.byref(ot), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_tangent_many_v(self.h, v[0], v[1], int(nrhs), C.byref(pr), C.byref(dt), C.byref(wk),
+                                                C.byref(ot), C.c_void_p(stream)))
 
     def factor_epoch(self):
         """``ab2_gar_factor_epoch``: bumped by every call that rewrites the factorisation or the records."""

@@ -480,6 +480,50 @@ int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int n
  * belong to is still the handle's.  A host-side increment; it changes nothing those calls compute. */
 int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch);
 
+/* Jacobians of the LQ solution with respect to the problem data: many cotangents (reverse mode) or many tangents
+ * (forward mode) on the last backward's factorisation, through ab2_gar_resolve's program (resolve(h) = -K^-1 h), without
+ * re-running the matrix recursion per right-hand side.
+ *   adjoint_many, for each cotangent j:  y_j = resolve(zbar_j), with the cotangent fields as resolve's rhs fields
+ *     (xs -> q, us -> r, vs -> d, vsT -> dN, lam0 -> g0, lams -> f).  y_j = -w_j with w_j as in ab2_gar_adjoint, so the
+ *     vector gradients are y_j itself (dq = y_x, dr = y_u, dd = y_v, df = y_l, dg0 = y_l0, and the terminal dq_N, dd_N)
+ *     and the matrix gradients are ab2_gar_adjoint's with -w replaced by y: dA = y_l,t+1 x_t^T + l_t+1 y_x,t^T,
+ *     dQ = 1/2 (y_x x^T + x y_x^T), dG0 = y_l0 x_0^T + l_0 y_x0^T, ...
+ *   tangent_many, for each tangent j:  rho_j = ab2_gar_tangent's right-hand side Kdot_j z + hdot_j, and
+ *     zdot_j = -K^-1 rho_j = resolve(rho_j).
+ * Layouts: `primal` is [batch][...] in the solver's output layouts, the solution of the current problem at this mu.
+ * Every per-right-hand-side array (cotangent, dot, work, grad, out) is [nrhs][batch][...] in DEVICE memory: block
+ * j * batch + b is right-hand side j of instance b.  grad and dot use the problem's record layouts (stage records'
+ * pad double written as 0, never read).  A NULL cotangent or dot field is zero for every right-hand side; a NULL grad
+ * field is not written.  `work` is caller-owned scratch in resolve's out layout (so the calls allocate nothing):
+ * adjoint_many leaves y there, which is the vector gradient in the solution's layouts (a result); tangent_many leaves
+ * rho there, in resolve's rhs layouts.
+ * Launches, in order on `stream` without host synchronisation: adjoint_many runs resolve (cotangent -> work), then a
+ * gradient kernel (work, primal -> grad); tangent_many runs a rho kernel (dot, primal -> work), then resolve
+ * (work -> out).  Only the caller's arrays are written: every handle output (FF .. LBDAS, status, pivot statistics) is
+ * unchanged and ab2_gar_factor_epoch does not move.  Records are read through the ring head (correct after
+ * cycle_append and a backward).  Right-hand side j's results are bit for bit independent of nrhs and of j's position.
+ * `mueq` must be the mu of the last backward.
+ * Errors (nothing is launched), as ab2_gar_resolve: AB2_ERR_UNSUPPORTED for dense, parametric (nth > 0) and parallel
+ * handles; AB2_ERR_STATE when no backward has run since the last set_problem, assemble or cycle_append;
+ * AB2_ERR_INVALID for nrhs < 0, a NULL work (or, for tangent_many, out) field of nonzero size, a NULL primal field of
+ * nonzero size, mueq <= 0 with constraints, or an overlap that would let one step read what an earlier step wrote:
+ * cotangent or dot with work, work with primal or out, grad or out with primal or with each other, grad with work.
+ * nrhs == 0 launches and writes nothing. */
+int ab2_gar_adjoint_many  (ab2_gar_solver *s, double mueq, int nrhs, const ab2_ls_iterate *primal,
+                           const ab2_ls_iterate *cotangent, const ab2_ls_trial *work,
+                           const ab2_lq_grad *grad, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_adjoint_many_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs,
+                           const ab2_ls_iterate *primal, const ab2_ls_iterate *cotangent,
+                           const ab2_ls_trial *work, const ab2_lq_grad *grad, void *stream);
+int ab2_gar_tangent_many  (ab2_gar_solver *s, double mueq, int nrhs, const ab2_ls_iterate *primal,
+                           const ab2_lq_tangent *dot, const ab2_ls_trial *work,
+                           const ab2_ls_trial *out, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs,
+                           const ab2_ls_iterate *primal, const ab2_lq_tangent *dot,
+                           const ab2_ls_trial *work, const ab2_ls_trial *out, void *stream);
+
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
  * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
