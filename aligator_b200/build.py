@@ -50,7 +50,7 @@ def build(verbose=False, force=False, ptxas_v=False):
     hdrs.append(os.path.join(PKG, "..", "include", "aligator_b200", "gar.h"))
     hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
                                                           "lq_assemble.h", "lq_adjoint.h", "lq_tangent.h", "lq_resolve.h",
-                                                          "lq_resolve.cuh", "lq_jacobian.h", "kkt_error.h",
+                                                          "lq_resolve.cuh", "lq_jacobian.h", "lq_refine.h", "kkt_error.h",
                                                           "linesearch.h", "proxddp_inner.h")]
     extra = ["-Xptxas", "-v"] if ptxas_v else []
     jobs = []
@@ -90,6 +90,11 @@ def build(verbose=False, force=False, ptxas_v=False):
     obj = os.path.join(OBJ, "jacobian_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_jacobian.h",
                                                                                        "lq_record.cuh")]
                                                       + [src], str(extra)))
+    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
+    src = os.path.join(CSRC, "lq_refine.cu")
+    obj = os.path.join(OBJ, "refine_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_refine.h",
+                                                                                     "lq_record.cuh")]
+                                                    + [src], str(extra)))
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "linesearch.cu")
     obj = os.path.join(OBJ, "linesearch_%s.o" % _digest([os.path.join(CSRC, "linesearch.h"), src], str(extra)))

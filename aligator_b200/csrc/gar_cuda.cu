@@ -23,6 +23,7 @@
 #include "lq_tangent.h"
 #include "lq_resolve.h"
 #include "lq_jacobian.h"
+#include "lq_refine.h"
 #include "lq_assemble.h"
 #include "proxddp_inner.h"
 #include "riccati_block_launch.h"
@@ -274,6 +275,9 @@ struct ab2_gar_solver {
   double *mu_dev = nullptr;    // [batch] host-given per-instance mu of the *_v sweeps, staged for the kernels
   double *adj_stage = nullptr, *adj_term = nullptr, *adj_g0 = nullptr; // the adjoint problem of ab2_gar_adjoint
   double *tan_rho = nullptr; // -rho of ab2_gar_tangent, in the cotangent layout (xs, us, vs, vsT, lam0, lams)
+  double *ref_buf = nullptr;   // ab2_gar_refine's residual (rhs layout) and correction (out layout)
+  double *ref_norms = nullptr; // staging of host norms of ab2_gar_refine / refine_many, ref_norms_n doubles
+  size_t ref_norms_n = 0;
   int nth = 0; // parameter dimension of the value function outputs (= nx in leg mode)
   int rec_nth = 0; // parameter blocks carried by the knot records (0 in leg mode)
   int legs = 0;    // >= 2: gar::ParallelRiccatiSolver (leg mode)
@@ -301,6 +305,9 @@ struct ab2_gar_solver {
   int out_knots[AB2_OUT_COUNT] = {};   // knots per instance (1 for per-instance arrays)
   int *status = nullptr, *pivstat = nullptr;
   bool have_problem = false, have_backward = false, have_forward = false;
+  // ab2_gar_refine: the last backward ran on the problem's own vectors (not an adjoint / tangent problem), and the
+  // trajectory outputs hold the primal solution of that factorisation (a forward since)
+  bool primal_factor = false, have_primal = false;
   // ab2_gar_resolve: FB / VXX belong to the current problem (a backward ran after the last set_problem, assemble or
   // cycle_append), and the count of calls that rewrote the factorisation or the records (ab2_gar_factor_epoch)
   bool factor_current = false;
@@ -555,7 +562,8 @@ int ab2_gar_destroy(ab2_gar_solver *s) {
   if (s->pg_done)
     cudaFree(s->pg_done);
   for (double *q : {s->own_stage_sym, s->own_stage, s->own_term, s->own_G0, s->own_g0, s->gains_tmp, s->kkt_tmp, s->theta_dev, s->cond, s->ls_tmp, s->fddp_slack, s->fddp_G0,
-                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev, s->adj_stage, s->adj_term, s->adj_g0, s->tan_rho})
+                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev, s->adj_stage, s->adj_term, s->adj_g0, s->tan_rho,
+                    s->ref_buf, s->ref_norms})
     if (q)
       cudaFree(q);
   for (int i = 0; i < ab2_gar_solver::kPipeStreams; ++i) {
@@ -764,8 +772,10 @@ static int launch(ab2_gar_solver *s, double mueq, const double *mueq_b, int bwd,
     s->vxx_packed = warp_kernel(s);
     s->factor_current = true;
     s->epoch += 1;
+    s->primal_factor = true;
   }
   s->have_forward = fwd != 0; // a backward-only launch invalidates the previous trajectory
+  s->have_primal = fwd != 0 && s->primal_factor;
   return AB2_OK;
 }
 
@@ -902,6 +912,8 @@ static int solve_cotangent_problem(ab2_gar_solver *s, double mueq, const double 
     return rc;
   s->have_backward = true;
   s->have_forward = true;
+  s->primal_factor = false; // the trajectory outputs are w or zdot, not the primal solution
+  s->have_primal = false;
   s->fac_head = 0;
   s->vxx_packed = warp_kernel(s);
   s->factor_current = true;
@@ -1284,6 +1296,223 @@ int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, 
   return tangent_many_impl(s, 0.0, mueq, memspace, nrhs, primal, dot, work, out, stream);
 }
 
+// ---- iterative refinement (lq_refine.cu): residual, resolve and update per step, on the last backward's factorisation ----
+static const char *const kRhsNames[6] = {"q", "r", "d", "dN", "g0", "f"};
+// fields in resolve's rhs layouts (the same sizes as the solution's), `blocks` instances
+static Fields rhs_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
+  Fields f = sol_fields(s, what, p, blocks);
+  f.names = kRhsNames;
+  return f;
+}
+static bool device_accessible(const void *p) {
+  cudaPointerAttributes at{};
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+    cudaGetLastError(); // a plain host pointer on an old runtime: not an error of this call
+    return false;
+  }
+  return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+}
+// `steps` refinement steps of z against h (own: the problem's own vectors; else rhs), [nrhs][batch][...]; r (in the
+// rhs layouts, named like the solution's fields) and dz are the scratch of the residual and the correction.  norms:
+// [nrhs][batch][steps + 1] in device or host memory, or null.  The arguments have been checked.
+static int run_refine(ab2_gar_solver *s, double mueq, const double *mu_dev, int nrhs, int steps, bool own,
+                      const ab2_lq_rhs *rhs, const ab2_ls_trial *z, const ab2_ls_trial *r, const ab2_ls_trial *dz,
+                      double *norms, cudaStream_t st) {
+  const ab2_gar_dims &d = s->d;
+  const int B = d.batch, N = d.horizon;
+  const size_t R = (size_t)nrhs * B, nnorm = R * (size_t)(steps + 1);
+  double *ndev = nullptr;
+  if (norms) {
+    if (device_accessible(norms)) {
+      ndev = norms;
+    } else {
+      if (s->ref_norms_n < nnorm) {
+        if (s->ref_norms)
+          CUDA_TRY(cudaFree(s->ref_norms));
+        s->ref_norms = nullptr;
+        s->ref_norms_n = 0;
+        CUDA_TRY(cudaMalloc(&s->ref_norms, nnorm * sizeof(double)));
+        s->ref_norms_n = nnorm;
+      }
+      ndev = s->ref_norms;
+    }
+    CUDA_TRY(cudaMemsetAsync(ndev, 0, nnorm * sizeof(double), st)); // the maxima meet by atomicMax from 0
+  }
+  const ab2::AdjointDims ad{B, N, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  auto residual = [&](int col, bool write) -> int {
+    ab2::RefineResidualArgs a{};
+    a.d = ad;
+    a.nrhs = nrhs;
+    a.stage_head = s->p.stage_head;
+    a.stage = s->p.stage;
+    a.term = s->p.term;
+    a.G0 = s->p.G0;
+    a.g0 = s->p.g0;
+    a.mueq = mueq;
+    a.mueq_b = mu_dev;
+    a.own = own;
+    if (!own) {
+      a.hq = rhs->q;
+      a.hr = rhs->r;
+      a.hd = rhs->d;
+      a.hdN = rhs->dN;
+      a.hg0 = rhs->g0;
+      a.hf = rhs->f;
+    }
+    a.xs = z->xs;
+    a.us = z->us;
+    a.vs = z->vs;
+    a.vsT = z->vsT;
+    a.lam0 = z->lam0;
+    a.lams = z->lams;
+    if (write) {
+      a.q = r->xs;
+      a.r = r->us;
+      a.dv = r->vs;
+      a.dN = r->vsT;
+      a.g0out = r->lam0;
+      a.f = r->lams;
+    }
+    a.norms = ndev;
+    a.nstride = steps + 1;
+    a.col = col;
+    CUDA_TRY(ab2::launch_refine_residual(a, st));
+    s->launches += 1;
+    return AB2_OK;
+  };
+  const size_t no[6] = {R * (N + 1) * d.nx, R * N * d.nu, R * N * d.nc, R * d.nct, R * d.nc0, R * N * d.nx};
+  const ab2_lq_rhs rr{r->xs, r->us, r->vs, r->vsT, r->lam0, r->lams};
+  for (int k = 0; k < steps; ++k) {
+    if (int rc = residual(k, true)) // r = K z + h
+      return rc;
+    if (int rc = run_resolve(s, mueq, mu_dev, nrhs, &rr, dz, st)) // dz = -K^-1 r
+      return rc;
+    ab2::RefineUpdateArgs u{{z->xs, z->us, z->vs, z->vsT, z->lam0, z->lams},
+                            {dz->xs, dz->us, dz->vs, dz->vsT, dz->lam0, dz->lams},
+                            {(long)no[0], (long)no[1], (long)no[2], (long)no[3], (long)no[4], (long)no[5]}};
+    CUDA_TRY(ab2::launch_refine_update(u, st)); // z += dz
+    s->launches += 1;
+  }
+  if (ndev) {
+    if (int rc = residual(steps, false)) // the last column: the norm of the refined iterate
+      return rc;
+    if (ndev != norms)
+      CUDA_TRY(cudaMemcpyAsync(norms, ndev, nnorm * sizeof(double), cudaMemcpyDeviceToHost, st));
+  }
+  return AB2_OK;
+}
+
+// The checks every refinement call shares after the handle's: steps, mu, shared memory.
+static int check_refine_args(const ab2_gar_solver *s, double mueq, const double *mueq_arr, int steps, const char *who) {
+  if (steps < 0)
+    return fail(AB2_ERR_INVALID, std::string(who) + ": steps < 0");
+  if (!mueq_arr && !(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  return check_resolve_fits(s, who);
+}
+
+static int refine_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int steps, double *norms,
+                       void *stream) {
+  const char *who = "refine";
+  if (!s)
+    return fail(AB2_ERR_INVALID, "null solver");
+  if (int rc = check_resolve_handle(s, 1, who))
+    return rc;
+  if (!s->have_primal)
+    return fail(AB2_ERR_STATE, std::string(who) + ": the trajectory outputs do not hold the primal solution of the last "
+                                                  "backward (no forward since, or an adjoint or tangent call)");
+  if (int rc = check_refine_args(s, mueq, mueq_arr, steps, who))
+    return rc;
+  if (steps == 0 && !norms)
+    return AB2_OK;
+  const ab2_gar_dims &d = s->d;
+  const int B = d.batch, N = d.horizon, nx = d.nx;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  const size_t nxs = (size_t)B * (N + 1) * nx, nus = (size_t)B * N * d.nu, nvs = (size_t)B * N * d.nc,
+               nvT = (size_t)B * d.nct, nl0 = (size_t)B * d.nc0, nls = (size_t)B * N * nx,
+               one = nxs + nus + nvs + nvT + nl0 + nls;
+  if (!s->ref_buf)
+    CUDA_TRY(cudaMalloc(&s->ref_buf, (2 * one + 1) * sizeof(double)));
+  auto split = [&](double *p) {
+    ab2_ls_trial t;
+    t.xs = p;
+    t.us = t.xs + nxs;
+    t.vs = t.us + nus;
+    t.vsT = t.vs + nvs;
+    t.lam0 = t.vsT + nvT;
+    t.lams = t.lam0 + nl0;
+    return t;
+  };
+  const ab2_ls_trial r = split(s->ref_buf), dz = split(s->ref_buf + one);
+  const ab2_ls_trial z{s->out[AB2_OUT_XS], s->out[AB2_OUT_US], s->out[AB2_OUT_VS], s->out[AB2_OUT_VST],
+                       s->out[AB2_OUT_LBD0], s->out[AB2_OUT_LBDAS]};
+  return run_refine(s, mueq, mu_dev, 1, steps, true, nullptr, &z, &r, &dz, norms, st);
+}
+int ab2_gar_refine(ab2_gar_solver *s, double mueq, int steps, double *norms, void *stream) {
+  return refine_impl(s, mueq, nullptr, AB2_DEVICE, steps, norms, stream);
+}
+int ab2_gar_refine_v(ab2_gar_solver *s, const double *mueq, int memspace, int steps, double *norms, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return refine_impl(s, 0.0, mueq, memspace, steps, norms, stream);
+}
+
+static int refine_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int nrhs, int steps,
+                            const ab2_lq_rhs *rhs, const ab2_ls_trial *z, const ab2_lq_refine_work *work,
+                            double *norms, void *stream) {
+  const char *who = "refine_many";
+  if (!s || !rhs || !z || !work)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_resolve_handle(s, nrhs, who))
+    return rc;
+  const size_t R = (size_t)nrhs * s->d.batch;
+  const double *ph[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
+  const double *pz[6] = {z->xs, z->us, z->vs, z->vsT, z->lam0, z->lams};
+  const double *pr[6] = {work->q, work->r, work->d, work->dN, work->g0, work->f};
+  const double *pd[6] = {work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
+  const Fields H = rhs_fields(s, "rhs", ph, R), Z = sol_fields(s, "z", pz, R), WR = rhs_fields(s, "work", pr, R),
+               WD = sol_fields(s, "work", pd, R);
+  for (const Fields *f : {&Z, &WR, &WD})
+    if (int rc = require(*f, who))
+      return rc;
+  if (int rc = check_refine_args(s, mueq, mueq_arr, steps, who))
+    return rc;
+  // the residual reads rhs and z and writes work's residual; resolve reads that and writes work's correction; the
+  // update reads the correction and writes z, which the next residual reads together with rhs
+  for (const FieldPair &ab : {FieldPair{&H, &Z}, FieldPair{&H, &WR}, FieldPair{&H, &WD}, FieldPair{&Z, &Z},
+                              FieldPair{&Z, &WR}, FieldPair{&Z, &WD}, FieldPair{&WR, &WR}, FieldPair{&WR, &WD},
+                              FieldPair{&WD, &WD}})
+    if (int rc = refuse_overlap(*ab.first, *ab.second, who))
+      return rc;
+  if (nrhs == 0 || (steps == 0 && !norms))
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(s->d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  const ab2_ls_trial r{work->q, work->r, work->d, work->dN, work->g0, work->f};
+  const ab2_ls_trial dz{work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
+  return run_refine(s, mueq, mu_dev, nrhs, steps, false, rhs, z, &r, &dz, norms, st);
+}
+int ab2_gar_refine_many(ab2_gar_solver *s, double mueq, int nrhs, int steps, const ab2_lq_rhs *rhs,
+                        const ab2_ls_trial *z, const ab2_lq_refine_work *work, double *norms, void *stream) {
+  return refine_many_impl(s, mueq, nullptr, AB2_DEVICE, nrhs, steps, rhs, z, work, norms, stream);
+}
+int ab2_gar_refine_many_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs, int steps,
+                          const ab2_lq_rhs *rhs, const ab2_ls_trial *z, const ab2_lq_refine_work *work, double *norms,
+                          void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return refine_many_impl(s, 0.0, mueq, memspace, nrhs, steps, rhs, z, work, norms, stream);
+}
+
 static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg_b, const double *mu_inv_b,
                          void *stream) {
   if (!s || !in)
@@ -1626,6 +1855,8 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
   }
   s->have_backward = true;
   s->have_forward = true;
+  s->primal_factor = true;
+  s->have_primal = true;
   s->fac_head = 0;
   s->vxx_packed = warp_kernel(s);
   s->factor_current = true;
@@ -2167,6 +2398,7 @@ int ab2_gar_cycle_append(ab2_gar_solver *s, const double *new_last, int memspace
   CUDA_TRY(cudaGetLastError());
   s->have_backward = false;
   s->have_forward = false;
+  s->have_primal = false;
   s->factor_current = false;
   s->epoch += 1;
   return AB2_OK;

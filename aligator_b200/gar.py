@@ -74,6 +74,12 @@ class LqRhs(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _RHS_KEYS]
 
 
+class LqRefineWork(C.Structure):
+    """``ab2_lq_refine_work``: caller-owned scratch of ``ab2_gar_refine_many``, the residual in resolve's rhs layouts
+    (q .. f) and the correction in the solution's layouts (xs .. lams)."""
+    _fields_ = [(k, C.c_void_p) for k in _RHS_KEYS + _LS_KEYS]
+
+
 _MULT_IN = ("xs", "lam0", "lams", "vs", "vsT", "prev_vs", "prev_vsT", "init_value", "xnext", "fs", "cval", "cval_N",
             "lo", "hi", "loN", "hiN")
 _MULT_OUT = ("slack", "lam0_plus", "lams_plus", "vs_plus", "vsT_plus", "shifted", "shifted_N", "Lv", "Lv_N")
@@ -203,6 +209,12 @@ def lib():
         L.ab2_gar_tangent_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LsIterate),
                                              C.POINTER(LqTangent), C.POINTER(LsIterate), C.POINTER(LsIterate),
                                              C.c_void_p]
+        L.ab2_gar_refine.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p]
+        L.ab2_gar_refine_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        L.ab2_gar_refine_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int, C.POINTER(LqRhs),
+                                          C.POINTER(LsIterate), C.POINTER(LqRefineWork), C.c_void_p, C.c_void_p]
+        L.ab2_gar_refine_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(LqRhs),
+                                            C.POINTER(LsIterate), C.POINTER(LqRefineWork), C.c_void_p, C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -737,6 +749,50 @@ class CudaRiccatiBatch:
         else:
             _check(lib().ab2_gar_tangent_many_v(self.h, v[0], v[1], int(nrhs), C.byref(pr), C.byref(dt), C.byref(wk),
                                                 C.byref(ot), C.c_void_p(stream)))
+
+    def refine(self, mueq, steps=1, norms=False, stream=0):
+        """Iterative refinement of the handle's own trajectory outputs (OUT_XS .. OUT_LBDAS) against the current
+        problem (``ab2_gar_refine``): ``steps`` times r = K z + h, z += resolve(r), on the last backward's
+        factorisation.  Every other output is unchanged.  ``mueq``: the mu of the last backward, a number or a [batch]
+        array / tensor (``ab2_gar_refine_v``).  With ``norms=True`` returns the [batch][steps + 1] infinity norms of the
+        residual of the input iterate and of each refined iterate (numpy; the call then synchronises ``stream``)."""
+        v = self._mueq_arg(mueq, stream)
+        out = np.empty((self.dims.batch, steps + 1), dtype=np.float64) if norms else None
+        if v is None:
+            _check(lib().ab2_gar_refine(self.h, C.c_double(mueq), int(steps), _ptr(out), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_refine_v(self.h, v[0], v[1], int(steps), _ptr(out), C.c_void_p(stream)))
+        if out is not None:
+            self.synchronize(stream)
+        return out
+
+    def refine_many(self, rhs, z, work, mueq, steps=1, norms=None, stream=0):
+        """Iterative refinement of many resolve solutions at once (``ab2_gar_refine_many``): ``z`` (dict with keys xs,
+        us, vs, vsT, lam0, lams of device tensors [nrhs][batch][...], e.g. ``resolve``'s ``out``) is refined in place
+        towards -K^-1 h for the right-hand sides ``rhs`` (dict with any of q, r, d, dN, g0, f as for ``resolve``; a key
+        that is missing or None is zero).  ``work``: dict with keys q, r, d, dN, g0, f (the last residual) and xs .. lams
+        (the last correction) of device tensors [nrhs][batch][...].  nrhs is read from ``z["xs"]``.  ``mueq``: the mu of
+        the last backward, a number or a [batch] array / tensor (``ab2_gar_refine_many_v``).  ``norms``: None (not
+        written), True (returns a host [nrhs][batch][steps + 1] array after synchronising ``stream``) or a device
+        tensor of that shape, written in stream order and returned."""
+        d = self.dims
+        nrhs = z["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
+        v = self._mueq_arg(mueq, stream)
+        rh = _fill(LqRhs(), _RHS_KEYS, rhs)
+        zz = _fill(LsIterate(), _LS_KEYS, z)
+        wk = _fill(LqRefineWork(), _RHS_KEYS + _LS_KEYS, work)
+        host = norms is True
+        out = np.empty((nrhs, d.batch, steps + 1), dtype=np.float64) if host else norms
+        self._keep_ref_many = (rhs, z, work, out)
+        if v is None:
+            _check(lib().ab2_gar_refine_many(self.h, C.c_double(mueq), int(nrhs), int(steps), C.byref(rh), C.byref(zz),
+                                             C.byref(wk), _ptr(out), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_refine_many_v(self.h, v[0], v[1], int(nrhs), int(steps), C.byref(rh), C.byref(zz),
+                                               C.byref(wk), _ptr(out), C.c_void_p(stream)))
+        if host:
+            self.synchronize(stream)
+        return out
 
     def factor_epoch(self):
         """``ab2_gar_factor_epoch``: bumped by every call that rewrites the factorisation or the records."""

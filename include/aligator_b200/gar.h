@@ -524,6 +524,60 @@ int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, 
                            const ab2_ls_iterate *primal, const ab2_lq_tangent *dot,
                            const ab2_ls_trial *work, const ab2_ls_trial *out, void *stream);
 
+/* Iterative refinement of the LQ solution on the last backward's factorisation (what ParallelRiccatiSolver does to its
+ * condensed system, parallel-solver.hxx:185-202, here for the whole serial solve).  At small penalties (mu = 1e-8 and
+ * below) the fp64 recursion loses digits to the conditioning of the stage KKT systems; a step or two of refinement
+ * with resolve as the correction solver recovers them.  For a solution estimate z = (x, u, v, lam) of K z = -h:
+ *   residual    r = K z + h,   correction  delta = resolve(r) = -K^-1 r,   update  z <- z + delta.
+ * With lam_{t+1} = lams[t] and lam_t = lams[t-1], the rows of r in resolve's rhs layouts are
+ *   q-row  Q x_t + S u_t + C^T v_t + A^T lam_{t+1} - lam_t + q_t     (t = 0: + G0^T lam_0 instead of - lam_0)
+ *   r-row  S^T x_t + R u_t + D^T v_t + B^T lam_{t+1} + r_t
+ *   d-row  C x_t + D u_t - mu v_t + d_t
+ *   f-row  A x_t + B u_t - x_{t+1} + f_t                             (in the row of lam_{t+1})
+ *   q_N    Q_N x_N + C_N^T v_N - lam_N + q_N  (N = 0: + G0^T lam_0 instead of - lam_N),   d_N  C_N x_N - mu v_N + d_N
+ *   g0     G0 x_0 + g0
+ * with Q and R used as stored.  These are the rows ab2_gar_kkt_error takes norms of, so ||r||_inf equals the largest
+ * of its three norms up to rounding.  h is the problem's own vectors (ab2_gar_refine: the primal solution) or a
+ * caller's resolve right-hand sides (ab2_gar_refine_many: the adjoint's w with h = -zbar, the tangent with h = rho,
+ * Jacobian columns, any resolve output).
+ *
+ * ab2_gar_refine / _v refine the handle's own trajectory outputs (XS, US, VS, VST, LBD0, LBDAS) in place against the
+ * current problem's vectors.  Every other output (FF, FB, VXX, VX, FFT, FBT, KKT0, status, pivot statistics) is
+ * bit-identical afterwards and ab2_gar_factor_epoch does not move.  The residual and correction live in a buffer the
+ * handle owns, allocated on the first call.
+ * ab2_gar_refine_many / _v refine z ([nrhs][batch][...] in the solution's layouts) in place against the right-hand
+ * sides rhs ([nrhs][batch][...] in resolve's rhs layouts; a NULL field is zero).  `work` is caller-owned: q .. f in
+ * resolve's rhs layouts for the residual, xs .. lams in the solution's layouts for the correction, all [nrhs][batch]
+ * [...] on the device.  After a call with steps >= 1 it holds the last residual (of the iterate before the last
+ * update) and the last correction.  Right-hand side j's result is bit for bit independent of nrhs and of j's position.
+ * norms (optional, NULL = not written): [nrhs][batch][steps + 1] doubles (nrhs = 1 for ab2_gar_refine) in device or
+ * host memory: ||r||_inf of the input iterate and of each refined iterate.  A host array is written by a stream-ordered
+ * copy from a buffer the handle owns (allocated when a larger one is first needed): read it after synchronising
+ * `stream`.  steps = 0 computes only the first column and changes nothing else; steps = 0 without norms does nothing.
+ * Launches, in order on `stream` without host synchronisation: per step a residual kernel, resolve's program and an
+ * update kernel; with norms, one more residual launch at the end for the last column.
+ * `mueq` must be the mu of the last backward; the _v twins take a per-instance mu as ab2_gar_resolve_v does.
+ * Errors (nothing is launched): AB2_ERR_UNSUPPORTED for dense, parametric (nth > 0) and parallel handles;
+ * AB2_ERR_STATE when no backward has run since the last set_problem, assemble or cycle_append, and for ab2_gar_refine
+ * also when the trajectory outputs do not hold the primal solution of that factorisation (no forward since the last
+ * backward, a backward alone, or an ab2_gar_adjoint / ab2_gar_tangent call since the last forward); AB2_ERR_INVALID for
+ * steps < 0, nrhs < 0, a NULL z or work field of nonzero size, mueq <= 0 with constraints, or an overlap that would let
+ * a launch read what an earlier launch of the same step wrote: rhs with z or work, z with itself or work, the two
+ * halves of work with each other or themselves.  nrhs == 0 launches and writes nothing. */
+typedef struct ab2_lq_refine_work {
+  double *q, *r, *d, *dN, *g0, *f;          /* residual, resolve's rhs layouts   */
+  double *xs, *us, *vs, *vsT, *lam0, *lams; /* correction, the solution's layouts */
+} ab2_lq_refine_work;
+int ab2_gar_refine  (ab2_gar_solver *s, double mueq, int steps, double *norms, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_refine_v(ab2_gar_solver *s, const double *mueq, int memspace, int steps, double *norms, void *stream);
+int ab2_gar_refine_many  (ab2_gar_solver *s, double mueq, int nrhs, int steps, const ab2_lq_rhs *rhs,
+                          const ab2_ls_trial *z, const ab2_lq_refine_work *work, double *norms, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_refine_many_v(ab2_gar_solver *s, const double *mueq, int memspace, int nrhs, int steps,
+                          const ab2_lq_rhs *rhs, const ab2_ls_trial *z, const ab2_lq_refine_work *work,
+                          double *norms, void *stream);
+
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
  * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
