@@ -20,6 +20,11 @@ tangents, the V cotangents or tangents go to the device in one call on one facto
 gradients and jvps are those of one ``adjoint`` or ``tangent`` call.  vmap over the problem data itself raises
 ``NotImplementedError``.
 
+:func:`lq_factor` returns the factorisation of the backward pass -- gains ``ff``, ``fb`` and cost-to-go ``vxx``, ``vx``,
+``fft``, ``fbt`` -- differentiable with respect to ``stage`` and ``term`` by one reverse pass of the matrix recursion
+on the device (``ab2_gar_factor_adjoint``).  Reverse mode only (``jacrev`` works, one device call per cotangent);
+G0 and g0 do not enter the factorisation.
+
 :func:`lq_resolve` re-solves the matrices of the handle's last backward for new vectors (``ab2_gar_resolve``), many
 right-hand sides in one call.  It is linear in the vectors and its own transpose, so its ``backward`` and ``jvp`` are
 ``lq_resolve`` calls again, and it has a vmap rule: ``torch.func.vmap``, ``jacrev``, ``jacfwd`` and higher orders work
@@ -341,3 +346,118 @@ def lq_resolve(batch, mueq, q=None, r=None, d=None, dN=None, g0=None, f=None):
     flat = [None if t is None else t.expand(*lead, *shapes[k]).reshape(nrhs, *shapes[k]) for k, t in h.items()]
     outs = _LqResolve.apply(batch, mueq, batch.factor_epoch(), *flat)
     return tuple(o.reshape(*lead, *o.shape[1:]) for o in outs)
+
+
+_FOUTS = (_gar.OUT_FF, _gar.OUT_FB, _gar.OUT_VXX, _gar.OUT_VX, _gar.OUT_FFT, _gar.OUT_FBT)
+_FKEYS = ("ff", "fb", "vxx", "vx", "fft", "fbt")
+_NO_FACTOR_DATA_VMAP = ("lq_factor: vmap over the problem data (stage, term, G0, g0, mueq) is not supported; vmap "
+                        "over cotangents is (torch.func.jacrev, vmap of a vjp function)")
+_NO_FACTOR_JVP = ("lq_factor: forward mode of the gains is not supported (torch.func.jvp, jacfwd, forward_ad); use "
+                  "reverse mode (backward, torch.func.vjp, jacrev)")
+
+
+def _factor_cotangent(gouts):
+    """Cotangents of lq_factor's outputs -> device layouts: vxx back to column-major blocks."""
+    cot = {}
+    for k, g in zip(_FKEYS, gouts):
+        if g is not None:
+            g = g.to(torch.float64)
+            if k == "vxx":
+                g = g.transpose(-1, -2)
+            g = g.contiguous()
+        cot[k] = g
+    return cot
+
+
+class _LqFactor(torch.autograd.Function):
+    @staticmethod
+    def forward(batch, stage, term, G0, g0, mueq):
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        batch.backward(mueq, stream=stream)
+        outs = []
+        for w in _FOUTS:
+            t = torch.empty(batch.out_shape(w), dtype=torch.float64, device=stage.device)
+            if t.numel():
+                batch.get_into(w, t, _gar.AB2_DEVICE, stream=stream)
+            outs.append(t.transpose(-1, -2).contiguous() if w == _gar.OUT_VXX else t)  # VXX blocks are column-major
+        return tuple(outs)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        batch, stage, term, G0, g0, mueq = inputs
+        ctx.batch, ctx.mueq = batch, mueq
+        ctx.save_for_backward(stage, term, G0, g0)
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *gouts):
+        stage, term, G0, g0 = ctx.saved_tensors
+        need = tuple(ctx.needs_input_grad[1:3])
+        if not any(need) or all(g is None for g in gouts):
+            return (None,) * 6
+        grads = iter(_LqFactorVjp.apply(ctx.batch, ctx.mueq, need, stage, term, G0, g0, *gouts))
+        return (None,) + tuple(next(grads) if n else None for n in need) + (None,) * 3
+
+    @staticmethod
+    def jvp(ctx, *_):
+        raise NotImplementedError(_NO_FACTOR_JVP)
+
+    @staticmethod
+    def vmap(info, in_dims, batch, stage, term, G0, g0, mueq):
+        raise NotImplementedError(_NO_FACTOR_DATA_VMAP)
+
+
+class _LqFactorVjp(torch.autograd.Function):
+    """Gradient records (stage, term) of ``lq_factor`` for the cotangents ``gouts`` of its outputs: a backward, then one
+    ``factor_adjoint`` call, or under vmap one ``factor_adjoint`` call per cotangent on that backward."""
+
+    @staticmethod
+    def forward(batch, mueq, need, stage, term, G0, g0, *gouts):
+        stage, term, G0, g0 = [_plain(t) for t in (stage, term, G0, g0)]
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        grads = {k: torch.empty_like(t) for (k, t), n in zip((("stage", stage), ("term", term)), need) if n}
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        batch.backward(mueq, stream=stream)
+        batch.factor_adjoint(_factor_cotangent(gouts), grads, mueq, stream=stream)
+        return tuple(grads.values())
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *_):
+        raise RuntimeError("lq_factor is differentiable once: its gradients have no derivatives")
+
+    @staticmethod
+    def vmap(info, in_dims, batch, mueq, need, stage, term, G0, g0, *gouts):
+        if any(d is not None for d in (in_dims[1],) + in_dims[3:7]):  # in_dims[2]: `need`, not a tensor
+            raise NotImplementedError(_NO_FACTOR_DATA_VMAP)
+        V = info.batch_size
+        stage, term, G0, g0 = [_plain(t) for t in (stage, term, G0, g0)]
+        cot = [_stacked(g, bd, V) for g, bd in zip(gouts, in_dims[7:])]
+        grads = {k: torch.empty((V,) + t.shape, dtype=torch.float64, device=stage.device)
+                 for (k, t), n in zip((("stage", stage), ("term", term)), need) if n}
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        batch.backward(mueq, stream=stream)
+        for j in range(V):
+            batch.factor_adjoint(_factor_cotangent([None if c is None else c[j] for c in cot]),
+                                 {k: g[j] for k, g in grads.items()}, mueq, stream=stream)
+        return tuple(grads.values()), 0
+
+
+def lq_factor(batch, stage, term, G0, g0, mueq):
+    """Run the backward pass of the batch's LQ problems on ``torch.cuda.current_stream()``; returns the factorisation
+    ``(ff, fb, vxx, vx, fft, fbt)``: ff [batch][N][nu+nc+nx] = [k; z; a], fb [batch][N][nu+nc+nx][nx] = [K; Z; Ahat],
+    vxx [batch][N+1][nx][nx] (indexed [b, t, i, j]), vx [batch][N+1][nx], fft [batch][nct] = z_N and fbt
+    [batch][nct][nx] = Z_N.  Differentiable in reverse mode with respect to ``stage`` and ``term`` (Q and R as
+    symmetric arguments, cotangents of vxx taken through their symmetric part); G0 and g0 do not enter the
+    factorisation and get no gradient.  Each backward re-sets the problem and reruns the backward pass, so losses that
+    mix ``lq_factor`` and ``lq_solve`` outputs of one handle get the summed gradient in any order.  Forward mode raises
+    ``NotImplementedError``.  Raises ``ValueError`` before any library call on a tensor that is not a contiguous float64
+    CUDA tensor of the handle's shape."""
+    _check_inputs(batch, dict(stage=stage, term=term, G0=G0, g0=g0))
+    return _LqFactor.apply(batch, stage, term, G0, g0, mueq)

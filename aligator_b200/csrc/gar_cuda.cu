@@ -22,6 +22,7 @@
 #include "lq_adjoint.h"
 #include "lq_tangent.h"
 #include "lq_resolve.h"
+#include "lq_factor_adjoint.h"
 #include "lq_jacobian.h"
 #include "lq_refine.h"
 #include "lq_assemble.h"
@@ -1022,10 +1023,8 @@ static int check_resolve_fits(const ab2_gar_solver *s, const char *who) {
     return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one right-hand side of this shape does not fit 227 KB of shared memory");
   return AB2_OK;
 }
-// resolve's program on the handle's current factorisation, rhs -> out (one launch).  mu_dev: the staged per-instance
-// mu, or null for the scalar mueq.
-static int run_resolve(ab2_gar_solver *s, double mueq, const double *mu_dev, int nrhs, const ab2_lq_rhs *rhs,
-                       const ab2_ls_trial *out, cudaStream_t st) {
+// The records and the last backward's factorisation as resolve's program reads them (no right-hand sides).
+static ab2::ResolveArgs factor_view(const ab2_gar_solver *s, double mueq, const double *mu_dev) {
   const ab2_gar_dims &d = s->d;
   ab2::ResolveArgs a{};
   a.batch = d.batch;
@@ -1038,7 +1037,6 @@ static int run_resolve(ab2_gar_solver *s, double mueq, const double *mu_dev, int
   a.srec = s->srec;
   a.trec = s->trec;
   a.stage_head = s->p.stage_head;
-  a.nrhs = nrhs;
   a.stage = s->p.stage;
   a.term = s->p.term;
   a.G0 = s->p.G0;
@@ -1048,6 +1046,14 @@ static int run_resolve(ab2_gar_solver *s, double mueq, const double *mu_dev, int
   a.Vxx0 = s->vxx_packed ? s->p.Vxx0 : nullptr;
   a.mueq = mueq;
   a.mueq_b = mu_dev;
+  return a;
+}
+// resolve's program on the handle's current factorisation, rhs -> out (one launch).  mu_dev: the staged per-instance
+// mu, or null for the scalar mueq.
+static int run_resolve(ab2_gar_solver *s, double mueq, const double *mu_dev, int nrhs, const ab2_lq_rhs *rhs,
+                       const ab2_ls_trial *out, cudaStream_t st) {
+  ab2::ResolveArgs a = factor_view(s, mueq, mu_dev);
+  a.nrhs = nrhs;
   a.q = rhs->q;
   a.r = rhs->r;
   a.d = rhs->d;
@@ -1112,6 +1118,74 @@ int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int n
     return fail(AB2_ERR_INVALID, "null mueq array");
   return resolve_impl(s, 0.0, mueq, memspace, nrhs, rhs, out, stream);
 }
+// ---- reverse mode of the backward recursion (lq_factor_adjoint.cu): cotangents of the factorisation -> gradients ----
+static int factor_adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
+                               const ab2_factor_cotangent *cot, const ab2_lq_grad *grad, void *stream) {
+  if (!s || !cot || !grad)
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_resolve_handle(s, 0, "factor_adjoint"))
+    return rc;
+  if (!s->primal_factor)
+    return fail(AB2_ERR_STATE, "factor_adjoint: FF and VX hold an adjoint or tangent solve; run a backward first");
+  const ab2_gar_dims &d = s->d;
+  const size_t B = d.batch, N = d.horizon, nx = d.nx, nr = d.nu + d.nc + d.nx;
+  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  // the gradients are written knot by knot while later knots' cotangents and factors are still to be read
+  const double *pc[6] = {cot->ff, cot->fb, cot->vxx, cot->vx, cot->fft, cot->fbt};
+  const size_t nc[6] = {B * N * nr, B * N * nr * nx, B * (N + 1) * nx * nx, B * (N + 1) * nx, B * d.nct,
+                        B * d.nct * nx};
+  double *const pg[4] = {grad->stage, grad->term, grad->G0, grad->g0};
+  const size_t ng[4] = {B * N * s->srec, B * s->trec, B * d.nc0 * nx, B * d.nc0};
+  static const char *gnames[4] = {"stage", "term", "G0", "g0"};
+  for (int i = 0; i < 4; ++i) {
+    if (!pg[i] || !ng[i])
+      continue;
+    for (int c = 0; c < 6; ++c)
+      if (pc[c] && nc[c] && pg[i] < pc[c] + nc[c] && pc[c] < pg[i] + ng[i])
+        return fail(AB2_ERR_INVALID, std::string("factor_adjoint: grad ") + gnames[i] + " overlaps a cotangent array");
+    for (int w = 0; w < AB2_OUT_COUNT; ++w)
+      if (s->out[w] && pg[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pg[i] + ng[i])
+        return fail(AB2_ERR_INVALID, std::string("factor_adjoint: grad ") + gnames[i] + " overlaps an output array of the handle");
+  }
+  if ((size_t)ab2::factor_adjoint_item_doubles(d.nx, d.nu, d.nc) * sizeof(double) > ab2::kFactorAdjointSmemMax)
+    return fail(AB2_ERR_UNSUPPORTED, "factor_adjoint: one instance of this shape does not fit 227 KB of shared memory");
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  ab2::FactorAdjointArgs a{};
+  a.fac = factor_view(s, mueq, mu_dev);
+  a.ff = s->out[AB2_OUT_FF];
+  a.vx = s->out[AB2_OUT_VX];
+  a.ffT = s->out[AB2_OUT_FFT];
+  a.c_ff = cot->ff;
+  a.c_fb = cot->fb;
+  a.c_vxx = cot->vxx;
+  a.c_vx = cot->vx;
+  a.c_fft = cot->fft;
+  a.c_fbt = cot->fbt;
+  a.g_stage = grad->stage;
+  a.g_term = grad->term;
+  a.g_G0 = grad->G0;
+  a.g_g0 = grad->g0;
+  CUDA_TRY(ab2::launch_factor_adjoint(a, st));
+  s->launches += 1;
+  return AB2_OK;
+}
+int ab2_gar_factor_adjoint(ab2_gar_solver *s, double mueq, const ab2_factor_cotangent *cot, const ab2_lq_grad *grad,
+                           void *stream) {
+  return factor_adjoint_impl(s, mueq, nullptr, AB2_DEVICE, cot, grad, stream);
+}
+int ab2_gar_factor_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace, const ab2_factor_cotangent *cot,
+                             const ab2_lq_grad *grad, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return factor_adjoint_impl(s, 0.0, mueq, memspace, cot, grad, stream);
+}
+
 int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch) {
   if (!s || !epoch)
     return fail(AB2_ERR_INVALID, "null argument");

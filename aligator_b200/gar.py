@@ -74,6 +74,15 @@ class LqRhs(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _RHS_KEYS]
 
 
+_FCOT_KEYS = ("ff", "fb", "vxx", "vx", "fft", "fbt")
+
+
+class FactorCotangent(C.Structure):
+    """``ab2_factor_cotangent``: device cotangents of ``ab2_gar_factor_adjoint`` (NULL = zero), in ``ab2_gar_get``'s
+    layouts."""
+    _fields_ = [(k, C.c_void_p) for k in _FCOT_KEYS]
+
+
 class LqRefineWork(C.Structure):
     """``ab2_lq_refine_work``: caller-owned scratch of ``ab2_gar_refine_many``, the residual in resolve's rhs layouts
     (q .. f) and the correction in the solution's layouts (xs .. lams)."""
@@ -215,6 +224,10 @@ def lib():
                                           C.POINTER(LsIterate), C.POINTER(LqRefineWork), C.c_void_p, C.c_void_p]
         L.ab2_gar_refine_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(LqRhs),
                                             C.POINTER(LsIterate), C.POINTER(LqRefineWork), C.c_void_p, C.c_void_p]
+        L.ab2_gar_factor_adjoint.argtypes = [C.c_void_p, C.c_double, C.POINTER(FactorCotangent), C.POINTER(LqGrad),
+                                             C.c_void_p]
+        L.ab2_gar_factor_adjoint_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(FactorCotangent),
+                                               C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -793,6 +806,23 @@ class CudaRiccatiBatch:
         if host:
             self.synchronize(stream)
         return out
+
+    def factor_adjoint(self, cotangent, grad, mueq, stream=0):
+        """Gradients of the factorisation (``ab2_gar_factor_adjoint``): ``grad`` receives the gradient records of a loss
+        whose cotangents with respect to the last backward's outputs are ``cotangent``, a dict with any of ff, fb, vxx,
+        vx, fft, fbt of device tensors laid out like ``get`` returns OUT_FF .. OUT_FBT (vxx as full blocks; a key that
+        is missing or None is zero).  ``grad``: dict with any of stage, term, G0, g0 of device tensors in the problem's
+        layouts, overwritten (G0 and g0 with zeros; a missing key is not written).  ``mueq``: the mu of the last
+        backward, a number or a [batch] array / tensor (``ab2_gar_factor_adjoint_v``).  Needs a backward on the
+        problem's own vectors since the last set_problem; the handle's outputs are not touched."""
+        v = self._mueq_arg(mueq, stream)
+        ct = _fill(FactorCotangent(), _FCOT_KEYS, cotangent)
+        gr = _fill(LqGrad(), _GRAD_KEYS, grad)
+        self._keep_fadj = (cotangent, grad)
+        if v is None:
+            _check(lib().ab2_gar_factor_adjoint(self.h, C.c_double(mueq), C.byref(ct), C.byref(gr), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_factor_adjoint_v(self.h, v[0], v[1], C.byref(ct), C.byref(gr), C.c_void_p(stream)))
 
     def factor_epoch(self):
         """``ab2_gar_factor_epoch``: bumped by every call that rewrites the factorisation or the records."""

@@ -578,6 +578,55 @@ int ab2_gar_refine_many_v(ab2_gar_solver *s, const double *mueq, int memspace, i
                           const ab2_lq_rhs *rhs, const ab2_ls_trial *z, const ab2_lq_refine_work *work,
                           double *norms, void *stream);
 
+/* Gradients of the factorisation with respect to the problem data: the reverse mode of the backward recursion, for
+ * losses on the gains and the cost-to-go (a feedback law u = k_0 + K_0 x fitted to demonstrations, inverse LQR on
+ * gains, a terminal cost trained against Vxx_0, vx_0).  The backward pass maps the records and mu to, per stage knot,
+ * FF_t = [k; z; a], FB_t = [K; Z; Ahat], Vxx_t, vx_t and, at the terminal knot, FFT = z_N, FBT = Z_N, Vxx_N, vx_N.  For
+ * cotangents of those outputs the call returns the gradient with respect to every record entry, with Q and R as
+ * symmetric arguments (as ab2_gar_adjoint).  Cotangents of Vxx_t are symmetrised, which is exact: Vxx_t is symmetric.
+ * Vxx_t is read only by knot t-1, so the pass runs forward in time, carrying Vbar, vbar (seeded with the Vxx_0, vx_0
+ * cotangents).  Per stage knot, with V' = Vxx_{t+1}, v' = vx_{t+1}, X = [[K, k], [Z, z]], Shat = S + A^T V' B,
+ * v+ = v' + V' f, M = [[R + B^T V' B, D^T], [D, -mu I]] (factored again from its lower triangle, as resolve does),
+ * sym(M) = (M + M^T) / 2 and the caller's cotangents marked 0:
+ *   closed loop  Kb = Kb0 + B^T Ahatb,  kb = kb0 + B^T ab,  Bb = Ahatb K^T + ab k^T,  Ab = Ahatb,  fb = ab
+ *   value        Qb = Vbar,  qb = vbar,  Shatb = Vbar K^T + vbar k^T,  Kb += Shat^T Vbar,  kb += Shat^T vbar,
+ *                Cb = Z Vbar + z vbar^T,  Zb = Zb0 + C Vbar,  zb = zb0 + C vbar
+ *   solve        P = -M^-1 [[Kb, kb], [Zb, zb]];  Shatb += P_u[:, :nx]^T,  rb = P_u[:, nx],  Cb += P_c[:, :nx],
+ *                db = P_c[:, nx],  Rb = sym(P_u X_u^T),  Db = P_c X_u^T + X_c P_u^T  (X_u = [K, k], X_c = [Z, z]),
+ *                Sb = Shatb
+ *   products     Ab += 2 V' A Qb + V' B Shatb^T + v+ qb^T,  Bb += 2 V' B Rb + V' A Shatb + v+ rb^T,
+ *                vb+ = A qb + B rb,  fb += V' vb+
+ *   carry        Vbar_{t+1} = sym(Vxxb0_{t+1}) + sym(A Qb A^T + B Rb B^T + A Shatb B^T + vb+ f^T),  vbar_{t+1} = vxb0_{t+1} + vb+
+ * and at the terminal knot (Z_N = C_N / mu, z_N = d_N / mu):  Zb = Zb0_N + C_N Vbar,  zb = zb0_N + C_N vbar,
+ *   C_Nb = Z_N Vbar + z_N vbar^T + Zb / mu,  d_Nb = zb / mu,  Q_Nb = Vbar,  q_Nb = vbar.
+ * G0 and g0 do not enter the factorisation: a non-NULL G0 / g0 grad field is zero-filled.  mu is not differentiated.
+ *
+ * Layouts (DEVICE arrays): cotangents as ab2_gar_get returns the outputs -- ff [batch][N][nu+nc+nx], fb
+ * [batch][N][(nu+nc+nx)*nx] row-major, vxx [batch][N+1][nx*nx] full column-major blocks (not the packed physical
+ * layout), vx [batch][N+1][nx], fft [batch][nct], fbt [batch][nct*nx]; a NULL field is a zero cotangent.  `grad` has
+ * the problem's layouts (stage records' pad double written as 0) and is overwritten; a NULL field is not written.
+ * One launch on `stream`: one warp per instance, or one CTA per instance when the shape's shared memory leaves room for
+ * no other.  Only the caller's grad arrays are written: every output of the handle, its status, pivot statistics and
+ * ab2_gar_factor_epoch are unchanged, and no memory is allocated (a host mueq array of the _v twin is staged like
+ * ab2_gar_sweep_v's).  Records are read through the ring head, Vxx in the layout the last backward wrote.  The
+ * results are deterministic: every entry is summed by one lane in a fixed order.  `mueq` must be the mu of the last
+ * backward.
+ * Errors (nothing is launched): AB2_ERR_UNSUPPORTED for dense, parametric (nth > 0) and parallel handles, and for a
+ * shape whose item needs more than 227 KB of shared memory (5 nx^2 + 3 nx nu + nc nx + nu^2 + 5 nx +
+ * (nu+nc)(2 nx + nu + nc + 3) doubles; C1-C5 fit);
+ * AB2_ERR_STATE unless a backward on the problem's own vectors has run since the last set_problem, assemble or
+ * cycle_append (after ab2_gar_adjoint or ab2_gar_tangent FF and VX hold that solve's vectors, until the next
+ * backward); AB2_ERR_INVALID for mueq <= 0 with constraints, or a grad array that overlaps a cotangent array or an
+ * output of the handle. */
+typedef struct ab2_factor_cotangent {
+  const double *ff, *fb, *vxx, *vx, *fft, *fbt;
+} ab2_factor_cotangent;
+int ab2_gar_factor_adjoint  (ab2_gar_solver *s, double mueq, const ab2_factor_cotangent *cot,
+                             const ab2_lq_grad *grad, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_factor_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace,
+                             const ab2_factor_cotangent *cot, const ab2_lq_grad *grad, void *stream);
+
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
  * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
