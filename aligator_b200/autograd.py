@@ -23,7 +23,10 @@ gradients and jvps are those of one ``adjoint`` or ``tangent`` call.  vmap over 
 :func:`lq_factor` returns the factorisation of the backward pass -- gains ``ff``, ``fb`` and cost-to-go ``vxx``, ``vx``,
 ``fft``, ``fbt`` -- differentiable with respect to ``stage`` and ``term`` by one reverse pass of the matrix recursion
 on the device (``ab2_gar_factor_adjoint``).  Reverse mode only (``jacrev`` works, one device call per cotangent);
-G0 and g0 do not enter the factorisation.
+G0 and g0 do not enter the factorisation.  :func:`lq_factor_fwd` returns the same outputs, bit for bit,
+differentiable in forward mode instead (``torch.func.jvp``, ``forward_ad``, ``jacfwd``) by one tangent pass of the
+matrix recursion on the device (``ab2_gar_factor_tangent``) per tangent: the cheap direction for the whole gain
+schedule's sensitivity to a few parameters.
 
 :func:`lq_resolve` re-solves the matrices of the handle's last backward for new vectors (``ab2_gar_resolve``), many
 right-hand sides in one call.  It is linear in the vectors and its own transpose, so its ``backward`` and ``jvp`` are
@@ -353,7 +356,7 @@ _FKEYS = ("ff", "fb", "vxx", "vx", "fft", "fbt")
 _NO_FACTOR_DATA_VMAP = ("lq_factor: vmap over the problem data (stage, term, G0, g0, mueq) is not supported; vmap "
                         "over cotangents is (torch.func.jacrev, vmap of a vjp function)")
 _NO_FACTOR_JVP = ("lq_factor: forward mode of the gains is not supported (torch.func.jvp, jacfwd, forward_ad); use "
-                  "reverse mode (backward, torch.func.vjp, jacrev)")
+                  "reverse mode (backward, torch.func.vjp, jacrev), or lq_factor_fwd for forward mode")
 
 
 def _factor_cotangent(gouts):
@@ -369,19 +372,25 @@ def _factor_cotangent(gouts):
     return cot
 
 
+def _factor_outputs(batch, stage, term, G0, g0, mueq):
+    """Set the problem, run the backward pass and copy the factorisation out: the outputs of lq_factor and
+    lq_factor_fwd."""
+    stream = torch.cuda.current_stream(stage.device).cuda_stream
+    batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+    batch.backward(mueq, stream=stream)
+    outs = []
+    for w in _FOUTS:
+        t = torch.empty(batch.out_shape(w), dtype=torch.float64, device=stage.device)
+        if t.numel():
+            batch.get_into(w, t, _gar.AB2_DEVICE, stream=stream)
+        outs.append(t.transpose(-1, -2).contiguous() if w == _gar.OUT_VXX else t)  # VXX blocks are column-major
+    return tuple(outs)
+
+
 class _LqFactor(torch.autograd.Function):
     @staticmethod
     def forward(batch, stage, term, G0, g0, mueq):
-        stream = torch.cuda.current_stream(stage.device).cuda_stream
-        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
-        batch.backward(mueq, stream=stream)
-        outs = []
-        for w in _FOUTS:
-            t = torch.empty(batch.out_shape(w), dtype=torch.float64, device=stage.device)
-            if t.numel():
-                batch.get_into(w, t, _gar.AB2_DEVICE, stream=stream)
-            outs.append(t.transpose(-1, -2).contiguous() if w == _gar.OUT_VXX else t)  # VXX blocks are column-major
-        return tuple(outs)
+        return _factor_outputs(batch, stage, term, G0, g0, mueq)
 
     @staticmethod
     def setup_context(ctx, inputs, output):
@@ -461,3 +470,102 @@ def lq_factor(batch, stage, term, G0, g0, mueq):
     CUDA tensor of the handle's shape."""
     _check_inputs(batch, dict(stage=stage, term=term, G0=G0, g0=g0))
     return _LqFactor.apply(batch, stage, term, G0, g0, mueq)
+
+
+_NO_FACTOR_FWD_DATA_VMAP = ("lq_factor_fwd: vmap over the problem data (stage, term, G0, g0, mueq) is not supported; "
+                            "vmap over tangents is (torch.func.jacfwd, vmap of a jvp function)")
+_NO_FACTOR_FWD_BACKWARD = ("lq_factor_fwd is differentiable in forward mode only (torch.func.jvp, jacfwd, forward_ad); "
+                           "use lq_factor for reverse mode")
+
+
+class _LqFactorFwd(torch.autograd.Function):
+    @staticmethod
+    def forward(batch, stage, term, G0, g0, mueq):
+        return _factor_outputs(batch, stage, term, G0, g0, mueq)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        batch, stage, term, G0, g0, mueq = inputs
+        ctx.batch, ctx.mueq = batch, mueq
+        ctx.save_for_forward(stage, term, G0, g0)
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *_):
+        raise RuntimeError(_NO_FACTOR_FWD_BACKWARD)
+
+    @staticmethod
+    def jvp(ctx, _batch_t, dstage, dterm, _dG0, _dg0, _mueq_t):
+        # G0 and g0 do not enter the factorisation.  The tangents are passed on as they are: under vmap (jacfwd) they
+        # are batched, and _LqFactorTangent's vmap rule takes them.
+        stage, term, G0, g0 = [_plain(t) for t in ctx.saved_tensors]
+        return _LqFactorTangent.apply(ctx.batch, ctx.mueq, stage, term, G0, g0, dstage, dterm)
+
+    @staticmethod
+    def vmap(info, in_dims, batch, stage, term, G0, g0, mueq):
+        # torch runs the forward unbatched when no input is batched (jacfwd); it needs this rule to exist all the same
+        raise NotImplementedError(_NO_FACTOR_FWD_DATA_VMAP)
+
+
+def _factor_tangent_into(batch, mueq, dot, outs, stream):
+    """One factor_tangent call: ``outs`` in lq_factor's shapes (vxx [..][i][j]) receive the tangents along ``dot``."""
+    dev = dict(zip(_FKEYS, outs))
+    vxx = torch.empty_like(dev["vxx"])  # the device writes column-major blocks
+    dev["vxx"] = vxx
+    batch.factor_tangent(dot, {k: t for k, t in dev.items() if t.numel()}, mueq, stream=stream)
+    outs[2].copy_(vxx.transpose(-1, -2))
+
+
+class _LqFactorTangent(torch.autograd.Function):
+    """The derivative of ``lq_factor_fwd``'s outputs along the data tangents ``dstage``, ``dterm``: a backward, then one
+    ``factor_tangent`` call, or under vmap one ``factor_tangent`` call per tangent on that backward."""
+
+    @staticmethod
+    def forward(batch, mueq, stage, term, G0, g0, dstage, dterm):
+        stage, term, G0, g0 = [_plain(t) for t in (stage, term, G0, g0)]
+        dot = {k: None if t is None else _plain(t.to(torch.float64).contiguous())
+               for k, t in (("stage", dstage), ("term", dterm))}
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        outs = [torch.empty(batch.out_shape(w), dtype=torch.float64, device=stage.device) for w in _FOUTS]
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        batch.backward(mueq, stream=stream)
+        _factor_tangent_into(batch, mueq, dot, outs, stream)
+        return tuple(outs)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *_):
+        raise RuntimeError("lq_factor_fwd is differentiable once: its jvps have no derivatives")
+
+    @staticmethod
+    def vmap(info, in_dims, batch, mueq, stage, term, G0, g0, dstage, dterm):
+        if any(d is not None for d in in_dims[2:6]):
+            raise NotImplementedError(_NO_FACTOR_FWD_DATA_VMAP)
+        V = info.batch_size
+        stage, term, G0, g0 = [_plain(t) for t in (stage, term, G0, g0)]
+        dot = {k: _stacked(t, bd, V) for k, t, bd in (("stage", dstage, in_dims[6]), ("term", dterm, in_dims[7]))}
+        stream = torch.cuda.current_stream(stage.device).cuda_stream
+        outs = [torch.empty((V,) + tuple(batch.out_shape(w)), dtype=torch.float64, device=stage.device)
+                for w in _FOUTS]
+        batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        batch.backward(mueq, stream=stream)
+        for j in range(V):
+            _factor_tangent_into(batch, mueq, {k: None if t is None else t[j] for k, t in dot.items()},
+                                 [o[j] for o in outs], stream)
+        return tuple(outs), (0,) * 6
+
+
+def lq_factor_fwd(batch, stage, term, G0, g0, mueq):
+    """:func:`lq_factor`'s outputs, bit for bit, differentiable in FORWARD mode with respect to ``stage`` and ``term``
+    (``torch.func.jvp``, ``torch.autograd.forward_ad``, ``jacfwd``): each jvp re-sets the problem, reruns the backward
+    pass and makes one ``factor_tangent`` call (under ``jacfwd`` one call per tangent on that backward).  The tangent
+    of Q and R enters through its symmetric part; G0 and g0 do not enter the factorisation.  Reverse mode raises
+    ``RuntimeError`` (use :func:`lq_factor`), and vmap over the problem data raises ``NotImplementedError``.  Raises
+    ``ValueError`` before any library call on a tensor that is not a contiguous float64 CUDA tensor of the handle's
+    shape."""
+    _check_inputs(batch, dict(stage=stage, term=term, G0=G0, g0=g0))
+    return _LqFactorFwd.apply(batch, stage, term, G0, g0, mueq)

@@ -51,6 +51,7 @@ def build(verbose=False, force=False, ptxas_v=False):
     hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
                                                           "lq_assemble.h", "lq_adjoint.h", "lq_tangent.h", "lq_resolve.h",
                                                           "lq_resolve.cuh", "lq_factor_adjoint.h", "lq_factor_adjoint.cuh",
+                                                          "lq_factor_tangent.h", "lq_factor_tangent.cuh",
                                                           "lq_jacobian.h", "lq_refine.h", "kkt_error.h",
                                                           "linesearch.h", "proxddp_inner.h")]
     extra = ["-Xptxas", "-v"] if ptxas_v else []
@@ -89,7 +90,13 @@ def build(verbose=False, force=False, ptxas_v=False):
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "lq_factor_adjoint.cu")
     obj = os.path.join(OBJ, "factor_adjoint_%s.o" % _digest([os.path.join(CSRC, f) for f in (
-        "vxx_layout.h", "lq_resolve.cuh", "lq_factor_adjoint.h", "lq_factor_adjoint.cuh")] + [src], str(extra)))
+        "vxx_layout.h", "lq_resolve.cuh", "item_launch.cuh", "lq_factor_adjoint.h", "lq_factor_adjoint.cuh")] + [src],
+        str(extra)))
+    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
+    src = os.path.join(CSRC, "lq_factor_tangent.cu")
+    obj = os.path.join(OBJ, "factor_tangent_%s.o" % _digest([os.path.join(CSRC, f) for f in (
+        "vxx_layout.h", "lq_resolve.cuh", "item_launch.cuh", "lq_factor_tangent.h", "lq_factor_tangent.cuh")] + [src],
+        str(extra)))
     jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
     src = os.path.join(CSRC, "lq_jacobian.cu")
     obj = os.path.join(OBJ, "jacobian_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_jacobian.h",

@@ -23,6 +23,7 @@
 #include "lq_tangent.h"
 #include "lq_resolve.h"
 #include "lq_factor_adjoint.h"
+#include "lq_factor_tangent.h"
 #include "lq_jacobian.h"
 #include "lq_refine.h"
 #include "lq_assemble.h"
@@ -1118,38 +1119,54 @@ int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int n
     return fail(AB2_ERR_INVALID, "null mueq array");
   return resolve_impl(s, 0.0, mueq, memspace, nrhs, rhs, out, stream);
 }
+// ---- derivatives of the backward recursion (lq_factor_adjoint.cu, lq_factor_tangent.cu) ----
+// The checks ab2_gar_factor_adjoint and ab2_gar_factor_tangent share, in this order: handle kind and a backward on the
+// problem's own vectors, mu, then that no array the call writes (`kind` wnames[i], pw[i], nw[i] doubles) overlaps an
+// array it reads (described by `reads`) or an output of the handle, and that one item fits `smem_max` bytes.
+static int check_factor_call(const ab2_gar_solver *s, double mueq, const double *mueq_arr, const char *who,
+                             const char *kind, int nwr, double *const *pw, const size_t *nw, const char *const *wnames,
+                             const char *reads, int nrd, const double *const *pr, const size_t *nr_, size_t item_bytes,
+                             size_t smem_max) {
+  if (int rc = check_resolve_handle(s, 0, who))
+    return rc;
+  if (!s->primal_factor)
+    return fail(AB2_ERR_STATE, std::string(who) + ": FF and VX hold an adjoint or tangent solve; run a backward first");
+  const ab2_gar_dims &d = s->d;
+  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
+    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  // the results are written knot by knot while later knots' inputs and factors are still to be read
+  for (int i = 0; i < nwr; ++i) {
+    if (!pw[i] || !nw[i])
+      continue;
+    for (int c = 0; c < nrd; ++c)
+      if (pr[c] && nr_[c] && pw[i] < pr[c] + nr_[c] && pr[c] < pw[i] + nw[i])
+        return fail(AB2_ERR_INVALID, std::string(who) + ": " + kind + " " + wnames[i] + " overlaps " + reads);
+    for (int w = 0; w < AB2_OUT_COUNT; ++w)
+      if (s->out[w] && pw[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pw[i] + nw[i])
+        return fail(AB2_ERR_INVALID, std::string(who) + ": " + kind + " " + wnames[i] + " overlaps an output array of the handle");
+  }
+  if (item_bytes > smem_max)
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one instance of this shape does not fit 227 KB of shared memory");
+  return AB2_OK;
+}
+
 // ---- reverse mode of the backward recursion (lq_factor_adjoint.cu): cotangents of the factorisation -> gradients ----
 static int factor_adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
                                const ab2_factor_cotangent *cot, const ab2_lq_grad *grad, void *stream) {
   if (!s || !cot || !grad)
     return fail(AB2_ERR_INVALID, "null argument");
-  if (int rc = check_resolve_handle(s, 0, "factor_adjoint"))
-    return rc;
-  if (!s->primal_factor)
-    return fail(AB2_ERR_STATE, "factor_adjoint: FF and VX hold an adjoint or tangent solve; run a backward first");
   const ab2_gar_dims &d = s->d;
   const size_t B = d.batch, N = d.horizon, nx = d.nx, nr = d.nu + d.nc + d.nx;
-  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
-  // the gradients are written knot by knot while later knots' cotangents and factors are still to be read
   const double *pc[6] = {cot->ff, cot->fb, cot->vxx, cot->vx, cot->fft, cot->fbt};
   const size_t nc[6] = {B * N * nr, B * N * nr * nx, B * (N + 1) * nx * nx, B * (N + 1) * nx, B * d.nct,
                         B * d.nct * nx};
   double *const pg[4] = {grad->stage, grad->term, grad->G0, grad->g0};
   const size_t ng[4] = {B * N * s->srec, B * s->trec, B * d.nc0 * nx, B * d.nc0};
   static const char *gnames[4] = {"stage", "term", "G0", "g0"};
-  for (int i = 0; i < 4; ++i) {
-    if (!pg[i] || !ng[i])
-      continue;
-    for (int c = 0; c < 6; ++c)
-      if (pc[c] && nc[c] && pg[i] < pc[c] + nc[c] && pc[c] < pg[i] + ng[i])
-        return fail(AB2_ERR_INVALID, std::string("factor_adjoint: grad ") + gnames[i] + " overlaps a cotangent array");
-    for (int w = 0; w < AB2_OUT_COUNT; ++w)
-      if (s->out[w] && pg[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pg[i] + ng[i])
-        return fail(AB2_ERR_INVALID, std::string("factor_adjoint: grad ") + gnames[i] + " overlaps an output array of the handle");
-  }
-  if ((size_t)ab2::factor_adjoint_item_doubles(d.nx, d.nu, d.nc) * sizeof(double) > ab2::kFactorAdjointSmemMax)
-    return fail(AB2_ERR_UNSUPPORTED, "factor_adjoint: one instance of this shape does not fit 227 KB of shared memory");
+  if (int rc = check_factor_call(s, mueq, mueq_arr, "factor_adjoint", "grad", 4, pg, ng, gnames, "a cotangent array",
+                                 6, pc, nc, (size_t)ab2::factor_adjoint_item_doubles(d.nx, d.nu, d.nc) * sizeof(double),
+                                 ab2::kFactorAdjointSmemMax))
+    return rc;
   CUDA_TRY(cudaSetDevice(d.device));
   cudaStream_t st = (cudaStream_t)stream;
   const double *mu_dev = nullptr;
@@ -1184,6 +1201,57 @@ int ab2_gar_factor_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace
   if (!mueq)
     return fail(AB2_ERR_INVALID, "null mueq array");
   return factor_adjoint_impl(s, 0.0, mueq, memspace, cot, grad, stream);
+}
+
+// ---- forward mode of the backward recursion (lq_factor_tangent.cu): tangent records -> tangents of the factorisation ----
+static int factor_tangent_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
+                               const ab2_lq_tangent *dot, const ab2_factor_tangent *out, void *stream) {
+  if (!s || !dot || !out)
+    return fail(AB2_ERR_INVALID, "null argument");
+  const ab2_gar_dims &d = s->d;
+  const size_t B = d.batch, N = d.horizon, nx = d.nx, nr = d.nu + d.nc + d.nx;
+  double *const po[6] = {out->ff, out->fb, out->vxx, out->vx, out->fft, out->fbt};
+  const size_t no[6] = {B * N * nr, B * N * nr * nx, B * (N + 1) * nx * nx, B * (N + 1) * nx, B * d.nct,
+                        B * d.nct * nx};
+  static const char *onames[6] = {"ff", "fb", "vxx", "vx", "fft", "fbt"};
+  const double *pd[4] = {dot->stage, dot->term, dot->G0, dot->g0};
+  const size_t nd[4] = {B * N * s->srec, B * s->trec, B * d.nc0 * nx, B * d.nc0};
+  if (int rc = check_factor_call(s, mueq, mueq_arr, "factor_tangent", "out", 6, po, no, onames, "a tangent array",
+                                 4, pd, nd, (size_t)ab2::factor_tangent_item_doubles(d.nx, d.nu, d.nc) * sizeof(double),
+                                 ab2::kFactorTangentSmemMax))
+    return rc;
+  CUDA_TRY(cudaSetDevice(d.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const double *mu_dev = nullptr;
+  if (mueq_arr)
+    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
+      return rc;
+  ab2::FactorTangentArgs a{};
+  a.fac = factor_view(s, mueq, mu_dev);
+  a.ff = s->out[AB2_OUT_FF];
+  a.vx = s->out[AB2_OUT_VX];
+  a.ffT = s->out[AB2_OUT_FFT];
+  a.d_stage = dot->stage;
+  a.d_term = dot->term;
+  a.o_ff = out->ff;
+  a.o_fb = out->fb;
+  a.o_vxx = out->vxx;
+  a.o_vx = out->vx;
+  a.o_fft = out->fft;
+  a.o_fbt = out->fbt;
+  CUDA_TRY(ab2::launch_factor_tangent(a, st));
+  s->launches += 1;
+  return AB2_OK;
+}
+int ab2_gar_factor_tangent(ab2_gar_solver *s, double mueq, const ab2_lq_tangent *dot, const ab2_factor_tangent *out,
+                           void *stream) {
+  return factor_tangent_impl(s, mueq, nullptr, AB2_DEVICE, dot, out, stream);
+}
+int ab2_gar_factor_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace, const ab2_lq_tangent *dot,
+                             const ab2_factor_tangent *out, void *stream) {
+  if (!mueq)
+    return fail(AB2_ERR_INVALID, "null mueq array");
+  return factor_tangent_impl(s, 0.0, mueq, memspace, dot, out, stream);
 }
 
 int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch) {

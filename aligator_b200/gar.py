@@ -83,6 +83,12 @@ class FactorCotangent(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in _FCOT_KEYS]
 
 
+class FactorTangent(C.Structure):
+    """``ab2_factor_tangent``: device outputs of ``ab2_gar_factor_tangent`` (NULL = not written), in ``ab2_gar_get``'s
+    layouts."""
+    _fields_ = [(k, C.c_void_p) for k in _FCOT_KEYS]
+
+
 class LqRefineWork(C.Structure):
     """``ab2_lq_refine_work``: caller-owned scratch of ``ab2_gar_refine_many``, the residual in resolve's rhs layouts
     (q .. f) and the correction in the solution's layouts (xs .. lams)."""
@@ -228,6 +234,10 @@ def lib():
                                              C.c_void_p]
         L.ab2_gar_factor_adjoint_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(FactorCotangent),
                                                C.POINTER(LqGrad), C.c_void_p]
+        L.ab2_gar_factor_tangent.argtypes = [C.c_void_p, C.c_double, C.POINTER(LqTangent), C.POINTER(FactorTangent),
+                                             C.c_void_p]
+        L.ab2_gar_factor_tangent_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LqTangent),
+                                               C.POINTER(FactorTangent), C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -823,6 +833,24 @@ class CudaRiccatiBatch:
             _check(lib().ab2_gar_factor_adjoint(self.h, C.c_double(mueq), C.byref(ct), C.byref(gr), C.c_void_p(stream)))
         else:
             _check(lib().ab2_gar_factor_adjoint_v(self.h, v[0], v[1], C.byref(ct), C.byref(gr), C.c_void_p(stream)))
+
+    def factor_tangent(self, dot, out, mueq, stream=0):
+        """Forward mode of the factorisation (``ab2_gar_factor_tangent``): ``out`` receives the derivative of the last
+        backward's outputs along the data tangent ``dot``, a dict with any of stage, term (G0 and g0 are ignored) of
+        device tensors in the problem's layouts (a key that is missing or None is zero).  ``out``: dict with any of ff,
+        fb, vxx, vx, fft, fbt of device tensors laid out like ``get`` returns OUT_FF .. OUT_FBT (vxx as full blocks),
+        overwritten (a missing key is not written).  The tangent of Q and R is taken through sym(.) = (. + .^T) / 2.
+        ``mueq``: the mu of the last backward, a number or a [batch] array / tensor (``ab2_gar_factor_tangent_v``).
+        Needs a backward on the problem's own vectors since the last set_problem; the handle's outputs are not
+        touched."""
+        v = self._mueq_arg(mueq, stream)
+        dt = _fill(LqTangent(), _GRAD_KEYS, dot)
+        ot = _fill(FactorTangent(), _FCOT_KEYS, out)
+        self._keep_ftan = (dot, out)
+        if v is None:
+            _check(lib().ab2_gar_factor_tangent(self.h, C.c_double(mueq), C.byref(dt), C.byref(ot), C.c_void_p(stream)))
+        else:
+            _check(lib().ab2_gar_factor_tangent_v(self.h, v[0], v[1], C.byref(dt), C.byref(ot), C.c_void_p(stream)))
 
     def factor_epoch(self):
         """``ab2_gar_factor_epoch``: bumped by every call that rewrites the factorisation or the records."""

@@ -627,6 +627,51 @@ int ab2_gar_factor_adjoint  (ab2_gar_solver *s, double mueq, const ab2_factor_co
 int ab2_gar_factor_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace,
                              const ab2_factor_cotangent *cot, const ab2_lq_grad *grad, void *stream);
 
+/* Forward mode of the factorisation: the tangents of FF, FB, VXX, VX, FFT, FBT along a tangent pdot of the problem
+ * records -- the sensitivity of the whole gain schedule K_t, or of every Vxx_t, to a few parameters that enter A, B,
+ * Q, ... in one call per parameter.  It is the exact transpose of ab2_gar_factor_adjoint: <cbar, ydot> =
+ * <factor_adjoint(cbar), pdot> for any cbar and pdot.  Q and R enter as sym(Qdot), sym(Rdot) (as ab2_gar_tangent), so an
+ * asymmetric Qdot acts as its symmetric part.  G0 and g0 do not enter the factorisation (their fields are ignored);
+ * mu is not differentiated.  The tangent recursion runs backward in time, as the sweep does, carrying Vd', vd' (the
+ * tangents of Vxx_{t+1}, vx_{t+1}).  At the terminal knot (Z_N = C_N / mu, z_N = d_N / mu as stored):
+ *   Zd_N = Cd_N / mu,  zd_N = dd_N / mu,  Vxxd_N = sym(Qd_N + Cd_N^T Z_N + C_N^T Zd_N),  vxd_N = qd_N + Cd_N^T z_N + C_N^T zd_N
+ * and per stage knot, with V' = Vxx_{t+1}, X = [[K, k], [Z, z]], Shat = S + A^T V' B, v+ = vx_{t+1} + V' f and
+ * M = [[R + B^T V' B, D^T], [D, -mu I]] recomputed from the record and the stored factor (M factored again from its
+ * lower triangle, as resolve does):
+ *   products     vd+ = vd' + Vd' f + V' fd,   Shatd = Sd + Ad^T V' B + A^T Vd' B + A^T V' Bd,
+ *                Rhatd = sym(Rd) + Bd^T V' B + B^T V' Bd + B^T Vd' B,   Qhatd = sym(Qd) + Ad^T V' A + A^T V' Ad + A^T Vd' A,
+ *                rhatd = rd + Bd^T v+ + B^T vd+,   qhatd = qd + Ad^T v+ + A^T vd+
+ *   solve        [[Kd, kd], [Zd, zd]] = -M^-1 [[Rhatd K + Dd^T Z + Shatd^T, Rhatd k + Dd^T z + rhatd], [Dd K + Cd, Dd k + dd]]
+ *   closed loop  Ahatd = Ad + Bd K + B Kd,   ad = fd + Bd k + B kd
+ *   value        Vxxd_t = sym(Qhatd + Shatd K + Shat Kd + Cd^T Z + C^T Zd),   vxd_t = qhatd + Shatd k + Shat kd + Cd^T z + C^T zd
+ * (Qhatd is formed as Qd + A^T (Vd' A + 2 V' Ad), which has the same symmetric part; only that part enters Vxxd_t.)
+ *
+ * Layouts (DEVICE arrays): `dot` is ab2_lq_tangent in the problem's layouts, logical knot order (stage
+ * [batch][N][stage_record], term [batch][term_record]; the pad double is never read); a NULL field is a zero tangent.
+ * `out` has ab2_gar_get's layouts, those of ab2_gar_factor_adjoint's cotangents: ff [batch][N][nu+nc+nx], fb
+ * [batch][N][(nu+nc+nx)*nx] row-major, vxx [batch][N+1][nx*nx] full column-major blocks (exactly symmetric), vx
+ * [batch][N+1][nx], fft [batch][nct], fbt [batch][nct*nx] row-major.  A NULL out field is not written (the recursion
+ * still carries Vxxd and vxd).
+ * One launch on `stream`: one warp per instance, or one CTA per instance when the shape's shared memory leaves room for
+ * no other.  Only the caller's out arrays are written: every output of the handle, its status, pivot statistics and
+ * ab2_gar_factor_epoch are unchanged, and no memory is allocated (a host mueq array of the _v twin is staged like
+ * ab2_gar_sweep_v's).  Records are read through the ring head, Vxx in the layout the last backward wrote.  The results
+ * are deterministic: every entry is summed by one lane in a fixed order.  `mueq` must be the mu of the last backward.
+ * Errors (nothing is launched): AB2_ERR_UNSUPPORTED for dense, parametric (nth > 0) and parallel handles, and for a
+ * shape whose item needs more than 227 KB of shared memory (4 nx^2 + 5 nx nu + nu^2 + nc nx + 4 nx +
+ * (nu+nc)(2 nx + nu + nc + 3) doubles, rounded up to even; C1-C5 fit); AB2_ERR_STATE unless a backward on the
+ * problem's own vectors has run since the last set_problem, assemble or cycle_append (not after ab2_gar_adjoint or
+ * ab2_gar_tangent, until the next backward); AB2_ERR_INVALID for mueq <= 0 with constraints, or an out array that
+ * overlaps a dot array or an output of the handle. */
+typedef struct ab2_factor_tangent {
+  double *ff, *fb, *vxx, *vx, *fft, *fbt;
+} ab2_factor_tangent;
+int ab2_gar_factor_tangent  (ab2_gar_solver *s, double mueq, const ab2_lq_tangent *dot,
+                             const ab2_factor_tangent *out, void *stream);
+/* The same with a per-instance mu: mueq [batch] in host or device memory, checked and staged like ab2_gar_sweep_v. */
+int ab2_gar_factor_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace,
+                             const ab2_lq_tangent *dot, const ab2_factor_tangent *out, void *stream);
+
 /* The rest of SolverProxDDP's inner iteration (solver-proxddp.hxx:555-699) around the sweep, batched over the
  * instances: multiplier estimates, Lagrangian gradients and stopping criteria.  With these, the LQ right-hand side
  * ab2_gar_assemble reads and the gradients ab2_gar_directional_derivative reads are produced on the device.
