@@ -36,6 +36,21 @@ def _digest(paths, extra=""):
     return h.hexdigest()[:16]
 
 
+_INCLUDE = re.compile(r'^\s*#\s*include\s+"([^"]+)"', re.M)
+
+
+def _sources(src):
+    """src and every file it reaches through #include "...", in a fixed order: what an object depends on."""
+    seen, todo = set(), [os.path.normpath(src)]
+    while todo:
+        p = todo.pop()
+        if p in seen or not os.path.exists(p):
+            continue
+        seen.add(p)
+        todo += [os.path.normpath(os.path.join(os.path.dirname(p), m)) for m in _INCLUDE.findall(open(p).read())]
+    return sorted(seen)
+
+
 def _run(cmd):
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
@@ -45,75 +60,24 @@ def _run(cmd):
 
 def build(verbose=False, force=False, ptxas_v=False):
     os.makedirs(OBJ, exist_ok=True)
-    hdrs = [os.path.join(CSRC, f) for f in ("riccati_group.cuh", "riccati_launch.cuh", "riccati_configs.h",
-                                            "vxx_layout.h")]
-    hdrs.append(os.path.join(PKG, "..", "include", "aligator_b200", "gar.h"))
-    hdrs_block = hdrs + [os.path.join(CSRC, f) for f in ("riccati_block.cuh", "riccati_block_launch.h",
-                                                          "lq_assemble.h", "lq_adjoint.h", "lq_tangent.h", "lq_resolve.h",
-                                                          "lq_resolve.cuh", "lq_factor_adjoint.h", "lq_factor_adjoint.cuh",
-                                                          "lq_factor_tangent.h", "lq_factor_tangent.cuh",
-                                                          "lq_jacobian.h", "lq_refine.h", "kkt_error.h",
-                                                          "linesearch.h", "proxddp_inner.h")]
     extra = ["-Xptxas", "-v"] if ptxas_v else []
     jobs = []
+
+    def obj(name, src, defines=(), tag=""):
+        # the -Xptxas -v flag is part of the digest, so a --ptxas build recompiles and prints every kernel
+        src = os.path.join(CSRC, src)
+        o = os.path.join(OBJ, "%s_%s.o" % (name, _digest(_sources(src), tag + str(extra))))
+        jobs.append((o, [NVCC] + ARCH + FLAGS + extra + list(defines) + ["-c", src, "-o", o]))
+
     for (nx, nu, nc, g) in configs():
-        src = os.path.join(CSRC, "kernel_inst.cu")
-        tag = _digest(hdrs + [src], "%d_%d_%d_%d%s" % (nx, nu, nc, g, extra))
-        obj = os.path.join(OBJ, "k_%d_%d_%d_%s.o" % (nx, nu, nc, tag))
-        cmd = [NVCC] + ARCH + FLAGS + extra + ["-DAB2_NX=%d" % nx, "-DAB2_NU=%d" % nu, "-DAB2_NC=%d" % nc,
-                                              "-DAB2_G=%d" % g, "-c", src, "-o", obj]
-        jobs.append((obj, cmd))
-    src = os.path.join(CSRC, "gar_cuda.cu")
-    tag = _digest(hdrs_block + [src])
-    obj = os.path.join(OBJ, "capi_%s.o" % tag)
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "block_kernel.cu")
-    obj = os.path.join(OBJ, "block_%s.o" % _digest(hdrs_block + [src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "kkt_error.cu")
-    obj = os.path.join(OBJ, "kkt_%s.o" % _digest([os.path.join(CSRC, "kkt_error.h"), src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_assemble.cu")
-    obj = os.path.join(OBJ, "assemble_%s.o" % _digest([hdrs[-1], os.path.join(CSRC, "lq_assemble.h"), src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_adjoint.cu")
-    obj = os.path.join(OBJ, "adjoint_%s.o" % _digest([os.path.join(CSRC, "lq_adjoint.h"), src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_tangent.cu")
-    obj = os.path.join(OBJ, "tangent_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_tangent.h")]
-                                                     + [src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_resolve.cu")
-    obj = os.path.join(OBJ, "resolve_%s.o" % _digest([os.path.join(CSRC, f) for f in ("vxx_layout.h", "lq_resolve.h",
-                                                                                      "lq_resolve.cuh")]
-                                                     + [src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_factor_adjoint.cu")
-    obj = os.path.join(OBJ, "factor_adjoint_%s.o" % _digest([os.path.join(CSRC, f) for f in (
-        "vxx_layout.h", "lq_resolve.cuh", "item_launch.cuh", "lq_factor_adjoint.h", "lq_factor_adjoint.cuh")] + [src],
-        str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_factor_tangent.cu")
-    obj = os.path.join(OBJ, "factor_tangent_%s.o" % _digest([os.path.join(CSRC, f) for f in (
-        "vxx_layout.h", "lq_resolve.cuh", "item_launch.cuh", "lq_factor_tangent.h", "lq_factor_tangent.cuh")] + [src],
-        str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_jacobian.cu")
-    obj = os.path.join(OBJ, "jacobian_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_jacobian.h",
-                                                                                       "lq_record.cuh")]
-                                                      + [src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "lq_refine.cu")
-    obj = os.path.join(OBJ, "refine_%s.o" % _digest([os.path.join(CSRC, f) for f in ("lq_adjoint.h", "lq_refine.h",
-                                                                                     "lq_record.cuh")]
-                                                    + [src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "linesearch.cu")
-    obj = os.path.join(OBJ, "linesearch_%s.o" % _digest([os.path.join(CSRC, "linesearch.h"), src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
-    src = os.path.join(CSRC, "proxddp_inner.cu")
-    obj = os.path.join(OBJ, "inner_%s.o" % _digest([hdrs[-1], os.path.join(CSRC, "proxddp_inner.h"), src], str(extra)))
-    jobs.append((obj, [NVCC] + ARCH + FLAGS + extra + ["-c", src, "-o", obj]))
+        obj("k_%d_%d_%d" % (nx, nu, nc), "kernel_inst.cu",
+            ["-DAB2_NX=%d" % nx, "-DAB2_NU=%d" % nu, "-DAB2_NC=%d" % nc, "-DAB2_G=%d" % g], "%d_%d_%d_%d" % (nx, nu, nc, g))
+    for name, src in (("capi", "gar_cuda.cu"), ("block", "block_kernel.cu"), ("kkt", "kkt_error.cu"),
+                      ("assemble", "lq_assemble.cu"), ("adjoint", "lq_adjoint.cu"), ("resolve", "lq_resolve.cu"),
+                      ("factor_adjoint", "lq_factor_adjoint.cu"), ("factor_tangent", "lq_factor_tangent.cu"),
+                      ("jacobian", "lq_jacobian.cu"), ("refine", "lq_refine.cu"), ("linesearch", "linesearch.cu"),
+                      ("inner", "proxddp_inner.cu")):
+        obj(name, src)
     todo =[(o, c) for (o, c) in jobs if force or not os.path.exists(o)]
     logs = []
     if todo:

@@ -20,7 +20,6 @@
 #include "kkt_error.h"
 #include "linesearch.h"
 #include "lq_adjoint.h"
-#include "lq_tangent.h"
 #include "lq_resolve.h"
 #include "lq_factor_adjoint.h"
 #include "lq_factor_tangent.h"
@@ -276,7 +275,7 @@ struct ab2_gar_solver {
   double *inner_tmp = nullptr; // [batch][2] per-instance scalars of multipliers / criterion, for host destinations
   double *mu_dev = nullptr;    // [batch] host-given per-instance mu of the *_v sweeps, staged for the kernels
   double *adj_stage = nullptr, *adj_term = nullptr, *adj_g0 = nullptr; // the adjoint problem of ab2_gar_adjoint
-  double *tan_rho = nullptr; // -rho of ab2_gar_tangent, in the cotangent layout (xs, us, vs, vsT, lam0, lams)
+  double *tan_rho = nullptr; // rho of ab2_gar_tangent, in the solution's layouts (xs, us, vs, vsT, lam0, lams)
   double *ref_buf = nullptr;   // ab2_gar_refine's residual (rhs layout) and correction (out layout)
   double *ref_norms = nullptr; // staging of host norms of ab2_gar_refine / refine_many, ref_norms_n doubles
   size_t ref_norms_n = 0;
@@ -847,41 +846,120 @@ int ab2_gar_forward_theta(ab2_gar_solver *s, const double *theta, int memspace, 
   return rc;
 }
 
-// ---- adjoint of the LQ solve (lq_adjoint.cu): records kernel, the sweep on the adjoint problem, gradient kernel ----
-// The checks shared by ab2_gar_adjoint and ab2_gar_tangent, in this order: handle kind, problem set, primal fields,
-// mu.  `refuse_overlap`: a primal field that overlaps an output of the handle is refused (the adjoint reads the
-// primal after its sweep has overwritten the outputs).
-static int check_vector_solve(ab2_gar_solver *s, double mueq, const double *mueq_arr, const ab2_ls_iterate *primal,
-                              const char *who, bool refuse_overlap) {
+// ---- argument checks and launch prologue shared by the derivative calls ----
+// The fields of one argument, for the NULL and overlap checks: pointers and sizes in doubles.
+struct Fields {
+  const char *what;
+  const char *const *names;
+  const double *p[AB2_OUT_COUNT];
+  size_t n[AB2_OUT_COUNT];
+  int count;
+};
+typedef std::pair<const Fields *, const Fields *> FieldPair;
+static const char *const kSolNames[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
+static const char *const kRecNames[4] = {"stage", "term", "G0", "g0"};
+// fields in the solution's layouts, `blocks` instances (batch, or nrhs * batch)
+static Fields sol_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
+  const ab2_gar_dims &d = s->d;
+  const int N = d.horizon;
+  const size_t per[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
+                         (size_t)N * d.nx};
+  Fields f{what, kSolNames, {}, {}, 6};
+  for (int i = 0; i < 6; ++i) {
+    f.p[i] = p[i];
+    f.n[i] = blocks * per[i];
+  }
+  return f;
+}
+// fields in the problem's record layouts (stage, term, G0, g0), `blocks` instances
+static Fields rec_fields(const ab2_gar_solver *s, const char *what, const double *const p[4], size_t blocks) {
+  const ab2_gar_dims &d = s->d;
+  const size_t per[4] = {(size_t)d.horizon * s->srec, (size_t)s->trec, (size_t)d.nc0 * d.nx, (size_t)d.nc0};
+  Fields f{what, kRecNames, {}, {}, 4};
+  for (int i = 0; i < 4; ++i) {
+    f.p[i] = p[i];
+    f.n[i] = blocks * per[i];
+  }
+  return f;
+}
+static int require(const Fields &f, const char *who) {
+  for (int i = 0; i < f.count; ++i)
+    if (f.n[i] && !f.p[i])
+      return fail(AB2_ERR_INVALID, std::string(who) + ": " + f.what + " " + f.names[i] + " is NULL");
+  return AB2_OK;
+}
+// no field of a may overlap a field of b (a and b the same argument: two different fields of it)
+static int refuse_overlap(const Fields &a, const Fields &b, const char *who) {
+  for (int i = 0; i < a.count; ++i)
+    for (int o = &a == &b ? i + 1 : 0; o < b.count; ++o)
+      if (a.p[i] && b.p[o] && a.n[i] && b.n[o] && a.p[i] < b.p[o] + b.n[o] && b.p[o] < a.p[i] + a.n[i])
+        return fail(AB2_ERR_INVALID, std::string(who) + ": " + a.what + " " + a.names[i] + " overlaps " + b.what + " " +
+                                         b.names[o]);
+  return AB2_OK;
+}
+static const char *const kRhsNames[6] = {"q", "r", "d", "dN", "g0", "f"};
+// fields in resolve's rhs layouts (the same sizes as the solution's), `blocks` instances
+static Fields rhs_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
+  Fields f = sol_fields(s, what, p, blocks);
+  f.names = kRhsNames;
+  return f;
+}
+static const char *const kFacNames[6] = {"ff", "fb", "vxx", "vx", "fft", "fbt"};
+// fields in ab2_gar_get's layouts of the factorisation (FF .. FBT, vxx as full blocks), `blocks` instances
+static Fields fac_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
+  const ab2_gar_dims &d = s->d;
+  const size_t N = d.horizon, nx = d.nx, nr = d.nu + d.nc + d.nx;
+  const size_t per[6] = {N * nr, N * nr * nx, (N + 1) * nx * nx, (N + 1) * nx, (size_t)d.nct, (size_t)d.nct * nx};
+  Fields f{what, kFacNames, {}, {}, 6};
+  for (int i = 0; i < 6; ++i) {
+    f.p[i] = p[i];
+    f.n[i] = blocks * per[i];
+  }
+  return f;
+}
+static const char *const kOutNames[AB2_OUT_COUNT] = {"FF",   "FB",    "VXX",  "VX",  "FFT",     "FBT",    "KKT0",
+                                                     "XS",   "US",    "VS",   "VST", "LBD0",    "LBDAS",  "FTH",
+                                                     "VXT",  "VTT",   "VT",   "KKT0FTH", "THGRAD", "THHESS"};
+// the handle's own output arrays, as allocated
+static Fields out_fields(const ab2_gar_solver *s) {
+  Fields f{"the handle's output", kOutNames, {}, {}, AB2_OUT_COUNT};
+  for (int w = 0; w < AB2_OUT_COUNT; ++w) {
+    f.p[w] = s->out[w];
+    f.n[w] = s->out_alloc[w];
+  }
+  return f;
+}
+// the scalar mu rule (a per-instance array is checked when it is staged)
+static int check_mu(const ab2_gar_solver *s, double mueq, const double *mueq_arr, const char *who) {
+  if (!mueq_arr && !(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
+    return fail(AB2_ERR_INVALID, std::string(who) + ": mueq must be > 0 when constraints are present");
+  return AB2_OK;
+}
+// The prologue of a call whose arguments have been checked: the handle's device, the caller's stream (*st) and the
+// per-instance mu mueq_arr (in memspace) as the kernels read it (*mu_dev; null for the scalar mu).
+static int begin_launch(ab2_gar_solver *s, const double *mueq_arr, int memspace, void *stream, cudaStream_t *st,
+                        const double **mu_dev) {
+  CUDA_TRY(cudaSetDevice(s->d.device));
+  *st = (cudaStream_t)stream;
+  *mu_dev = nullptr;
+  return mueq_arr ? stage_mueq(s, mueq_arr, memspace, *st, mu_dev) : AB2_OK;
+}
+
+// ---- adjoint of the LQ solve: records kernel (lq_adjoint.cu), the sweep on the adjoint problem, gradient kernel
+//      (lq_jacobian.cu) ----
+// The handle checks shared by ab2_gar_adjoint and ab2_gar_tangent, in this order: handle kind, problem set.
+static int check_solve_handle(const ab2_gar_solver *s, const char *who) {
   if (s->nth > 0 || s->legs > 1)
     return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": parametric (nth > 0) and parallel handles are not supported");
   if (!s->have_problem)
-    return fail(AB2_ERR_STATE, "set_problem has not been called with all four buffers");
-  const ab2_gar_dims &d = s->d;
-  const int B = d.batch, N = d.horizon, nx = d.nx;
-  const double *pz[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
-  const size_t nz[6] = {(size_t)B * (N + 1) * nx, (size_t)B * N * d.nu, (size_t)B * N * d.nc,
-                        (size_t)B * d.nct, (size_t)B * d.nc0, (size_t)B * N * nx};
-  static const char *names[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
-  for (int i = 0; i < 6; ++i) {
-    if (nz[i] == 0)
-      continue;
-    if (!pz[i])
-      return fail(AB2_ERR_INVALID, std::string(who) + ": primal " + names[i] + " is NULL");
-    if (refuse_overlap)
-      for (int w = 0; w < AB2_OUT_COUNT; ++w)
-        if (s->out[w] && pz[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pz[i] + nz[i])
-          return fail(AB2_ERR_INVALID, std::string(who) + ": primal " + names[i] + " overlaps an output array of the handle");
-  }
-  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+    return fail(AB2_ERR_STATE, std::string(who) + ": set_problem has not been called with all four buffers");
   return AB2_OK;
 }
 
-// The current problem's matrices with the vectors q, r, d, f, q_N, d_N, g0 = -cot, solved by the handle's own sweep
-// (two launches).  mu_dev: the staged per-instance mu, or null for the scalar mueq.
+// The current problem's matrices with the vectors q, r, d, f, q_N, d_N, g0 = -cot (copy: = cot), solved by the
+// handle's own sweep (two launches).  mu_dev: the staged per-instance mu, or null for the scalar mueq.
 static int solve_cotangent_problem(ab2_gar_solver *s, double mueq, const double *mu_dev, const ab2_ls_iterate *cot,
-                                   cudaStream_t st) {
+                                   bool copy, cudaStream_t st) {
   const ab2_gar_dims &d = s->d;
   const int B = d.batch, N = d.horizon, nx = d.nx;
   auto own = [&](double *&buf, size_t n) -> int {
@@ -894,9 +972,9 @@ static int solve_cotangent_problem(ab2_gar_solver *s, double mueq, const double 
       (rc = own(s->adj_g0, (size_t)B * d.nc0)) != AB2_OK)
     return rc;
   const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
-  // 1. the problem: same matrices, vectors = -cot
+  // 1. the problem: same matrices, vectors = -cot (copy: cot)
   ab2::AdjointRecordArgs ra{ad, s->p.stage_head, s->p.stage, s->p.term, cot->xs, cot->us, cot->vs, cot->vsT,
-                            cot->lam0, cot->lams, s->adj_stage, s->adj_term, s->adj_g0};
+                            cot->lam0, cot->lams, s->adj_stage, s->adj_term, s->adj_g0, copy};
   CUDA_TRY(ab2::launch_adjoint_records(ra, st));
   s->launches += 1;
   // 2. backward + forward on it; the problem pointers change in this launch's copy of the parameters only, and a
@@ -928,28 +1006,36 @@ static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
                         const ab2_ls_iterate *primal, const ab2_ls_iterate *cot, const ab2_lq_grad *grad, void *stream) {
   if (!s || !primal || !cot || !grad)
     return fail(AB2_ERR_INVALID, "null argument");
-  if (int rc = check_vector_solve(s, mueq, mueq_arr, primal, "adjoint", true))
+  const char *who = "adjoint";
+  if (int rc = check_solve_handle(s, who))
+    return rc;
+  // the gradient kernel reads the primal after the sweep has overwritten the handle's outputs
+  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
+  const Fields P = sol_fields(s, "primal", pp, s->d.batch);
+  if (int rc = require(P, who))
+    return rc;
+  if (int rc = refuse_overlap(P, out_fields(s), who))
+    return rc;
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
     return rc;
   const ab2_gar_dims &d = s->d;
   const int B = d.batch, N = d.horizon, nx = d.nx;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   // 1. + 2. the adjoint problem (vectors = -cotangent) and its solve
   int rc;
-  if ((rc = solve_cotangent_problem(s, mueq, mu_dev, cot, st)) != AB2_OK)
+  if ((rc = solve_cotangent_problem(s, mueq, mu_dev, cot, false, st)) != AB2_OK)
     return rc;
   const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
-  // 3. gradient records from the primal z and the adjoint w (the trajectory outputs)
-  ab2::AdjointGradArgs ga{ad,
-                          primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
-                          s->out[AB2_OUT_XS], s->out[AB2_OUT_US], s->out[AB2_OUT_VS], s->out[AB2_OUT_VST],
-                          s->out[AB2_OUT_LBD0], s->out[AB2_OUT_LBDAS],
-                          grad->stage, grad->term, grad->G0, grad->g0};
-  CUDA_TRY(ab2::launch_adjoint_grad(ga, st));
+  // 3. gradient records from the primal z and the adjoint w (the trajectory outputs): dh = -w, dK = -w z^T
+  ab2::JacobianGradArgs ga{ad, 1,
+                           primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
+                           s->out[AB2_OUT_XS], s->out[AB2_OUT_US], s->out[AB2_OUT_VS], s->out[AB2_OUT_VST],
+                           s->out[AB2_OUT_LBD0], s->out[AB2_OUT_LBDAS],
+                           grad->stage, grad->term, grad->G0, grad->g0, true};
+  CUDA_TRY(ab2::launch_jacobian_grad(ga, st));
   s->launches += 1;
   return AB2_OK;
 }
@@ -964,37 +1050,41 @@ int ab2_gar_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace, const
   return adjoint_impl(s, 0.0, mueq, memspace, primal, cotangent, grad, stream);
 }
 
-// ---- tangent of the LQ solve (lq_tangent.cu): right-hand-side kernel, then the adjoint's records kernel and sweep ----
+// ---- tangent of the LQ solve: right-hand-side kernel (lq_jacobian.cu), then the adjoint's records kernel and sweep ----
 static int tangent_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
                         const ab2_ls_iterate *primal, const ab2_lq_tangent *dot, void *stream) {
   if (!s || !primal || !dot)
     return fail(AB2_ERR_INVALID, "null argument");
+  const char *who = "tangent";
+  if (int rc = check_solve_handle(s, who))
+    return rc;
   // the primal is read completely by the first launch, before the sweep writes any output: it may alias them
-  if (int rc = check_vector_solve(s, mueq, mueq_arr, primal, "tangent", false))
+  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
+  if (int rc = require(sol_fields(s, "primal", pp, s->d.batch), who))
+    return rc;
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
     return rc;
   const ab2_gar_dims &d = s->d;
   const int B = d.batch, N = d.horizon, nx = d.nx;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   const size_t nxs = (size_t)B * (N + 1) * nx, nus = (size_t)B * N * d.nu, nvs = (size_t)B * N * d.nc,
                nvT = (size_t)B * d.nct, nl0 = (size_t)B * d.nc0, nls = (size_t)B * N * nx;
   if (!s->tan_rho)
     CUDA_TRY(cudaMalloc(&s->tan_rho, (nxs + nus + nvs + nvT + nl0 + nls + 1) * sizeof(double)));
   double *rxs = s->tan_rho, *rus = rxs + nxs, *rvs = rus + nus, *rvT = rvs + nvs, *rl0 = rvT + nvT, *rls = rl0 + nl0;
-  // 1. -rho = -(Kdot z + hdot), in the cotangent layout
+  // 1. rho = Kdot z + hdot, in the solution's layouts
   const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
-  ab2::TangentRhsArgs ta{ad, dot->stage, dot->term, dot->G0, dot->g0,
-                         primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
-                         rxs, rus, rvs, rvT, rl0, rls};
-  CUDA_TRY(ab2::launch_tangent_rhs(ta, st));
+  ab2::JacobianRhsArgs ra{ad, 1, dot->stage, dot->term, dot->G0, dot->g0,
+                          primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
+                          rxs, rus, rvs, rvT, rl0, rls};
+  CUDA_TRY(ab2::launch_jacobian_rhs(ra, st));
   s->launches += 1;
   // 2. + 3. the tangent problem (vectors = rho) and its solve: the trajectory outputs become zdot
   const ab2_ls_iterate rho{rxs, rus, rvs, rvT, rl0, rls};
-  return solve_cotangent_problem(s, mueq, mu_dev, &rho, st);
+  return solve_cotangent_problem(s, mueq, mu_dev, &rho, true, st);
 }
 int ab2_gar_tangent(ab2_gar_solver *s, double mueq, const ab2_ls_iterate *primal, const ab2_lq_tangent *dot,
                     void *stream) {
@@ -1075,38 +1165,28 @@ static int resolve_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
                         const ab2_lq_rhs *rhs, const ab2_ls_trial *out, void *stream) {
   if (!s || !rhs || !out)
     return fail(AB2_ERR_INVALID, "null argument");
-  if (int rc = check_resolve_handle(s, nrhs, "resolve"))
+  const char *who = "resolve";
+  if (int rc = check_resolve_handle(s, nrhs, who))
     return rc;
-  const ab2_gar_dims &d = s->d;
-  const int N = d.horizon;
-  double *const po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
-  const size_t no[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
-                        (size_t)N * d.nx};
-  static const char *names[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
-  for (int i = 0; i < 6; ++i)
-    if (no[i] && !po[i])
-      return fail(AB2_ERR_INVALID, std::string("resolve: out ") + names[i] + " is NULL");
-  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  const size_t R = (size_t)nrhs * s->d.batch;
+  const double *po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
+  const double *ph[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
+  if (int rc = require(sol_fields(s, "out", po, 1), who)) // (refused even at nrhs = 0)
+    return rc;
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
+    return rc;
   // the backward pass parks its per-knot vectors in the out arrays before it has read every rhs entry: an out array
   // that overlaps an rhs array would be read after it was overwritten
-  const double *pr[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
-  static const char *rnames[6] = {"q", "r", "d", "dN", "g0", "f"};
-  const size_t R = (size_t)nrhs * d.batch;
-  for (int i = 0; i < 6; ++i)
-    for (int o = 0; o < 6; ++o)
-      if (pr[i] && po[o] && no[i] && no[o] && pr[i] < po[o] + R * no[o] && po[o] < pr[i] + R * no[i])
-        return fail(AB2_ERR_INVALID, std::string("resolve: rhs ") + rnames[i] + " overlaps out " + names[o]);
-  if (int rc = check_resolve_fits(s, "resolve"))
+  if (int rc = refuse_overlap(rhs_fields(s, "rhs", ph, R), sol_fields(s, "out", po, R), who))
+    return rc;
+  if (int rc = check_resolve_fits(s, who))
     return rc;
   if (nrhs == 0)
     return AB2_OK;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   return run_resolve(s, mueq, mu_dev, nrhs, rhs, out, st);
 }
 int ab2_gar_resolve(ab2_gar_solver *s, double mueq, int nrhs, const ab2_lq_rhs *rhs, const ab2_ls_trial *out,
@@ -1120,33 +1200,13 @@ int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int n
   return resolve_impl(s, 0.0, mueq, memspace, nrhs, rhs, out, stream);
 }
 // ---- derivatives of the backward recursion (lq_factor_adjoint.cu, lq_factor_tangent.cu) ----
-// The checks ab2_gar_factor_adjoint and ab2_gar_factor_tangent share, in this order: handle kind and a backward on the
-// problem's own vectors, mu, then that no array the call writes (`kind` wnames[i], pw[i], nw[i] doubles) overlaps an
-// array it reads (described by `reads`) or an output of the handle, and that one item fits `smem_max` bytes.
-static int check_factor_call(const ab2_gar_solver *s, double mueq, const double *mueq_arr, const char *who,
-                             const char *kind, int nwr, double *const *pw, const size_t *nw, const char *const *wnames,
-                             const char *reads, int nrd, const double *const *pr, const size_t *nr_, size_t item_bytes,
-                             size_t smem_max) {
+// The handle checks ab2_gar_factor_adjoint and ab2_gar_factor_tangent share: handle kind, and a backward on the
+// problem's own vectors.
+static int check_factor_handle(const ab2_gar_solver *s, const char *who) {
   if (int rc = check_resolve_handle(s, 0, who))
     return rc;
   if (!s->primal_factor)
     return fail(AB2_ERR_STATE, std::string(who) + ": FF and VX hold an adjoint or tangent solve; run a backward first");
-  const ab2_gar_dims &d = s->d;
-  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
-  // the results are written knot by knot while later knots' inputs and factors are still to be read
-  for (int i = 0; i < nwr; ++i) {
-    if (!pw[i] || !nw[i])
-      continue;
-    for (int c = 0; c < nrd; ++c)
-      if (pr[c] && nr_[c] && pw[i] < pr[c] + nr_[c] && pr[c] < pw[i] + nw[i])
-        return fail(AB2_ERR_INVALID, std::string(who) + ": " + kind + " " + wnames[i] + " overlaps " + reads);
-    for (int w = 0; w < AB2_OUT_COUNT; ++w)
-      if (s->out[w] && pw[i] < s->out[w] + s->out_alloc[w] && s->out[w] < pw[i] + nw[i])
-        return fail(AB2_ERR_INVALID, std::string(who) + ": " + kind + " " + wnames[i] + " overlaps an output array of the handle");
-  }
-  if (item_bytes > smem_max)
-    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one instance of this shape does not fit 227 KB of shared memory");
   return AB2_OK;
 }
 
@@ -1155,24 +1215,26 @@ static int factor_adjoint_impl(ab2_gar_solver *s, double mueq, const double *mue
                                const ab2_factor_cotangent *cot, const ab2_lq_grad *grad, void *stream) {
   if (!s || !cot || !grad)
     return fail(AB2_ERR_INVALID, "null argument");
-  const ab2_gar_dims &d = s->d;
-  const size_t B = d.batch, N = d.horizon, nx = d.nx, nr = d.nu + d.nc + d.nx;
-  const double *pc[6] = {cot->ff, cot->fb, cot->vxx, cot->vx, cot->fft, cot->fbt};
-  const size_t nc[6] = {B * N * nr, B * N * nr * nx, B * (N + 1) * nx * nx, B * (N + 1) * nx, B * d.nct,
-                        B * d.nct * nx};
-  double *const pg[4] = {grad->stage, grad->term, grad->G0, grad->g0};
-  const size_t ng[4] = {B * N * s->srec, B * s->trec, B * d.nc0 * nx, B * d.nc0};
-  static const char *gnames[4] = {"stage", "term", "G0", "g0"};
-  if (int rc = check_factor_call(s, mueq, mueq_arr, "factor_adjoint", "grad", 4, pg, ng, gnames, "a cotangent array",
-                                 6, pc, nc, (size_t)ab2::factor_adjoint_item_doubles(d.nx, d.nu, d.nc) * sizeof(double),
-                                 ab2::kFactorAdjointSmemMax))
+  const char *who = "factor_adjoint";
+  if (int rc = check_factor_handle(s, who))
     return rc;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
+    return rc;
+  // the gradients are written knot by knot while later knots' cotangents and factors are still to be read
+  const ab2_gar_dims &d = s->d;
+  const double *pc[6] = {cot->ff, cot->fb, cot->vxx, cot->vx, cot->fft, cot->fbt};
+  const double *pg[4] = {grad->stage, grad->term, grad->G0, grad->g0};
+  const Fields G = rec_fields(s, "grad", pg, d.batch);
+  if (int rc = refuse_overlap(G, fac_fields(s, "cotangent", pc, d.batch), who))
+    return rc;
+  if (int rc = refuse_overlap(G, out_fields(s), who))
+    return rc;
+  if ((size_t)ab2::factor_adjoint_item_doubles(d.nx, d.nu, d.nc) * sizeof(double) > ab2::kFactorAdjointSmemMax)
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one instance of this shape does not fit 227 KB of shared memory");
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   ab2::FactorAdjointArgs a{};
   a.fac = factor_view(s, mueq, mu_dev);
   a.ff = s->out[AB2_OUT_FF];
@@ -1208,24 +1270,26 @@ static int factor_tangent_impl(ab2_gar_solver *s, double mueq, const double *mue
                                const ab2_lq_tangent *dot, const ab2_factor_tangent *out, void *stream) {
   if (!s || !dot || !out)
     return fail(AB2_ERR_INVALID, "null argument");
-  const ab2_gar_dims &d = s->d;
-  const size_t B = d.batch, N = d.horizon, nx = d.nx, nr = d.nu + d.nc + d.nx;
-  double *const po[6] = {out->ff, out->fb, out->vxx, out->vx, out->fft, out->fbt};
-  const size_t no[6] = {B * N * nr, B * N * nr * nx, B * (N + 1) * nx * nx, B * (N + 1) * nx, B * d.nct,
-                        B * d.nct * nx};
-  static const char *onames[6] = {"ff", "fb", "vxx", "vx", "fft", "fbt"};
-  const double *pd[4] = {dot->stage, dot->term, dot->G0, dot->g0};
-  const size_t nd[4] = {B * N * s->srec, B * s->trec, B * d.nc0 * nx, B * d.nc0};
-  if (int rc = check_factor_call(s, mueq, mueq_arr, "factor_tangent", "out", 6, po, no, onames, "a tangent array",
-                                 4, pd, nd, (size_t)ab2::factor_tangent_item_doubles(d.nx, d.nu, d.nc) * sizeof(double),
-                                 ab2::kFactorTangentSmemMax))
+  const char *who = "factor_tangent";
+  if (int rc = check_factor_handle(s, who))
     return rc;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
+    return rc;
+  // the tangents are written knot by knot while later knots' tangent records and factors are still to be read
+  const ab2_gar_dims &d = s->d;
+  const double *po[6] = {out->ff, out->fb, out->vxx, out->vx, out->fft, out->fbt};
+  const double *pd[4] = {dot->stage, dot->term, dot->G0, dot->g0};
+  const Fields O = fac_fields(s, "out", po, d.batch);
+  if (int rc = refuse_overlap(O, rec_fields(s, "tangent", pd, d.batch), who))
+    return rc;
+  if (int rc = refuse_overlap(O, out_fields(s), who))
+    return rc;
+  if ((size_t)ab2::factor_tangent_item_doubles(d.nx, d.nu, d.nc) * sizeof(double) > ab2::kFactorTangentSmemMax)
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one instance of this shape does not fit 227 KB of shared memory");
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   ab2::FactorTangentArgs a{};
   a.fac = factor_view(s, mueq, mu_dev);
   a.ff = s->out[AB2_OUT_FF];
@@ -1262,56 +1326,6 @@ int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch) {
 }
 
 // ---- Jacobians (lq_jacobian.cu): many cotangents or tangents on the last backward's factorisation, through resolve ----
-// The fields of one argument, for the NULL and overlap checks: pointers and sizes in doubles.
-struct Fields {
-  const char *what;
-  const char *const *names;
-  const double *p[6];
-  size_t n[6];
-  int count;
-};
-typedef std::pair<const Fields *, const Fields *> FieldPair;
-static const char *const kSolNames[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
-static const char *const kRecNames[4] = {"stage", "term", "G0", "g0"};
-// fields in the solution's layouts, `blocks` instances (batch, or nrhs * batch)
-static Fields sol_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
-  const ab2_gar_dims &d = s->d;
-  const int N = d.horizon;
-  const size_t per[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
-                         (size_t)N * d.nx};
-  Fields f{what, kSolNames, {}, {}, 6};
-  for (int i = 0; i < 6; ++i) {
-    f.p[i] = p[i];
-    f.n[i] = blocks * per[i];
-  }
-  return f;
-}
-// fields in the problem's record layouts (stage, term, G0, g0), `blocks` instances
-static Fields rec_fields(const ab2_gar_solver *s, const char *what, const double *const p[4], size_t blocks) {
-  const ab2_gar_dims &d = s->d;
-  const size_t per[4] = {(size_t)d.horizon * s->srec, (size_t)s->trec, (size_t)d.nc0 * d.nx, (size_t)d.nc0};
-  Fields f{what, kRecNames, {}, {}, 4};
-  for (int i = 0; i < 4; ++i) {
-    f.p[i] = p[i];
-    f.n[i] = blocks * per[i];
-  }
-  return f;
-}
-static int require(const Fields &f, const char *who) {
-  for (int i = 0; i < f.count; ++i)
-    if (f.n[i] && !f.p[i])
-      return fail(AB2_ERR_INVALID, std::string(who) + ": " + f.what + " " + f.names[i] + " is NULL");
-  return AB2_OK;
-}
-// no field of a may overlap a field of b (a and b the same argument: two different fields of it)
-static int refuse_overlap(const Fields &a, const Fields &b, const char *who) {
-  for (int i = 0; i < a.count; ++i)
-    for (int o = &a == &b ? i + 1 : 0; o < b.count; ++o)
-      if (a.p[i] && b.p[o] && a.n[i] && b.n[o] && a.p[i] < b.p[o] + b.n[o] && b.p[o] < a.p[i] + a.n[i])
-        return fail(AB2_ERR_INVALID, std::string(who) + ": " + a.what + " " + a.names[i] + " overlaps " + b.what + " " +
-                                         b.names[o]);
-  return AB2_OK;
-}
 
 static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int nrhs,
                              const ab2_ls_iterate *primal, const ab2_ls_iterate *cot, const ab2_ls_trial *work,
@@ -1333,8 +1347,8 @@ static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
     return rc;
   if (int rc = require(P, who))
     return rc;
-  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
+    return rc;
   // resolve writes work while it reads the cotangent; the gradient kernel then reads work and the primal
   for (const FieldPair &ab : {FieldPair{&Z, &W}, FieldPair{&W, &P}, FieldPair{&G, &P}, FieldPair{&G, &W},
                               FieldPair{&G, &G}})
@@ -1344,12 +1358,10 @@ static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
     return rc;
   if (nrhs == 0)
     return AB2_OK;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   // 1. y_j = resolve(zbar_j) = -K^-1 zbar_j: the cotangent fields are resolve's rhs fields
   const ab2_lq_rhs rhs{cot->xs, cot->us, cot->vs, cot->vsT, cot->lam0, cot->lams};
   if (int rc = run_resolve(s, mueq, mu_dev, nrhs, &rhs, work, st))
@@ -1359,7 +1371,7 @@ static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
   ab2::JacobianGradArgs ga{ad, nrhs,
                            primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
                            work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams,
-                           grad->stage, grad->term, grad->G0, grad->g0};
+                           grad->stage, grad->term, grad->G0, grad->g0, false};
   CUDA_TRY(ab2::launch_jacobian_grad(ga, st));
   s->launches += 1;
   return AB2_OK;
@@ -1399,8 +1411,8 @@ static int tangent_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
     return rc;
   if (int rc = require(P, who))
     return rc;
-  if (!mueq_arr && !(mueq > 0.0) && (d.nc > 0 || d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
+    return rc;
   // the rho kernel writes work while it reads the tangent and the primal; resolve then writes out while it reads work
   for (const FieldPair &ab : {FieldPair{&D, &W}, FieldPair{&P, &W}, FieldPair{&W, &O}, FieldPair{&O, &P},
                               FieldPair{&O, &O}})
@@ -1410,12 +1422,10 @@ static int tangent_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
     return rc;
   if (nrhs == 0)
     return AB2_OK;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   // 1. rho_j = Kdot_j z + hdot_j into work, in resolve's rhs layouts
   const ab2::AdjointDims ad{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
   ab2::JacobianRhsArgs ra{ad, nrhs, dot->stage, dot->term, dot->G0, dot->g0,
@@ -1439,13 +1449,6 @@ int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, 
 }
 
 // ---- iterative refinement (lq_refine.cu): residual, resolve and update per step, on the last backward's factorisation ----
-static const char *const kRhsNames[6] = {"q", "r", "d", "dN", "g0", "f"};
-// fields in resolve's rhs layouts (the same sizes as the solution's), `blocks` instances
-static Fields rhs_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
-  Fields f = sol_fields(s, what, p, blocks);
-  f.names = kRhsNames;
-  return f;
-}
 static bool device_accessible(const void *p) {
   cudaPointerAttributes at{};
   if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
@@ -1548,8 +1551,8 @@ static int run_refine(ab2_gar_solver *s, double mueq, const double *mu_dev, int 
 static int check_refine_args(const ab2_gar_solver *s, double mueq, const double *mueq_arr, int steps, const char *who) {
   if (steps < 0)
     return fail(AB2_ERR_INVALID, std::string(who) + ": steps < 0");
-  if (!mueq_arr && !(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
-    return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
+  if (int rc = check_mu(s, mueq, mueq_arr, who))
+    return rc;
   return check_resolve_fits(s, who);
 }
 
@@ -1569,12 +1572,10 @@ static int refine_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, i
     return AB2_OK;
   const ab2_gar_dims &d = s->d;
   const int B = d.batch, N = d.horizon, nx = d.nx;
-  CUDA_TRY(cudaSetDevice(d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   const size_t nxs = (size_t)B * (N + 1) * nx, nus = (size_t)B * N * d.nu, nvs = (size_t)B * N * d.nc,
                nvT = (size_t)B * d.nct, nl0 = (size_t)B * d.nc0, nls = (size_t)B * N * nx,
                one = nxs + nus + nvs + nvT + nl0 + nls;
@@ -1633,12 +1634,10 @@ static int refine_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_a
       return rc;
   if (nrhs == 0 || (steps == 0 && !norms))
     return AB2_OK;
-  CUDA_TRY(cudaSetDevice(s->d.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const double *mu_dev = nullptr;
-  if (mueq_arr)
-    if (int rc = stage_mueq(s, mueq_arr, memspace, st, &mu_dev))
-      return rc;
+  cudaStream_t st;
+  const double *mu_dev;
+  if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
+    return rc;
   const ab2_ls_trial r{work->q, work->r, work->d, work->dN, work->g0, work->f};
   const ab2_ls_trial dz{work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
   return run_refine(s, mueq, mu_dev, nrhs, steps, false, rhs, z, &r, &dz, norms, st);

@@ -1,6 +1,6 @@
-// item_launch.cuh -- launch selection shared by the per-instance programs of the factorisation's derivatives
-// (lq_factor_adjoint.cu, lq_factor_tangent.cu): items that leave room for others run one per warp, several warps per
-// CTA; an item too large to share an SM runs alone on a CTA of kItemCtaThreads lanes.
+// item_launch.cuh -- launch selection shared by the per-item programs of resolve and the factorisation's derivatives
+// (lq_resolve.cu, lq_factor_adjoint.cu, lq_factor_tangent.cu): items that leave room for others run one per warp,
+// several warps per CTA; an item too large to share an SM runs alone on a CTA of kItemCtaThreads lanes (not resolve).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -19,6 +19,12 @@ struct ItemCtaCtx {
   __device__ __forceinline__ void sync() const { __syncthreads(); }
 };
 
+// warps (items) per CTA of warp items of item_bytes each
+inline int item_warps_per_cta(size_t item_bytes) {
+  const int wpc = (int)(kItemCtaBudget / item_bytes);
+  return wpc < 1 ? 1 : (wpc > kItemMaxWarps ? kItemMaxWarps : wpc);
+}
+
 // warp(args, item_doubles): item b = blockIdx.x * warps + warp index; cta(args): item b = blockIdx.x.  One launch.
 template <class Args>
 cudaError_t launch_items(void (*warp)(const Args, int), void (*cta)(const Args), const Args &a, long batch,
@@ -31,8 +37,7 @@ cudaError_t launch_items(void (*warp)(const Args, int), void (*cta)(const Args),
     cta<<<(unsigned)batch, kItemCtaThreads, item_bytes, st>>>(a);
     return cudaGetLastError();
   }
-  int wpc = (int)(kItemCtaBudget / item_bytes);
-  wpc = wpc < 1 ? 1 : (wpc > kItemMaxWarps ? kItemMaxWarps : wpc);
+  const int wpc = item_warps_per_cta(item_bytes);
   const size_t smem = item_bytes * wpc;
   e = cudaFuncSetAttribute(warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)

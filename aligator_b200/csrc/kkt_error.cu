@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include "kkt_error.h"
+#include "lq_record.cuh"
 
 namespace ab2 {
 
@@ -36,7 +37,7 @@ __global__ void __launch_bounds__(256) kkt_error_kernel(const KktErrorArgs a) {
     const double *u = term ? nullptr : a.us + (b * N + t) * nu;
     const int ncc = term ? nct : nc, nuu = term ? 0 : nu;
     const double *v = term ? a.vsT + b * nct : a.vs + (b * N + t) * nc;
-    const int slot = term ? 0 : ((t + a.stage_head) >= N ? t + a.stage_head - N : t + a.stage_head);
+    const int slot = term ? 0 : ring_slot(t, a.stage_head, N);
     const double *rec = term ? a.term + b * a.trec : a.stage + (b * N + slot) * a.srec;
     // block pointers inside the record
     const double *A = rec, *B = rec + nxx, *f = B + nxu;

@@ -79,10 +79,8 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
   }
 
   for (int t = 0; t < N; ++t) {
-    const double *rec = r.stage + ((long)b * N + (t + r.stage_head >= N ? t + r.stage_head - N : t + r.stage_head)) * r.srec;
-    // stage record [A | B | f | Q | S | R | q | r | C | D | d]
-    const long oB = nx * nx, of = oB + nx * nu, oQ = of + nx, oS = oQ + nx * nx, oR = oS + nx * nu, oq = oR + nu * nu,
-               orr = oq + nx, oC = orr + nu, oD = oC + nc * nx, od = oD + nc * nu, oend = od + nc;
+    const StageOffsets so = stage_offsets(nx, nu, nc);
+    const double *rec = r.stage + ((long)b * N + ring_slot(t, r.stage_head, N)) * r.srec;
     double *g = a.g_stage ? a.g_stage + ((long)b * N + t) * r.srec : nullptr;
     const double *fbk = r.fb + (b * N + t) * (long)nr * nx, *ffk = a.ff + (b * N + t) * (long)nr;
     const double *cfb = a.c_fb ? a.c_fb + (b * N + t) * (long)nr * nx : nullptr;
@@ -96,9 +94,9 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
       Ahb[e] = cfb ? cfb[(n + i) * nx + j] : 0.0;
     }
     for (int e = ctx.lane; e < nx * nu; e += ctx.nl)
-      Bm[e] = rec[oB + e];
+      Bm[e] = rec[so.B + e];
     for (int e = ctx.lane; e < nc * nx; e += ctx.nl)
-      Cm[e] = rec[oC + e];
+      Cm[e] = rec[so.C + e];
     for (int e = ctx.lane; e < n * m; e += ctx.nl) {
       const int i = e % n, j = e / n;
       if (j < nx) {
@@ -110,7 +108,7 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
       }
     }
     for (int i = ctx.lane; i < nx; i += ctx.nl) {
-      f[i] = rec[of + i];
+      f[i] = rec[so.f + i];
       ab[i] = cff ? cff[n + i] : 0.0;
     }
     ctx.sync();
@@ -133,28 +131,12 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
     // 3. Shat = S + A^T W; M (lower) = [[R + B^T W, .], [D, -mu I]]
     for (int e = ctx.lane; e < nx * nu; e += ctx.nl) {
       const int i = e % nx, c = e / nx;
-      double s = rec[oS + e];
+      double s = rec[so.S + e];
       for (int k = 0; k < nx; ++k)
         s += Am[k + i * nx] * W[k + c * nx];
       Sh[e] = s;
     }
-    for (int e = ctx.lane; e < n * n; e += ctx.nl) {
-      const int i = e % n, j = e / n;
-      if (i < j)
-        continue;
-      double v;
-      if (i < nu) {
-        double s = 0.0;
-        for (int k = 0; k < nx; ++k)
-          s += Bm[k + i * nx] * W[k + j * nx];
-        v = rec[oR + i + j * nu] + s;
-      } else if (j < nu) {
-        v = rec[oD + (i - nu) + j * nc];
-      } else {
-        v = i == j ? -mu : 0.0;
-      }
-      M[e] = v;
-    }
+    rs::kkt_lower(ctx, M, Bm, W, rec + so.R, rec + so.D, nx, nu, nc, mu);
     ctx.sync();
     // 4. P += [[B^T Ahatb + Shat^T Vbar, B^T ab + Shat^T vbar], [C Vbar, C vbar]]; factor M; P <- -M^-1 P
     for (int e = ctx.lane; e < n * m; e += ctx.nl) {
@@ -173,12 +155,7 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
       P[e] += s;
     }
     ctx.sync();
-    rs::bk_factor(ctx, M, piv, n);
-    for (int j = ctx.lane; j < m; j += ctx.nl) {
-      rs::bk_solve(M, piv, n, P + j * n);
-      for (int i = 0; i < n; ++i)
-        P[i + j * n] = -P[i + j * n];
-    }
+    rs::kkt_solve(ctx, M, piv, n, P, n, m, true);
     ctx.sync();
     // 5. Shatb (over Shat), Rb; the gradients of Q, q, r, d, C, D, S
     for (int e = ctx.lane; e < nx * nu; e += ctx.nl) {
@@ -201,17 +178,17 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
     }
     if (g) {
       for (int e = ctx.lane; e < nx * nx; e += ctx.nl)
-        g[oQ + e] = Vb[e];
+        g[so.Q + e] = Vb[e];
       for (int i = ctx.lane; i < nx; i += ctx.nl)
-        g[oq + i] = vb[i];
+        g[so.q + i] = vb[i];
       for (int i = ctx.lane; i < n; i += ctx.nl)
-        g[(i < nu ? orr : od - nu) + i] = P[i + nx * n];
+        g[(i < nu ? so.r : so.d - nu) + i] = P[i + nx * n];
       for (int e = ctx.lane; e < nc * nx; e += ctx.nl) { // Cb = Z Vbar + z vbar^T + P_c[:, :nx]
         const int c = e % nc, i = e / nc;
         double s = 0.0;
         for (int k = 0; k < nx; ++k)
           s += KZ[(nu + c) + k * n] * Vb[k + i * nx];
-        g[oC + e] = (s + kz[nu + c] * vb[i]) + P[(nu + c) + i * n];
+        g[so.C + e] = (s + kz[nu + c] * vb[i]) + P[(nu + c) + i * n];
       }
       for (int e = ctx.lane; e < nc * nu; e += ctx.nl) { // Db = P_c X_u^T + X_c P_u^T
         const int c = e % nc, j = e / nc;
@@ -221,10 +198,10 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
           s1 += P[(nu + c) + l * n] * xu;
           s2 += xc * P[j + l * n];
         }
-        g[oD + e] = s1 + s2;
+        g[so.D + e] = s1 + s2;
       }
-      if (ctx.lane == 0 && r.srec > oend)
-        g[oend] = 0.0;
+      if (ctx.lane == 0 && r.srec > so.end)
+        g[so.end] = 0.0;
     }
     ctx.sync();
     // 6. Ab, Bb, the gradients of S and R; vb+ = A qb + B rb
@@ -251,13 +228,13 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
       for (int k = 0; k < nx; ++k)
         h += T[i + k * nx] * Sh[k + c * nx];
       if (g) {
-        g[oB + e] = (((s + ab[i] * kz[c]) + 2.0 * w) + h) + vp[i] * P[c + nx * n];
-        g[oS + e] = Sh[e];
+        g[so.B + e] = (((s + ab[i] * kz[c]) + 2.0 * w) + h) + vp[i] * P[c + nx * n];
+        g[so.S + e] = Sh[e];
       }
     }
     if (g)
       for (int e = ctx.lane; e < nu * nu; e += ctx.nl)
-        g[oR + e] = Rb[e];
+        g[so.R + e] = Rb[e];
     for (int i = ctx.lane; i < nx; i += ctx.nl) {
       double s = 0.0;
       for (int k = 0; k < nx; ++k)
@@ -273,7 +250,7 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
         double s = 0.0;
         for (int k = 0; k < nx; ++k)
           s += Vp[i + k * nx] * vbp[k];
-        g[of + i] = ab[i] + s;
+        g[so.f + i] = ab[i] + s;
       }
     for (int e = ctx.lane; e < nx * nx; e += ctx.nl) {
       const int i = e % nx, j = e / nx;
@@ -320,13 +297,14 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
 
   // ---- terminal knot ----
   if (a.g_term) {
-    const double *rec = r.term + b * r.trec, *CN = rec + nx * nx + nx;
+    const TermOffsets to = term_offsets(nx, nct);
+    const double *rec = r.term + b * r.trec, *CN = rec + to.C;
     const double *ZN = r.fbT + b * nct * nx, *zN = a.ffT + b * nct;
     double *g = a.g_term + b * r.trec;
     for (int e = ctx.lane; e < nx * nx; e += ctx.nl)
       g[e] = Vb[e];
     for (int i = ctx.lane; i < nx; i += ctx.nl)
-      g[nx * nx + i] = vb[i];
+      g[to.q + i] = vb[i];
     for (int e = ctx.lane; e < nct * nx; e += ctx.nl) { // C_Nb = Z_N Vbar + z_N vbar^T + Zb / mu
       const int c = e % nct, i = e / nct;
       double s = 0.0, z = a.c_fbt ? a.c_fbt[b * nct * nx + c * nx + i] : 0.0;
@@ -334,13 +312,13 @@ AB2_RS_HD void factor_adjoint_item(const FactorAdjointArgs &a, const Ctx &ctx, d
         s += ZN[c * nx + k] * Vb[k + i * nx];
       for (int k = 0; k < nx; ++k)
         z += CN[c + k * nct] * Vb[k + i * nx];
-      g[nx * nx + nx + e] = (s + zN[c] * vb[i]) + z / mu;
+      g[to.C + e] = (s + zN[c] * vb[i]) + z / mu;
     }
     for (int c = ctx.lane; c < nct; c += ctx.nl) { // d_Nb = (zb0_N + C_N vbar) / mu
       double z = a.c_fft ? a.c_fft[b * nct + c] : 0.0;
       for (int k = 0; k < nx; ++k)
         z += CN[c + k * nct] * vb[k];
-      g[nx * nx + nx + nct * nx + c] = z / mu;
+      g[to.d + c] = z / mu;
     }
   }
 }

@@ -66,10 +66,11 @@ AB2_RS_HD void factor_tangent_item(const FactorTangentArgs &a, const Ctx &ctx, d
 
   // ---- terminal knot: record [Q | q | C | d] ----
   {
-    const double *rec = r.term + b * r.trec, *CN = rec + nx * nx + nx;
+    const TermOffsets to = term_offsets(nx, nct);
+    const double *rec = r.term + b * r.trec, *CN = rec + to.C;
     const double *ZN = r.fbT + b * nct * nx, *zN = a.ffT + b * nct;
     const double *dt = a.d_term ? a.d_term + b * r.trec : nullptr;
-    const double *dC = dt ? dt + nx * nx + nx : nullptr, *dd = dC ? dC + nct * nx : nullptr;
+    const double *dC = dt ? dt + to.C : nullptr, *dd = dt ? dt + to.d : nullptr;
     // g(p, q) = Qd_N + Cd_N^T Z_N + C_N^T Zd_N
     const auto g = [&](int p, int q) {
       double x = dt ? dt[p + q * nx] : 0.0, y = 0.0, z = 0.0;
@@ -87,7 +88,7 @@ AB2_RS_HD void factor_tangent_item(const FactorTangentArgs &a, const Ctx &ctx, d
         a.o_vxx[(b * (N + 1) + N) * nx * nx + e] = Vd[e];
     }
     for (int i = ctx.lane; i < nx; i += ctx.nl) {
-      double x = dt ? dt[nx * nx + i] : 0.0, y = 0.0, z = 0.0;
+      double x = dt ? dt[to.q + i] : 0.0, y = 0.0, z = 0.0;
       if (dC)
         for (int c = 0; c < nct; ++c) {
           y += dC[c + i * nct] * zN[c];
@@ -109,10 +110,11 @@ AB2_RS_HD void factor_tangent_item(const FactorTangentArgs &a, const Ctx &ctx, d
   }
 
   for (int t = N - 1; t >= 0; --t) {
-    const double *rec = r.stage + ((long)b * N + (t + r.stage_head >= N ? t + r.stage_head - N : t + r.stage_head)) * r.srec;
-    // stage record [A | B | f | Q | S | R | q | r | C | D | d]
+    // stage record [A | B | f | Q | S | R | q | r | C | D | d] (stage_offsets as 64-bit values typed out here: read
+    // through StageOffsets, the CTA kernel takes 157 registers instead of 127)
     const long oB = nx * nx, of = oB + nx * nu, oQ = of + nx, oS = oQ + nx * nx, oR = oS + nx * nu, oq = oR + nu * nu,
                orr = oq + nx, oC = orr + nu, oD = oC + nc * nx, od = oD + nc * nu;
+    const double *rec = r.stage + ((long)b * N + ring_slot(t, r.stage_head, N)) * r.srec;
     const double *ds = a.d_stage ? a.d_stage + ((long)b * N + t) * r.srec : nullptr; // the dotted record, read in place
     const double *fbk = r.fb + (b * N + t) * (long)nr * nx, *ffk = a.ff + (b * N + t) * (long)nr;
 
@@ -204,23 +206,7 @@ AB2_RS_HD void factor_tangent_item(const FactorTangentArgs &a, const Ctx &ctx, d
         w += Bm[k + i * nx] * Wd[k + j * nx];
       Rd[e] = ((ds ? 0.5 * (ds[oR + e] + ds[oR + j + i * nu]) : 0.0) + s) + w;
     }
-    for (int e = ctx.lane; e < n * n; e += ctx.nl) {
-      const int i = e % n, j = e / n;
-      if (i < j)
-        continue;
-      double v;
-      if (i < nu) {
-        double s = 0.0;
-        for (int k = 0; k < nx; ++k)
-          s += Bm[k + i * nx] * W[k + j * nx];
-        v = rec[oR + i + j * nu] + s;
-      } else if (j < nu) {
-        v = rec[oD + (i - nu) + j * nc];
-      } else {
-        v = i == j ? -mu : 0.0;
-      }
-      M[e] = v;
-    }
+    rs::kkt_lower(ctx, M, Bm, W, rec + oR, rec + oD, nx, nu, nc, mu);
     for (int i = ctx.lane; i < nx; i += ctx.nl) {
       double s = 0.0, w = 0.0;
       if (ds)
@@ -263,12 +249,7 @@ AB2_RS_HD void factor_tangent_item(const FactorTangentArgs &a, const Ctx &ctx, d
       P[e] = (s + w) + h;
     }
     ctx.sync();
-    rs::bk_factor(ctx, M, piv, n);
-    for (int j = ctx.lane; j < m; j += ctx.nl) {
-      rs::bk_solve(M, piv, n, P + j * n);
-      for (int i = 0; i < n; ++i)
-        P[i + j * n] = -P[i + j * n];
-    }
+    rs::kkt_solve(ctx, M, piv, n, P, n, m, true);
     ctx.sync();
     // 5. outputs: FB rows [Kd; Zd; Ahatd], FF [kd; zd; ad]; Td <- Vxxd_t = sym(g), vd <- vxd_t
     if (a.o_fb) {

@@ -1,9 +1,11 @@
 // lq_jacobian.cu -- the two streaming kernels of ab2_gar_adjoint_many and ab2_gar_tangent_many: many cotangents or
 // tangents per factorisation, around ab2_gar_resolve's program (lq_resolve.cu), which solves z = resolve(h) = -K^-1 h.
+// ab2_gar_adjoint and ab2_gar_tangent run the same kernels at nrhs = 1 around their own sweep (gar_cuda.cu).
 //  * jacobian_grad_kernel: reverse mode.  For cotangent j, y_j = resolve(zbar_j) = -K^-1 zbar_j, so the gradients of
 //    ab2_gar_adjoint (dh = -w, dK = -w z^T with w = K^-1 zbar) are dh = y_j and dK = y_j z^T read out of K's blocks:
 //      dA = y_l x^T + l y_x^T, dQ = 1/2 (y_x x^T + x y_x^T), dq = y_x, ...   (gar.h, ab2_gar_adjoint)
-//    Every element is one or two products, computed by one lane: no sums, no atomics.
+//    Every element is one or two products, computed by one lane: no sums, no atomics.  ab2_gar_adjoint passes its
+//    own w as y and asks for the values negated.
 //  * jacobian_rhs_kernel: forward mode.  rho_j = Kdot_j z + hdot_j, ab2_gar_tangent's right-hand side for tangent j,
 //    written (not negated) in resolve's rhs layouts; resolve(rho_j) is then zdot_j.
 //
@@ -21,8 +23,7 @@
 // So right-hand side j's result is bit for bit independent of nrhs and of j's position, and of timing.
 #include <cuda_runtime.h>
 
-#include <stdint.h>
-
+#include "cp_async.cuh"
 #include "lq_jacobian.h"
 #include "lq_record.cuh"
 
@@ -40,39 +41,25 @@ enum : unsigned { G_PAIR = 0, G_HALF = 1, G_SINGLE = 2, G_ZERO = 3 }; // y_a p_b
 __device__ __forceinline__ unsigned gentry(int a, int b, unsigned mode) {
   return (unsigned)a | ((unsigned)b << 15) | (mode << 30);
 }
-__device__ __forceinline__ double gvalue(unsigned ent, const double *p, const double *y) {
+// times sgn = +1 or -1 (exact: -1 negates; a pad element stays +0.0).  A pair is rounded as fma(y_a, p_b, p_a y_b), or
+// with swap as fma(p_a, y_b, y_a p_b), the order ab2_gar_adjoint's stage gradients have always had.
+__device__ __forceinline__ double gvalue(unsigned ent, const double *p, const double *y, double sgn, bool swap) {
   const unsigned mode = ent >> 30;
   const int ia = (int)(ent & 0x7fff), ib = (int)((ent >> 15) & 0x7fff);
   if (mode == G_ZERO)
     return 0.0;
-  if (mode == G_SINGLE)
-    return y[ia];
-  const double s = y[ia] * p[ib] + p[ia] * y[ib];
-  return mode == G_HALF ? 0.5 * s : s;
+  double s;
+  if (mode == G_SINGLE) {
+    s = y[ia];
+  } else {
+    s = swap ? fma(p[ia], y[ib], y[ia] * p[ib]) : fma(y[ia], p[ib], p[ia] * y[ib]);
+    if (mode == G_HALF)
+      s = 0.5 * s;
+  }
+  return sgn * s;
 }
 
 // ---- rho rows from a staged tile holding record elements [e0, e1) ----
-__device__ __forceinline__ void cp8(double *dst, const double *src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src)
-               : "memory");
-}
-__device__ __forceinline__ void cp16(double *dst, const double *src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src)
-               : "memory");
-}
-__device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-// n doubles from global src to shared dst (dst 16-byte aligned), issued by the lanes of one warp
-__device__ __forceinline__ void stage_copy(double *dst, const double *src, int n, int lane) {
-  if (((uintptr_t)src & 15) == 0) {
-    for (int k = lane; 2 * k + 1 < n; k += 32)
-      cp16(dst + 2 * k, src + 2 * k);
-    if ((n & 1) && lane == 0)
-      cp8(dst + n - 1, src + n - 1);
-  } else {
-    for (int k = lane; k < n; k += 32)
-      cp8(dst + k, src + k);
-  }
-}
 // Part of row i of M y (col = false) or of M^T y (col = true) in the tile, for the m x n block M at record offset o.
 __device__ __forceinline__ double mv(const double *tile, int e0, int e1, int o, int m, int n, int i, bool col,
                                      const double *y) {
@@ -146,6 +133,8 @@ int sm_count() {
 }
 } // namespace
 
+// NEG: a.neg, as a template argument so that the flag costs no register
+template <bool NEG>
 __global__ void __launch_bounds__(kWarps * 32) jacobian_grad_kernel(const JacobianGradArgs a, int chunk,
                                                                     int warp_doubles) {
   extern __shared__ __align__(16) double smem[];
@@ -156,6 +145,7 @@ __global__ void __launch_bounds__(kWarps * 32) jacobian_grad_kernel(const Jacobi
   // stage vector buffer [x | u | v | l]; terminal [x_N | v_N | x_0 | l_0]
   const int X = 0, U = nx, V = nx + nu, L = nx + nu + nc, nrow = 2 * nx + nu + nc;
   const int TV = nx, TX0 = nx + nct, TL0 = 2 * nx + nct, tvec = 2 * nx + nct + nc0;
+  constexpr double sgn = NEG ? -1.0 : 1.0;
   const StageOffsets so = stage_offsets(nx, nu, nc);
   for (int e = threadIdx.x; e < srec; e += blockDim.x) {
     const RecElem el = stage_elem(so, nx, nu, nc, e);
@@ -214,7 +204,7 @@ __global__ void __launch_bounds__(kWarps * 32) jacobian_grad_kernel(const Jacobi
           ++g;
         }
         for (int p = lane; p < R * srec; p += 32) {
-          out[g * rstride + e] = gvalue(map[e], pv, yv + g * nrow);
+          out[g * rstride + e] = gvalue(map[e], pv, yv + g * nrow, sgn, NEG);
           e += 32;
           while (e >= srec) {
             e -= srec;
@@ -247,21 +237,24 @@ __global__ void __launch_bounds__(kWarps * 32) jacobian_grad_kernel(const Jacobi
       __syncwarp();
       if (a.term)
         for (int e = lane; e < d.trec; e += 32)
-          a.term[jb * d.trec + e] = gvalue(map[srec + e], pv, yv);
+          a.term[jb * d.trec + e] = gvalue(map[srec + e], pv, yv, sgn, false);
       if (a.G0) // dG0 = y_l0 x_0^T + l_0 y_x0^T, column-major [nc0][nx]
         for (int e = lane; e < nc0 * nx; e += 32) {
           const int r = e % nc0, c = e / nc0;
-          a.G0[jb * nc0 * nx + e] = yv[TL0 + r] * pv[TX0 + c] + pv[TL0 + r] * yv[TX0 + c];
+          const double v = fma(yv[TL0 + r], pv[TX0 + c], pv[TL0 + r] * yv[TX0 + c]);
+          a.G0[jb * nc0 * nx + e] = sgn * v;
         }
       if (a.g0)
         for (int i = lane; i < nc0; i += 32)
-          a.g0[jb * nc0 + i] = yv[TL0 + i];
+          a.g0[jb * nc0 + i] = sgn * yv[TL0 + i];
       __syncwarp();
     }
   }
 }
 
-__global__ void __launch_bounds__(kWarps * 32, 3) jacobian_rhs_kernel(const JacobianRhsArgs a, int slice, int group,
+// ONE: nrhs = 1 (ab2_gar_tangent), where the right-hand-side loop is a single pass and 4 CTAs per SM fit the registers
+template <bool ONE>
+__global__ void __launch_bounds__(kWarps * 32, ONE ? 4 : 3) jacobian_rhs_kernel(const JacobianRhsArgs a, int slice, int group,
                                                                       int warp_doubles) {
   extern __shared__ __align__(16) double smem[];
   const AdjointDims d = a.d;
@@ -283,8 +276,8 @@ __global__ void __launch_bounds__(kWarps * 32, 3) jacobian_rhs_kernel(const Jaco
         vec[k] = k < nx ? a.xs[(it + b) * nx + k] : k < nx + nu ? a.us[it * nu + k - nx]
                  : k < nx + nu + nc ? a.vs[it * nc + k - nx - nu] : a.lams[it * nx + k - nx - nu - nc];
       __syncwarp();
-      for (int j0 = 0; j0 < a.nrhs; j0 += group) {
-        const int R = a.nrhs - j0 < group ? a.nrhs - j0 : group;
+      for (int j0 = 0; j0 < (ONE ? 1 : a.nrhs); j0 += group) {
+        const int R = ONE ? 1 : (a.nrhs - j0 < group ? a.nrhs - j0 : group);
         for (int p = lane; p < R * nrow; p += 32)
           acc[p] = 0.0;
         if (a.stage) {
@@ -292,7 +285,7 @@ __global__ void __launch_bounds__(kWarps * 32, 3) jacobian_rhs_kernel(const Jaco
             const int e1 = e0 + slice < d.srec ? e0 + slice : d.srec;
             for (int g = 0; g < R; ++g)
               stage_copy(tile + g * slice, a.stage + ((long)(j0 + g) * nS + it) * d.srec + e0, e1 - e0, lane);
-            cp_wait();
+            cp_wait_all();
             __syncwarp();
             for (int p = lane; p < R * nrow; p += 32) {
               const int g = p / nrow;
@@ -337,7 +330,7 @@ __global__ void __launch_bounds__(kWarps * 32, 3) jacobian_rhs_kernel(const Jaco
         for (int e0 = 0; e0 < d.trec; e0 += kTile) {
           const int e1 = e0 + kTile < d.trec ? e0 + kTile : d.trec;
           stage_copy(tile, a.term + jb * d.trec + e0, e1 - e0, lane);
-          cp_wait();
+          cp_wait_all();
           __syncwarp();
           for (int r = lane; r < nx + nct; r += 32)
             acc[r] += term_row(tile, e0, e1, to, nx, nct, r, x, v);
@@ -387,17 +380,18 @@ cudaError_t launch_jacobian_grad(const JacobianGradArgs &a, cudaStream_t st) {
   int warp_doubles = nrow * (1 + chunk) > 2 * tvec ? nrow * (1 + chunk) : 2 * tvec;
   warp_doubles = (warp_doubles + 1) & ~1;
   const size_t smem = (size_t)warp_doubles * kWarps * sizeof(double) + (size_t)(d.srec + d.trec) * sizeof(unsigned);
-  cudaError_t e = cudaFuncSetAttribute(jacobian_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  void (*kernel)(const JacobianGradArgs, int, int) = a.neg ? jacobian_grad_kernel<true> : jacobian_grad_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;
   int per_sm = 1;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, jacobian_grad_kernel, kWarps * 32, smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kWarps * 32, smem);
   if (e != cudaSuccess)
     return e;
   long grid = (items + kWarps - 1) / kWarps;
   const long full = (long)sm_count() * (per_sm > 0 ? per_sm : 1);
   grid = grid < full ? grid : full;
-  jacobian_grad_kernel<<<(int)grid, kWarps * 32, smem, st>>>(a, chunk, warp_doubles);
+  kernel<<<(int)grid, kWarps * 32, smem, st>>>(a, chunk, warp_doubles);
   return cudaGetLastError();
 }
 
@@ -417,17 +411,18 @@ cudaError_t launch_jacobian_rhs(const JacobianRhsArgs &a, cudaStream_t st) {
   const int vecs = nrow + group * nrow > d.nx + d.nct + trows ? nrow + group * nrow : d.nx + d.nct + trows;
   const int warp_doubles = (kTile + vecs + 1) & ~1;
   const size_t smem = (size_t)warp_doubles * kWarps * sizeof(double);
-  cudaError_t e = cudaFuncSetAttribute(jacobian_rhs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  void (*kernel)(const JacobianRhsArgs, int, int, int) = a.nrhs == 1 ? jacobian_rhs_kernel<true> : jacobian_rhs_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;
   int per_sm = 1;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, jacobian_rhs_kernel, kWarps * 32, smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kWarps * 32, smem);
   if (e != cudaSuccess)
     return e;
   long grid = (items + kWarps - 1) / kWarps;
   const long full = (long)sm_count() * (per_sm > 0 ? per_sm : 1);
   grid = grid < full ? grid : full;
-  jacobian_rhs_kernel<<<(int)grid, kWarps * 32, smem, st>>>(a, slice, group, warp_doubles);
+  kernel<<<(int)grid, kWarps * 32, smem, st>>>(a, slice, group, warp_doubles);
   return cudaGetLastError();
 }
 

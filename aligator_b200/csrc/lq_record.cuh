@@ -1,9 +1,14 @@
-// lq_record.cuh -- the knot-record layouts of gar.h, for the Jacobian kernels (lq_jacobian.cu): where each block of a
-// stage record [A | B | f | Q | S | R | q | r | C | D | d | pad] and of a terminal record [Q | q | C | d] starts, and
-// which block, row and column an element of a record is.  Matrices are column-major.
+// lq_record.cuh -- the knot-record layouts of gar.h, for the programs of the LQ solve's derivatives: where each block
+// of a stage record [A | B | f | Q | S | R | q | r | C | D | d | pad] and of a terminal record [Q | q | C | d] starts,
+// which block, row and column an element of a record is, and which ring slot holds a knot's record.  Matrices are
+// column-major.  Includable from plain C++ (the emulation library).
 #pragma once
 
-#include <cuda_runtime.h>
+#if defined(__CUDACC__)
+#define AB2_REC_HD __host__ __device__ __forceinline__
+#else
+#define AB2_REC_HD inline
+#endif
 
 namespace ab2 {
 
@@ -14,7 +19,7 @@ struct TermOffsets {
   int Q, q, C, d, end;
 };
 
-__host__ __device__ __forceinline__ StageOffsets stage_offsets(int nx, int nu, int nc) {
+AB2_REC_HD StageOffsets stage_offsets(int nx, int nu, int nc) {
   StageOffsets o;
   o.A = 0;
   o.B = o.A + nx * nx;
@@ -30,7 +35,7 @@ __host__ __device__ __forceinline__ StageOffsets stage_offsets(int nx, int nu, i
   o.end = o.d + nc;
   return o;
 }
-__host__ __device__ __forceinline__ TermOffsets term_offsets(int nx, int nct) {
+AB2_REC_HD TermOffsets term_offsets(int nx, int nct) {
   TermOffsets o;
   o.Q = 0;
   o.q = nx * nx;
@@ -40,16 +45,19 @@ __host__ __device__ __forceinline__ TermOffsets term_offsets(int nx, int nct) {
   return o;
 }
 
+// storage slot of knot t's stage record in a ring of N records whose first knot is at slot `head` (cycle_append)
+AB2_REC_HD int ring_slot(int t, int head, int N) { return t + head >= N ? t + head - N : t + head; }
+
 // the blocks of a stage record, in storage order; the terminal record uses BK_Q, BK_QV, BK_C, BK_DV
 enum : int { BK_A, BK_B, BK_F, BK_Q, BK_S, BK_R, BK_QV, BK_RV, BK_C, BK_D, BK_DV, BK_PAD };
 struct RecElem {
   int blk, row, col; // a vector block has col = 0
 };
 
-__host__ __device__ __forceinline__ RecElem mat_elem(int blk, int r, int m) { return RecElem{blk, r % m, r / m}; }
+AB2_REC_HD RecElem mat_elem(int blk, int r, int m) { return RecElem{blk, r % m, r / m}; }
 
 // element e of a stage record
-__host__ __device__ __forceinline__ RecElem stage_elem(const StageOffsets &o, int nx, int nu, int nc, int e) {
+AB2_REC_HD RecElem stage_elem(const StageOffsets &o, int nx, int nu, int nc, int e) {
   if (e < o.B)
     return mat_elem(BK_A, e - o.A, nx);
   if (e < o.f)
@@ -75,7 +83,7 @@ __host__ __device__ __forceinline__ RecElem stage_elem(const StageOffsets &o, in
   return RecElem{BK_PAD, 0, 0};
 }
 // element e of a terminal record (C and d have nct rows)
-__host__ __device__ __forceinline__ RecElem term_elem(const TermOffsets &o, int nx, int nct, int e) {
+AB2_REC_HD RecElem term_elem(const TermOffsets &o, int nx, int nct, int e) {
   if (e < o.q)
     return mat_elem(BK_Q, e - o.Q, nx);
   if (e < o.C)

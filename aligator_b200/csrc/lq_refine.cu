@@ -24,8 +24,7 @@
 // independent of nrhs, of j's position and of timing.
 #include <cuda_runtime.h>
 
-#include <stdint.h>
-
+#include "cp_async.cuh"
 #include "lq_record.cuh"
 #include "lq_refine.h"
 
@@ -34,30 +33,6 @@ namespace ab2 {
 namespace {
 constexpr int kWarps = 8;  // warps per CTA
 constexpr int kTile = 512; // records of at most this many doubles are staged in shared memory
-
-__device__ __forceinline__ void cp8(double *dst, const double *src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src)
-               : "memory");
-}
-__device__ __forceinline__ void cp16(double *dst, const double *src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src)
-               : "memory");
-}
-__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_wait_prev() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
-__device__ __forceinline__ void cp_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-// n doubles from global src to shared dst (dst 16-byte aligned), issued by the lanes of one warp
-__device__ __forceinline__ void stage_copy(double *dst, const double *src, int n, int lane) {
-  if (((uintptr_t)src & 15) == 0) {
-    for (int k = lane; 2 * k + 1 < n; k += 32)
-      cp16(dst + 2 * k, src + 2 * k);
-    if ((n & 1) && lane == 0)
-      cp8(dst + n - 1, src + n - 1);
-  } else {
-    for (int k = lane; k < n; k += 32)
-      cp8(dst + k, src + k);
-  }
-}
 
 // row i of M y for the column-major m x n block M
 __device__ __forceinline__ double rowdot(const double *M, int m, int n, int i, const double *y) {
@@ -92,9 +67,7 @@ __device__ __forceinline__ void atomic_max_nonneg(double *addr, double v) {
 __device__ __forceinline__ const double *record(const RefineResidualArgs &a, long it) {
   const int N = a.d.N;
   const long b = it / N;
-  int slot = (int)(it - b * N) + a.stage_head;
-  slot = slot >= N ? slot - N : slot;
-  return a.stage + (b * N + slot) * a.d.srec;
+  return a.stage + (b * N + ring_slot((int)(it - b * N), a.stage_head, N)) * a.d.srec;
 }
 // the records of the K knots of group g (fewer in the last group) to dst
 __device__ __forceinline__ void issue(const RefineResidualArgs &a, int K, long nS, long g, double *dst, int lane) {

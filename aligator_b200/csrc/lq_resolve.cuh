@@ -37,6 +37,7 @@
 
 #include <math.h>
 
+#include "lq_record.cuh"
 #include "vxx_layout.h"
 
 namespace ab2 {
@@ -262,6 +263,44 @@ AB2_RS_HD void bk_solve(const double *A, const double *piv, int n, double *x) {
   }
 }
 
+// M (n x n, n = nu + nc, lower triangle, column-major) = [[R + B^T W, .], [D, -mu I]], the KKT matrix of a stage knot,
+// from the staged B (nx x nu) and W = V' B, and the record's R (nu x nu) and D (nc x nu).  No synchronisation.
+template <class Ctx>
+AB2_RS_HD void kkt_lower(const Ctx &ctx, double *M, const double *Bm, const double *W, const double *R, const double *D,
+                         int nx, int nu, int nc, double mu) {
+  const int n = nu + nc;
+  for (int e = ctx.lane; e < n * n; e += ctx.nl) {
+    const int i = e % n, j = e / n;
+    if (i < j)
+      continue;
+    double v;
+    if (i < nu) {
+      double s = 0.0;
+      for (int k = 0; k < nx; ++k)
+        s += Bm[k + i * nx] * W[k + j * nx];
+      v = R[i + j * nu] + s;
+    } else if (j < nu) {
+      v = D[(i - nu) + j * nc];
+    } else {
+      v = i == j ? -mu : 0.0;
+    }
+    M[e] = v;
+  }
+}
+
+// Factors the n x n matrix M (lower triangle) in place and solves `cols` columns X + j ld in place, negated with neg
+// (each column by one lane).  No synchronisation after the solves.
+template <class Ctx>
+AB2_RS_HD void kkt_solve(const Ctx &ctx, double *M, double *piv, int n, double *X, int ld, int cols, bool neg) {
+  bk_factor(ctx, M, piv, n);
+  for (int j = ctx.lane; j < cols; j += ctx.nl) {
+    bk_solve(M, piv, n, X + j * ld);
+    if (neg)
+      for (int i = 0; i < n; ++i)
+        X[j * ld + i] = -X[j * ld + i];
+  }
+}
+
 } // namespace rs
 
 // One work item: instance b, right-hand sides [j0, j0 + R).  sm: resolve_item_doubles(..., a.chunk) doubles.
@@ -271,6 +310,7 @@ AB2_RS_HD void resolve_item(const ResolveArgs &a, const Ctx &ctx, double *sm, lo
   const int n = nu + nc, n0 = nx + nc0, nr = nu + nc + nx, m = resolve_nkkt(nu, nc, nx, nc0);
   const long B = a.batch;
   const double mu = a.mueq_b ? a.mueq_b[b] : a.mueq;
+  const StageOffsets so = stage_offsets(nx, nu, nc);
   double *V = sm, *FB = V + nx * nx, *Bm = FB + nr * nx, *W = Bm + nx * nu, *KKT = W + nx * nu, *piv = KKT + n * n;
   double *K0 = sm, *piv0 = K0 + n0 * n0; // the initial saddle system, over the dead stage buffers
   double *X = sm + resolve_mat_doubles(nx, nu, nc, nc0), *Y = X + a.chunk * nx, *VP = Y + a.chunk * nx, *VX = VP + a.chunk * nx, *S = VX + a.chunk * nx;
@@ -279,7 +319,7 @@ AB2_RS_HD void resolve_item(const ResolveArgs &a, const Ctx &ctx, double *sm, lo
 
   // ---- terminal knot: z_N = d_N / mu, vx_N = q_N + C_N^T z_N ----
   {
-    const double *rec = a.term + b * a.trec, *CN = rec + nx * nx + nx;
+    const double *CN = a.term + b * a.trec + term_offsets(nx, nct).C;
     for (int e = ctx.lane; e < R * nct; e += ctx.nl) {
       const int j = e / nct, i = e % nct;
       a.vsT[rix(j, nct) + i] = (a.dN ? a.dN[rix(j, nct) + i] : 0.0) / mu;
@@ -296,10 +336,8 @@ AB2_RS_HD void resolve_item(const ResolveArgs &a, const Ctx &ctx, double *sm, lo
 
   // ---- stage knots, backward ----
   for (int t = N - 1; t >= 0; --t) {
-    const double *rec = a.stage + ((long)b * N + (t + a.stage_head >= N ? t + a.stage_head - N : t + a.stage_head)) * a.srec;
-    // stage record [A | B | f | Q | S | R | q | r | C | D | d]
-    const double *Br = rec + nx * nx, *Rr = Br + nx * nu + nx + nx * nx + nx * nu;
-    const double *Sr = Br + nx * nu + nx + nx * nx, *Cr = Rr + nu * nu + nx + nu, *Dr = Cr + nc * nx;
+    const double *rec = a.stage + ((long)b * N + ring_slot(t, a.stage_head, N)) * a.srec;
+    const double *Br = rec + so.B, *Sr = rec + so.S, *Cr = rec + so.C;
     // the backward pass needs A, S and C instead of the gains: they take the FB rows' place (the same nr * nx doubles)
     double *Am = FB, *Sm = Am + nx * nx, *Cm = Sm + nx * nu;
     rs::load_v(a, ctx, b, t + 1, V);
@@ -335,23 +373,7 @@ AB2_RS_HD void resolve_item(const ResolveArgs &a, const Ctx &ctx, double *sm, lo
     }
     ctx.sync();
     // KKT (lower) = [[R + B^T V' B, .], [D, -mu I]]; solve vector [r_t + B^T v+; d_t]
-    for (int e = ctx.lane; e < n * n; e += ctx.nl) {
-      const int i = e % n, j = e / n;
-      if (i < j)
-        continue;
-      double v;
-      if (i < nu) {
-        double s = 0.0;
-        for (int k = 0; k < nx; ++k)
-          s += Bm[k + i * nx] * W[k + j * nx];
-        v = Rr[i + j * nu] + s;
-      } else if (j < nu) {
-        v = Dr[(i - nu) + j * nc];
-      } else {
-        v = i == j ? -mu : 0.0;
-      }
-      KKT[i + j * n] = v;
-    }
+    rs::kkt_lower(ctx, KKT, Bm, W, rec + so.R, rec + so.D, nx, nu, nc, mu);
     for (int e = ctx.lane; e < R * n; e += ctx.nl) {
       const int j = e / n, i = e % n;
       double v;
@@ -366,12 +388,7 @@ AB2_RS_HD void resolve_item(const ResolveArgs &a, const Ctx &ctx, double *sm, lo
       S[j * m + i] = v;
     }
     ctx.sync();
-    rs::bk_factor(ctx, KKT, piv, n);
-    for (int j = ctx.lane; j < R; j += ctx.nl) {
-      rs::bk_solve(KKT, piv, n, S + j * m);
-      for (int i = 0; i < n; ++i)
-        S[j * m + i] = -S[j * m + i];
-    }
+    rs::kkt_solve(ctx, KKT, piv, n, S, m, R, true);
     ctx.sync();
     // k -> us[t], z -> vs[t]; a = f + B k -> xs[t+1]; Y = V' B k
     for (int e = ctx.lane; e < R * n; e += ctx.nl) {
@@ -428,9 +445,7 @@ AB2_RS_HD void resolve_item(const ResolveArgs &a, const Ctx &ctx, double *sm, lo
       S[j * m + i] = i < nx ? -VX[j * nx + i] : -(a.g0 ? a.g0[rix(j, nc0) + (i - nx)] : 0.0);
     }
     ctx.sync();
-    rs::bk_factor(ctx, K0, piv0, n0);
-    for (int j = ctx.lane; j < R; j += ctx.nl)
-      rs::bk_solve(K0, piv0, n0, S + j * m);
+    rs::kkt_solve(ctx, K0, piv0, n0, S, m, R, false); // the right-hand side is negated already
     ctx.sync();
     for (int e = ctx.lane; e < R * n0; e += ctx.nl) {
       const int j = e / n0, i = e % n0;

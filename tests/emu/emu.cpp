@@ -1,12 +1,17 @@
-// The host emulation library of the sweep programs: the warp-per-instance group program (group_emu.cpp), the
-// CTA-per-instance program with its leg mode, and the stage-dense program (block_emu.cpp), in one translation unit.
+// The host emulation library of the device programs: the warp-per-instance group program (group_emu.cpp), the
+// CTA-per-instance program with its leg mode, and the stage-dense program (block_emu.cpp), and the per-item programs of
+// resolve and the factorisation's derivatives (resolve_emu.cpp, factor_adjoint_emu.cpp, factor_tangent_emu.cpp), in one
+// translation unit.
 // TEST INFRASTRUCTURE.  Every entry point takes a complete ab2::SweepParams; the layout exports below let the
 // caller's mirror of that struct check itself against this build.
 #include <cstddef>
 #include <cstring>
 
 #include "block_emu.cpp"
+#include "factor_adjoint_emu.cpp"
+#include "factor_tangent_emu.cpp"
 #include "group_emu.cpp"
+#include "resolve_emu.cpp"
 
 extern "C" int emu_sweep_params_size() { return (int)sizeof(ab2::SweepParams); }
 

@@ -1,19 +1,7 @@
 // Host emulation of the ab2_gar_factor_tangent program (aligator_b200/csrc/lq_factor_tangent.cuh): each instance runs
-// on `nl` std::threads that synchronise through a std::barrier, as the lanes of one warp or CTA do on the device.
-// Built by tests/test_factor_tangent_oracle.py with g++ -std=c++20 -pthread.
-#include <barrier>
-#include <thread>
-#include <vector>
-
+// on `nl` emulated lanes (item_emu.h).  Part of the emulation library (emu.cpp).
 #include "../../aligator_b200/csrc/lq_factor_tangent.cuh"
-
-namespace {
-struct EmuCtx {
-  int lane, nl;
-  std::barrier<> *bar;
-  void sync() const { bar->arrive_and_wait(); }
-};
-} // namespace
+#include "item_emu.h"
 
 // dims: batch, N, nx, nu, nc, nct, nc0, srec, trec, stage_head, lanes
 // in:   stage, term, fb, fbT, Vxx, Vxx0, ff, vx, ffT, d_stage, d_term
@@ -33,12 +21,7 @@ extern "C" int emu_factor_tangent(const int *dims, double mueq, const double *mu
   r.mueq_b = mueq_b;
   std::vector<double> sm(ab2::factor_tangent_item_doubles(r.nx, r.nu, r.nc));
   for (long b = 0; b < r.batch; ++b) {
-    std::barrier<> bar(nl);
-    std::vector<std::thread> th;
-    for (int l = 0; l < nl; ++l)
-      th.emplace_back([&, l] { ab2::factor_tangent_item(a, EmuCtx{l, nl, &bar}, sm.data(), b); });
-    for (auto &t : th)
-      t.join();
+    run_lanes(nl, [&](const EmuCtx &ctx) { ab2::factor_tangent_item(a, ctx, sm.data(), b); });
   }
   return 0;
 }

@@ -1,19 +1,7 @@
 // Host emulation of the ab2_gar_resolve program (aligator_b200/csrc/lq_resolve.cuh): each work item runs on `nl`
-// std::threads that synchronise through a std::barrier, as the lanes of one warp do through __syncwarp.
-// Built by tests/test_resolve_emulation.py with g++ -std=c++20 -pthread.
-#include <barrier>
-#include <thread>
-#include <vector>
-
+// emulated lanes (item_emu.h).  Part of the emulation library (emu.cpp).
 #include "../../aligator_b200/csrc/lq_resolve.cuh"
-
-namespace {
-struct EmuCtx {
-  int lane, nl;
-  std::barrier<> *bar;
-  void sync() const { bar->arrive_and_wait(); }
-};
-} // namespace
+#include "item_emu.h"
 
 // dims: batch, N, nx, nu, nc, nct, nc0, srec, trec, stage_head, nrhs, chunk, lanes
 // in:   stage, term, G0, fb, fbT, Vxx, Vxx0, q, r, d, dN, g0, f     out: xs, us, vs, vsT, lam0, lams
@@ -33,12 +21,7 @@ extern "C" int emu_resolve(const int *dims, double mueq, const double *mueq_b, c
   for (long b = 0; b < a.batch; ++b)
     for (int c = 0; c < chunks; ++c) {
       const int j0 = c * a.chunk, R = a.nrhs - j0 < a.chunk ? a.nrhs - j0 : a.chunk;
-      std::barrier<> bar(nl);
-      std::vector<std::thread> th;
-      for (int l = 0; l < nl; ++l)
-        th.emplace_back([&, l] { ab2::resolve_item(a, EmuCtx{l, nl, &bar}, sm.data(), b, j0, R); });
-      for (auto &t : th)
-        t.join();
+      run_lanes(nl, [&](const EmuCtx &ctx) { ab2::resolve_item(a, ctx, sm.data(), b, j0, R); });
     }
   return 0;
 }

@@ -4,15 +4,13 @@ differences of that recursion; and the device program itself, compiled for the h
 (tests/emu/factor_adjoint_emu.cpp), against the restatement."""
 import ctypes as C
 import functools
-import hashlib
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
+import emu_harness
 import gen
 import lq_adjoint_ref as aref
 import lq_factor_adjoint_ref as ref
@@ -171,18 +169,7 @@ def test_restatement_matches_finite_differences(case):
 # ---- host emulation of the device program ----
 @functools.lru_cache(maxsize=None)
 def _emu():
-    src = os.path.join(HERE, "emu", "factor_adjoint_emu.cpp")
-    hdrs = [os.path.join(HERE, "..", "aligator_b200", "csrc", f)
-            for f in ("lq_factor_adjoint.cuh", "lq_resolve.cuh", "vxx_layout.h")]
-    tag = hashlib.sha256(b"".join(open(p, "rb").read() for p in [src] + hdrs)).hexdigest()[:16]
-    lib = os.path.join(tempfile.gettempdir(), "ab2_factor_adjoint_emu_%d_%s.so" % (os.getuid(), tag))
-    if not os.path.exists(lib):
-        fd, tmp = tempfile.mkstemp(suffix=".so")
-        os.close(fd)
-        subprocess.check_call(["/usr/bin/g++", "-O1", "-std=c++20", "-fPIC", "-shared", "-pthread", "-w", "-o", tmp,
-                               src])
-        os.replace(tmp, lib)
-    h = C.CDLL(lib)
+    h = emu_harness.lib()
     h.emu_factor_adjoint.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
     h.emu_factor_adjoint_size_scan.restype = C.c_long
     h.emu_factor_adjoint_size_scan.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]

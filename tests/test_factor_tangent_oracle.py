@@ -5,15 +5,13 @@ reverse mode by duality; and the device program itself, compiled for the host an
 (tests/emu/factor_tangent_emu.cpp), against the restatement."""
 import ctypes as C
 import functools
-import hashlib
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
+import emu_harness
 import gen
 import lq_adjoint_ref as aref
 import lq_factor_adjoint_ref as adj
@@ -117,18 +115,7 @@ def test_duality_with_factor_adjoint(case):
 # ---- host emulation of the device program ----
 @functools.lru_cache(maxsize=None)
 def _emu():
-    src = os.path.join(HERE, "emu", "factor_tangent_emu.cpp")
-    hdrs = [os.path.join(HERE, "..", "aligator_b200", "csrc", f)
-            for f in ("lq_factor_tangent.cuh", "lq_resolve.cuh", "vxx_layout.h")]
-    tag = hashlib.sha256(b"".join(open(p, "rb").read() for p in [src] + hdrs)).hexdigest()[:16]
-    lib = os.path.join(tempfile.gettempdir(), "ab2_factor_tangent_emu_%d_%s.so" % (os.getuid(), tag))
-    if not os.path.exists(lib):
-        fd, tmp = tempfile.mkstemp(suffix=".so")
-        os.close(fd)
-        subprocess.check_call(["/usr/bin/g++", "-O1", "-std=c++20", "-fPIC", "-shared", "-pthread", "-w", "-o", tmp,
-                               src])
-        os.replace(tmp, lib)
-    h = C.CDLL(lib)
+    h = emu_harness.lib()
     h.emu_factor_tangent.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
     h.emu_factor_tangent_size_scan.restype = C.c_long
     h.emu_factor_tangent_size_scan.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -5,14 +5,12 @@ and the device program itself, compiled for the host and run on emulated lanes (
 the restatement."""
 import ctypes as C
 import functools
-import hashlib
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 
+import emu_harness
 import gen
 import lq_adjoint_ref as aref
 import lq_resolve_ref as ref
@@ -146,17 +144,7 @@ def test_identities(case):
 # ---- host emulation of the device program ----
 @functools.lru_cache(maxsize=None)
 def _emu():
-    src = os.path.join(HERE, "emu", "resolve_emu.cpp")
-    hdrs = [os.path.join(HERE, "..", "aligator_b200", "csrc", f) for f in ("lq_resolve.cuh", "vxx_layout.h")]
-    tag = hashlib.sha256(b"".join(open(p, "rb").read() for p in [src] + hdrs)).hexdigest()[:16]
-    lib = os.path.join(tempfile.gettempdir(), "ab2_resolve_emu_%d_%s.so" % (os.getuid(), tag))
-    if not os.path.exists(lib):
-        fd, tmp = tempfile.mkstemp(suffix=".so")
-        os.close(fd)
-        subprocess.check_call(["/usr/bin/g++", "-O1", "-std=c++20", "-fPIC", "-shared", "-pthread", "-w", "-o", tmp,
-                               src])
-        os.replace(tmp, lib)
-    h = C.CDLL(lib)
+    h = emu_harness.lib()
     h.emu_resolve.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
     return h
 

@@ -84,7 +84,7 @@ def main():
             if ev.device_type.name != "CUDA" or ev.count == 0:
                 continue
             t = getattr(ev, "device_time_total", None) or ev.cuda_time_total
-            key = ("records" if "adjoint_records" in ev.key else "grad" if "adjoint_grad" in ev.key
+            key = ("records" if "adjoint_records" in ev.key else "grad" if "jacobian_grad" in ev.key
                    else "sweep" if "kernel" in ev.key and "Memcpy" not in ev.key else None)
             if key:
                 kern[key] = kern.get(key, 0.0) + t / ev.count / 1e3  # ms per call

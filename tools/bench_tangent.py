@@ -73,7 +73,7 @@ def main():
             if ev.device_type.name != "CUDA" or ev.count == 0:
                 continue
             t = getattr(ev, "device_time_total", None) or ev.cuda_time_total
-            key = ("rhs" if "tangent_rhs" in ev.key else "records" if "adjoint_records" in ev.key
+            key = ("rhs" if "jacobian_rhs" in ev.key else "records" if "adjoint_records" in ev.key
                    else "sweep" if "kernel" in ev.key and "Memcpy" not in ev.key else None)
             if key:
                 kern[key] = kern.get(key, 0.0) + t / ev.count / 1e3  # ms per call
