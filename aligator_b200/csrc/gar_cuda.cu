@@ -335,22 +335,12 @@ extern "C" {
 const char *ab2_gar_last_error(void) { return g_err.c_str(); }
 const char *ab2_gar_version(void) { return "aligator_b200 gar 0.1 (sm_90a)"; }
 
-size_t ab2_gar_stage_record_doubles(int nx, int nu, int nc) {
-  size_t n = 2 * (size_t)nx * nx + 2 * (size_t)nx * nu + (size_t)nu * nu + 2 * (size_t)nx + nu +
-             (size_t)nc * (nx + nu + 1);
-  return (n + 1) & ~(size_t)1;
-}
-size_t ab2_gar_term_record_doubles(int nx, int nct) {
-  return (size_t)nx * nx + nx + (size_t)nct * nx + nct;
-}
+size_t ab2_gar_stage_record_doubles(int nx, int nu, int nc) { return ab2::stage_record_len(nx, nu, nc); }
+size_t ab2_gar_term_record_doubles(int nx, int nct) { return ab2::term_record_len(nx, nct); }
 size_t ab2_gar_stage_record_doubles_th(int nx, int nu, int nc, int nth) {
-  size_t n = 2 * (size_t)nx * nx + 2 * (size_t)nx * nu + (size_t)nu * nu + 2 * (size_t)nx + nu +
-             (size_t)nc * (nx + nu + 1) + (size_t)nth * (nx + nu + nc + nth + 1);
-  return (n + 1) & ~(size_t)1;
+  return ab2::stage_record_len(nx, nu, nc, nth);
 }
-size_t ab2_gar_term_record_doubles_th(int nx, int nct, int nth) {
-  return ab2_gar_term_record_doubles(nx, nct) + (size_t)nth * (nx + nct + nth + 1);
-}
+size_t ab2_gar_term_record_doubles_th(int nx, int nct, int nth) { return ab2::term_record_len(nx, nct, nth); }
 int ab2_gar_supported(int nx, int nu, int nc, int nc0) {
   if (nx < 1 || nu < 1 || nc < 0 || nc0 < 0)
     return 0;
@@ -1757,37 +1747,6 @@ int ab2_gar_get_problem(ab2_gar_solver *s, int what, double *dst, int memspace, 
 }
 
 // ---- symmetric blocks travel as lower triangles (ab2_gar_sweep_host_sym) ----
-// source offset, in the triangle-packed record, of element e of the full record [A|B|f|Q|S|R|q|r|C|D|d]
-static inline __host__ __device__ int sym_source(int e, int nx, int nu, int nc) {
-  const int off_q = nx * nx + nx * nu + nx, tq = nx * (nx + 1) / 2, tr = nu * (nu + 1) / 2;
-  if (e < off_q)
-    return e;
-  e -= off_q;
-  if (e < nx * nx) { // Q(i, j), column-major; the lower triangle column by column: column j holds rows j..nx-1
-    int i = e % nx, j = e / nx;
-    if (i < j) {
-      const int t = i;
-      i = j;
-      j = t;
-    }
-    return off_q + j * nx - j * (j - 1) / 2 + (i - j);
-  }
-  e -= nx * nx;
-  if (e < nx * nu)
-    return off_q + tq + e;
-  e -= nx * nu;
-  if (e < nu * nu) {
-    int i = e % nu, j = e / nu;
-    if (i < j) {
-      const int t = i;
-      i = j;
-      j = t;
-    }
-    return off_q + tq + nx * nu + j * nu - j * (j - 1) / 2 + (i - j);
-  }
-  e -= nu * nu;
-  return off_q + tq + nx * nu + tr + e; // q, r, C, D, d
-}
 namespace ab2 {
 // full records from triangle-packed ones: HBM -> HBM, a table look-up per element (built once per CTA)
 __global__ void __launch_bounds__(256) expand_sym_kernel(const double *__restrict__ src, double *__restrict__ dst, const long nrec,
@@ -1795,7 +1754,7 @@ __global__ void __launch_bounds__(256) expand_sym_kernel(const double *__restric
                                                          const int srec_pad, const int srec_sym) {
   extern __shared__ int lut[];
   for (int e = threadIdx.x; e < srec_pad; e += blockDim.x)
-    lut[e] = e < srec_full ? sym_source(e, nx, nu, nc) : -1;
+    lut[e] = e < srec_full ? ab2::sym_source(e, nx, nu, nc) : -1;
   __syncthreads();
   const long total = nrec * srec_pad;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -1809,28 +1768,18 @@ __global__ void __launch_bounds__(256) expand_sym_kernel(const double *__restric
 size_t ab2_gar_stage_record_doubles_sym(int nx, int nu, int nc) {
   if (nx < 1 || nu < 0 || nc < 0)
     return 0;
-  return (size_t)nx * nx + (size_t)nx * nu + nx + (size_t)nx * (nx + 1) / 2 + (size_t)nx * nu + (size_t)nu * (nu + 1) / 2 + nx + nu +
-         (size_t)nc * nx + (size_t)nc * nu + nc;
+  return ab2::stage_sym_len(nx, nu, nc);
 }
 
 int ab2_gar_pack_stage_sym(int nx, int nu, int nc, const double *stage, double *stage_sym, long nrec) {
   if (!stage || !stage_sym || nrec < 0 || nx < 1 || nu < 0 || nc < 0)
     return fail(AB2_ERR_INVALID, "bad argument");
-  const int full = nx * nx + nx * nu + nx + nx * nx + nx * nu + nu * nu + nx + nu + nc * nx + nc * nu + nc;
   const size_t pad = ab2_gar_stage_record_doubles(nx, nu, nc), sym = ab2_gar_stage_record_doubles_sym(nx, nu, nc);
-  std::vector<int> dst_of(sym, 0); // one full-record element per packed slot (the lower-triangle one)
-  for (int e = full - 1; e >= 0; --e) {
-    const int off_q = nx * nx + nx * nu + nx;
-    int keep = 1;
-    int r = e - off_q;
-    if (r >= 0 && r < nx * nx)
-      keep = (r % nx) >= (r / nx);
-    r -= nx * nx + nx * nu;
-    if (r >= 0 && r < nu * nu)
-      keep = (r % nu) >= (r / nu);
-    if (keep)
-      dst_of[sym_source(e, nx, nu, nc)] = e;
-  }
+  // one full-record element per packed slot: the lower-triangle one, which of a symmetric pair has the smaller
+  // column-major index and so is written last
+  std::vector<int> dst_of(sym, 0);
+  for (int e = ab2::stage_offsets(nx, nu, nc).end - 1; e >= 0; --e)
+    dst_of[ab2::sym_source(e, nx, nu, nc)] = e;
   for (long k = 0; k < nrec; ++k)
     for (size_t o = 0; o < sym; ++o)
       stage_sym[(size_t)k * sym + o] = stage[(size_t)k * pad + dst_of[o]];
@@ -1951,8 +1900,6 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
         return rc;
       const long nrec = (long)nb * N;
       if (nrec > 0) {
-        const int full = nx * nx + nx * s->d.nu + nx + nx * nx + nx * s->d.nu + s->d.nu * s->d.nu + nx + s->d.nu +
-                         s->d.nc * nx + s->d.nc * s->d.nu + s->d.nc;
         long blocks = (nrec * (long)s->srec + 255) / 256;
         if (blocks > s->p.num_sms * 8L)
           blocks = s->p.num_sms * 8L;
@@ -1968,7 +1915,7 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
                                         (int)(s->srec * sizeof(int))));
         ab2::expand_sym_kernel<<<(int)blocks, 256, s->srec * sizeof(int), st>>>(
             s->own_stage_sym + (size_t)b0 * N * srec_sym, s->own_stage + (size_t)b0 * N * s->srec, nrec, nx, s->d.nu, s->d.nc,
-            full, (int)s->srec, (int)srec_sym);
+            ab2::stage_offsets(nx, s->d.nu, s->d.nc).end, (int)s->srec, (int)srec_sym);
         CUDA_TRY(cudaGetLastError());
         s->launches += 1;
       }

@@ -11,6 +11,7 @@
 
 #include "../../include/aligator_b200/gar.h"
 #include "lq_assemble.h"
+#include "lq_record.cuh"
 
 namespace ab2 {
 
@@ -169,11 +170,12 @@ __global__ void __launch_bounds__(256)
   const long warp = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long nwarps = ((long)gridDim.x * blockDim.x) >> 5;
   const int nxx = nx * nx;
+  const TermOffsets to = term_offsets(nx, nct);
   for (long b = warp; b < batch; b += nwarps) {
     double *dst = term + b * trec;
     const double preg = preg_b ? preg_b[b] : in.preg, mu_inv = mu_inv_b ? mu_inv_b[b] : in.mu_inv;
     for (int e = lane; e < nxx; e += 32) // knot.Q = tcd.Lxx_; diag += preg
-      dst[e] = in.Lxx_N[b * nxx + e] + ((e % (nx + 1) == 0) ? preg : 0.0) +
+      dst[to.Q + e] = in.Lxx_N[b * nxx + e] + ((e % (nx + 1) == 0) ? preg : 0.0) +
                ((N == 0 && in.Hxx0) ? in.Hxx0[b * nxx + e] : 0.0); // stages[0] is the terminal knot when N = 0 (:803-804)
     for (int j = lane; j < nx; j += 32) { // knot.q = Lxs[N] + cstr_lx_corr[N]
       double full = 0.0, proj = 0.0;
@@ -184,15 +186,15 @@ __global__ void __launch_bounds__(256)
         full += pij * lv;
         proj += (pij * a) * lv;
       }
-      dst[nxx + j] = in.Lx_N[b * nx + j] + (full - proj);
+      dst[to.q + j] = in.Lx_N[b * nx + j] + (full - proj);
     }
     for (int e = lane; e < nct * nx; e += 32) {
       const int i = e % nct;
-      dst[nxx + nx + e] =
+      dst[to.C + e] =
           row_active(in.shifted_N[b * nct + i], in.loN[i], in.hiN[i]) ? in.cJx_N[b * nct * nx + e] : 0.0;
     }
     for (int e = lane; e < nct; e += 32)
-      dst[nxx + nx + nct * nx + e] = in.Lv_N[b * nct + e];
+      dst[to.d + e] = in.Lv_N[b * nct + e];
     for (int e = lane; e < nc0 * nx; e += 32) // prob.G0 = id.Jx(), prob.g0 = id.value_
       G0[b * nc0 * nx + e] = in.G0[b * nc0 * nx + e];
     for (int e = lane; e < nc0; e += 32)

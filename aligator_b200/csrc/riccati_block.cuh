@@ -72,22 +72,24 @@ AB2_HD constexpr BlockDims make_block_dims(int nx, int nu, int nc, int nc0, int 
   d.nt2 = (nx + 1 + 7) / 8;
   d.kt2 = (d.nk + 3) / 4;
   d.njp = 8 * d.nt;
-  d.off_b = nx * nx;
-  d.off_f = d.off_b + nx * nu;
-  d.off_q = d.off_f + nx;
-  d.off_s = d.off_q + nx * nx;
-  d.off_r = d.off_s + nx * nu;
-  d.off_qv = d.off_r + nu * nu;
-  d.off_rv = d.off_qv + nx;
-  d.off_c = d.off_rv + nu;
-  d.off_d = d.off_c + nc * nx;
-  d.off_dv = d.off_d + nc * nu;
-  d.off_gx = d.off_dv + nc;
-  d.off_gu = d.off_gx + nx * rec_nth;
-  d.off_gv = d.off_gu + nu * rec_nth;
-  d.off_gth = d.off_gv + nc * rec_nth;
-  d.off_gam = d.off_gth + rec_nth * rec_nth;
-  d.srec_pad = blk_ev(d.off_gam + rec_nth);
+  const StageOffsets so = stage_offsets(nx, nu, nc);
+  const TailOffsets tail = stage_tail(so, nx, nu, nc, rec_nth);
+  d.off_b = so.B;
+  d.off_f = so.f;
+  d.off_q = so.Q;
+  d.off_s = so.S;
+  d.off_r = so.R;
+  d.off_qv = so.q;
+  d.off_rv = so.r;
+  d.off_c = so.C;
+  d.off_d = so.D;
+  d.off_dv = so.d;
+  d.off_gx = tail.Gx;
+  d.off_gu = tail.Gu;
+  d.off_gv = tail.Gv;
+  d.off_gth = tail.Gth;
+  d.off_gam = tail.gamma;
+  d.srec_pad = stage_pad(tail.end);
   // (parametric knots read [Gx .. gamma] at the end of the step: no early refill of the tail)
   d.split = (d.off_q % 2 == 0 && rec_nth == 0) ? d.off_q : d.srec_pad;
   d.vs = blk_fstride(4 * d.kt);

@@ -31,8 +31,8 @@ AB2_HD constexpr DenseDims make_dense_dims(int nx, int nu, int nc, int nct, int 
   d.nct = nct;
   d.nc0 = nc0;
   d.n = nu + nc + 2 * nx;
-  d.srec = blk_ev(2 * nx * nx + 2 * nx * nu + nu * nu + 2 * nx + nu + nc * (nx + nu + 1));
-  d.trec = nx * nx + nx + nct * nx + nct;
+  d.srec = stage_record_len(nx, nu, nc);
+  d.trec = term_record_len(nx, nct);
   const int n0 = nx + nc0;
   const int nmax = d.n > n0 ? d.n : n0;
   int o = 0;

@@ -33,6 +33,7 @@
 #include <cstdint>
 #include <utility>
 
+#include "lq_record.cuh"
 #include "vxx_layout.h"
 
 #if defined(__CUDACC__)
@@ -142,10 +143,7 @@ AB2_D void flag_bad_mu(const SweepParams &p, const int inst, const bool constrai
 }
 
 // physical slot of stage knot t in the (ring-indexed) stage-record array
-AB2_HD int stage_slot(const SweepParams &p, int t) {
-  const int s = t + p.stage_head;
-  return s >= p.N ? s - p.N : s;
-}
+AB2_HD int stage_slot(const SweepParams &p, int t) { return ring_slot(t, p.stage_head, p.N); }
 // leg i of T over a horizon of N stage knots + the terminal knot (get_work, parallel-solver.hxx:23-28)
 AB2_HD int leg_begin(int N, int i, int T) { return (int)((long long)i * (N + 1) / T); }
 // doubles before block b of the condensed vector: blocks [nc0, nx, nx, nx, ...]
@@ -202,20 +200,12 @@ struct Cfg {
   // packed Vxx_t store of the tensor-core step: lane l writes the packed pairs l, l + 32, ...
   static constexpr int VPU = (PK_ && MMA_) ? (VP / 2 + 31) / 32 : 0;
   static constexpr int LUT_INTS = MMA ? 32 * (NT + NT * NT + VPU) : 0; // per-CTA table of per-lane constants
-  // stage record offsets (doubles) -- the reference's 11 buffers, concatenated
-  static constexpr int OFF_A = 0;
-  static constexpr int OFF_B = OFF_A + NX * NX;
-  static constexpr int OFF_F = OFF_B + NX * NU;
-  static constexpr int OFF_Q = OFF_F + NX;
-  static constexpr int OFF_S = OFF_Q + NX * NX;
-  static constexpr int OFF_R = OFF_S + NX * NU;
-  static constexpr int OFF_QV = OFF_R + NU * NU;
-  static constexpr int OFF_RV = OFF_QV + NX;
-  static constexpr int OFF_C = OFF_RV + NU;
-  static constexpr int OFF_D = OFF_C + NC * NX;
-  static constexpr int OFF_DV = OFF_D + NC * NU;
-  static constexpr int SREC = OFF_DV + NC;
-  static constexpr int SREC_PAD = ev(SREC);  // 16-byte granularity for bulk copies
+  // stage record offsets (doubles), lq_record.cuh
+  static constexpr StageOffsets REC = stage_offsets(NX, NU, NC);
+  static constexpr int OFF_A = REC.A, OFF_B = REC.B, OFF_F = REC.f, OFF_Q = REC.Q, OFF_S = REC.S, OFF_R = REC.R;
+  static constexpr int OFF_QV = REC.q, OFF_RV = REC.r, OFF_C = REC.C, OFF_D = REC.D, OFF_DV = REC.d;
+  static constexpr int SREC = REC.end;
+  static constexpr int SREC_PAD = stage_pad(SREC); // 16-byte granularity for bulk copies
   static constexpr int M_DBL = OFF_Q;        // [A|B|f]
   static constexpr int SPLIT = ev(M_DBL);    // part 0 = [0,SPLIT), part 1 = rest
   static constexpr int RS = ev(NX + 1);      // row stride of rhs0 / sol

@@ -7,6 +7,7 @@
 #include <cstddef>
 #include <cstring>
 
+#include "../../aligator_b200/csrc/lq_record.cuh"
 #include "block_emu.cpp"
 #include "factor_adjoint_emu.cpp"
 #include "factor_tangent_emu.cpp"
@@ -37,4 +38,21 @@ extern "C" int emu_sweep_params_offset(const char *name) {
     if (std::strcmp(f.name, name) == 0)
       return (int)f.off;
   return -1;
+}
+
+// the record layouts of lq_record.cuh, for the tests' mirror of them.  Stage: A B f Q S R q r C D d end, the tail
+// Gx Gu Gv Gth gamma end, the stored length and the triangle-packed length (20 ints).  Terminal: Q q C d end, the tail
+// Gx Gv Gth gamma end and the length (11 ints).
+extern "C" void emu_stage_layout(int nx, int nu, int nc, int nth, int *out) {
+  const ab2::StageOffsets o = ab2::stage_offsets(nx, nu, nc);
+  const ab2::TailOffsets t = ab2::stage_tail(o, nx, nu, nc, nth);
+  const int v[] = {o.A, o.B, o.f, o.Q, o.S, o.R, o.q, o.r, o.C, o.D, o.d, o.end, t.Gx, t.Gu, t.Gv, t.Gth, t.gamma, t.end,
+                   ab2::stage_record_len(nx, nu, nc, nth), ab2::stage_sym_len(nx, nu, nc)};
+  std::memcpy(out, v, sizeof(v));
+}
+extern "C" void emu_term_layout(int nx, int nct, int nth, int *out) {
+  const ab2::TermOffsets o = ab2::term_offsets(nx, nct);
+  const ab2::TailOffsets t = ab2::term_tail(o, nx, nct, nth);
+  const int v[] = {o.Q, o.q, o.C, o.d, o.end, t.Gx, t.Gv, t.Gth, t.gamma, t.end, ab2::term_record_len(nx, nct, nth)};
+  std::memcpy(out, v, sizeof(v));
 }

@@ -14,6 +14,7 @@ import tempfile
 import numpy as np
 
 import gen
+import lq_adjoint_ref
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 EMU_DIR = os.path.join(HERE, "emu")
@@ -83,14 +84,20 @@ def _F(a):
 
 
 def _parametric_records(probs, N):
-    """Stage / terminal records of parametric problems: the plain record followed by Gx, Gu, Gv, Gth, gamma."""
+    """Stage / terminal records of parametric problems: the plain record followed by Gx, Gu, Gv, Gth, gamma, each
+    block at its offset in the tests' mirror of the record layout."""
+    def record(k, off):
+        rec = np.zeros(max(e for _, e in off.values()))
+        for name, (s, e) in off.items():
+            rec[s:e] = _F(getattr(k, name))
+        return rec
+
+    rows = lambda *ms: (np.shape(m)[0] for m in ms)
     stage = []
     for p in probs:
-        rows = [np.concatenate([gen.stage_record(k), _F(k.Gx), _F(k.Gu), _F(k.Gv), _F(k.Gth), _F(k.gamma)])
-                for k in p.stages[:N]]
-        stage.append(np.stack(rows) if rows else np.zeros((0, 0)))
-    kts = [p.stages[N] for p in probs]
-    term = np.stack([np.concatenate([gen.term_record(k), _F(k.Gx), _F(k.Gv), _F(k.Gth), _F(k.gamma)]) for k in kts])
+        recs = [record(k, lq_adjoint_ref.stage_offsets(*rows(k.Q, k.R, k.C, k.Gth))[0]) for k in p.stages[:N]]
+        stage.append(np.stack(recs) if recs else np.zeros((0, 0)))
+    term = np.stack([record(k, lq_adjoint_ref.term_offsets(*rows(k.Q, k.C, k.Gth))[0]) for k in (p.stages[N] for p in probs)])
     return stage, term, np.stack([_F(p.G0) for p in probs]), np.stack([np.asarray(p.g0) for p in probs])
 
 

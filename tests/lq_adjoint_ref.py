@@ -15,10 +15,13 @@ import numpy as np
 KEYS = ("xs", "us", "vs", "vsT", "lam0", "lams")
 
 
-def stage_offsets(nx, nu, nc):
-    """Start of each block of a stage record, and the padded record length."""
+def stage_offsets(nx, nu, nc, nth=0):
+    """(start, end) of each block of a stage record, with the parametric tail when nth > 0, and the padded record
+    length.  Mirrors csrc/lq_record.cuh (checked by test_record_layout.py)."""
     sizes = [("A", nx * nx), ("B", nx * nu), ("f", nx), ("Q", nx * nx), ("S", nx * nu), ("R", nu * nu), ("q", nx),
              ("r", nu), ("C", nc * nx), ("D", nc * nu), ("d", nc)]
+    if nth:
+        sizes += [("Gx", nx * nth), ("Gu", nu * nth), ("Gv", nc * nth), ("Gth", nth * nth), ("gamma", nth)]
     off, o = {}, 0
     for k, n in sizes:
         off[k] = (o, o + n)
@@ -26,8 +29,11 @@ def stage_offsets(nx, nu, nc):
     return off, o + (o % 2)
 
 
-def term_offsets(nx, nct):
+def term_offsets(nx, nct, nth=0):
+    """(start, end) of each block of a terminal record, with the parametric tail when nth > 0, and the record length."""
     sizes = [("Q", nx * nx), ("q", nx), ("C", nct * nx), ("d", nct)]
+    if nth:
+        sizes += [("Gx", nx * nth), ("Gv", nct * nth), ("Gth", nth * nth), ("gamma", nth)]
     off, o = {}, 0
     for k, n in sizes:
         off[k] = (o, o + n)

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import gen
+import lq_adjoint_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -32,11 +33,11 @@ def _records(gar, s, nx, nu, nc, nct, nc0, N, B, seed):
     rec_nth = 0 if s.legs else s.nth
     if rec_nth:
         rng = np.random.default_rng(seed)
-        plain = 2 * nx * nx + 2 * nx * nu + nu * nu + 2 * nx + nu + nc * (nx + nu + 1)
+        off, _ = lq_adjoint_ref.stage_offsets(nx, nu, nc, rec_nth)
+        plain, end = off["d"][1], off["gamma"][1]
         st = np.zeros((B, N, s.srec))
         st[..., :plain] = stage.reshape(B, N, -1)[..., :plain]
-        st[..., plain:plain + rec_nth * (nx + nu + nc + rec_nth + 1)] = 0.1 * rng.standard_normal(
-            (B, N, rec_nth * (nx + nu + nc + rec_nth + 1)))
+        st[..., plain:end] = 0.1 * rng.standard_normal((B, N, end - plain))
         tt = np.zeros((B, s.trec))
         tt[:, :term.shape[1]] = term
         tt[:, term.shape[1]:] = 0.1 * rng.standard_normal((B, s.trec - term.shape[1]))
