@@ -72,7 +72,7 @@ def build(verbose=False, force=False, ptxas_v=False):
     for (nx, nu, nc, g) in configs():
         obj("k_%d_%d_%d" % (nx, nu, nc), "kernel_inst.cu",
             ["-DAB2_NX=%d" % nx, "-DAB2_NU=%d" % nu, "-DAB2_NC=%d" % nc, "-DAB2_G=%d" % g], "%d_%d_%d_%d" % (nx, nu, nc, g))
-    for name, src in (("capi", "gar_cuda.cu"), ("block", "block_kernel.cu"), ("kkt", "kkt_error.cu"),
+    for name, src in (("capi", "gar_cuda.cu"), ("block", "block_kernel.cu"),
                       ("assemble", "lq_assemble.cu"), ("adjoint", "lq_adjoint.cu"), ("resolve", "lq_resolve.cu"),
                       ("factor_adjoint", "lq_factor_adjoint.cu"), ("factor_tangent", "lq_factor_tangent.cu"),
                       ("jacobian", "lq_jacobian.cu"), ("refine", "lq_refine.cu"), ("linesearch", "linesearch.cu"),

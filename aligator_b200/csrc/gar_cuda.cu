@@ -17,7 +17,6 @@
 #include <vector>
 
 #include "../../include/aligator_b200/gar.h"
-#include "kkt_error.h"
 #include "linesearch.h"
 #include "lq_adjoint.h"
 #include "lq_resolve.h"
@@ -1511,21 +1510,23 @@ static int run_refine(ab2_gar_solver *s, double mueq, const double *mu_dev, int 
     a.norms = ndev;
     a.nstride = steps + 1;
     a.col = col;
-    CUDA_TRY(ab2::launch_refine_residual(a, st));
+    CUDA_TRY(ab2::launch_refine_residual(a, false, st));
     s->launches += 1;
     return AB2_OK;
   };
-  const size_t no[6] = {R * (N + 1) * d.nx, R * N * d.nu, R * N * d.nc, R * d.nct, R * d.nc0, R * N * d.nx};
   const ab2_lq_rhs rr{r->xs, r->us, r->vs, r->vsT, r->lam0, r->lams};
+  // z += dz as a linear step of length 1 over nrhs * batch instances (the [nrhs][batch][...] arrays are contiguous);
+  // z + 1.0 * dz rounds to z + dz
+  const ab2::LineSearchArgs step{(int)R, N, d.nx, d.nu, d.nc, d.nct, d.nc0,
+                                 dz->xs, dz->us, dz->vs, dz->vsT, dz->lam0, dz->lams};
+  const ab2::LinearStepIO io{z->xs, z->us, z->vs, z->vsT, z->lam0, z->lams,
+                             z->xs, z->us, z->vs, z->vsT, z->lam0, z->lams};
   for (int k = 0; k < steps; ++k) {
     if (int rc = residual(k, true)) // r = K z + h
       return rc;
     if (int rc = run_resolve(s, mueq, mu_dev, nrhs, &rr, dz, st)) // dz = -K^-1 r
       return rc;
-    ab2::RefineUpdateArgs u{{z->xs, z->us, z->vs, z->vsT, z->lam0, z->lams},
-                            {dz->xs, dz->us, dz->vs, dz->vsT, dz->lam0, dz->lams},
-                            {(long)no[0], (long)no[1], (long)no[2], (long)no[3], (long)no[4], (long)no[5]}};
-    CUDA_TRY(ab2::launch_refine_update(u, st)); // z += dz
+    CUDA_TRY(ab2::launch_linear_step(step, io, 1.0, nullptr, st)); // z += dz
     s->launches += 1;
   }
   if (ndev) {
@@ -2090,31 +2091,30 @@ static int kkt_error_impl(ab2_gar_solver *s, double mueq, const double *mueq_b, 
   CUDA_TRY(cudaSetDevice(s->d.device));
   if (!s->kkt_tmp)
     CUDA_TRY(cudaMalloc(&s->kkt_tmp, (size_t)s->d.batch * 3 * sizeof(double)));
-  ab2::KktErrorArgs a;
-  a.batch = s->d.batch;
-  a.N = s->d.horizon;
-  a.nx = s->d.nx;
-  a.nu = s->d.nu;
-  a.nc = s->d.nc;
-  a.nct = s->d.nct;
-  a.nc0 = s->d.nc0;
-  a.srec = s->srec;
-  a.trec = s->trec;
+  // the refinement's residual of the last forward pass against the problem's own vectors, with one norm per row family
+  const ab2_gar_dims &d = s->d;
+  ab2::RefineResidualArgs a{};
+  a.d = ab2::AdjointDims{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  a.nrhs = 1;
   a.stage_head = s->p.stage_head;
-  a.mueq = mueq;
-  a.mueq_b = mueq_b;
   a.stage = s->p.stage;
   a.term = s->p.term;
   a.G0 = s->p.G0;
   a.g0 = s->p.g0;
+  a.mueq = mueq;
+  a.mueq_b = mueq_b;
+  a.own = true;
   a.xs = s->out[AB2_OUT_XS];
   a.us = s->out[AB2_OUT_US];
   a.vs = s->out[AB2_OUT_VS];
   a.vsT = s->out[AB2_OUT_VST];
-  a.lbd0 = s->out[AB2_OUT_LBD0];
-  a.lbdas = s->out[AB2_OUT_LBDAS];
-  a.out = (memspace == AB2_DEVICE) ? dst : s->kkt_tmp;
-  CUDA_TRY(ab2::launch_kkt_error(a, (cudaStream_t)stream));
+  a.lam0 = s->out[AB2_OUT_LBD0];
+  a.lams = s->out[AB2_OUT_LBDAS];
+  a.norms = (memspace == AB2_DEVICE) ? dst : s->kkt_tmp;
+  a.nstride = 3;
+  a.col = 0;
+  CUDA_TRY(cudaMemsetAsync(a.norms, 0, (size_t)d.batch * 3 * sizeof(double), (cudaStream_t)stream));
+  CUDA_TRY(ab2::launch_refine_residual(a, true, (cudaStream_t)stream));
   s->launches += 1;
   if (memspace != AB2_DEVICE)
     CUDA_TRY(cudaMemcpyAsync(dst, s->kkt_tmp, (size_t)s->d.batch * 3 * sizeof(double), cudaMemcpyDeviceToHost,

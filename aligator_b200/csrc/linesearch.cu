@@ -15,33 +15,33 @@
 
 namespace ab2 {
 
-// PI: per-instance step lengths alpha_b (ab2_gar_linear_step_v); false = the scalar alpha
+// PI: per-instance step lengths alpha_b (ab2_gar_linear_step_v); false = the scalar alpha.  The arrays one after the
+// other, each a plain grid-stride loop (`trial` may be `current`, as in the refinement's z += delta).
 template <bool PI>
 __global__ void __launch_bounds__(256)
     linear_step_kernel(const LineSearchArgs a, const LinearStepIO io, const double alpha, const double *__restrict__ alpha_b) {
-  const long nX = (long)a.batch * (a.N + 1) * a.nx, nU = (long)a.batch * a.N * a.nu, nV = (long)a.batch * a.N * a.nc,
-             nVT = (long)a.batch * a.nct, nL0 = (long)a.batch * a.nc0, nL = (long)a.batch * a.N * a.nx;
-  const long total = nX + nU + nV + nVT + nL0 + nL;
-  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    long j = i, per; // per: elements of one instance in this array
+#pragma unroll 1
+  for (int f = 0; f < 6; ++f) {
+    long per; // per: elements of one instance in this array
     const double *cur, *stp;
     double *out;
-    if (j < nX) {
+    if (f == 0) {
       cur = io.xs, stp = a.dxs, out = io.txs, per = (long)(a.N + 1) * a.nx;
-    } else if ((j -= nX) < nU) {
+    } else if (f == 1) {
       cur = io.us, stp = a.dus, out = io.tus, per = (long)a.N * a.nu;
-    } else if ((j -= nU) < nV) {
+    } else if (f == 2) {
       cur = io.vs, stp = a.dvs, out = io.tvs, per = (long)a.N * a.nc;
-    } else if ((j -= nV) < nVT) {
+    } else if (f == 3) {
       cur = io.vsT, stp = a.dvsT, out = io.tvsT, per = a.nct;
-    } else if ((j -= nVT) < nL0) {
+    } else if (f == 4) {
       cur = io.lam0, stp = a.dlam0, out = io.tlam0, per = a.nc0;
     } else {
-      j -= nL0;
       cur = io.lams, stp = a.dlams, out = io.tlams, per = (long)a.N * a.nx;
     }
-    const double al = PI ? alpha_b[j / per] : alpha; // the alpha of the instance that owns the element
-    out[j] = cur[j] + al * stp[j]; // results + alpha * step, as vectorMultiplyAdd / integrate write it
+    for (long j = blockIdx.x * (long)blockDim.x + threadIdx.x; j < per * a.batch; j += (long)gridDim.x * blockDim.x) {
+      const double al = PI ? alpha_b[j / per] : alpha; // the alpha of the instance that owns the element
+      out[j] = cur[j] + al * stp[j]; // results + alpha * step, as vectorMultiplyAdd / integrate write it
+    }
   }
 }
 

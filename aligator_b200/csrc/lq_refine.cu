@@ -1,6 +1,8 @@
-// lq_refine.cu -- the two kernels of ab2_gar_refine and ab2_gar_refine_many: iterative refinement of a solution
-// estimate z of K z = -h on the last backward's factorisation, with resolve(r) = -K^-1 r (lq_resolve.cu) as the
-// correction solver.
+// lq_refine.cu -- the residual kernel of ab2_gar_refine, ab2_gar_refine_many and ab2_gar_kkt_error.  Refinement
+// improves a solution estimate z of K z = -h on the last backward's factorisation, with resolve(r) = -K^-1 r
+// (lq_resolve.cu) as the correction solver and linear_step_kernel (linesearch.cu) as the update z += delta.  The update
+// cannot be fused into the next residual launch: the residual of knot t reads x_{t+1} and lambda_t, which other warps
+// would be updating.
 //  * refine_residual_kernel: r = K z + h in resolve's rhs layouts, row by row (lambda_{t+1} = lams[t], lambda_t =
 //    lams[t-1]):
 //      q-row  Q x_t + S u_t + C^T v_t + A^T lambda_{t+1} - lambda_t + q_t     (t = 0: + G0^T lambda_0 instead of -lambda_0)
@@ -9,10 +11,11 @@
 //      f-row  A x_t + B u_t - x_{t+1} + f_t
 //      q_N    Q_N x_N + C_N^T v_N - lambda_N + q_N   (N = 0: + G0^T lambda_0),   d_N  C_N x_N - mu v_N + d_N,
 //      g0     G0 x_0 + g0
-//    Q and R are used as stored.  These are the rows of lqrComputeKktError (kkt_error.cu), so max |r| is the largest
-//    of its three norms.  h is the problem's own vectors (read from the records) or a caller's right-hand sides.
-//  * refine_update_kernel: z += delta, streaming.  It cannot be fused into the next residual launch: the residual of
-//    knot t reads x_{t+1} and lambda_t, which other warps would be updating.
+//    Q and R are used as stored.  These are the rows of lqrComputeKktError (gar/utils.hxx:88-182).  With FAMILIES the
+//    kernel keeps one maximum per row family, lqrComputeKktError's three norms: column col + 0 the f and g0 rows
+//    (dynamics), col + 1 the d and d_N rows (constraints), col + 2 the q, r and q_N rows (stationarity).  That is
+//    ab2_gar_kkt_error, with h the problem's own vectors and z the last forward pass.  Without it, one maximum of every
+//    row in column col.  h is the problem's own vectors (read from the records) or a caller's right-hand sides.
 //
 // Layout of the residual kernel: one warp per group of K consecutive stage knots, grid-stride, with K = 32 / rows per
 // knot (2 at C3, 1 at C2), so that short records leave few lanes idle.  A record of at most kTile doubles is staged
@@ -90,6 +93,7 @@ int knots_per_warp(const AdjointDims &d) {
 }
 } // namespace
 
+template <bool FAMILIES>
 __global__ void __launch_bounds__(kWarps * 32, 2) refine_residual_kernel(const RefineResidualArgs a, int K, int staged,
                                                                        int warp_doubles) {
   extern __shared__ __align__(16) double smem[];
@@ -137,7 +141,7 @@ __global__ void __launch_bounds__(kWarps * 32, 2) refine_residual_kernel(const R
         vec[p] = v;
       }
       __syncwarp();
-      double m = 0.0;
+      double m = 0.0, mc = 0.0, ms = 0.0; // FAMILIES: m the f rows, mc the d rows, ms the q and r rows
       for (int p = lane; p < kn * nrow; p += 32) {
         const int k = p / nrow, row = p - k * nrow;
         const long it = k0 + k, b = it / N, t = it - b * N, jit = (long)j * nS + it, jb = (long)j * B + b;
@@ -185,14 +189,28 @@ __global__ void __launch_bounds__(kWarps * 32, 2) refine_residual_kernel(const R
           if (a.f)
             a.f[jit * nx + i] = s;
         }
-        m = upd(m, s);
+        if constexpr (FAMILIES) {
+          if (row < nx + nu)
+            ms = upd(ms, s);
+          else if (row < nx + nu + nc)
+            mc = upd(mc, s);
+          else
+            m = upd(m, s);
+        } else {
+          m = upd(m, s);
+        }
       }
       if (a.norms)
-        for (int k = 0; k < kn; ++k) { // one maximum per knot of the group
-          const double mk = warp_max(klane == k ? m : 0.0);
+        for (int k = 0; k < kn; ++k) { // one maximum per knot of the group and family
+          double mk[FAMILIES ? 3 : 1];   // the families' warp reductions overlap when no atomic sits between them
+#pragma unroll
+          for (int f = 0; f < (FAMILIES ? 3 : 1); ++f)
+            mk[f] = warp_max(klane == k ? (f == 0 ? m : f == 1 ? mc : ms) : 0.0);
           if (lane == 0) {
             const long b = (k0 + k) / N;
-            atomic_max_nonneg(a.norms + ((long)j * B + b) * a.nstride + a.col, mk);
+#pragma unroll
+            for (int f = 0; f < (FAMILIES ? 3 : 1); ++f)
+              atomic_max_nonneg(a.norms + ((long)j * B + b) * a.nstride + a.col + f, mk[f]);
           }
         }
       __syncwarp(); // the vectors are overwritten next
@@ -208,7 +226,7 @@ __global__ void __launch_bounds__(kWarps * 32, 2) refine_residual_kernel(const R
     const double *T = a.term + b * d.trec, *G = a.G0 + b * nc0 * nx;
     const double *x = a.xs + (jb * (N + 1) + N) * nx, *vT = a.vsT + jb * nct, *x0 = a.xs + jb * (N + 1) * nx;
     const double *l0 = a.lam0 + jb * nc0, *lN = N > 0 ? a.lams + (jb * N + N - 1) * nx : nullptr;
-    double m = 0.0;
+    double m = 0.0, mc = 0.0, ms = 0.0; // FAMILIES: m the g0 rows, mc the d_N rows, ms the q_N rows
     for (int row = lane; row < trows; row += 32) {
       double s;
       if (row < nx) {
@@ -236,28 +254,32 @@ __global__ void __launch_bounds__(kWarps * 32, 2) refine_residual_kernel(const R
         if (a.g0out)
           a.g0out[jb * nc0 + i] = s;
       }
-      m = upd(m, s);
+      if constexpr (FAMILIES) {
+        if (row < nx)
+          ms = upd(ms, s);
+        else if (row < nx + nct)
+          mc = upd(mc, s);
+        else
+          m = upd(m, s);
+      } else {
+        m = upd(m, s);
+      }
     }
     if (a.norms) {
-      m = warp_max(m);
-      if (lane == 0)
-        atomic_max_nonneg(a.norms + jb * a.nstride + a.col, m);
+      double mk[FAMILIES ? 3 : 1];
+#pragma unroll
+      for (int f = 0; f < (FAMILIES ? 3 : 1); ++f)
+        mk[f] = warp_max(f == 0 ? m : f == 1 ? mc : ms);
+      if (lane == 0) {
+#pragma unroll
+        for (int f = 0; f < (FAMILIES ? 3 : 1); ++f)
+          atomic_max_nonneg(a.norms + jb * a.nstride + a.col + f, mk[f]);
+      }
     }
   }
 }
 
-__global__ void __launch_bounds__(256) refine_update_kernel(const RefineUpdateArgs a) {
-  const long i0 = (long)blockIdx.x * blockDim.x + threadIdx.x, is = (long)gridDim.x * blockDim.x;
-#pragma unroll 1
-  for (int f = 0; f < 6; ++f) {
-    double *z = a.z[f];
-    const double *dz = a.dz[f];
-    for (long i = i0; i < a.n[f]; i += is)
-      z[i] += dz[i];
-  }
-}
-
-cudaError_t launch_refine_residual(const RefineResidualArgs &a, cudaStream_t st) {
+cudaError_t launch_refine_residual(const RefineResidualArgs &a, bool families, cudaStream_t st) {
   const AdjointDims &d = a.d;
   const int K = knots_per_warp(d);
   const long nG = d.N > 0 ? ((long)d.batch * d.N + K - 1) / K : 0, items = nG + (long)d.batch * a.nrhs;
@@ -267,30 +289,18 @@ cudaError_t launch_refine_residual(const RefineResidualArgs &a, cudaStream_t st)
   const int nvec = 4 * d.nx + d.nu + d.nc;
   const int warp_doubles = ((staged ? 2 * K * d.srec : 0) + K * nvec + 1) & ~1; // (srec is even)
   const size_t smem = (size_t)warp_doubles * kWarps * sizeof(double);
-  cudaError_t e = cudaFuncSetAttribute(refine_residual_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  const auto kernel = families ? refine_residual_kernel<true> : refine_residual_kernel<false>;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;
   int per_sm = 1;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, refine_residual_kernel, kWarps * 32, smem);
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kWarps * 32, smem);
   if (e != cudaSuccess)
     return e;
   long grid = (items + kWarps - 1) / kWarps;
   const long full = (long)sm_count() * (per_sm > 0 ? per_sm : 1);
   grid = grid < full ? grid : full;
-  refine_residual_kernel<<<(int)grid, kWarps * 32, smem, st>>>(a, K, staged, warp_doubles);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_refine_update(const RefineUpdateArgs &a, cudaStream_t st) {
-  long total = 0;
-  for (int f = 0; f < 6; ++f)
-    total += a.n[f];
-  if (total <= 0)
-    return cudaSuccess;
-  long grid = (total + 255) / 256;
-  const long full = (long)sm_count() * 8;
-  grid = grid < full ? grid : full;
-  refine_update_kernel<<<(int)grid, 256, 0, st>>>(a);
+  kernel<<<(int)grid, kWarps * 32, smem, st>>>(a, K, staged, warp_doubles);
   return cudaGetLastError();
 }
 

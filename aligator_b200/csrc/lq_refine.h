@@ -1,6 +1,6 @@
-// lq_refine.h -- host interface of the two kernels of ab2_gar_refine / ab2_gar_refine_many (lq_refine.cu): the
-// residual r = K z + h of a solution estimate z and the update z += delta.  Every per-right-hand-side array is
-// [nrhs][batch][...]: block j * batch + b is right-hand side j of instance b.
+// lq_refine.h -- host interface of the residual kernel of ab2_gar_refine / ab2_gar_refine_many and ab2_gar_kkt_error
+// (lq_refine.cu): the residual r = K z + h of a solution estimate z and its infinity norms.  Every per-right-hand-side
+// array is [nrhs][batch][...]: block j * batch + b is right-hand side j of instance b.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -21,12 +21,8 @@ struct RefineResidualArgs {
   double *norms;                                  // norms[(j * batch + b) * nstride + col] = max |r|; NULL = none
   int nstride, col;
 };
-// z[i] += dz[i] for the six fields of a solution (sizes in doubles; a field of size 0 is skipped)
-struct RefineUpdateArgs {
-  double *z[6];
-  const double *dz[6];
-  long n[6];
-};
-cudaError_t launch_refine_residual(const RefineResidualArgs &a, cudaStream_t st);
-cudaError_t launch_refine_update(const RefineUpdateArgs &a, cudaStream_t st);
+// families: norms[(j * batch + b) * nstride + col + 0 / 1 / 2] = the maxima of the dynamics (f, g0), constraint
+// (d, d_N) and stationarity (q, r, q_N) rows instead of one maximum in column col.  The norms are maxima: the caller
+// zeroes them first.
+cudaError_t launch_refine_residual(const RefineResidualArgs &a, bool families, cudaStream_t st);
 } // namespace ab2

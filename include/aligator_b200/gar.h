@@ -288,7 +288,8 @@ int ab2_gar_get_gains(ab2_gar_solver *s, double *dst, int memspace, void *stream
 /* lqrComputeKktError (gar/utils.hxx:88-182) of the current problem and the solution of the last
  * forward pass, for every instance: dst[batch][3] = infinity norms of the dynamics (incl. the
  * initial condition), constraint (C x + D u + d - mu v) and stationarity residuals.  Computed on
- * the device (one warp per (instance, knot)); dst in host or device memory. */
+ * the device by ab2_gar_refine's residual kernel (one launch), with one maximum per row family; dst in
+ * host or device memory. */
 int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace, void *stream);
 /* The same with a per-instance mu: mueq [batch] in DEVICE memory (dst in host or device memory). */
 int ab2_gar_kkt_error_v(ab2_gar_solver *s, const double *mueq, double *dst, int memspace, void *stream);
@@ -536,10 +537,10 @@ int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, 
  *   f-row  A x_t + B u_t - x_{t+1} + f_t                             (in the row of lam_{t+1})
  *   q_N    Q_N x_N + C_N^T v_N - lam_N + q_N  (N = 0: + G0^T lam_0 instead of - lam_N),   d_N  C_N x_N - mu v_N + d_N
  *   g0     G0 x_0 + g0
- * with Q and R used as stored.  These are the rows ab2_gar_kkt_error takes norms of, so ||r||_inf equals the largest
- * of its three norms up to rounding.  h is the problem's own vectors (ab2_gar_refine: the primal solution) or a
- * caller's resolve right-hand sides (ab2_gar_refine_many: the adjoint's w with h = -zbar, the tangent with h = rho,
- * Jacobian columns, any resolve output).
+ * with Q and R used as stored.  These are the rows ab2_gar_kkt_error takes norms of, summed by the same kernel, so
+ * ||r||_inf equals the largest of its three norms exactly.  h is the problem's own vectors (ab2_gar_refine: the primal
+ * solution) or a caller's resolve right-hand sides (ab2_gar_refine_many: the adjoint's w with h = -zbar, the tangent
+ * with h = rho, Jacobian columns, any resolve output).
  *
  * ab2_gar_refine / _v refine the handle's own trajectory outputs (XS, US, VS, VST, LBD0, LBDAS) in place against the
  * current problem's vectors.  Every other output (FF, FB, VXX, VX, FFT, FBT, KKT0, status, pivot statistics) is

@@ -13,6 +13,7 @@ import lq_adjoint_ref as aref
 import lq_refine_ref as fref
 import lq_resolve_ref as rref
 from test_gpu_adjoint import HANDLES, _outputs, env  # noqa: F401  (env is the module fixture)
+from test_gpu_packed_vxx import _DeviceArray
 from test_refine_oracle import errors, refine_case, refined_on_oracle
 from test_resolve_oracle import _records
 
@@ -122,6 +123,41 @@ def test_norms_state_and_kernel_kinds(env, name, kw, dims):
     for k in rref.SOL:
         assert gen.rel_fro(z[k], z0[k]) <= 1e-8, (name, k)
     s.close()
+
+
+@pytest.mark.parametrize("dims,general_g0", [((12, 6, 0, 0, 12, 20, 64), False), ((4, 2, 2, 2, 3, 20, 96), True),
+                                             ((57, 28, 0, 0, 57, 6, 4), False)], ids=["C2", "C3_nct_G0", "C5"])
+def test_kkt_error_is_the_residual_norm(env, dims, general_g0):
+    """kkt_error's three norms are the per-family maxima of refine's residual: their maximum equals refine's first norm
+    bit for bit, with a scalar and a per-instance mu, on a fresh handle and after cycle_append and a sweep (nonzero ring
+    head).  A NaN in one instance's x makes that instance's dynamics and stationarity norms NaN and leaves every other
+    instance's norms as they were."""
+    gar, _, torch = env
+    nx, nu, nc, nct, nc0, N, B = dims
+    probs = gen.generate_batch(81, B, N, nx, nu, nc, nct)
+    if general_g0:
+        gen.general_initial_condition(probs, nc0, 82)
+    _, srec = aref.stage_offsets(nx, nu, nc)
+    new_last = np.zeros((B, srec))
+    new_last[:, :gen.stage_record(probs[0].stages[1]).size] = [gen.stage_record(p.stages[1]) for p in probs]
+    for mu in (1e-6, np.geomspace(1e-8, 1e-4, B)):
+        s, _ = _handle(env, {}, dims, 0, mu, probs=probs)
+        for ring in (False, True):
+            if ring:
+                s.cycle_append(new_last)
+                s.sweep(mu)
+            k = s.kkt_error(mu)
+            n = s.refine(mu, 0, norms=True)[:, 0]
+            assert np.all(np.isfinite(k)) and np.any(k > 0)
+            assert np.array_equal(k.max(axis=1).view(np.uint64), n.view(np.uint64)), (ring, k.max(axis=1), n)
+        xs = torch.as_tensor(_DeviceArray(s.device_ptr(gar.OUT_XS), B * (N + 1) * nx), device="cuda")
+        xs[(1 * (N + 1) + N // 2) * nx] = float("nan")  # instance 1, knot N / 2, x[0]
+        torch.cuda.synchronize()
+        kn = s.kkt_error(mu)
+        assert np.isnan(kn[1, 0]) and np.isnan(kn[1, 2]), kn[1]
+        others = np.arange(B) != 1
+        assert np.array_equal(kn[others].view(np.uint64), k[others].view(np.uint64))
+        s.close()
 
 
 @pytest.mark.parametrize("name,kw,dims", [KINDS[i] for i in (0, 8, 16, 17, 18)],

@@ -7,8 +7,10 @@ Per config: ms per refinement step, from CUDA events over `iters` back-to-back r
 calls (a refined trajectory stays refined, so every call does the same work), divided by two; the sweep timed the same
 way in the same run.  A separate torch.profiler run gives each kernel of a step its time, and for the residual kernel
 the HBM bandwidth its byte count implies (per stage knot: the record, z read once with x_{t+1} and lambda_t from the
-neighbours' rows in cache, r written) as a fraction of the 3350 GB/s data-sheet peak.  Prints one JSON line per config
-with the card's name and power limit read in the same run."""
+neighbours' rows in cache, r written) as a fraction of the 3350 GB/s data-sheet peak.  kkt_error is timed the same
+two ways: the call (a memset, the residual kernel with one norm per row family, a copy to the host and a synchronise)
+from CUDA events, and its kernel from torch.profiler.  Prints one JSON line per config with the card's name and power
+limit read in the same run."""
 import argparse
 import json
 import os
@@ -42,7 +44,7 @@ def profiled(torch, f):
         if ev.device_type.name != "CUDA" or ev.count == 0:
             continue
         t = getattr(ev, "device_time_total", None) or ev.cuda_time_total
-        key = ("residual" if "refine_residual" in ev.key else "update" if "refine_update" in ev.key
+        key = ("residual" if "refine_residual" in ev.key else "update" if "linear_step" in ev.key
                else "resolve" if "resolve_kernel" in ev.key else None)
         if key:
             kern[key] = kern.get(key, 0.0) + t / 1e3 / 3
@@ -83,6 +85,8 @@ def main():
         norms = s.refine(MU, 2, norms=True)
         k2 = s.kkt_error(MU).max(axis=1)
         step_ms = timed(lambda: s.refine(MU, 2)) / 2
+        kkt_ms = timed(lambda: s.kkt_error(MU))
+        kkt_kernel_ms = profiled(torch, lambda: s.kkt_error(MU))["residual"]  # the residual kernel's norms
         kern = profiled(torch, lambda: s.refine(MU, 1))
         rb = residual_bytes(nx, nu, nc, s.srec, B, N)
         res_ms = kern.get("residual", float("nan"))
@@ -91,6 +95,7 @@ def main():
                               sweep_ms=round(sweep_ms, 4), step_ms=round(step_ms, 4),
                               step_over_sweep=round(step_ms / sweep_ms, 2),
                               kernels_ms={k: round(v, 4) for k, v in kern.items()},
+                              kkt_error_ms=round(kkt_ms, 4), kkt_error_kernel_ms=round(kkt_kernel_ms, 4),
                               residual_bytes=rb, residual_GBps=round(gbs, 1), residual_frac_of_3350=round(gbs / 3350, 3),
                               kkt_max_unrefined=float(k0.max()), kkt_max_refined=float(k2.max()),
                               norm_first_max=float(norms[:, 0].max()), norm_last_max=float(norms[:, -1].max()))),
