@@ -259,6 +259,40 @@ int fail(int code, const std::string &msg) {
     if (_e != cudaSuccess)                                                                  \
       return fail(AB2_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));        \
   } while (0)
+// A device array the handle owns: allocated on first use (at least one element), reallocated when a larger size is
+// asked for (the old contents are dropped), freed with the handle.  Reads as the pointer it holds.
+template <class T> struct DevBuf {
+  T *p = nullptr;
+  size_t n = 0; // elements allocated
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  ~DevBuf() {
+    if (p)
+      cudaFree(p);
+  }
+  operator T *() const { return p; }
+  cudaError_t ensure(size_t want) {
+    if (want == 0)
+      want = 1;
+    if (n >= want)
+      return cudaSuccess;
+    if (p) {
+      const cudaError_t e = cudaFree(p);
+      p = nullptr;
+      n = 0;
+      if (e != cudaSuccess)
+        return e;
+    }
+    const cudaError_t e = cudaMalloc(&p, want * sizeof(T));
+    if (e != cudaSuccess) {
+      p = nullptr;
+      return e;
+    }
+    n = want;
+    return cudaSuccess;
+  }
+};
 } // namespace
 
 struct ab2_gar_solver {
@@ -267,17 +301,16 @@ struct ab2_gar_solver {
   int srec, trec, nr;
   ab2::SweepParams p;
   // owned device storage
-  double *own_stage = nullptr, *own_term = nullptr, *own_G0 = nullptr, *own_g0 = nullptr;
-  double *own_stage_sym = nullptr; // triangle-packed stage records as uploaded by ab2_gar_sweep_host_sym
-  double *gains_tmp = nullptr, *kkt_tmp = nullptr, *theta_dev = nullptr, *ls_tmp = nullptr;
-  double *fddp_slack = nullptr, *fddp_G0 = nullptr, *fddp_g0 = nullptr, *fddp_vx = nullptr;
-  double *inner_tmp = nullptr; // [batch][2] per-instance scalars of multipliers / criterion, for host destinations
-  double *mu_dev = nullptr;    // [batch] host-given per-instance mu of the *_v sweeps, staged for the kernels
-  double *adj_stage = nullptr, *adj_term = nullptr, *adj_g0 = nullptr; // the adjoint problem of ab2_gar_adjoint
-  double *tan_rho = nullptr; // rho of ab2_gar_tangent, in the solution's layouts (xs, us, vs, vsT, lam0, lams)
-  double *ref_buf = nullptr;   // ab2_gar_refine's residual (rhs layout) and correction (out layout)
-  double *ref_norms = nullptr; // staging of host norms of ab2_gar_refine / refine_many, ref_norms_n doubles
-  size_t ref_norms_n = 0;
+  DevBuf<double> own_stage, own_term, own_G0, own_g0;
+  DevBuf<double> own_stage_sym; // triangle-packed stage records as uploaded by ab2_gar_sweep_host_sym
+  DevBuf<double> gains_tmp, kkt_tmp, theta_dev, ls_tmp;
+  DevBuf<double> fddp_slack, fddp_G0, fddp_g0, fddp_vx;
+  DevBuf<double> inner_tmp; // [batch][2] per-instance scalars of multipliers / criterion, for host destinations
+  DevBuf<double> mu_dev;    // [batch] host-given per-instance mu of the *_v sweeps, staged for the kernels
+  DevBuf<double> adj_stage, adj_term, adj_g0; // the adjoint problem of ab2_gar_adjoint
+  DevBuf<double> tan_rho; // rho of ab2_gar_tangent, in the solution's layouts (xs, us, vs, vsT, lam0, lams)
+  DevBuf<double> ref_buf;   // ab2_gar_refine's residual (rhs layout) and correction (out layout)
+  DevBuf<double> ref_norms; // staging of host norms of ab2_gar_refine / refine_many
   int nth = 0; // parameter dimension of the value function outputs (= nx in leg mode)
   int rec_nth = 0; // parameter blocks carried by the knot records (0 in leg mode)
   int legs = 0;    // >= 2: gar::ParallelRiccatiSolver (leg mode)
@@ -287,7 +320,7 @@ struct ab2_gar_solver {
   // in place; seen by the getters only.  p.stage_head: the same for the solver-owned copy of the stage records,
   // read by the kernels through stage_slot().
   int fac_head = 0;
-  double *cond = nullptr;
+  DevBuf<double> cond;
   // fused pack + all-gather over peer memory (multi-GPU)
   int pg_world = 0, pg_rank = 0;
   unsigned long long pg_step = 0;
@@ -298,12 +331,13 @@ struct ab2_gar_solver {
   size_t pg_buf_doubles = 0;
   unsigned long long pg_pushed_step = 0; // the step whose blocks the last sweep stored into the peers itself
   bool pg_in_sweep = true;               // env AB2_PEER_IN_SWEEP=0: always use the separate pack + store kernel
-  double *out[AB2_OUT_COUNT] = {};
+  DevBuf<double> out[AB2_OUT_COUNT];  // out[w].n: doubles allocated (>= out_doubles[w])
   size_t out_doubles[AB2_OUT_COUNT] = {};
-  size_t out_alloc[AB2_OUT_COUNT] = {}; // doubles allocated behind out[w] (>= out_doubles[w])
   size_t out_rec[AB2_OUT_COUNT] = {};  // doubles per knot (or per instance)
   int out_knots[AB2_OUT_COUNT] = {};   // knots per instance (1 for per-instance arrays)
-  int *status = nullptr, *pivstat = nullptr;
+  DevBuf<int> status, pivstat;
+  // What the handle holds.  Only the transitions below (problem_replaced, factored, rolled_out, swept_host, cycled)
+  // assign these nine fields; DESIGN §1 "Handle state" tabulates them per call.
   bool have_problem = false, have_backward = false, have_forward = false;
   // ab2_gar_refine: the last backward ran on the problem's own vectors (not an adjoint / tangent problem), and the
   // trajectory outputs hold the primal solution of that factorisation (a forward since)
@@ -327,6 +361,116 @@ struct ab2_gar_solver {
 
 static size_t stage_total(const ab2_gar_solver *s) {
   return (size_t)s->d.batch * s->d.horizon * s->srec;
+}
+
+// The configured backward runs the warp-per-instance kernel, which stores Vxx packed.
+static bool warp_kernel(const ab2_gar_solver *s) { return s->k && s->variant != 9; }
+
+// ---- the handle's state transitions: each call that changes what the handle holds goes through these, after its
+//      launches have been enqueued ----
+// set_problem, assemble: new records (complete: all four arrays are held); any factorisation is stale.
+static void problem_replaced(ab2_gar_solver *s, bool complete) {
+  s->have_problem = complete;
+  s->factor_current = false;
+  s->epoch += 1;
+}
+// A backward rewrote every factor slot in knot order at this mu (mu_dev: a per-instance mu, which is not kept).
+// primal: on the problem's own vectors, not an adjoint or tangent problem.  The trajectory outputs are stale.
+static void factored(ab2_gar_solver *s, bool primal, double mueq, const double *mu_dev) {
+  if (!mu_dev)
+    s->p.mueq = mueq;
+  s->have_backward = true;
+  s->factor_current = true;
+  s->primal_factor = primal;
+  s->have_forward = false;
+  s->have_primal = false;
+  s->fac_head = 0;
+  s->vxx_packed = warp_kernel(s);
+  s->epoch += 1;
+}
+// A forward pass wrote the trajectory outputs from the last backward's factorisation.
+static void rolled_out(ab2_gar_solver *s) {
+  s->have_forward = true;
+  s->have_primal = s->primal_factor;
+}
+// ab2_gar_sweep_host: new records, factored and rolled out, counted as one change of the factorisation.
+static void swept_host(ab2_gar_solver *s, double mueq, const double *mu_dev) {
+  s->have_problem = true;
+  factored(s, true, mueq, mu_dev);
+  rolled_out(s);
+}
+// cycle_append: the rings advanced by one knot (the parallel solver zeroed its factors instead); nothing is current.
+static void cycled(ab2_gar_solver *s) {
+  if (s->legs <= 1)
+    s->fac_head = (s->fac_head + 1) % s->d.horizon;
+  s->have_backward = false;
+  s->have_forward = false;
+  s->have_primal = false;
+  s->factor_current = false;
+  s->epoch += 1;
+}
+
+// ---- small shared pieces of the calls ----
+// the copy kind of a result for the caller's memspace
+static cudaMemcpyKind out_kind(int memspace) {
+  return memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+}
+// grid of a 256-thread grid-stride kernel over n elements: at most 8 CTAs per SM
+static int grid_for(const ab2_gar_solver *s, size_t n) {
+  const long blocks = (long)((n + 255) / 256);
+  return (int)(blocks > s->p.num_sms * 8L ? s->p.num_sms * 8L : blocks);
+}
+static ab2::AdjointDims adjoint_dims(const ab2_gar_solver *s) {
+  const ab2_gar_dims &d = s->d;
+  return ab2::AdjointDims{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+}
+// the handle's trajectory outputs
+static ab2_ls_trial trajectory(const ab2_gar_solver *s) {
+  return ab2_ls_trial{s->out[AB2_OUT_XS], s->out[AB2_OUT_US],   s->out[AB2_OUT_VS],
+                      s->out[AB2_OUT_VST], s->out[AB2_OUT_LBD0], s->out[AB2_OUT_LBDAS]};
+}
+// `count` arrays t[0 .. count) of the solution's layouts (xs .. lams, one batch each) in the handle's buffer buf
+static int sol_scratch(ab2_gar_solver *s, DevBuf<double> &buf, int count, ab2_ls_trial *t) {
+  const ab2_gar_dims &d = s->d;
+  const size_t B = d.batch, N = d.horizon;
+  const size_t n[6] = {B * (N + 1) * d.nx, B * N * d.nu, B * N * d.nc, B * d.nct, B * d.nc0, B * N * d.nx};
+  const size_t one = n[0] + n[1] + n[2] + n[3] + n[4] + n[5];
+  CUDA_TRY(buf.ensure(count * one));
+  for (int i = 0; i < count; ++i) {
+    t[i].xs = buf.p + i * one;
+    t[i].us = t[i].xs + n[0];
+    t[i].vs = t[i].us + n[1];
+    t[i].vsT = t[i].vs + n[2];
+    t[i].lam0 = t[i].vsT + n[3];
+    t[i].lams = t[i].lam0 + n[4];
+  }
+  return AB2_OK;
+}
+// the SweepParams member of each output, indexed by AB2_OUT_*
+static double *ab2::SweepParams::*const kOutMember[AB2_OUT_COUNT] = {
+    &ab2::SweepParams::ff,   &ab2::SweepParams::fb,     &ab2::SweepParams::Vxx,     &ab2::SweepParams::vx,
+    &ab2::SweepParams::ffT,  &ab2::SweepParams::fbT,    &ab2::SweepParams::kkt0,    &ab2::SweepParams::xs,
+    &ab2::SweepParams::us,   &ab2::SweepParams::vs,     &ab2::SweepParams::vsT,     &ab2::SweepParams::lbd0,
+    &ab2::SweepParams::lbdas, &ab2::SweepParams::fth,   &ab2::SweepParams::Vxt,     &ab2::SweepParams::Vtt,
+    &ab2::SweepParams::vt,   &ab2::SweepParams::kkt0fth, &ab2::SweepParams::thGrad, &ab2::SweepParams::thHess};
+// An n-double result of a call: the kernels write it at dev, which is the caller's buffer dst when that is device
+// memory and the handle's scratch otherwise; copy_out() then copies the scratch to dst.
+struct Staged {
+  double *dst, *dev;
+  size_t n;
+  int copy_out(cudaStream_t st) const {
+    if (dev != dst)
+      CUDA_TRY(cudaMemcpyAsync(dst, dev, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+    return AB2_OK;
+  }
+};
+static int stage_result(DevBuf<double> &scratch, double *dst, bool on_device, size_t n, Staged *r) {
+  *r = Staged{dst, dst, n};
+  if (!on_device) {
+    CUDA_TRY(scratch.ensure(n));
+    r->dev = scratch;
+  }
+  return AB2_OK;
 }
 
 extern "C" {
@@ -440,84 +584,48 @@ static int create_impl(const ab2_gar_dims *dims, int nth, int legs, ab2_gar_solv
   setup(AB2_OUT_THHESS, (size_t)nth * nth, 1);
   // warp-per-instance handles: VXX holds either layout (packed + the full slot-0 array, or full blocks for variant 9)
   const size_t vxx_packed_total = (size_t)B * (N + 1) * ab2::vxx_packed_doubles(nx) + (size_t)B * nx * nx;
+  // allocated and zeroed; on failure the handle is destroyed and the message names the array
+  auto alloc = [&](auto &buf, size_t n, const char *what) -> int {
+    cudaError_t e = buf.ensure(n);
+    if (e == cudaSuccess)
+      e = cudaMemset(buf.p, 0, n * sizeof(*buf.p));
+    if (e != cudaSuccess) {
+      ab2_gar_destroy(s);
+      return fail(AB2_ERR_CUDA, std::string("cudaMalloc ") + what + ": " + cudaGetErrorString(e));
+    }
+    return AB2_OK;
+  };
+  ab2::SweepParams &p = s->p;
+  std::memset(&p, 0, sizeof(p));
   for (int w = 0; w < AB2_OUT_COUNT; ++w) {
     // (+2: the forward pass of the CTA-per-instance kernel fetches odd-sized gain records
     // with 16-byte granularity, up to one double past the end of the array)
     size_t n = s->out_doubles[w];
     if (w == AB2_OUT_VXX && s->k && vxx_packed_total > n)
       n = vxx_packed_total;
-    const size_t bytes = (n > 0 ? n + 2 : 2) * sizeof(double);
-    s->out_alloc[w] = bytes / sizeof(double);
-    cudaError_t e = cudaMalloc(&s->out[w], bytes);
-    if (e == cudaSuccess)
-      e = cudaMemset(s->out[w], 0, bytes);
-    if (e != cudaSuccess) {
-      ab2_gar_destroy(s);
-      return fail(AB2_ERR_CUDA, std::string("cudaMalloc outputs: ") + cudaGetErrorString(e));
-    }
+    if (int rc = alloc(s->out[w], n + 2, "outputs"))
+      return rc;
+    p.*kOutMember[w] = s->out[w];
   }
-  {
-    cudaError_t e = cudaMalloc(&s->status, sizeof(int) * B);
-    if (e == cudaSuccess)
-      e = cudaMemset(s->status, 0, sizeof(int) * B);
-    if (e != cudaSuccess) {
-      ab2_gar_destroy(s);
-      return fail(AB2_ERR_CUDA, std::string("cudaMalloc status: ") + cudaGetErrorString(e));
-    }
-  }
-  {
-    cudaError_t e = cudaMalloc(&s->pivstat, sizeof(int) * B);
-    if (e == cudaSuccess)
-      e = cudaMemset(s->pivstat, 0, sizeof(int) * B);
-    if (e != cudaSuccess) {
-      ab2_gar_destroy(s);
-      return fail(AB2_ERR_CUDA, std::string("cudaMalloc pivstat: ") + cudaGetErrorString(e));
-    }
-  }
-  if (legs > 1) {
-    const size_t td = (size_t)d.nc0 + (size_t)d.nx * (2 * legs - 1);
-    cudaError_t e = cudaMalloc(&s->cond, sizeof(double) * B * td);
-    if (e == cudaSuccess)
-      e = cudaMemset(s->cond, 0, sizeof(double) * B * td);
-    if (e != cudaSuccess) {
-      ab2_gar_destroy(s);
-      return fail(AB2_ERR_CUDA, std::string("cudaMalloc cond: ") + cudaGetErrorString(e));
-    }
-  }
-  ab2::SweepParams &p = s->p;
-  std::memset(&p, 0, sizeof(p));
+  if (int rc = alloc(s->status, B, "status"))
+    return rc;
+  if (int rc = alloc(s->pivstat, B, "pivstat"))
+    return rc;
+  if (legs > 1)
+    if (int rc = alloc(s->cond, (size_t)B * ((size_t)d.nc0 + (size_t)d.nx * (2 * legs - 1)), "cond"))
+      return rc;
   p.legs = legs;
   p.cond = s->cond;
   p.N = N;
   p.nct = d.nct;
   p.nc0 = d.nc0;
   p.batch = B;
-  p.ff = s->out[AB2_OUT_FF];
-  p.fb = s->out[AB2_OUT_FB];
-  p.Vxx = s->out[AB2_OUT_VXX];
   if (s->k)
     p.Vxx0 = p.Vxx + (size_t)B * (N + 1) * ab2::vxx_packed_doubles(nx);
-  p.vx = s->out[AB2_OUT_VX];
-  p.ffT = s->out[AB2_OUT_FFT];
-  p.fbT = s->out[AB2_OUT_FBT];
-  p.kkt0 = s->out[AB2_OUT_KKT0];
-  p.xs = s->out[AB2_OUT_XS];
-  p.us = s->out[AB2_OUT_US];
-  p.vs = s->out[AB2_OUT_VS];
-  p.vsT = s->out[AB2_OUT_VST];
-  p.lbd0 = s->out[AB2_OUT_LBD0];
-  p.lbdas = s->out[AB2_OUT_LBDAS];
   p.status = s->status;
   p.pivstat = s->pivstat;
   p.nth = nth;
   p.theta = nullptr;
-  p.fth = s->out[AB2_OUT_FTH];
-  p.Vxt = s->out[AB2_OUT_VXT];
-  p.Vtt = s->out[AB2_OUT_VTT];
-  p.vt = s->out[AB2_OUT_VT];
-  p.kkt0fth = s->out[AB2_OUT_KKT0FTH];
-  p.thGrad = s->out[AB2_OUT_THGRAD];
-  p.thHess = s->out[AB2_OUT_THHESS];
   {
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d.device);
@@ -536,14 +644,7 @@ static int create_impl(const ab2_gar_dims *dims, int nth, int legs, ab2_gar_solv
 int ab2_gar_destroy(ab2_gar_solver *s) {
   if (!s)
     return AB2_OK;
-  cudaSetDevice(s->d.device);
-  for (int w = 0; w < AB2_OUT_COUNT; ++w)
-    if (s->out[w])
-      cudaFree(s->out[w]);
-  if (s->status)
-    cudaFree(s->status);
-  if (s->pivstat)
-    cudaFree(s->pivstat);
+  cudaSetDevice(s->d.device); // (the DevBuf members are freed by delete, on this device)
   for (int w = 0; w < s->pg_world; ++w)
     if (w != s->pg_rank && s->pg_peer_base[w])
       cudaIpcCloseMemHandle(s->pg_peer_base[w]);
@@ -551,11 +652,6 @@ int ab2_gar_destroy(ab2_gar_solver *s) {
     cudaFree(s->pg_local);
   if (s->pg_done)
     cudaFree(s->pg_done);
-  for (double *q : {s->own_stage_sym, s->own_stage, s->own_term, s->own_G0, s->own_g0, s->gains_tmp, s->kkt_tmp, s->theta_dev, s->cond, s->ls_tmp, s->fddp_slack, s->fddp_G0,
-                    s->fddp_g0, s->fddp_vx, s->inner_tmp, s->mu_dev, s->adj_stage, s->adj_term, s->adj_g0, s->tan_rho,
-                    s->ref_buf, s->ref_norms})
-    if (q)
-      cudaFree(q);
   for (int i = 0; i < ab2_gar_solver::kPipeStreams; ++i) {
     if (s->pipe_done[i])
       cudaEventDestroy(s->pipe_done[i]);
@@ -603,11 +699,10 @@ int ab2_gar_set_problem(ab2_gar_solver *s, const double *stage, const double *te
     if (g0)
       s->p.g0 = g0;
   } else if (memspace == AB2_HOST) {
-    auto up = [&](double *&own, const double *src, size_t n, const double *&dst) -> int {
+    auto up = [&](DevBuf<double> &own, const double *src, size_t n, const double *&dst) -> int {
       if (!src)
         return AB2_OK;
-      if (!own)
-        CUDA_TRY(cudaMalloc(&own, (n > 0 ? n : 1) * sizeof(double)));
+      CUDA_TRY(own.ensure(n));
       if (n)
         CUDA_TRY(cudaMemcpyAsync(own, src, n * sizeof(double), cudaMemcpyHostToDevice, st));
       dst = own;
@@ -627,16 +722,10 @@ int ab2_gar_set_problem(ab2_gar_solver *s, const double *stage, const double *te
   } else {
     return fail(AB2_ERR_INVALID, "memspace must be AB2_HOST or AB2_DEVICE");
   }
-  s->have_problem = s->p.stage && s->p.term && (s->p.G0 || s->d.nc0 == 0) && (s->p.g0 || s->d.nc0 == 0);
-  if (s->d.horizon == 0 && s->p.term)
-    s->have_problem = true;
-  s->factor_current = false;
-  s->epoch += 1;
+  problem_replaced(s, (s->p.stage && s->p.term && (s->p.G0 || s->d.nc0 == 0) && (s->p.g0 || s->d.nc0 == 0)) ||
+                          (s->d.horizon == 0 && s->p.term));
   return AB2_OK;
 }
-
-// The configured backward runs the warp-per-instance kernel, which stores Vxx packed.
-static bool warp_kernel(const ab2_gar_solver *s) { return s->k && s->variant != 9; }
 
 // SweepParams of the instances [b0, b0 + nb) of a backward + forward launch: every array leads with the batch index.
 static ab2::SweepParams slice_params(const ab2_gar_solver *s, int b0, int nb) {
@@ -650,37 +739,17 @@ static ab2::SweepParams slice_params(const ab2_gar_solver *s, int b0, int nb) {
     q.G0 += b * s->d.nc0 * nx;
   if (q.g0)
     q.g0 += b * s->d.nc0;
-  q.ff += b * s->out_knots[AB2_OUT_FF] * s->out_rec[AB2_OUT_FF];
-  q.fb += b * s->out_knots[AB2_OUT_FB] * s->out_rec[AB2_OUT_FB];
+  for (int w = 0; w < AB2_OUT_COUNT; ++w) // (the value-function outputs of nth = 0 have zero-sized records)
+    if (w != AB2_OUT_VXX || !warp_kernel(s))
+      q.*kOutMember[w] += b * s->out_knots[w] * s->out_rec[w];
   if (warp_kernel(s)) {
     q.Vxx += b * (N + 1) * ab2::vxx_packed_doubles(nx);
     q.Vxx0 += b * nx * nx;
-  } else {
-    q.Vxx += b * s->out_knots[AB2_OUT_VXX] * s->out_rec[AB2_OUT_VXX];
   }
-  q.vx +=b * s->out_knots[AB2_OUT_VX] * s->out_rec[AB2_OUT_VX];
-  q.ffT += b * s->out_rec[AB2_OUT_FFT];
-  q.fbT += b * s->out_rec[AB2_OUT_FBT];
-  q.kkt0 += b * s->out_rec[AB2_OUT_KKT0];
-  q.xs += b * s->out_knots[AB2_OUT_XS] * s->out_rec[AB2_OUT_XS];
-  q.us += b * s->out_knots[AB2_OUT_US] * s->out_rec[AB2_OUT_US];
-  q.vs += b * s->out_knots[AB2_OUT_VS] * s->out_rec[AB2_OUT_VS];
-  q.vsT += b * s->out_rec[AB2_OUT_VST];
-  q.lbd0 += b * s->out_rec[AB2_OUT_LBD0];
-  q.lbdas += b * s->out_knots[AB2_OUT_LBDAS] * s->out_rec[AB2_OUT_LBDAS];
   q.status += b;
   q.pivstat += b;
-  if (s->nth > 0) {
-    q.fth += b * s->out_knots[AB2_OUT_FTH] * s->out_rec[AB2_OUT_FTH];
-    q.Vxt += b * s->out_knots[AB2_OUT_VXT] * s->out_rec[AB2_OUT_VXT];
-    q.Vtt += b * s->out_knots[AB2_OUT_VTT] * s->out_rec[AB2_OUT_VTT];
-    q.vt += b * s->out_knots[AB2_OUT_VT] * s->out_rec[AB2_OUT_VT];
-    q.kkt0fth += b * s->out_rec[AB2_OUT_KKT0FTH];
-    q.thGrad += b * s->out_rec[AB2_OUT_THGRAD];
-    q.thHess += b * s->out_rec[AB2_OUT_THHESS];
-    if (q.theta)
-      q.theta += b * s->nth;
-  }
+  if (q.theta)
+    q.theta += b * s->nth;
   if (q.cond)
     q.cond += b * ((size_t)s->d.nc0 + (size_t)nx * (2 * s->legs - 1));
   return q;
@@ -735,11 +804,11 @@ static int launch(ab2_gar_solver *s, double mueq, const double *mueq_b, int bwd,
   if (bwd && !mueq_b && !(mueq > 0.0) && (s->d.nc > 0 || s->d.nct > 0))
     return fail(AB2_ERR_INVALID, "mueq must be > 0 when constraints are present");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  if (!mueq_b)
-    s->p.mueq = mueq;
   s->p.do_bwd = bwd;
   s->p.do_fwd = fwd;
   ab2::SweepParams q = s->p;
+  if (!mueq_b)
+    q.mueq = mueq;
   q.mueq_b = mueq_b;
   q.peer_world = 0;
   if (bwd && s->pg_in_sweep && s->pg_peer_base[0] && s->k && s->variant != 9 && s->legs <= 1 && !s->dense &&
@@ -756,16 +825,10 @@ static int launch(ab2_gar_solver *s, double mueq, const double *mueq_b, int bwd,
   }
   if (int rc = run_kernels(s, q, bwd, fwd, (cudaStream_t)stream))
     return rc;
-  if (bwd) {
-    s->have_backward = true;
-    s->fac_head = 0; // every factor slot was rewritten in knot order
-    s->vxx_packed = warp_kernel(s);
-    s->factor_current = true;
-    s->epoch += 1;
-    s->primal_factor = true;
-  }
-  s->have_forward = fwd != 0; // a backward-only launch invalidates the previous trajectory
-  s->have_primal = fwd != 0 && s->primal_factor;
+  if (bwd)
+    factored(s, true, mueq, mueq_b);
+  if (fwd)
+    rolled_out(s);
   return AB2_OK;
 }
 
@@ -790,8 +853,7 @@ static int stage_mueq(ab2_gar_solver *s, const double *mueq, int memspace, cudaS
       if (!(mueq[b] > 0.0))
         return fail(AB2_ERR_INVALID, "mueq[" + std::to_string(b) + "] must be > 0 when constraints are present");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  if (!s->mu_dev)
-    CUDA_TRY(cudaMalloc(&s->mu_dev, (size_t)s->d.batch * sizeof(double)));
+  CUDA_TRY(s->mu_dev.ensure(s->d.batch));
   CUDA_TRY(cudaMemcpyAsync(s->mu_dev, mueq, (size_t)s->d.batch * sizeof(double), cudaMemcpyHostToDevice, st));
   *dev = s->mu_dev;
   return AB2_OK;
@@ -823,8 +885,7 @@ int ab2_gar_forward_theta(ab2_gar_solver *s, const double *theta, int memspace, 
     if (memspace == AB2_DEVICE) {
       s->p.theta = theta;
     } else {
-      if (!s->theta_dev)
-        CUDA_TRY(cudaMalloc(&s->theta_dev, (size_t)s->d.batch * s->nth * sizeof(double)));
+      CUDA_TRY(s->theta_dev.ensure((size_t)s->d.batch * s->nth));
       CUDA_TRY(cudaMemcpyAsync(s->theta_dev, theta, (size_t)s->d.batch * s->nth * sizeof(double),
                                cudaMemcpyHostToDevice, (cudaStream_t)stream));
       s->p.theta = s->theta_dev;
@@ -847,29 +908,33 @@ struct Fields {
 typedef std::pair<const Fields *, const Fields *> FieldPair;
 static const char *const kSolNames[6] = {"xs", "us", "vs", "vsT", "lam0", "lams"};
 static const char *const kRecNames[4] = {"stage", "term", "G0", "g0"};
-// fields in the solution's layouts, `blocks` instances (batch, or nrhs * batch)
-static Fields sol_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
+} // extern "C"
+// the fields p, per[i] doubles per instance, `blocks` instances
+static Fields make_fields(const char *what, const char *const *names, std::initializer_list<const double *> p,
+                          const size_t *per, size_t blocks) {
+  Fields f{what, names, {}, {}, (int)p.size()};
+  int i = 0;
+  for (const double *q : p) {
+    f.p[i] = q;
+    f.n[i] = blocks * per[i];
+    ++i;
+  }
+  return f;
+}
+// the fields xs .. lams of v (an ab2_ls_iterate, ab2_ls_trial or the correction of ab2_lq_refine_work) in the
+// solution's layouts, `blocks` instances (batch, or nrhs * batch)
+template <class T> static Fields sol_fields(const ab2_gar_solver *s, const char *what, const T &v, size_t blocks) {
   const ab2_gar_dims &d = s->d;
   const int N = d.horizon;
   const size_t per[6] = {(size_t)(N + 1) * d.nx, (size_t)N * d.nu, (size_t)N * d.nc, (size_t)d.nct, (size_t)d.nc0,
                          (size_t)N * d.nx};
-  Fields f{what, kSolNames, {}, {}, 6};
-  for (int i = 0; i < 6; ++i) {
-    f.p[i] = p[i];
-    f.n[i] = blocks * per[i];
-  }
-  return f;
+  return make_fields(what, kSolNames, {v.xs, v.us, v.vs, v.vsT, v.lam0, v.lams}, per, blocks);
 }
-// fields in the problem's record layouts (stage, term, G0, g0), `blocks` instances
-static Fields rec_fields(const ab2_gar_solver *s, const char *what, const double *const p[4], size_t blocks) {
+// the fields stage, term, G0, g0 of v (an ab2_lq_grad or ab2_lq_tangent) in the problem's record layouts
+template <class T> static Fields rec_fields(const ab2_gar_solver *s, const char *what, const T &v, size_t blocks) {
   const ab2_gar_dims &d = s->d;
   const size_t per[4] = {(size_t)d.horizon * s->srec, (size_t)s->trec, (size_t)d.nc0 * d.nx, (size_t)d.nc0};
-  Fields f{what, kRecNames, {}, {}, 4};
-  for (int i = 0; i < 4; ++i) {
-    f.p[i] = p[i];
-    f.n[i] = blocks * per[i];
-  }
-  return f;
+  return make_fields(what, kRecNames, {v.stage, v.term, v.G0, v.g0}, per, blocks);
 }
 static int require(const Fields &f, const char *who) {
   for (int i = 0; i < f.count; ++i)
@@ -887,25 +952,23 @@ static int refuse_overlap(const Fields &a, const Fields &b, const char *who) {
   return AB2_OK;
 }
 static const char *const kRhsNames[6] = {"q", "r", "d", "dN", "g0", "f"};
-// fields in resolve's rhs layouts (the same sizes as the solution's), `blocks` instances
-static Fields rhs_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
-  Fields f = sol_fields(s, what, p, blocks);
+// the fields q .. f of v (an ab2_lq_rhs or the residual of ab2_lq_refine_work) in resolve's rhs layouts (the same
+// sizes as the solution's)
+template <class T> static Fields rhs_fields(const ab2_gar_solver *s, const char *what, const T &v, size_t blocks) {
+  Fields f = sol_fields(s, what, ab2_ls_iterate{v.q, v.r, v.d, v.dN, v.g0, v.f}, blocks);
   f.names = kRhsNames;
   return f;
 }
 static const char *const kFacNames[6] = {"ff", "fb", "vxx", "vx", "fft", "fbt"};
-// fields in ab2_gar_get's layouts of the factorisation (FF .. FBT, vxx as full blocks), `blocks` instances
-static Fields fac_fields(const ab2_gar_solver *s, const char *what, const double *const p[6], size_t blocks) {
+// the fields of v (an ab2_factor_cotangent or ab2_factor_tangent) in ab2_gar_get's layouts of the factorisation
+// (FF .. FBT, vxx as full blocks)
+template <class T> static Fields fac_fields(const ab2_gar_solver *s, const char *what, const T &v, size_t blocks) {
   const ab2_gar_dims &d = s->d;
   const size_t N = d.horizon, nx = d.nx, nr = d.nu + d.nc + d.nx;
   const size_t per[6] = {N * nr, N * nr * nx, (N + 1) * nx * nx, (N + 1) * nx, (size_t)d.nct, (size_t)d.nct * nx};
-  Fields f{what, kFacNames, {}, {}, 6};
-  for (int i = 0; i < 6; ++i) {
-    f.p[i] = p[i];
-    f.n[i] = blocks * per[i];
-  }
-  return f;
+  return make_fields(what, kFacNames, {v.ff, v.fb, v.vxx, v.vx, v.fft, v.fbt}, per, blocks);
 }
+extern "C" {
 static const char *const kOutNames[AB2_OUT_COUNT] = {"FF",   "FB",    "VXX",  "VX",  "FFT",     "FBT",    "KKT0",
                                                      "XS",   "US",    "VS",   "VST", "LBD0",    "LBDAS",  "FTH",
                                                      "VXT",  "VTT",   "VT",   "KKT0FTH", "THGRAD", "THHESS"};
@@ -914,7 +977,7 @@ static Fields out_fields(const ab2_gar_solver *s) {
   Fields f{"the handle's output", kOutNames, {}, {}, AB2_OUT_COUNT};
   for (int w = 0; w < AB2_OUT_COUNT; ++w) {
     f.p[w] = s->out[w];
-    f.n[w] = s->out_alloc[w];
+    f.n[w] = s->out[w].n;
   }
   return f;
 }
@@ -949,44 +1012,30 @@ static int check_solve_handle(const ab2_gar_solver *s, const char *who) {
 // handle's own sweep (two launches).  mu_dev: the staged per-instance mu, or null for the scalar mueq.
 static int solve_cotangent_problem(ab2_gar_solver *s, double mueq, const double *mu_dev, const ab2_ls_iterate *cot,
                                    bool copy, cudaStream_t st) {
-  const ab2_gar_dims &d = s->d;
-  const int B = d.batch, N = d.horizon, nx = d.nx;
-  auto own = [&](double *&buf, size_t n) -> int {
-    if (!buf)
-      CUDA_TRY(cudaMalloc(&buf, (n > 0 ? n : 1) * sizeof(double)));
-    return AB2_OK;
-  };
-  int rc;
-  if ((rc = own(s->adj_stage, stage_total(s))) != AB2_OK || (rc = own(s->adj_term, (size_t)B * s->trec)) != AB2_OK ||
-      (rc = own(s->adj_g0, (size_t)B * d.nc0)) != AB2_OK)
-    return rc;
-  const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  const size_t B = s->d.batch;
+  CUDA_TRY(s->adj_stage.ensure(stage_total(s)));
+  CUDA_TRY(s->adj_term.ensure(B * s->trec));
+  CUDA_TRY(s->adj_g0.ensure(B * s->d.nc0));
   // 1. the problem: same matrices, vectors = -cot (copy: cot)
-  ab2::AdjointRecordArgs ra{ad, s->p.stage_head, s->p.stage, s->p.term, cot->xs, cot->us, cot->vs, cot->vsT,
-                            cot->lam0, cot->lams, s->adj_stage, s->adj_term, s->adj_g0, copy};
+  ab2::AdjointRecordArgs ra{adjoint_dims(s), s->p.stage_head, s->p.stage, s->p.term, cot->xs, cot->us, cot->vs,
+                            cot->vsT, cot->lam0, cot->lams, s->adj_stage, s->adj_term, s->adj_g0, copy};
   CUDA_TRY(ab2::launch_adjoint_records(ra, st));
   s->launches += 1;
   // 2. backward + forward on it; the problem pointers change in this launch's copy of the parameters only, and a
   //    sharded handle never publishes these gains to its peers
-  if (!mu_dev)
-    s->p.mueq = mueq;
   ab2::SweepParams q = s->p;
+  if (!mu_dev)
+    q.mueq = mueq;
   q.stage = s->adj_stage;
   q.stage_head = 0;
   q.term = s->adj_term;
   q.g0 = s->adj_g0;
   q.mueq_b = mu_dev;
   q.peer_world = 0;
-  if ((rc = run_kernels(s, q, 1, 1, st)) != AB2_OK)
+  if (int rc = run_kernels(s, q, 1, 1, st))
     return rc;
-  s->have_backward = true;
-  s->have_forward = true;
-  s->primal_factor = false; // the trajectory outputs are w or zdot, not the primal solution
-  s->have_primal = false;
-  s->fac_head = 0;
-  s->vxx_packed = warp_kernel(s);
-  s->factor_current = true;
-  s->epoch += 1;
+  factored(s, false, mueq, mu_dev); // the trajectory outputs are w or zdot, not the primal solution
+  rolled_out(s);
   return AB2_OK;
 }
 
@@ -999,30 +1048,25 @@ static int adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
   if (int rc = check_solve_handle(s, who))
     return rc;
   // the gradient kernel reads the primal after the sweep has overwritten the handle's outputs
-  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
-  const Fields P = sol_fields(s, "primal", pp, s->d.batch);
+  const Fields P = sol_fields(s, "primal", *primal, s->d.batch);
   if (int rc = require(P, who))
     return rc;
   if (int rc = refuse_overlap(P, out_fields(s), who))
     return rc;
   if (int rc = check_mu(s, mueq, mueq_arr, who))
     return rc;
-  const ab2_gar_dims &d = s->d;
-  const int B = d.batch, N = d.horizon, nx = d.nx;
   cudaStream_t st;
   const double *mu_dev;
   if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
     return rc;
   // 1. + 2. the adjoint problem (vectors = -cotangent) and its solve
-  int rc;
-  if ((rc = solve_cotangent_problem(s, mueq, mu_dev, cot, false, st)) != AB2_OK)
+  if (int rc = solve_cotangent_problem(s, mueq, mu_dev, cot, false, st))
     return rc;
-  const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
   // 3. gradient records from the primal z and the adjoint w (the trajectory outputs): dh = -w, dK = -w z^T
-  ab2::JacobianGradArgs ga{ad, 1,
+  const ab2_ls_trial w = trajectory(s);
+  ab2::JacobianGradArgs ga{adjoint_dims(s), 1,
                            primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
-                           s->out[AB2_OUT_XS], s->out[AB2_OUT_US], s->out[AB2_OUT_VS], s->out[AB2_OUT_VST],
-                           s->out[AB2_OUT_LBD0], s->out[AB2_OUT_LBDAS],
+                           w.xs, w.us, w.vs, w.vsT, w.lam0, w.lams,
                            grad->stage, grad->term, grad->G0, grad->g0, true};
   CUDA_TRY(ab2::launch_jacobian_grad(ga, st));
   s->launches += 1;
@@ -1048,32 +1092,26 @@ static int tangent_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
   if (int rc = check_solve_handle(s, who))
     return rc;
   // the primal is read completely by the first launch, before the sweep writes any output: it may alias them
-  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
-  if (int rc = require(sol_fields(s, "primal", pp, s->d.batch), who))
+  if (int rc = require(sol_fields(s, "primal", *primal, s->d.batch), who))
     return rc;
   if (int rc = check_mu(s, mueq, mueq_arr, who))
     return rc;
-  const ab2_gar_dims &d = s->d;
-  const int B = d.batch, N = d.horizon, nx = d.nx;
   cudaStream_t st;
   const double *mu_dev;
   if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
     return rc;
-  const size_t nxs = (size_t)B * (N + 1) * nx, nus = (size_t)B * N * d.nu, nvs = (size_t)B * N * d.nc,
-               nvT = (size_t)B * d.nct, nl0 = (size_t)B * d.nc0, nls = (size_t)B * N * nx;
-  if (!s->tan_rho)
-    CUDA_TRY(cudaMalloc(&s->tan_rho, (nxs + nus + nvs + nvT + nl0 + nls + 1) * sizeof(double)));
-  double *rxs = s->tan_rho, *rus = rxs + nxs, *rvs = rus + nus, *rvT = rvs + nvs, *rl0 = rvT + nvT, *rls = rl0 + nl0;
+  ab2_ls_trial rho;
+  if (int rc = sol_scratch(s, s->tan_rho, 1, &rho))
+    return rc;
   // 1. rho = Kdot z + hdot, in the solution's layouts
-  const ab2::AdjointDims ad{B, N, nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
-  ab2::JacobianRhsArgs ra{ad, 1, dot->stage, dot->term, dot->G0, dot->g0,
+  ab2::JacobianRhsArgs ra{adjoint_dims(s), 1, dot->stage, dot->term, dot->G0, dot->g0,
                           primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
-                          rxs, rus, rvs, rvT, rl0, rls};
+                          rho.xs, rho.us, rho.vs, rho.vsT, rho.lam0, rho.lams};
   CUDA_TRY(ab2::launch_jacobian_rhs(ra, st));
   s->launches += 1;
   // 2. + 3. the tangent problem (vectors = rho) and its solve: the trajectory outputs become zdot
-  const ab2_ls_iterate rho{rxs, rus, rvs, rvT, rl0, rls};
-  return solve_cotangent_problem(s, mueq, mu_dev, &rho, true, st);
+  const ab2_ls_iterate rho_in{rho.xs, rho.us, rho.vs, rho.vsT, rho.lam0, rho.lams};
+  return solve_cotangent_problem(s, mueq, mu_dev, &rho_in, true, st);
 }
 int ab2_gar_tangent(ab2_gar_solver *s, double mueq, const ab2_ls_iterate *primal, const ab2_lq_tangent *dot,
                     void *stream) {
@@ -1158,15 +1196,13 @@ static int resolve_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
   if (int rc = check_resolve_handle(s, nrhs, who))
     return rc;
   const size_t R = (size_t)nrhs * s->d.batch;
-  const double *po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
-  const double *ph[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
-  if (int rc = require(sol_fields(s, "out", po, 1), who)) // (refused even at nrhs = 0)
+  if (int rc = require(sol_fields(s, "out", *out, 1), who)) // (refused even at nrhs = 0)
     return rc;
   if (int rc = check_mu(s, mueq, mueq_arr, who))
     return rc;
   // the backward pass parks its per-knot vectors in the out arrays before it has read every rhs entry: an out array
   // that overlaps an rhs array would be read after it was overwritten
-  if (int rc = refuse_overlap(rhs_fields(s, "rhs", ph, R), sol_fields(s, "out", po, R), who))
+  if (int rc = refuse_overlap(rhs_fields(s, "rhs", *rhs, R), sol_fields(s, "out", *out, R), who))
     return rc;
   if (int rc = check_resolve_fits(s, who))
     return rc;
@@ -1211,10 +1247,8 @@ static int factor_adjoint_impl(ab2_gar_solver *s, double mueq, const double *mue
     return rc;
   // the gradients are written knot by knot while later knots' cotangents and factors are still to be read
   const ab2_gar_dims &d = s->d;
-  const double *pc[6] = {cot->ff, cot->fb, cot->vxx, cot->vx, cot->fft, cot->fbt};
-  const double *pg[4] = {grad->stage, grad->term, grad->G0, grad->g0};
-  const Fields G = rec_fields(s, "grad", pg, d.batch);
-  if (int rc = refuse_overlap(G, fac_fields(s, "cotangent", pc, d.batch), who))
+  const Fields G = rec_fields(s, "grad", *grad, d.batch);
+  if (int rc = refuse_overlap(G, fac_fields(s, "cotangent", *cot, d.batch), who))
     return rc;
   if (int rc = refuse_overlap(G, out_fields(s), who))
     return rc;
@@ -1266,10 +1300,8 @@ static int factor_tangent_impl(ab2_gar_solver *s, double mueq, const double *mue
     return rc;
   // the tangents are written knot by knot while later knots' tangent records and factors are still to be read
   const ab2_gar_dims &d = s->d;
-  const double *po[6] = {out->ff, out->fb, out->vxx, out->vx, out->fft, out->fbt};
-  const double *pd[4] = {dot->stage, dot->term, dot->G0, dot->g0};
-  const Fields O = fac_fields(s, "out", po, d.batch);
-  if (int rc = refuse_overlap(O, rec_fields(s, "tangent", pd, d.batch), who))
+  const Fields O = fac_fields(s, "out", *out, d.batch);
+  if (int rc = refuse_overlap(O, rec_fields(s, "tangent", *dot, d.batch), who))
     return rc;
   if (int rc = refuse_overlap(O, out_fields(s), who))
     return rc;
@@ -1326,12 +1358,8 @@ static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
     return rc;
   const ab2_gar_dims &d = s->d;
   const size_t B = d.batch, R = (size_t)nrhs * B;
-  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
-  const double *pc[6] = {cot->xs, cot->us, cot->vs, cot->vsT, cot->lam0, cot->lams};
-  const double *pw[6] = {work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
-  const double *pg[4] = {grad->stage, grad->term, grad->G0, grad->g0};
-  const Fields P = sol_fields(s, "primal", pp, B), Z = sol_fields(s, "cotangent", pc, R),
-               W = sol_fields(s, "work", pw, R), G = rec_fields(s, "grad", pg, R);
+  const Fields P = sol_fields(s, "primal", *primal, B), Z = sol_fields(s, "cotangent", *cot, R),
+               W = sol_fields(s, "work", *work, R), G = rec_fields(s, "grad", *grad, R);
   if (int rc = require(W, who))
     return rc;
   if (int rc = require(P, who))
@@ -1356,8 +1384,7 @@ static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
   if (int rc = run_resolve(s, mueq, mu_dev, nrhs, &rhs, work, st))
     return rc;
   // 2. gradient records from y_j and z
-  const ab2::AdjointDims ad{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
-  ab2::JacobianGradArgs ga{ad, nrhs,
+  ab2::JacobianGradArgs ga{adjoint_dims(s), nrhs,
                            primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
                            work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams,
                            grad->stage, grad->term, grad->G0, grad->g0, false};
@@ -1388,12 +1415,8 @@ static int tangent_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
     return rc;
   const ab2_gar_dims &d = s->d;
   const size_t B = d.batch, R = (size_t)nrhs * B;
-  const double *pp[6] = {primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams};
-  const double *pd[4] = {dot->stage, dot->term, dot->G0, dot->g0};
-  const double *pw[6] = {work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
-  const double *po[6] = {out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
-  const Fields P = sol_fields(s, "primal", pp, B), D = rec_fields(s, "dot", pd, R),
-               W = sol_fields(s, "work", pw, R), O = sol_fields(s, "out", po, R);
+  const Fields P = sol_fields(s, "primal", *primal, B), D = rec_fields(s, "dot", *dot, R),
+               W = sol_fields(s, "work", *work, R), O = sol_fields(s, "out", *out, R);
   if (int rc = require(W, who))
     return rc;
   if (int rc = require(O, who))
@@ -1416,8 +1439,7 @@ static int tangent_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
   if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
     return rc;
   // 1. rho_j = Kdot_j z + hdot_j into work, in resolve's rhs layouts
-  const ab2::AdjointDims ad{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
-  ab2::JacobianRhsArgs ra{ad, nrhs, dot->stage, dot->term, dot->G0, dot->g0,
+  ab2::JacobianRhsArgs ra{adjoint_dims(s), nrhs, dot->stage, dot->term, dot->G0, dot->g0,
                           primal->xs, primal->us, primal->vs, primal->vsT, primal->lam0, primal->lams,
                           work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
   CUDA_TRY(ab2::launch_jacobian_rhs(ra, st));
@@ -1455,27 +1477,15 @@ static int run_refine(ab2_gar_solver *s, double mueq, const double *mu_dev, int 
   const ab2_gar_dims &d = s->d;
   const int B = d.batch, N = d.horizon;
   const size_t R = (size_t)nrhs * B, nnorm = R * (size_t)(steps + 1);
-  double *ndev = nullptr;
+  Staged nr{nullptr, nullptr, nnorm};
   if (norms) {
-    if (device_accessible(norms)) {
-      ndev = norms;
-    } else {
-      if (s->ref_norms_n < nnorm) {
-        if (s->ref_norms)
-          CUDA_TRY(cudaFree(s->ref_norms));
-        s->ref_norms = nullptr;
-        s->ref_norms_n = 0;
-        CUDA_TRY(cudaMalloc(&s->ref_norms, nnorm * sizeof(double)));
-        s->ref_norms_n = nnorm;
-      }
-      ndev = s->ref_norms;
-    }
-    CUDA_TRY(cudaMemsetAsync(ndev, 0, nnorm * sizeof(double), st)); // the maxima meet by atomicMax from 0
+    if (int rc = stage_result(s->ref_norms, norms, device_accessible(norms), nnorm, &nr))
+      return rc;
+    CUDA_TRY(cudaMemsetAsync(nr.dev, 0, nnorm * sizeof(double), st)); // the maxima meet by atomicMax from 0
   }
-  const ab2::AdjointDims ad{B, N, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
   auto residual = [&](int col, bool write) -> int {
     ab2::RefineResidualArgs a{};
-    a.d = ad;
+    a.d = adjoint_dims(s);
     a.nrhs = nrhs;
     a.stage_head = s->p.stage_head;
     a.stage = s->p.stage;
@@ -1507,7 +1517,7 @@ static int run_refine(ab2_gar_solver *s, double mueq, const double *mu_dev, int 
       a.g0out = r->lam0;
       a.f = r->lams;
     }
-    a.norms = ndev;
+    a.norms = nr.dev;
     a.nstride = steps + 1;
     a.col = col;
     CUDA_TRY(ab2::launch_refine_residual(a, false, st));
@@ -1529,11 +1539,10 @@ static int run_refine(ab2_gar_solver *s, double mueq, const double *mu_dev, int 
     CUDA_TRY(ab2::launch_linear_step(step, io, 1.0, nullptr, st)); // z += dz
     s->launches += 1;
   }
-  if (ndev) {
+  if (nr.dev) {
     if (int rc = residual(steps, false)) // the last column: the norm of the refined iterate
       return rc;
-    if (ndev != norms)
-      CUDA_TRY(cudaMemcpyAsync(norms, ndev, nnorm * sizeof(double), cudaMemcpyDeviceToHost, st));
+    return nr.copy_out(st);
   }
   return AB2_OK;
 }
@@ -1561,31 +1570,15 @@ static int refine_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, i
     return rc;
   if (steps == 0 && !norms)
     return AB2_OK;
-  const ab2_gar_dims &d = s->d;
-  const int B = d.batch, N = d.horizon, nx = d.nx;
   cudaStream_t st;
   const double *mu_dev;
   if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
     return rc;
-  const size_t nxs = (size_t)B * (N + 1) * nx, nus = (size_t)B * N * d.nu, nvs = (size_t)B * N * d.nc,
-               nvT = (size_t)B * d.nct, nl0 = (size_t)B * d.nc0, nls = (size_t)B * N * nx,
-               one = nxs + nus + nvs + nvT + nl0 + nls;
-  if (!s->ref_buf)
-    CUDA_TRY(cudaMalloc(&s->ref_buf, (2 * one + 1) * sizeof(double)));
-  auto split = [&](double *p) {
-    ab2_ls_trial t;
-    t.xs = p;
-    t.us = t.xs + nxs;
-    t.vs = t.us + nus;
-    t.vsT = t.vs + nvs;
-    t.lam0 = t.vsT + nvT;
-    t.lams = t.lam0 + nl0;
-    return t;
-  };
-  const ab2_ls_trial r = split(s->ref_buf), dz = split(s->ref_buf + one);
-  const ab2_ls_trial z{s->out[AB2_OUT_XS], s->out[AB2_OUT_US], s->out[AB2_OUT_VS], s->out[AB2_OUT_VST],
-                       s->out[AB2_OUT_LBD0], s->out[AB2_OUT_LBDAS]};
-  return run_refine(s, mueq, mu_dev, 1, steps, true, nullptr, &z, &r, &dz, norms, st);
+  ab2_ls_trial rdz[2]; // the residual and the correction
+  if (int rc = sol_scratch(s, s->ref_buf, 2, rdz))
+    return rc;
+  const ab2_ls_trial z = trajectory(s);
+  return run_refine(s, mueq, mu_dev, 1, steps, true, nullptr, &z, &rdz[0], &rdz[1], norms, st);
 }
 int ab2_gar_refine(ab2_gar_solver *s, double mueq, int steps, double *norms, void *stream) {
   return refine_impl(s, mueq, nullptr, AB2_DEVICE, steps, norms, stream);
@@ -1605,12 +1598,8 @@ static int refine_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_a
   if (int rc = check_resolve_handle(s, nrhs, who))
     return rc;
   const size_t R = (size_t)nrhs * s->d.batch;
-  const double *ph[6] = {rhs->q, rhs->r, rhs->d, rhs->dN, rhs->g0, rhs->f};
-  const double *pz[6] = {z->xs, z->us, z->vs, z->vsT, z->lam0, z->lams};
-  const double *pr[6] = {work->q, work->r, work->d, work->dN, work->g0, work->f};
-  const double *pd[6] = {work->xs, work->us, work->vs, work->vsT, work->lam0, work->lams};
-  const Fields H = rhs_fields(s, "rhs", ph, R), Z = sol_fields(s, "z", pz, R), WR = rhs_fields(s, "work", pr, R),
-               WD = sol_fields(s, "work", pd, R);
+  const Fields H = rhs_fields(s, "rhs", *rhs, R), Z = sol_fields(s, "z", *z, R), WR = rhs_fields(s, "work", *work, R),
+               WD = sol_fields(s, "work", *work, R);
   for (const Fields *f : {&Z, &WR, &WD})
     if (int rc = require(*f, who))
       return rc;
@@ -1645,6 +1634,16 @@ int ab2_gar_refine_many_v(ab2_gar_solver *s, const double *mueq, int memspace, i
   return refine_many_impl(s, 0.0, mueq, memspace, nrhs, steps, rhs, z, work, norms, stream);
 }
 
+// the handle's own copy of the records (assemble, sweep_host), allocated on first use
+static int own_records(ab2_gar_solver *s) {
+  const size_t B = s->d.batch;
+  CUDA_TRY(s->own_stage.ensure(stage_total(s)));
+  CUDA_TRY(s->own_term.ensure(B * s->trec));
+  CUDA_TRY(s->own_G0.ensure(B * s->d.nc0 * s->d.nx));
+  CUDA_TRY(s->own_g0.ensure(B * s->d.nc0));
+  return AB2_OK;
+}
+
 static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const double *preg_b, const double *mu_inv_b,
                          void *stream) {
   if (!s || !in)
@@ -1662,14 +1661,7 @@ static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const doubl
   if (!stage_ok || !cstr_ok || !hess_ok || !term_ok || !init_ok)
     return fail(AB2_ERR_INVALID, "ab2_lq_inputs: a required array is NULL for these dimensions");
   CUDA_TRY(cudaSetDevice(d.device));
-  auto own = [&](double *&buf, size_t n) -> int {
-    if (!buf)
-      CUDA_TRY(cudaMalloc(&buf, (n > 0 ? n : 1) * sizeof(double)));
-    return AB2_OK;
-  };
-  int rc;
-  if ((rc = own(s->own_stage, stage_total(s))) != AB2_OK || (rc = own(s->own_term, (size_t)d.batch * s->trec)) != AB2_OK ||
-      (rc = own(s->own_G0, (size_t)d.batch * d.nc0 * d.nx)) != AB2_OK || (rc = own(s->own_g0, (size_t)d.batch * d.nc0)) != AB2_OK)
+  if (int rc = own_records(s))
     return rc;
   CUDA_TRY(ab2::launch_lq_assemble(*in, preg_b, mu_inv_b, s->own_stage, s->own_term, s->own_G0, s->own_g0, d.batch, d.horizon, d.nx,
                                    d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec, (cudaStream_t)stream));
@@ -1679,9 +1671,7 @@ static int assemble_impl(ab2_gar_solver *s, const ab2_lq_inputs *in, const doubl
   s->p.term = s->own_term;
   s->p.G0 = s->own_G0;
   s->p.g0 = s->own_g0;
-  s->have_problem = true;
-  s->factor_current = false;
-  s->epoch += 1;
+  problem_replaced(s, true);
   return AB2_OK;
 }
 int ab2_gar_assemble(ab2_gar_solver *s, const ab2_lq_inputs *in, void *stream) {
@@ -1706,10 +1696,7 @@ static int get_vxx_packed(ab2_gar_solver *s, int head, int b0, int nb, int t0, i
   double *out = dst;
   if (memspace != AB2_DEVICE)
     CUDA_TRY(cudaMallocAsync(&out, n * sizeof(double), st));
-  long blocks = (long)((n + 255) / 256);
-  if (blocks > s->p.num_sms * 8L)
-    blocks = s->p.num_sms * 8L;
-  ab2::vxx_expand_kernel<<<(int)blocks, 256, 0, st>>>(s->out[AB2_OUT_VXX], s->p.Vxx0, out, s->d.horizon, s->d.nx, head,
+  ab2::vxx_expand_kernel<<<grid_for(s, n), 256, 0, st>>>(s->out[AB2_OUT_VXX], s->p.Vxx0, out, s->d.horizon, s->d.nx, head,
                                                       b0, nb, t0, nt);
   CUDA_TRY(cudaGetLastError()); // (a copy for the caller, like cudaMemcpy: not in ab2_gar_launch_count)
   if (memspace != AB2_DEVICE) {
@@ -1738,12 +1725,9 @@ int ab2_gar_get_problem(ab2_gar_solver *s, int what, double *dst, int memspace, 
   CUDA_TRY(cudaSetDevice(s->d.device));
   if (what == 0 && s->p.stage_head != 0 && n[0]) // the solver-owned copy after cycle_append: knot order through the head
     return copy_ring(s->p.stage, (size_t)s->srec, s->d.horizon, s->d.horizon, s->p.stage_head, 0, s->d.batch, 0,
-                     s->d.horizon, dst, memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                     (cudaStream_t)stream);
+                     s->d.horizon, dst, out_kind(memspace), (cudaStream_t)stream);
   if (n[what])
-    CUDA_TRY(cudaMemcpyAsync(dst, ptrs[what], n[what] * sizeof(double),
-                             memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                             (cudaStream_t)stream));
+    CUDA_TRY(cudaMemcpyAsync(dst, ptrs[what], n[what] * sizeof(double), out_kind(memspace), (cudaStream_t)stream));
   return AB2_OK;
 }
 
@@ -1844,26 +1828,17 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
       CUDA_TRY(cudaEventCreateWithFlags(&s->pipe_done[i], cudaEventDisableTiming));
     }
   }
-  auto own = [&](double *&buf, size_t n) -> int {
-    if (!buf)
-      CUDA_TRY(cudaMalloc(&buf, (n > 0 ? n : 1) * sizeof(double)));
-    return AB2_OK;
-  };
   int rc;
-  if ((rc = own(s->own_stage, stage_total(s))) != AB2_OK || (rc = own(s->own_term, (size_t)B * s->trec)) != AB2_OK ||
-      (rc = own(s->own_G0, (size_t)B * nc0 * nx)) != AB2_OK || (rc = own(s->own_g0, (size_t)B * nc0)) != AB2_OK)
+  if ((rc = own_records(s)) != AB2_OK)
     return rc;
   const size_t srec_sym = ab2_gar_stage_record_doubles_sym(nx, s->d.nu, s->d.nc);
-  if (sym && (rc = own(s->own_stage_sym, (size_t)B * N * srec_sym)) != AB2_OK)
-    return rc;
+  if (sym)
+    CUDA_TRY(s->own_stage_sym.ensure((size_t)B * N * srec_sym));
   s->p.stage = s->own_stage;
   s->p.stage_head = 0;
   s->p.term = s->own_term;
   s->p.G0 = s->own_G0;
   s->p.g0 = s->own_g0;
-  s->have_problem = true;
-  if (!mueq_b)
-    s->p.mueq = mueq;
   s->p.do_bwd = 1;
   s->p.do_fwd = 1;
   if (nchunks <= 0) { // enough slices to hide the first upload / last download, each still one full wave
@@ -1901,9 +1876,6 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
         return rc;
       const long nrec = (long)nb * N;
       if (nrec > 0) {
-        long blocks = (nrec * (long)s->srec + 255) / 256;
-        if (blocks > s->p.num_sms * 8L)
-          blocks = s->p.num_sms * 8L;
         // same shared-memory carve-out as the sweeps it runs beside (an SM is configured for one carve-out at a time)
         static bool carve = false;
         if (!carve) {
@@ -1914,7 +1886,7 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
         if (s->srec * sizeof(int) > 48 * 1024) // (records beyond 12 288 doubles: opt in to the larger table)
           CUDA_TRY(cudaFuncSetAttribute(ab2::expand_sym_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)(s->srec * sizeof(int))));
-        ab2::expand_sym_kernel<<<(int)blocks, 256, s->srec * sizeof(int), st>>>(
+        ab2::expand_sym_kernel<<<grid_for(s, (size_t)nrec * s->srec), 256, s->srec * sizeof(int), st>>>(
             s->own_stage_sym + (size_t)b0 * N * srec_sym, s->own_stage + (size_t)b0 * N * s->srec, nrec, nx, s->d.nu, s->d.nc,
             ab2::stage_offsets(nx, s->d.nu, s->d.nc).end, (int)s->srec, (int)srec_sym);
         CUDA_TRY(cudaGetLastError());
@@ -1925,6 +1897,8 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
     ab2::SweepParams q = slice_params(s, b0, nb);
     if (mu_dev)
       q.mueq_b = mu_dev + b0;
+    else
+      q.mueq = mueq;
     if (int rc2 = run_kernels(s, q, 1, 1, st))
       return rc2;
     for (int i = 0; i < nwhat; ++i) {
@@ -1942,14 +1916,7 @@ static int sweep_host_impl(ab2_gar_solver *s, const double *stage, const double 
     CUDA_TRY(cudaEventRecord(s->pipe_done[i], s->pipe_stream[i]));
     CUDA_TRY(cudaStreamWaitEvent(user, s->pipe_done[i], 0));
   }
-  s->have_backward = true;
-  s->have_forward = true;
-  s->primal_factor = true;
-  s->have_primal = true;
-  s->fac_head = 0;
-  s->vxx_packed = warp_kernel(s);
-  s->factor_current = true;
-  s->epoch += 1;
+  swept_host(s, mueq, mu_dev);
   return AB2_OK;
 }
 
@@ -1997,10 +1964,8 @@ int ab2_gar_get(ab2_gar_solver *s, int what, double *dst, int memspace, void *st
     return get_vxx_packed(s, s->fac_head, 0, s->d.batch, 0, s->d.horizon + 1, dst, memspace, (cudaStream_t)stream);
   if (ring_indexed(s, what)) // between a cycle_append and the next backward: knot order through the ring head
     return copy_ring(s->out[what], s->out_rec[what], s->out_knots[what], s->d.horizon, s->fac_head, 0, s->d.batch, 0,
-                     s->out_knots[what], dst, memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                     (cudaStream_t)stream);
-  CUDA_TRY(cudaMemcpyAsync(dst, s->out[what], s->out_doubles[what] * sizeof(double),
-                           memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                     s->out_knots[what], dst, out_kind(memspace), (cudaStream_t)stream);
+  CUDA_TRY(cudaMemcpyAsync(dst, s->out[what], s->out_doubles[what] * sizeof(double), out_kind(memspace),
                            (cudaStream_t)stream));
   return AB2_OK;
 }
@@ -2019,13 +1984,11 @@ int ab2_gar_get_range(ab2_gar_solver *s, int what, int b0, int nb, int t0, int n
   if (what == AB2_OUT_VXX && s->vxx_packed)
     return get_vxx_packed(s, s->fac_head, b0, nb, t0, nt, dst, memspace, (cudaStream_t)stream);
   if (ring_indexed(s, what))
-    return copy_ring(s->out[what], rec, knots, s->d.horizon, s->fac_head, b0, nb, t0, nt, dst,
-                     memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, (cudaStream_t)stream);
+    return copy_ring(s->out[what], rec, knots, s->d.horizon, s->fac_head, b0, nb, t0, nt, dst, out_kind(memspace),
+                     (cudaStream_t)stream);
   const double *src = s->out[what] + ((size_t)b0 * knots + t0) * rec;
   CUDA_TRY(cudaMemcpy2DAsync(dst, (size_t)nt * rec * sizeof(double), src, (size_t)knots * rec * sizeof(double),
-                             (size_t)nt * rec * sizeof(double), (size_t)nb,
-                             memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                             (cudaStream_t)stream));
+                             (size_t)nt * rec * sizeof(double), (size_t)nb, out_kind(memspace), (cudaStream_t)stream));
   return AB2_OK;
 }
 
@@ -2039,12 +2002,8 @@ int ab2_gar_first_step_policy(ab2_gar_solver *s, double *dst, void *stream) {
   if (!s->have_backward)
     return fail(AB2_ERR_STATE, "first_step_policy before backward()");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  const long total = (long)s->d.batch * s->d.nu * (s->d.nx + 1);
-  const int threads = 256;
-  long blocks = (total + threads - 1) / threads;
-  if (blocks > s->p.num_sms * 8L)
-    blocks = s->p.num_sms * 8L;
-  ab2::first_step_policy_kernel<<<(int)blocks, threads, 0, (cudaStream_t)stream>>>(
+  const size_t total = (size_t)s->d.batch * s->d.nu * (s->d.nx + 1);
+  ab2::first_step_policy_kernel<<<grid_for(s, total), 256, 0, (cudaStream_t)stream>>>(
       s->out[AB2_OUT_FB], s->out[AB2_OUT_FF], dst, s->d.batch, s->d.horizon, s->nr, s->d.nu, s->d.nx, s->fac_head);
   CUDA_TRY(cudaGetLastError());
   s->launches += 1;
@@ -2063,22 +2022,14 @@ int ab2_gar_get_gains(ab2_gar_solver *s, double *dst, int memspace, void *stream
   const size_t total = (size_t)nrec * s->nr * (s->d.nx + 1);
   if (total == 0)
     return AB2_OK;
-  double *out = dst;
-  if (memspace != AB2_DEVICE) { // stage on the device, then one copy
-    if (!s->gains_tmp)
-      CUDA_TRY(cudaMalloc(&s->gains_tmp, total * sizeof(double)));
-    out = s->gains_tmp;
-  }
-  long blocks = ((long)total + 255) / 256;
-  if (blocks > s->p.num_sms * 8L)
-    blocks = s->p.num_sms * 8L;
-  ab2::gains_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(s->out[AB2_OUT_FB], s->out[AB2_OUT_FF], out, nrec,
-                                                                    s->nr, s->d.nx, s->d.horizon, s->fac_head);
+  Staged r;
+  if (int rc = stage_result(s->gains_tmp, dst, memspace == AB2_DEVICE, total, &r))
+    return rc;
+  ab2::gains_kernel<<<grid_for(s, total), 256, 0, (cudaStream_t)stream>>>(s->out[AB2_OUT_FB], s->out[AB2_OUT_FF], r.dev,
+                                                                          nrec, s->nr, s->d.nx, s->d.horizon, s->fac_head);
   CUDA_TRY(cudaGetLastError());
   s->launches += 1;
-  if (memspace != AB2_DEVICE)
-    CUDA_TRY(cudaMemcpyAsync(dst, out, total * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  return AB2_OK;
+  return r.copy_out((cudaStream_t)stream);
 }
 
 static int kkt_error_impl(ab2_gar_solver *s, double mueq, const double *mueq_b, double *dst, int memspace, void *stream) {
@@ -2089,12 +2040,12 @@ static int kkt_error_impl(ab2_gar_solver *s, double mueq, const double *mueq_b, 
   if (s->rec_nth > 0)
     return fail(AB2_ERR_UNSUPPORTED, "kkt_error: parametric problems (nth > 0) are not supported");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  if (!s->kkt_tmp)
-    CUDA_TRY(cudaMalloc(&s->kkt_tmp, (size_t)s->d.batch * 3 * sizeof(double)));
+  Staged r;
+  if (int rc = stage_result(s->kkt_tmp, dst, memspace == AB2_DEVICE, (size_t)s->d.batch * 3, &r))
+    return rc;
   // the refinement's residual of the last forward pass against the problem's own vectors, with one norm per row family
-  const ab2_gar_dims &d = s->d;
   ab2::RefineResidualArgs a{};
-  a.d = ab2::AdjointDims{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0, s->srec, s->trec};
+  a.d = adjoint_dims(s);
   a.nrhs = 1;
   a.stage_head = s->p.stage_head;
   a.stage = s->p.stage;
@@ -2104,22 +2055,20 @@ static int kkt_error_impl(ab2_gar_solver *s, double mueq, const double *mueq_b, 
   a.mueq = mueq;
   a.mueq_b = mueq_b;
   a.own = true;
-  a.xs = s->out[AB2_OUT_XS];
-  a.us = s->out[AB2_OUT_US];
-  a.vs = s->out[AB2_OUT_VS];
-  a.vsT = s->out[AB2_OUT_VST];
-  a.lam0 = s->out[AB2_OUT_LBD0];
-  a.lams = s->out[AB2_OUT_LBDAS];
-  a.norms = (memspace == AB2_DEVICE) ? dst : s->kkt_tmp;
+  const ab2_ls_trial z = trajectory(s);
+  a.xs = z.xs;
+  a.us = z.us;
+  a.vs = z.vs;
+  a.vsT = z.vsT;
+  a.lam0 = z.lam0;
+  a.lams = z.lams;
+  a.norms = r.dev;
   a.nstride = 3;
   a.col = 0;
-  CUDA_TRY(cudaMemsetAsync(a.norms, 0, (size_t)d.batch * 3 * sizeof(double), (cudaStream_t)stream));
+  CUDA_TRY(cudaMemsetAsync(a.norms, 0, r.n * sizeof(double), (cudaStream_t)stream));
   CUDA_TRY(ab2::launch_refine_residual(a, true, (cudaStream_t)stream));
   s->launches += 1;
-  if (memspace != AB2_DEVICE)
-    CUDA_TRY(cudaMemcpyAsync(dst, s->kkt_tmp, (size_t)s->d.batch * 3 * sizeof(double), cudaMemcpyDeviceToHost,
-                             (cudaStream_t)stream));
-  return AB2_OK;
+  return r.copy_out((cudaStream_t)stream);
 }
 int ab2_gar_kkt_error(ab2_gar_solver *s, double mueq, double *dst, int memspace, void *stream) {
   return kkt_error_impl(s, mueq, nullptr, dst, memspace, stream);
@@ -2141,9 +2090,7 @@ int ab2_gar_status(ab2_gar_solver *s, int *dst, int memspace, void *stream) {
   if (!s || !dst)
     return fail(AB2_ERR_INVALID, "bad argument");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  CUDA_TRY(cudaMemcpyAsync(dst, s->status, sizeof(int) * s->d.batch,
-                           memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                           (cudaStream_t)stream));
+  CUDA_TRY(cudaMemcpyAsync(dst, s->status, sizeof(int) * s->d.batch, out_kind(memspace), (cudaStream_t)stream));
   return AB2_OK;
 }
 
@@ -2157,24 +2104,14 @@ static ab2::LineSearchArgs ls_args(const ab2_gar_solver *s) {
   a.nc = s->d.nc;
   a.nct = s->d.nct;
   a.nc0 = s->d.nc0;
-  a.dxs = s->out[AB2_OUT_XS];
-  a.dus = s->out[AB2_OUT_US];
-  a.dvs = s->out[AB2_OUT_VS];
-  a.dvsT = s->out[AB2_OUT_VST];
-  a.dlam0 = s->out[AB2_OUT_LBD0];
-  a.dlams = s->out[AB2_OUT_LBDAS];
+  const ab2_ls_trial z = trajectory(s);
+  a.dxs = z.xs;
+  a.dus = z.us;
+  a.dvs = z.vs;
+  a.dvsT = z.vsT;
+  a.dlam0 = z.lam0;
+  a.dlams = z.lams;
   return a;
-}
-static int ls_result(ab2_gar_solver *s, double *dst, int memspace, cudaStream_t st, double **dev) {
-  if (memspace == AB2_DEVICE) {
-    *dev = dst;
-    return AB2_OK;
-  }
-  if (!s->ls_tmp)
-    CUDA_TRY(cudaMalloc(&s->ls_tmp, (size_t)s->d.batch * sizeof(double)));
-  *dev = s->ls_tmp;
-  (void)st;
-  return AB2_OK;
 }
 static int linear_step_impl(ab2_gar_solver *s, double alpha, const double *alpha_b, const ab2_ls_iterate *cur,
                             const ab2_ls_trial *trial, void *stream) {
@@ -2212,14 +2149,12 @@ int ab2_gar_directional_derivative(ab2_gar_solver *s, const double *Lxs, const d
   if (!s->have_forward)
     return fail(AB2_ERR_STATE, "directional_derivative needs the step of a forward pass");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  double *dev = nullptr;
-  if (int rc = ls_result(s, dst, memspace, (cudaStream_t)stream, &dev))
+  Staged r;
+  if (int rc = stage_result(s->ls_tmp, dst, memspace == AB2_DEVICE, s->d.batch, &r))
     return rc;
-  CUDA_TRY(ab2::launch_directional_derivative(ls_args(s), Lxs, Lus, dev, (cudaStream_t)stream));
+  CUDA_TRY(ab2::launch_directional_derivative(ls_args(s), Lxs, Lus, r.dev, (cudaStream_t)stream));
   s->launches += 1;
-  if (memspace != AB2_DEVICE)
-    CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)s->d.batch * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  return AB2_OK;
+  return r.copy_out((cudaStream_t)stream);
 }
 static int al_value_impl(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, double mudyn, double mucstr,
                          const double *mudyn_b, const double *mucstr_b, double *dst, int memspace, void *stream) {
@@ -2230,15 +2165,13 @@ static int al_value_impl(ab2_gar_solver *s, const ab2_ls_iterate *plus, const do
       (d.nct > 0 && !plus->vsT))
     return fail(AB2_ERR_INVALID, "al_value: a required multiplier array is NULL for these dimensions");
   CUDA_TRY(cudaSetDevice(d.device));
-  double *dev = nullptr;
-  if (int rc = ls_result(s, dst, memspace, (cudaStream_t)stream, &dev))
+  Staged r;
+  if (int rc = stage_result(s->ls_tmp, dst, memspace == AB2_DEVICE, d.batch, &r))
     return rc;
   CUDA_TRY(ab2::launch_al_value(d.batch, d.horizon, d.nx, d.nc, d.nct, d.nc0, plus->lam0, plus->lams, plus->vs, plus->vsT,
-                                cost, mudyn, mucstr, mudyn_b, mucstr_b, dev, (cudaStream_t)stream));
+                                cost, mudyn, mucstr, mudyn_b, mucstr_b, r.dev, (cudaStream_t)stream));
   s->launches += 1;
-  if (memspace != AB2_DEVICE)
-    CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  return AB2_OK;
+  return r.copy_out((cudaStream_t)stream);
 }
 int ab2_gar_al_value(ab2_gar_solver *s, const ab2_ls_iterate *plus, const double *cost, double mudyn, double mucstr,
                      double *dst, int memspace, void *stream) {
@@ -2255,17 +2188,6 @@ int ab2_gar_al_value_v(ab2_gar_solver *s, const ab2_ls_iterate *plus, const doub
 static ab2::InnerDims inner_dims(const ab2_gar_solver *s) {
   const ab2_gar_dims &d = s->d;
   return ab2::InnerDims{d.batch, d.horizon, d.nx, d.nu, d.nc, d.nct, d.nc0};
-}
-// device destination of a [batch][2] result: the caller's buffer or the handle's scratch (copied out afterwards)
-static int inner_result(ab2_gar_solver *s, double *dst, int memspace, double **dev) {
-  if (memspace == AB2_DEVICE) {
-    *dev = dst;
-    return AB2_OK;
-  }
-  if (!s->inner_tmp)
-    CUDA_TRY(cudaMalloc(&s->inner_tmp, (size_t)s->d.batch * 2 * sizeof(double)));
-  *dev = s->inner_tmp;
-  return AB2_OK;
 }
 static int multipliers_impl(ab2_gar_solver *s, const ab2_mult_inputs *in, const double *mu_b, const double *mu_dyn_b,
                             const ab2_mult_outputs *out, double *dst, int memspace, void *stream) {
@@ -2286,14 +2208,12 @@ static int multipliers_impl(ab2_gar_solver *s, const ab2_mult_inputs *in, const 
   if (!mu_b && (!(in->mu > 0.0) || !(in->mu_dyn > 0.0)))
     return fail(AB2_ERR_INVALID, "multipliers: mu and mu_dyn must be positive");
   CUDA_TRY(cudaSetDevice(d.device));
-  double *dev = nullptr;
-  if (int rc = inner_result(s, dst, memspace, &dev))
+  Staged r;
+  if (int rc = stage_result(s->inner_tmp, dst, memspace == AB2_DEVICE, (size_t)d.batch * 2, &r))
     return rc;
-  CUDA_TRY(ab2::launch_multipliers(inner_dims(s), *in, mu_b, mu_dyn_b, *out, dev, (cudaStream_t)stream));
+  CUDA_TRY(ab2::launch_multipliers(inner_dims(s), *in, mu_b, mu_dyn_b, *out, r.dev, (cudaStream_t)stream));
   s->launches += 1;
-  if (memspace != AB2_DEVICE)
-    CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * 2 * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  return AB2_OK;
+  return r.copy_out((cudaStream_t)stream);
 }
 int ab2_gar_multipliers(ab2_gar_solver *s, const ab2_mult_inputs *in, const ab2_mult_outputs *out, double *dst,
                         int memspace, void *stream) {
@@ -2334,14 +2254,12 @@ int ab2_gar_criterion(ab2_gar_solver *s, const double *Lxs, const double *Lus, c
   if (!ok)
     return fail(AB2_ERR_INVALID, "criterion: a required array is NULL for these dimensions");
   CUDA_TRY(cudaSetDevice(d.device));
-  double *dev = nullptr;
-  if (int rc = inner_result(s, dst, memspace, &dev))
+  Staged r;
+  if (int rc = stage_result(s->inner_tmp, dst, memspace == AB2_DEVICE, (size_t)d.batch * 2, &r))
     return rc;
-  CUDA_TRY(ab2::launch_criterion(inner_dims(s), Lxs, Lus, init_value, slack, Lv, Lv_N, dev, (cudaStream_t)stream));
+  CUDA_TRY(ab2::launch_criterion(inner_dims(s), Lxs, Lus, init_value, slack, Lv, Lv_N, r.dev, (cudaStream_t)stream));
   s->launches += 1;
-  if (memspace != AB2_DEVICE)
-    CUDA_TRY(cudaMemcpyAsync(dst, dev, (size_t)d.batch * 2 * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  return AB2_OK;
+  return r.copy_out((cudaStream_t)stream);
 }
 
 static int fddp_backward_impl(ab2_gar_solver *s, const ab2_fddp_inputs *in, const double *preg_b, double *Vx_out,
@@ -2356,15 +2274,10 @@ static int fddp_backward_impl(ab2_gar_solver *s, const ab2_fddp_inputs *in, cons
   CUDA_TRY(cudaSetDevice(d.device));
   cudaStream_t st = (cudaStream_t)stream;
   const int B = d.batch, N = d.horizon, nx = d.nx, nu = d.nu;
-  auto own = [&](double *&buf, size_t n) -> int {
-    if (!buf)
-      CUDA_TRY(cudaMalloc(&buf, (n > 0 ? n : 1) * sizeof(double)));
-    return AB2_OK;
-  };
-  int rc;
-  if ((rc = own(s->fddp_slack, (size_t)B * N * nx)) != AB2_OK || (rc = own(s->fddp_G0, (size_t)B * nx * nx)) != AB2_OK ||
-      (rc = own(s->fddp_g0, (size_t)B * nx)) != AB2_OK || (rc = own(s->fddp_vx, (size_t)B * (N + 1) * nx)) != AB2_OK)
-    return rc;
+  CUDA_TRY(s->fddp_slack.ensure((size_t)B * N * nx));
+  CUDA_TRY(s->fddp_G0.ensure((size_t)B * nx * nx));
+  CUDA_TRY(s->fddp_g0.ensure((size_t)B * nx));
+  CUDA_TRY(s->fddp_vx.ensure((size_t)B * (N + 1) * nx));
   ab2::fddp_prep_kernel<<<s->p.num_sms * 4, 256, 0, st>>>(in->fs, s->fddp_slack, s->fddp_G0, s->fddp_g0, B, N, nx);
   CUDA_TRY(cudaGetLastError());
   s->launches += 1;
@@ -2384,11 +2297,11 @@ static int fddp_backward_impl(ab2_gar_solver *s, const ab2_fddp_inputs *in, cons
   lq.g0 = s->fddp_g0;
   lq.preg = in->preg; // Q, R and the terminal Q carry + preg I (:217, :246, :273)
   lq.mu_inv = 1.0;
-  if ((rc = assemble_impl(s, &lq, preg_b, nullptr, stream)) != AB2_OK)
+  if (int rc = assemble_impl(s, &lq, preg_b, nullptr, stream))
     return rc;
-  if ((rc = ab2_gar_backward(s, 1.0, stream)) != AB2_OK) // (mueq is unused without constraints)
+  if (int rc = ab2_gar_backward(s, 1.0, stream)) // (mueq is unused without constraints)
     return rc;
-  double *vxo = Vx_out ? Vx_out : s->fddp_vx;
+  double *vxo = Vx_out ? Vx_out : s->fddp_vx.p;
   ab2::fddp_vx_kernel<<<s->p.num_sms * 4, 256, 0, st>>>(s->out[AB2_OUT_VXX], s->vxx_packed ? s->p.Vxx0 : nullptr,
                                                       s->out[AB2_OUT_VX], in->fs, vxo, B, N, nx);
   CUDA_TRY(cudaGetLastError());
@@ -2431,9 +2344,7 @@ int ab2_gar_pivot_stats(ab2_gar_solver *s, int *dst, int memspace, void *stream)
   if (!s->have_backward)
     return fail(AB2_ERR_STATE, "pivot_stats before backward()");
   CUDA_TRY(cudaSetDevice(s->d.device));
-  CUDA_TRY(cudaMemcpyAsync(dst, s->pivstat, sizeof(int) * s->d.batch,
-                           memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
-                           (cudaStream_t)stream));
+  CUDA_TRY(cudaMemcpyAsync(dst, s->pivstat, sizeof(int) * s->d.batch, out_kind(memspace), (cudaStream_t)stream));
   return AB2_OK;
 }
 
@@ -2458,8 +2369,8 @@ int ab2_gar_cycle_append(ab2_gar_solver *s, const double *new_last, int memspace
   // rotating left = advancing the head by one.  What is touched is ONE knot slot per instance and array:
   // the factor slot of the new last knot is zeroed (datas[N-1] re-created, :82-83), its record is written.
   if (s->legs <= 1) {
-    s->fac_head = (s->fac_head + 1) % N;
-    const int slot = (N - 1 + s->fac_head) % N; // physical slot of the new stage knot N-1 (= the old knot 0's)
+    const int slot = s->fac_head; // the old knot 0's slot, which holds the new stage knot N-1 once cycled() has
+                                  // advanced the head by one
     for (int w : {AB2_OUT_FF, AB2_OUT_FB, AB2_OUT_VXX, AB2_OUT_VX}) {
       const size_t rec = (w == AB2_OUT_VXX && s->vxx_packed) ? (size_t)ab2::vxx_packed_doubles(s->d.nx) : s->out_rec[w];
       if (rec == 0)
@@ -2484,11 +2395,7 @@ int ab2_gar_cycle_append(ab2_gar_solver *s, const double *new_last, int memspace
                                memspace == AB2_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
   }
   CUDA_TRY(cudaGetLastError());
-  s->have_backward = false;
-  s->have_forward = false;
-  s->have_primal = false;
-  s->factor_current = false;
-  s->epoch += 1;
+  cycled(s);
   return AB2_OK;
 }
 

@@ -138,6 +138,9 @@ class GarError(RuntimeError):
 
 
 _lib = None
+# the calls ab2_gar_<name>(h, double mueq, ...) whose twin ab2_gar_<name>_v takes (mueq array, memspace) in its place
+_MU_TWINS = ("backward", "sweep", "adjoint", "tangent", "resolve", "adjoint_many", "tangent_many", "refine",
+             "refine_many", "factor_adjoint", "factor_tangent")
 
 
 def lib():
@@ -164,8 +167,6 @@ def lib():
         L.ab2_gar_backward.argtypes = [C.c_void_p, C.c_double, C.c_void_p]
         L.ab2_gar_forward.argtypes = [C.c_void_p, C.c_void_p]
         L.ab2_gar_sweep.argtypes = [C.c_void_p, C.c_double, C.c_void_p]
-        L.ab2_gar_backward_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
-        L.ab2_gar_sweep_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_create_parametric.argtypes = [C.POINTER(GarDims), C.c_int, C.POINTER(C.c_void_p)]
         L.ab2_gar_create_parallel.argtypes = [C.POINTER(GarDims), C.c_int, C.POINTER(C.c_void_p)]
         L.ab2_gar_create_dense.argtypes = [C.POINTER(GarDims), C.POINTER(C.c_void_p)]
@@ -205,39 +206,21 @@ def lib():
         L.ab2_gar_al_value_v.argtypes = [C.c_void_p] * 6 + [C.c_int, C.c_void_p]
         L.ab2_gar_adjoint.argtypes = [C.c_void_p, C.c_double, C.POINTER(LsIterate), C.POINTER(LsIterate),
                                       C.POINTER(LqGrad), C.c_void_p]
-        L.ab2_gar_adjoint_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LsIterate), C.POINTER(LsIterate),
-                                        C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_tangent.argtypes = [C.c_void_p, C.c_double, C.POINTER(LsIterate), C.POINTER(LqTangent), C.c_void_p]
-        L.ab2_gar_tangent_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LsIterate), C.POINTER(LqTangent),
-                                        C.c_void_p]
         L.ab2_gar_resolve.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LqRhs), C.POINTER(LsIterate),
                                       C.c_void_p]
-        L.ab2_gar_resolve_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LqRhs),
-                                        C.POINTER(LsIterate), C.c_void_p]
         L.ab2_gar_factor_epoch.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
         L.ab2_gar_adjoint_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LsIterate), C.POINTER(LsIterate),
                                            C.POINTER(LsIterate), C.POINTER(LqGrad), C.c_void_p]
-        L.ab2_gar_adjoint_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LsIterate),
-                                             C.POINTER(LsIterate), C.POINTER(LsIterate), C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_tangent_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LsIterate), C.POINTER(LqTangent),
                                            C.POINTER(LsIterate), C.POINTER(LsIterate), C.c_void_p]
-        L.ab2_gar_tangent_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(LsIterate),
-                                             C.POINTER(LqTangent), C.POINTER(LsIterate), C.POINTER(LsIterate),
-                                             C.c_void_p]
         L.ab2_gar_refine.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p]
-        L.ab2_gar_refine_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         L.ab2_gar_refine_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int, C.POINTER(LqRhs),
                                           C.POINTER(LsIterate), C.POINTER(LqRefineWork), C.c_void_p, C.c_void_p]
-        L.ab2_gar_refine_many_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(LqRhs),
-                                            C.POINTER(LsIterate), C.POINTER(LqRefineWork), C.c_void_p, C.c_void_p]
         L.ab2_gar_factor_adjoint.argtypes = [C.c_void_p, C.c_double, C.POINTER(FactorCotangent), C.POINTER(LqGrad),
                                              C.c_void_p]
-        L.ab2_gar_factor_adjoint_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(FactorCotangent),
-                                               C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_factor_tangent.argtypes = [C.c_void_p, C.c_double, C.POINTER(LqTangent), C.POINTER(FactorTangent),
                                              C.c_void_p]
-        L.ab2_gar_factor_tangent_v.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(LqTangent),
-                                               C.POINTER(FactorTangent), C.c_void_p]
         L.ab2_gar_multipliers.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.POINTER(MultOutputs), C.c_void_p, C.c_int,
                                           C.c_void_p]
         L.ab2_gar_multipliers_v.argtypes = [C.c_void_p, C.POINTER(MultInputs), C.c_void_p, C.c_void_p,
@@ -252,6 +235,9 @@ def lib():
         L.ab2_gar_cycle_append.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         L.ab2_gar_synchronize.argtypes = [C.c_void_p, C.c_void_p]
         L.ab2_gar_kernel_info.argtypes = [C.c_void_p] + [C.POINTER(C.c_int)] * 5
+        for name in _MU_TWINS:  # ab2_gar_<name>_v(h, mueq array, memspace, ...): the scalar mueq's place
+            getattr(L, "ab2_gar_%s_v" % name).argtypes = ([C.c_void_p, C.c_void_p, C.c_int]
+                                                          + getattr(L, "ab2_gar_" + name).argtypes[2:])
         _lib = L
     return _lib
 
@@ -312,7 +298,7 @@ class CudaRiccatiBatch:
         rec_nth = 0 if self.legs else self.nth
         self.srec = int(lib().ab2_gar_stage_record_doubles_th(nx, nu, nc, rec_nth))
         self.trec = int(lib().ab2_gar_term_record_doubles_th(nx, nct, rec_nth))
-        self._keep = None
+        self._keep = {}  # call name -> the arguments of its last call, alive while the device may still read them
         self._keep_v = {}
 
     # ---- per-instance scalars (the *_v twins of the C ABI) ----------------------
@@ -376,6 +362,17 @@ class CudaRiccatiBatch:
             return _ptr(self._device_array(v, "mueq", stream)), AB2_DEVICE
         return _ptr(self._host_array(v, "mueq")), AB2_HOST
 
+    def _mu_call(self, name, mueq, stream, keep, *args):
+        """``ab2_gar_<name>(h, mueq, *args, stream)`` for a number ``mueq``, else ``ab2_gar_<name>_v(h, array,
+        memspace, *args, stream)``.  ``keep``: the arrays behind ``args``, kept alive until the next call of ``name``."""
+        v = self._mueq_arg(mueq, stream)
+        if keep is not None:
+            self._keep[name] = keep
+        if v is None:
+            _check(getattr(lib(), "ab2_gar_" + name)(self.h, float(mueq), *args, C.c_void_p(stream)))
+        else:
+            _check(getattr(lib(), "ab2_gar_%s_v" % name)(self.h, v[0], v[1], *args, C.c_void_p(stream)))
+
     def close(self):
         if getattr(self, "h", None) is not None and self.h.value:
             lib().ab2_gar_destroy(self.h)
@@ -395,7 +392,7 @@ class CudaRiccatiBatch:
                 assert stage.size == d.batch * d.horizon * self.srec, "stage size"
             if term is not None:
                 assert term.size == d.batch * self.trec, "term size"
-        self._keep = (stage, term, G0, g0)
+        self._keep["set_problem"] = (stage, term, G0, g0)
         _check(lib().ab2_gar_set_problem(self.h, _ptr(stage), _ptr(term), _ptr(G0), _ptr(g0),
                                          memspace, C.c_void_p(stream)))
 
@@ -403,11 +400,7 @@ class CudaRiccatiBatch:
     def backward(self, mueq, stream=0):
         """``mueq``: a number, or a [batch] float64 array / tensor of per-instance values (``ab2_gar_backward_v``;
         CUDA tensors are read on the device, host arrays are staged by the library)."""
-        v = self._mueq_arg(mueq, stream)
-        if v is None:
-            _check(lib().ab2_gar_backward(self.h, float(mueq), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_backward_v(self.h, v[0], v[1], C.c_void_p(stream)))
+        self._mu_call("backward", mueq, stream, None)
 
     def forward(self, stream=0, theta=None):
         """forward(); with ``theta`` ([batch][nth] host array) the parametric rollout."""
@@ -416,7 +409,7 @@ class CudaRiccatiBatch:
         else:
             th = np.ascontiguousarray(theta, dtype=np.float64)
             assert th.size == self.dims.batch * self.nth
-            self._keep_theta = th
+            self._keep["forward"] = th
             _check(lib().ab2_gar_forward_theta(self.h, _ptr(th), AB2_HOST, C.c_void_p(stream)))
             self.synchronize(stream)
 
@@ -425,14 +418,23 @@ class CudaRiccatiBatch:
 
     def sweep(self, mueq, stream=0):
         """``mueq``: a number or a [batch] array / tensor (``ab2_gar_sweep_v``), as for ``backward``."""
-        v = self._mueq_arg(mueq, stream)
-        if v is None:
-            _check(lib().ab2_gar_sweep(self.h, float(mueq), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_sweep_v(self.h, v[0], v[1], C.c_void_p(stream)))
+        self._mu_call("sweep", mueq, stream, None)
 
     def synchronize(self, stream=0):
         _check(lib().ab2_gar_synchronize(self.h, C.c_void_p(stream)))
+
+    def _sweep_host(self, name, stage, term, G0, g0, mueq, outputs, nchunks, stream):
+        """``ab2_gar_<name>`` or, for a per-instance ``mueq``, ``ab2_gar_<name>_v`` (the array staged from the host)."""
+        v = self._per_instance(mueq, "mueq")
+        whats = (C.c_int * len(outputs))(*outputs.keys())
+        dsts = (C.c_void_p * len(outputs))(*[_ptr(a).value for a in outputs.values()])
+        self._keep["sweep_host"] = (stage, term, G0, g0, outputs)
+        if v is None:
+            f, mu = getattr(lib(), "ab2_gar_" + name), C.c_double(mueq)
+        else:
+            f, mu = getattr(lib(), "ab2_gar_%s_v" % name), _ptr(self._host_array(v, "mueq"))
+        _check(f(self.h, _ptr(stage), _ptr(term), _ptr(G0), _ptr(g0), mu, int(nchunks), whats, dsts, len(outputs),
+                 C.c_void_p(stream)))
 
     def sweep_host(self, stage, term, G0, g0, mueq, outputs, nchunks=0, stream=0):
         """Upload + sweep + download in one pipelined call (``ab2_gar_sweep_host``): the batch
@@ -440,35 +442,13 @@ class CudaRiccatiBatch:
         ``outputs``: {OUT_*: host array of the full output size}; pinned arrays make the
         copies asynchronous.  Asynchronous w.r.t. the host: call ``synchronize(stream)``.  ``mueq``: a number or a
         [batch] array / tensor of per-instance values (``ab2_gar_sweep_host_v``)."""
-        v = self._per_instance(mueq, "mueq")
-        whats = (C.c_int * len(outputs))(*outputs.keys())
-        dsts = (C.c_void_p * len(outputs))(*[_ptr(a).value for a in outputs.values()])
-        self._keep = (stage, term, G0, g0, outputs)
-        if v is None:
-            _check(lib().ab2_gar_sweep_host(self.h, _ptr(stage), _ptr(term), _ptr(G0), _ptr(g0),
-                                            C.c_double(mueq), int(nchunks), whats, dsts, len(outputs),
-                                            C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_sweep_host_v(self.h, _ptr(stage), _ptr(term), _ptr(G0), _ptr(g0),
-                                              _ptr(self._host_array(v, "mueq")), int(nchunks), whats, dsts,
-                                              len(outputs), C.c_void_p(stream)))
+        self._sweep_host("sweep_host", stage, term, G0, g0, mueq, outputs, nchunks, stream)
 
     def sweep_host_sym(self, stage_sym, term, G0, g0, mueq, outputs, nchunks=0, stream=0):
         """``sweep_host`` with the symmetric blocks Q, R of every stage knot sent as lower triangles
         (``ab2_gar_sweep_host_sym``; records made by ``pack_stage_sym``): fewer bytes over PCIe.  ``mueq``: a number
         or a [batch] array / tensor (``ab2_gar_sweep_host_sym_v``)."""
-        v = self._per_instance(mueq, "mueq")
-        whats = (C.c_int * len(outputs))(*outputs.keys())
-        dsts = (C.c_void_p * len(outputs))(*[_ptr(a).value for a in outputs.values()])
-        self._keep = (stage_sym, term, G0, g0, outputs)
-        if v is None:
-            _check(lib().ab2_gar_sweep_host_sym(self.h, _ptr(stage_sym), _ptr(term), _ptr(G0), _ptr(g0),
-                                                C.c_double(mueq), int(nchunks), whats, dsts, len(outputs),
-                                                C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_sweep_host_sym_v(self.h, _ptr(stage_sym), _ptr(term), _ptr(G0), _ptr(g0),
-                                                  _ptr(self._host_array(v, "mueq")), int(nchunks), whats, dsts,
-                                                  len(outputs), C.c_void_p(stream)))
+        self._sweep_host("sweep_host_sym", stage_sym, term, G0, g0, mueq, outputs, nchunks, stream)
 
     def pack_stage_sym(self, stage, out=None):
         """Full stage records [batch][N][srec] (host) -> triangle-packed records (``ab2_gar_pack_stage_sym``)."""
@@ -532,7 +512,7 @@ class CudaRiccatiBatch:
             a = arrays.get(n)
             setattr(inp, n, None if a is None else _ptr(a).value)
         v = self._device_pair(preg, mu_inv, ("preg", "mu_inv"), stream)
-        self._keep = (arrays,)
+        self._keep["assemble"] = (arrays,)
         if v is None:
             inp.preg, inp.mu_inv = float(preg), float(mu_inv)
             _check(lib().ab2_gar_assemble(self.h, C.byref(inp), C.c_void_p(stream)))
@@ -641,7 +621,7 @@ class CudaRiccatiBatch:
         v = self._per_instance(alpha, "alpha")
         cur = LsIterate(*[_ptr(current.get(k)).value if current.get(k) is not None else None for k in _LS_KEYS])
         tr = LsIterate(*[_ptr(trial.get(k)).value if trial.get(k) is not None else None for k in _LS_KEYS])
-        self._keep_ls = (current, trial)
+        self._keep["linear_step"] = (current, trial)
         if v is None:
             _check(lib().ab2_gar_linear_step(self.h, C.c_double(alpha), C.byref(cur), C.byref(tr), C.c_void_p(stream)))
         else:
@@ -676,17 +656,10 @@ class CudaRiccatiBatch:
         mu; a cotangent key that is missing or None is zero).  ``grad``: dict with any of stage, term, G0, g0 of
         device tensors in the problem's layouts, overwritten.  ``mueq``: a number or a [batch] array / tensor
         (``ab2_gar_adjoint_v``).  Afterwards the handle's outputs are those of the adjoint solve."""
-        v = self._mueq_arg(mueq, stream)
         pr = _fill(LsIterate(), _LS_KEYS, primal)
         ct = _fill(LsIterate(), _LS_KEYS, cotangent)
         gr = _fill(LqGrad(), _GRAD_KEYS, grad)
-        self._keep_adj = (primal, cotangent, grad)
-        if v is None:
-            _check(lib().ab2_gar_adjoint(self.h, C.c_double(mueq), C.byref(pr), C.byref(ct), C.byref(gr),
-                                         C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_adjoint_v(self.h, v[0], v[1], C.byref(pr), C.byref(ct), C.byref(gr),
-                                           C.c_void_p(stream)))
+        self._mu_call("adjoint", mueq, stream, (primal, cotangent, grad), C.byref(pr), C.byref(ct), C.byref(gr))
 
     def tangent(self, primal, tangent, mueq, stream=0):
         """Forward mode of the LQ solve (``ab2_gar_tangent``): afterwards the handle's trajectory outputs (OUT_XS ..
@@ -696,14 +669,9 @@ class CudaRiccatiBatch:
         the solution of the current problem at this mu; it may be the handle's own outputs (``device_ptr``).  The
         tangent of Q and R is taken through sym(.) = (. + .^T) / 2, as ``adjoint``'s gradient is.  ``mueq``: a number
         or a [batch] array / tensor (``ab2_gar_tangent_v``)."""
-        v = self._mueq_arg(mueq, stream)
         pr = _fill(LsIterate(), _LS_KEYS, primal)
         dt = _fill(LqTangent(), _GRAD_KEYS, tangent)
-        self._keep_tan = (primal, tangent)
-        if v is None:
-            _check(lib().ab2_gar_tangent(self.h, C.c_double(mueq), C.byref(pr), C.byref(dt), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_tangent_v(self.h, v[0], v[1], C.byref(pr), C.byref(dt), C.c_void_p(stream)))
+        self._mu_call("tangent", mueq, stream, (primal, tangent), C.byref(pr), C.byref(dt))
 
     def resolve(self, rhs, out, mueq, stream=0):
         """Re-solve the last backward's LQ matrices for new vectors (``ab2_gar_resolve``): ``out`` receives
@@ -714,16 +682,9 @@ class CudaRiccatiBatch:
         or a [batch] array / tensor (``ab2_gar_resolve_v``).  The handle's own outputs are not touched."""
         d = self.dims
         nrhs = out["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
-        v = self._mueq_arg(mueq, stream)
         rh = _fill(LqRhs(), _RHS_KEYS, rhs)
         ot = _fill(LsIterate(), _LS_KEYS, out)
-        self._keep_rs = (rhs, out)
-        if v is None:
-            _check(lib().ab2_gar_resolve(self.h, C.c_double(mueq), int(nrhs), C.byref(rh), C.byref(ot),
-                                         C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_resolve_v(self.h, v[0], v[1], int(nrhs), C.byref(rh), C.byref(ot),
-                                           C.c_void_p(stream)))
+        self._mu_call("resolve", mueq, stream, (rhs, out), int(nrhs), C.byref(rh), C.byref(ot))
 
     def adjoint_many(self, primal, cotangent, work, grad, mueq, stream=0):
         """Many cotangents on the last backward's factorisation (``ab2_gar_adjoint_many``): ``grad`` receives, for every
@@ -736,18 +697,12 @@ class CudaRiccatiBatch:
         or a [batch] array / tensor (``ab2_gar_adjoint_many_v``).  The handle's own outputs are not touched."""
         d = self.dims
         nrhs = work["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
-        v = self._mueq_arg(mueq, stream)
         pr = _fill(LsIterate(), _LS_KEYS, primal)
         ct = _fill(LsIterate(), _LS_KEYS, cotangent)
         wk = _fill(LsIterate(), _LS_KEYS, work)
         gr = _fill(LqGrad(), _GRAD_KEYS, grad)
-        self._keep_adj_many = (primal, cotangent, work, grad)
-        if v is None:
-            _check(lib().ab2_gar_adjoint_many(self.h, C.c_double(mueq), int(nrhs), C.byref(pr), C.byref(ct),
-                                              C.byref(wk), C.byref(gr), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_adjoint_many_v(self.h, v[0], v[1], int(nrhs), C.byref(pr), C.byref(ct), C.byref(wk),
-                                                C.byref(gr), C.c_void_p(stream)))
+        self._mu_call("adjoint_many", mueq, stream, (primal, cotangent, work, grad), int(nrhs), C.byref(pr), C.byref(ct),
+                      C.byref(wk), C.byref(gr))
 
     def tangent_many(self, primal, tangent, work, out, mueq, stream=0):
         """Many tangents on the last backward's factorisation (``ab2_gar_tangent_many``): ``out`` receives, for every
@@ -760,18 +715,12 @@ class CudaRiccatiBatch:
         touched."""
         d = self.dims
         nrhs = out["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
-        v = self._mueq_arg(mueq, stream)
         pr = _fill(LsIterate(), _LS_KEYS, primal)
         dt = _fill(LqTangent(), _GRAD_KEYS, tangent)
         wk = _fill(LsIterate(), _LS_KEYS, work)
         ot = _fill(LsIterate(), _LS_KEYS, out)
-        self._keep_tan_many = (primal, tangent, work, out)
-        if v is None:
-            _check(lib().ab2_gar_tangent_many(self.h, C.c_double(mueq), int(nrhs), C.byref(pr), C.byref(dt),
-                                              C.byref(wk), C.byref(ot), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_tangent_many_v(self.h, v[0], v[1], int(nrhs), C.byref(pr), C.byref(dt), C.byref(wk),
-                                                C.byref(ot), C.c_void_p(stream)))
+        self._mu_call("tangent_many", mueq, stream, (primal, tangent, work, out), int(nrhs), C.byref(pr), C.byref(dt),
+                      C.byref(wk), C.byref(ot))
 
     def refine(self, mueq, steps=1, norms=False, stream=0):
         """Iterative refinement of the handle's own trajectory outputs (OUT_XS .. OUT_LBDAS) against the current
@@ -779,12 +728,8 @@ class CudaRiccatiBatch:
         factorisation.  Every other output is unchanged.  ``mueq``: the mu of the last backward, a number or a [batch]
         array / tensor (``ab2_gar_refine_v``).  With ``norms=True`` returns the [batch][steps + 1] infinity norms of the
         residual of the input iterate and of each refined iterate (numpy; the call then synchronises ``stream``)."""
-        v = self._mueq_arg(mueq, stream)
         out = np.empty((self.dims.batch, steps + 1), dtype=np.float64) if norms else None
-        if v is None:
-            _check(lib().ab2_gar_refine(self.h, C.c_double(mueq), int(steps), _ptr(out), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_refine_v(self.h, v[0], v[1], int(steps), _ptr(out), C.c_void_p(stream)))
+        self._mu_call("refine", mueq, stream, None, int(steps), _ptr(out))
         if out is not None:
             self.synchronize(stream)
         return out
@@ -800,19 +745,13 @@ class CudaRiccatiBatch:
         tensor of that shape, written in stream order and returned."""
         d = self.dims
         nrhs = z["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
-        v = self._mueq_arg(mueq, stream)
         rh = _fill(LqRhs(), _RHS_KEYS, rhs)
         zz = _fill(LsIterate(), _LS_KEYS, z)
         wk = _fill(LqRefineWork(), _RHS_KEYS + _LS_KEYS, work)
         host = norms is True
         out = np.empty((nrhs, d.batch, steps + 1), dtype=np.float64) if host else norms
-        self._keep_ref_many = (rhs, z, work, out)
-        if v is None:
-            _check(lib().ab2_gar_refine_many(self.h, C.c_double(mueq), int(nrhs), int(steps), C.byref(rh), C.byref(zz),
-                                             C.byref(wk), _ptr(out), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_refine_many_v(self.h, v[0], v[1], int(nrhs), int(steps), C.byref(rh), C.byref(zz),
-                                               C.byref(wk), _ptr(out), C.c_void_p(stream)))
+        self._mu_call("refine_many", mueq, stream, (rhs, z, work, out), int(nrhs), int(steps), C.byref(rh), C.byref(zz),
+                      C.byref(wk), _ptr(out))
         if host:
             self.synchronize(stream)
         return out
@@ -825,14 +764,9 @@ class CudaRiccatiBatch:
         layouts, overwritten (G0 and g0 with zeros; a missing key is not written).  ``mueq``: the mu of the last
         backward, a number or a [batch] array / tensor (``ab2_gar_factor_adjoint_v``).  Needs a backward on the
         problem's own vectors since the last set_problem; the handle's outputs are not touched."""
-        v = self._mueq_arg(mueq, stream)
         ct = _fill(FactorCotangent(), _FCOT_KEYS, cotangent)
         gr = _fill(LqGrad(), _GRAD_KEYS, grad)
-        self._keep_fadj = (cotangent, grad)
-        if v is None:
-            _check(lib().ab2_gar_factor_adjoint(self.h, C.c_double(mueq), C.byref(ct), C.byref(gr), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_factor_adjoint_v(self.h, v[0], v[1], C.byref(ct), C.byref(gr), C.c_void_p(stream)))
+        self._mu_call("factor_adjoint", mueq, stream, (cotangent, grad), C.byref(ct), C.byref(gr))
 
     def factor_tangent(self, dot, out, mueq, stream=0):
         """Forward mode of the factorisation (``ab2_gar_factor_tangent``): ``out`` receives the derivative of the last
@@ -843,14 +777,9 @@ class CudaRiccatiBatch:
         ``mueq``: the mu of the last backward, a number or a [batch] array / tensor (``ab2_gar_factor_tangent_v``).
         Needs a backward on the problem's own vectors since the last set_problem; the handle's outputs are not
         touched."""
-        v = self._mueq_arg(mueq, stream)
         dt = _fill(LqTangent(), _GRAD_KEYS, dot)
         ot = _fill(FactorTangent(), _FCOT_KEYS, out)
-        self._keep_ftan = (dot, out)
-        if v is None:
-            _check(lib().ab2_gar_factor_tangent(self.h, C.c_double(mueq), C.byref(dt), C.byref(ot), C.c_void_p(stream)))
-        else:
-            _check(lib().ab2_gar_factor_tangent_v(self.h, v[0], v[1], C.byref(dt), C.byref(ot), C.c_void_p(stream)))
+        self._mu_call("factor_tangent", mueq, stream, (dot, out), C.byref(dt), C.byref(ot))
 
     def factor_epoch(self):
         """``ab2_gar_factor_epoch``: bumped by every call that rewrites the factorisation or the records."""
@@ -878,7 +807,7 @@ class CudaRiccatiBatch:
         v = self._device_pair(mu, mu_dyn, ("mu", "mu_dyn"), stream)
         inp = _fill(MultInputs(), _MULT_IN, inputs)
         o = _fill(MultOutputs(), _MULT_OUT, outputs)
-        self._keep_inner = (inputs, outputs)
+        self._keep["inner"] = (inputs, outputs)
         if v is None:
             inp.mu, inp.mu_dyn = float(mu), float(mu_dyn)
             return self._scalars(lambda dst, ms: _check(lib().ab2_gar_multipliers(
@@ -893,14 +822,14 @@ class CudaRiccatiBatch:
         inp = _fill(LagInputs(), _LAG_IN, inputs)
         inp.force_initial_condition = int(bool(force_initial_condition))
         o = _fill(LagOutputs(), _LAG_OUT, outputs)
-        self._keep_inner = (inputs, outputs)
+        self._keep["inner"] = (inputs, outputs)
         _check(lib().ab2_gar_lagrangian_gradient(self.h, C.byref(inp), C.byref(o), C.c_void_p(stream)))
 
     def criterion(self, arrays, out=None, stream=0):
         """computeCriterion on the device (``ab2_gar_criterion``).  ``arrays``: dict of device tensors Lxs, Lus,
         init_value, slack, Lv, Lv_N.  Returns [batch][2] = [inner_criterion, dual_infeas] (numpy, or into ``out``)."""
         ptrs = [_ptr(arrays.get(k)) for k in ("Lxs", "Lus", "init_value", "slack", "Lv", "Lv_N")]
-        self._keep_inner = (arrays,)
+        self._keep["inner"] = (arrays,)
         return self._scalars(lambda dst, ms: _check(lib().ab2_gar_criterion(
             self.h, *ptrs, dst, ms, C.c_void_p(stream))), out, stream)
 
@@ -910,7 +839,7 @@ class CudaRiccatiBatch:
         per-instance values (``ab2_fddp_backward_pass_v``)."""
         v = self._per_instance(preg, "preg")
         inp = FddpInputs(*[_ptr(arrays[k]).value for k in _FDDP_KEYS], 0.0 if v is not None else float(preg))
-        self._keep = (arrays, Vx_out, Quuks_out)
+        self._keep["fddp_backward_pass"] = (arrays, Vx_out, Quuks_out)
         if v is None:
             _check(lib().ab2_fddp_backward_pass(self.h, C.byref(inp), _ptr(Vx_out), _ptr(Quuks_out),
                                                 C.c_void_p(stream)))

@@ -114,7 +114,7 @@ def main():
                        adjoint_speedup=round(adj_ms / (ms / nrhs), 2))
             kr = profiled(torch, f) if nrhs >= 8 else {}
             del cot, work, grad, f
-            s._keep_adj_many = None  # the handle keeps the last call's arrays alive: release them before allocating
+            s._keep.pop("adjoint_many", None)  # the handle keeps the last call's arrays alive: release them before allocating
             torch.cuda.empty_cache()
             # forward mode
             dot = {k: torch.randn((nrhs,) + tuple(v.shape), dtype=torch.float64, device="cuda") for k, v in rec.items()}
@@ -125,7 +125,7 @@ def main():
                        tangent_speedup=round(tan_ms / (ms / nrhs), 2))
             kf = profiled(torch, f) if nrhs >= 8 else {}
             del dot, work, out, f
-            s._keep_tan_many = None
+            s._keep.pop("tangent_many", None)
             torch.cuda.empty_cache()
             if kr or kf:
                 by = kernel_bytes(nx, nu, nc, s.srec, B, N, nrhs)
