@@ -7,11 +7,18 @@ nothing depends on Bunch-Kaufman pivot decisions.  The fp64 inputs are exact in 
 computes from them is accurate to ~cond * 1e-50, far below anything fp64 can resolve.
 
 `solve` returns the outputs in the product's layouts (fp64, rounded from the extended-precision values);
-`error_families` measures an implementation against them, family by family."""
+`error_families` measures an implementation against them, family by family.
+
+Derivatives of the solve, exact to far below fp64, without any derivative formula or with the closed forms evaluated in
+extended precision: `tangent_problem` is the forward mode of every output of the sweep by central differences of the
+recursion at 100 digits; `grad_solution` and `grad_factor` are the reverse modes of the solution and of the
+factorisation, the restatements of tests/lq_adjoint_ref.py and tests/lq_factor_adjoint_ref.py evaluated on object
+arrays.  `grad_errors`, `factor_errors` and `solution_errors` measure an implementation's derivatives against them."""
 import mpmath
 import numpy as np
 
 import gen
+import lq_adjoint_ref as aref
 
 MP = mpmath.MPContext()
 MP.dps = 50
@@ -61,15 +68,70 @@ def lu_solve(M, Rhs):
     return X
 
 
+STAGE_BLOCKS = ("A", "B", "f", "Q", "S", "R", "q", "r", "C", "D", "d")
+TERM_BLOCKS = ("Q", "q", "C", "d")
+
+
 def _mp_knot(k):
     return {n: mpa(getattr(k, n)) for n in ("Q", "S", "R", "q", "r", "A", "B", "f", "C", "D", "d")}
 
 
-def solve_problem(p, mueq):
+def dims_of(p):
+    """(nx, nu, nc, nct, nc0, N) of an LqrProblem, in the restatements' order."""
+    N = p.horizon
+    return (p.stages[0].nx, p.stages[0].nu if N else 0, p.stages[0].nc if N else 0, p.stages[N].nc, p.nc0, N)
+
+
+def _record_blocks(rec, off, shapes):
+    """{block: fp64 array} of one packed record (column-major matrix blocks)."""
+    out = {}
+    for n, shape in shapes.items():
+        a, b = off[n]
+        out[n] = np.asarray(rec[a:b], dtype=np.float64).reshape(shape[::-1]).T if len(shape) == 2 else \
+            np.asarray(rec[a:b], dtype=np.float64)
+    return out
+
+
+def _displace(p, st, G0, g0, pdot, h):
+    """The extended-precision data st (knot dicts), G0, g0 moved to p + h pdot.  pdot: one instance's tangent in the
+    records' layouts, a dict with any of stage [N][srec], term [trec], G0 [nc0 * nx] (column-major), g0 [nc0] (a
+    missing or None entry is zero).  Q, R and the terminal Q must move symmetrically."""
+    nx, nu, nc, nct, nc0, N = dims_of(p)
+    so, _ = aref.stage_offsets(nx, nu, nc)
+    to, _ = aref.term_offsets(nx, nct)
+    get = lambda k: None if pdot.get(k) is None else np.asarray(pdot[k], dtype=np.float64)
+    move = lambda x, d: x + h * mpa(d)
+    sd, td = get("stage"), get("term")
+    for t in range(N + 1):
+        k = p.stages[t]
+        if t < N:
+            if sd is None:
+                continue
+            d = _record_blocks(sd.reshape(N, -1)[t], so, {n: getattr(k, n).shape for n in STAGE_BLOCKS})
+        else:
+            if td is None:
+                continue
+            d = _record_blocks(td.ravel(), to, {n: getattr(k, n).shape for n in TERM_BLOCKS})
+        for n, v in d.items():
+            if n in ("Q", "R"):
+                assert np.array_equal(v, v.T), "a tangent of %s must be symmetric" % n
+            st[t][n] = move(st[t][n], v)
+    if get("G0") is not None:
+        G0 = move(G0, get("G0").reshape(nx, nc0).T)
+    if get("g0") is not None:
+        g0 = move(g0, get("g0").ravel())
+    return st, G0, g0
+
+
+def solve_problem(p, mueq, pdot=None, h=0):
     """One LqrProblem (uniform stage dims, terminal knot nu = 0) at penalty mueq -> dict of extended-precision
-    outputs (object arrays) in the product's layouts."""
+    outputs (object arrays) in the product's layouts.  With a data direction `pdot` (see _displace), the problem
+    p + h pdot, its data formed exactly in the working precision."""
     N = p.horizon
     st = [_mp_knot(k) for k in p.stages]
+    G0, g0 = mpa(p.G0), mpa(p.g0)
+    if pdot is not None:
+        st, G0, g0 = _displace(p, st, G0, g0, pdot, MP.mpf(h))
     nx, nu, nc = p.stages[0].nx, (p.stages[0].nu if N else 0), (p.stages[0].nc if N else 0)
     nct, nc0 = p.stages[N].nc, p.nc0
     mu = MP.mpf(float(mueq))
@@ -100,7 +162,6 @@ def solve_problem(p, mueq):
         Vxx[t] = Qh + Sh @ K + m["C"].T @ KZ[nu:]
         vx[t] = qh + Sh @ k + m["C"].T @ kz[nu:]
     # initial saddle-point system [[Vxx_0, G0^T], [G0, 0]] [x0; lbd0] = -[vx_0; g0]
-    G0, g0 = mpa(p.G0), mpa(p.g0)
     M0 = np.block([[Vxx[0], G0.T], [G0, zeros(nc0, nc0)]]) if nc0 else Vxx[0]
     s0 = -lu_solve(M0, np.concatenate([vx[0], g0])[:, None])[:, 0]
     xs, us, vs, lbdas = [s0[:nx]], [], [], []
@@ -187,8 +248,10 @@ def _rel(a, b):
 
 def _pieces(o, nu, nc, N):
     """family -> list of per-(instance, knot) blocks of output dict o (fp64, product layouts); families whose
-    outputs o does not have are left out (an implementation that computes only the trajectory)."""
-    B = o["xs"].shape[0]
+    outputs o does not have are left out (an implementation that computes only the trajectory, or only the
+    factorisation)."""
+    traj = "xs" in o
+    B = o["xs" if traj else "fb"].shape[0]
     P = {f: [] for f in FAMILIES}
     for b in range(B):
         for t in range(N):
@@ -199,19 +262,22 @@ def _pieces(o, nu, nc, N):
                     P["Z"].append(fb[nu:nu + nc]); P["z"].append(ff[nu:nu + nc])
                 if fb.shape[0] > nu + nc:
                     P["Ahat"].append(fb[nu + nc:]); P["a"].append(ff[nu + nc:])
-            if nc:
-                P["vs"].append(o["vs"][b, t])
-            P["us"].append(o["us"][b, t]); P["lbd"].append(o["lbdas"][b, t])
-        if o["vsT"].shape[1]:
+            if traj:
+                if nc:
+                    P["vs"].append(o["vs"][b, t])
+                P["us"].append(o["us"][b, t]); P["lbd"].append(o["lbdas"][b, t])
+        if (o["vsT"] if traj else o["fbT"]).shape[1]:
             if "fbT" in o:
                 P["Z"].append(o["fbT"][b]); P["z"].append(o["ffT"][b])
-            P["vs"].append(o["vsT"][b])
-        if o["lbd0"].shape[1]:
+            if traj:
+                P["vs"].append(o["vsT"][b])
+        if traj and o["lbd0"].shape[1]:
             P["lbd"].append(o["lbd0"][b])
         for t in range(N + 1):
             if "Vxx" in o:
                 P["Vxx"].append(o["Vxx"][b, t]); P["vx"].append(o["vx"][b, t])
-            P["xs"].append(o["xs"][b, t])
+            if traj:
+                P["xs"].append(o["xs"][b, t])
     return P
 
 
@@ -237,9 +303,182 @@ def violations(e_kernel, e_oracle):
     return {f: (e_kernel[f], e_oracle[f]) for f in e_kernel if not e_kernel[f] <= tolerance(e_oracle[f])}
 
 
-def table(title, e_oracle, e_kernel):
-    rows = ["%s\n  %-5s %10s %10s %7s" % (title, "family", "e_oracle", "e_kernel", "ratio")]
+def table(title, e_oracle, e_kernel, e_torch=None):
+    """One row per family: the oracle's error, the kernel's and their ratio; with `e_torch`, the error of the fp64
+    torch.autograd derivation beside them."""
+    extra = lambda f: "" if e_torch is None else " %10.2e" % e_torch.get(f, float("nan"))
+    rows = ["%s\n  %-5s %10s %10s %7s%s" % (title, "family", "e_oracle", "e_kernel", "ratio",
+                                           "" if e_torch is None else " %10s" % "e_torch")]
     for f in e_kernel:
         ratio = e_kernel[f] / e_oracle[f] if e_oracle[f] > 0 else float("inf") if e_kernel[f] > 0 else 0.0
-        rows.append("  %-5s %10.2e %10.2e %7.2f" % (f, e_oracle[f], e_kernel[f], ratio))
+        rows.append("  %-5s %10.2e %10.2e %7.2f%s" % (f, e_oracle[f], e_kernel[f], ratio, extra(f)))
     return "\n".join(rows)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Derivatives
+# ---------------------------------------------------------------------------------------------------------------------
+TANGENT_DPS = 100      # working precision of the central differences
+TANGENT_STEP = 1e-40   # rounding ~1e-100 cond / h, truncation ~h^2 cond^2: both far below 1e-30 for cond up to 1e11
+SELF_CHECK = 1e-30     # the differences at h and at 2h agree to this, relative, output by output
+NOISE = 1e-45          # the differences' rounding is ~1e-60 cond (cond <= 1e11): anything below this is zero
+OUTPUT_KEYS = ("fb", "ff", "Vxx", "vx", "fbT", "ffT", "xs", "us", "vs", "vsT", "lbd0", "lbdas")
+
+
+def _norm(a):
+    return MP.sqrt(MP.fsum(v * v for v in np.ravel(a))) if np.size(a) else _ZERO
+
+
+def tangent_problem(p, mueq, pdot, h=TANGENT_STEP):
+    """The derivative of every output of the sweep of p along the data direction pdot (see _displace): central
+    differences (y(p + h pdot) - y(p - h pdot)) / 2h of the recursion at TANGENT_DPS digits -> dict of object arrays
+    keyed as solve_problem's outputs.  Checked against the differences at 2h: they agree to SELF_CHECK relative to the
+    larger of the derivative and the output itself, output by output.  An entry below NOISE times that scale is the
+    rounding of a derivative that is exactly zero (x_0 when G0 pins it, say) and is returned as exactly zero."""
+    with MP.workdps(TANGENT_DPS):
+        hh = MP.mpf(h)
+
+        def central(step):
+            plus, minus = solve_problem(p, mueq, pdot, step), solve_problem(p, mueq, pdot, -step)
+            return {k: (plus[k] - minus[k]) / (2 * step) for k in OUTPUT_KEYS}, plus
+
+        (d1, y), (d2, _) = central(hh), central(2 * hh)
+        for k in OUTPUT_KEYS:
+            scale = max(_norm(d1[k]), _norm(d2[k]), _norm(y[k]))
+            assert _norm(d1[k] - d2[k]) <= SELF_CHECK * scale, (k, float(_norm(d1[k] - d2[k]) / scale))
+            small = np.vectorize(lambda v: abs(v) <= NOISE * scale, otypes=[bool])(d1[k]) if d1[k].size else False
+            d1[k] = np.where(small, _ZERO, d1[k])
+    return d1
+
+
+def tangents(probs, mueq, dots):
+    """tangent_problem over a batch: dots is a dict of [B, ...] arrays in the records' layouts.  -> (fp64 dict [B, ...],
+    list of extended-precision dicts)."""
+    mus = np.broadcast_to(np.asarray(mueq, dtype=np.float64), (len(probs),))
+    hp = [tangent_problem(p, m, {k: None if v is None else np.asarray(v)[b] for k, v in dots.items()})
+          for b, (p, m) in enumerate(zip(probs, mus))]
+    return {k: np.stack([to64(h[k]) for h in hp]) for k in hp[0]}, hp
+
+
+def solution_dict(hps):
+    """Per-instance extended-precision outputs -> the batched solution dict of tests/lq_adjoint_ref.py (object)."""
+    st = lambda k: np.stack([h[k] for h in hps])
+    return dict(xs=st("xs"), us=st("us"), vs=st("vs"), vsT=st("vsT"), lam0=st("lbd0"), lams=st("lbdas"))
+
+
+def factor_dict(hps):
+    """Per-instance extended-precision outputs -> the factorisation in the restatements' keys (object)."""
+    st = lambda k: np.stack([h[k] for h in hps])
+    return dict(ff=st("ff"), fb=st("fb"), vxx=st("Vxx"), vx=st("vx"), fft=st("ffT"), fbt=st("fbT"))
+
+
+def records(probs):
+    """The packed records (stage [B][N][srec] zero-padded, term, G0 column-major, g0) of a batch, fp64."""
+    nx, nu, nc, nct, nc0, N = dims_of(probs[0])
+    _, srec = aref.stage_offsets(nx, nu, nc)
+    stage = np.zeros((len(probs), N, srec))
+    for b, p in enumerate(probs):
+        for t in range(N):
+            r = gen.stage_record(p.stages[t])
+            stage[b, t, :r.size] = r
+    term = np.stack([gen.term_record(p.stages[N]) for p in probs])
+    G0 = np.stack([np.asarray(p.G0, dtype=np.float64).ravel(order="F") for p in probs]).reshape(len(probs), nc0 * nx)
+    g0 = np.stack([np.asarray(p.g0, dtype=np.float64) for p in probs]).reshape(len(probs), nc0)
+    return stage, term, G0, g0
+
+
+def _mus(mueq, B):
+    return np.array([MP.mpf(float(m)) for m in np.broadcast_to(np.asarray(mueq, dtype=np.float64), (B,))],
+                    dtype=object)
+
+
+def grad_solution(probs, mueq, cot, hps=None):
+    """Extended-precision gradient records of <cot, z(p)> (z the solution, cot in tests/lq_adjoint_ref.py's layouts,
+    fp64): w = K^-1 cot is the extended-precision solve of the problem with its vectors replaced by -cot (exact), then
+    lq_adjoint_ref.grad_records on object arrays.  hps: the problems' extended-precision outputs, if at hand."""
+    import lq_resolve_ref as rref
+    d6 = dims_of(probs[0])
+    c = aref._full(cot, d6, len(probs))
+    hj = dict(q=-c["xs"], r=-c["us"], d=-c["vs"], dN=-c["vsT"], g0=-c["lam0"], f=-c["lams"])
+    if hps is None:
+        _, hps = solve(probs, mueq)
+    _, w = solve(rref.replaced_problems(probs, hj), mueq)
+    return aref.grad_records(solution_dict(hps), solution_dict(w), d6)
+
+
+def grad_factor(probs, mueq, cot, hps=None):
+    """Extended-precision gradient records of <cot, factorisation> (cot in tests/lq_factor_adjoint_ref.py's keys and
+    shapes, fp64): lq_factor_adjoint_ref.factor_adjoint on object arrays, fed with the extended-precision
+    factorisation."""
+    import lq_factor_adjoint_ref as fadj
+    d6 = dims_of(probs[0])
+    if hps is None:
+        _, hps = solve(probs, mueq)
+    stage, term, _, _ = records(probs)
+    f = factor_dict(hps)
+    return fadj.factor_adjoint(mpa(stage), mpa(term), f["ff"], f["fb"], f["vxx"], f["vx"], f["fft"], f["fbt"],
+                               {k: None if v is None else mpa(v) for k, v in cot.items()}, d6, _mus(mueq, len(probs)),
+                               solve=lu_solve)
+
+
+def grads64(g):
+    return {k: to64(v) for k, v in g.items()}
+
+
+# error families of the derivatives: one per record block (gradients), per factor block (factor tangents), per
+# trajectory family (solution tangents); each the worst per-(instance, knot) relative error
+GRAD_FAMILIES = STAGE_BLOCKS + tuple("N" + n for n in TERM_BLOCKS) + ("G0", "g0")
+FACTOR_FAMILIES = ("K", "k", "Z", "z", "Ahat", "a", "Vxx", "vx")
+TRAJ_FAMILIES = ("xs", "us", "vs", "lbd")
+
+
+def _grad_pieces(g, d6):
+    nx, nu, nc, nct, nc0, N = d6
+    so, _ = aref.stage_offsets(nx, nu, nc)
+    to, _ = aref.term_offsets(nx, nct)
+    tt = np.asarray(g["term"], dtype=np.float64)
+    B = tt.shape[0]
+    st, tt = np.asarray(g["stage"], dtype=np.float64).reshape(B, N, -1 if N else 0), tt.reshape(B, -1)
+    G0, g0 = (np.asarray(g[k], dtype=np.float64).reshape(B, -1) for k in ("G0", "g0"))
+    P = {f: [] for f in GRAD_FAMILIES}
+    for b in range(B):
+        for t in range(N):
+            for n, (a, e) in so.items():
+                P[n].append(st[b, t, a:e])
+        for n, (a, e) in to.items():
+            P["N" + n].append(tt[b, a:e])
+        P["G0"].append(G0[b]); P["g0"].append(g0[b])
+    return P
+
+
+def grad_errors(got, ref, d6, families=GRAD_FAMILIES):
+    """Per record block: the worst per-(instance, knot) relative error of the gradient records `got` against `ref`
+    (the fp64-rounded extended-precision records); blocks of zero size are left out."""
+    g, r = _grad_pieces(got, d6), _grad_pieces(ref, d6)
+    return {f: max(_rel(a, b) for a, b in zip(g[f], r[f])) for f in families if r[f] and np.size(r[f][0])}
+
+
+def factor_errors(got, ref, d6):
+    """Per factor block (K .. vx): the worst per-(instance, knot) relative error of a factorisation (or its tangent,
+    in the restatements' keys ff, fb, vxx, vx, fft, fbt) against `ref` in the same keys."""
+    nx, nu, nc, nct, nc0, N = d6
+    conv = lambda o: dict(fb=o["fb"], ff=o["ff"], Vxx=o["vxx"], vx=o["vx"], fbT=o["fbt"], ffT=o["fft"])
+    return error_families(conv(got), conv(ref), nu, nc, N, FACTOR_FAMILIES)
+
+
+def solution_errors(got, ref, d6):
+    """Per trajectory family: the worst per-(instance, knot) relative error of a solution (or its tangent) in
+    tests/lq_adjoint_ref.py's keys against `ref` in the same keys."""
+    nx, nu, nc, nct, nc0, N = d6
+    conv = lambda o: dict(xs=o["xs"], us=o["us"], vs=o["vs"], vsT=o["vsT"], lbd0=o["lam0"], lbdas=o["lams"])
+    return error_families(conv(got), conv(ref), nu, nc, N, TRAJ_FAMILIES)
+
+
+def solution_of(o):
+    """hp_reference / oracle output keys -> tests/lq_adjoint_ref.py's solution keys."""
+    return dict(xs=o["xs"], us=o["us"], vs=o["vs"], vsT=o["vsT"], lam0=o["lbd0"], lams=o["lbdas"])
+
+
+def factor_of(o):
+    """hp_reference / oracle output keys -> the restatements' factor keys."""
+    return dict(ff=o["ff"], fb=o["fb"], vxx=o["Vxx"], vx=o["vx"], fft=o["ffT"], fbt=o["fbT"])

@@ -7,6 +7,10 @@ dK = -w z^T read out of K's blocks (`grad_records`; the symmetric Q and R get th
 Solutions and cotangents are dicts of batched arrays in the solver's output layouts: xs [B][N+1][nx], us [B][N][nu],
 vs [B][N][nc], vsT [B][nct], lam0 [B][nc0], lams [B][N][nx] (lambda_1 .. lambda_N).  Records are the packed
 [B][N][stage_record] / [B][term_record] / [B][nc0*nx] / [B][nc0] arrays of gar.h.
+
+Every function here and in the other restatements (lq_tangent_ref, lq_factor_adjoint_ref, lq_factor_tangent_ref)
+computes in the dtype of its inputs: float64, or object arrays of extended-precision numbers (tests/hp_reference.py),
+for which every buffer is allocated as object and every linear solve goes through the `solve` hook.
 """
 from __future__ import annotations
 
@@ -41,14 +45,32 @@ def term_offsets(nx, nct, nth=0):
     return off, o
 
 
+def dtype_of(*arrays):
+    """object when any input holds extended-precision numbers (an object array), else float64."""
+    return object if any(getattr(a, "dtype", None) == object for a in arrays) else np.float64
+
+
+def batched_solve(solve, M, X):
+    """M^-1 X for stacks of systems M [..., n, n], X [..., n, m]: np.linalg.solve, or `solve` (a 2-D solver of object
+    arrays, hp_reference.lu_solve) system by system."""
+    if solve is None:
+        return np.linalg.solve(M, X)
+    lead = np.broadcast_shapes(M.shape[:-2], X.shape[:-2])
+    M, X = np.broadcast_to(M, lead + M.shape[-2:]), np.broadcast_to(X, lead + X.shape[-2:])
+    out = np.empty(lead + X.shape[-2:], dtype=object)
+    for i in np.ndindex(*lead):
+        out[i] = solve(M[i], X[i].copy()) if M.shape[-1] else X[i]
+    return out
+
+
 def _shapes(dims, B):
     nx, nu, nc, nct, nc0, N = dims
     return dict(xs=(B, N + 1, nx), us=(B, N, nu), vs=(B, N, nc), vsT=(B, nct), lam0=(B, nc0), lams=(B, N, nx))
 
 
-def _full(cot, dims, B):
+def _full(cot, dims, B, dt=np.float64):
     """Cotangent dict with missing / None entries as zeros."""
-    return {k: np.zeros(s) if cot.get(k) is None else np.asarray(cot[k], dtype=np.float64).reshape(s)
+    return {k: np.zeros(s, dtype=dt) if cot.get(k) is None else np.asarray(cot[k], dtype=dt).reshape(s)
             for k, s in _shapes(dims, B).items()}
 
 
@@ -56,16 +78,17 @@ def adjoint_records(stage, term, G0, g0, cot, dims):
     """The adjoint problem: the matrices of (stage, term, G0) and the vectors q, r, d, f, q_N, d_N, g0 = -cotangent."""
     nx, nu, nc, nct, nc0, N = dims
     B = term.shape[0]
-    c = _full(cot, dims, B)
+    dt = dtype_of(stage, term, G0, *cot.values())
+    c = _full(cot, dims, B, dt)
     so, srec = stage_offsets(nx, nu, nc)
     to, _ = term_offsets(nx, nct)
-    st = np.array(stage, dtype=np.float64).reshape(B, N, srec)
-    tt = np.array(term, dtype=np.float64).reshape(B, -1)
+    st = np.array(stage, dtype=dt).reshape(B, N, srec)
+    tt = np.array(term, dtype=dt).reshape(B, -1)
     for k, v in (("q", c["xs"][:, :N]), ("r", c["us"]), ("d", c["vs"]), ("f", c["lams"])):
         st[..., so[k][0]:so[k][1]] = -v
     tt[:, to["q"][0]:to["q"][1]] = -c["xs"][:, N]
     tt[:, to["d"][0]:to["d"][1]] = -c["vsT"]
-    return st, tt, np.array(G0, dtype=np.float64).reshape(B, -1), -c["lam0"]
+    return st, tt, np.array(G0, dtype=dt).reshape(B, -1), -c["lam0"]
 
 
 def _outer(a, b):
@@ -81,7 +104,8 @@ def grad_records(z, w, dims):
     """Gradient records from the primal solution z and the adjoint solution w (dicts of batched arrays)."""
     nx, nu, nc, nct, nc0, N = dims
     B = np.asarray(z["xs"]).shape[0]
-    z, w = _full(z, dims, B), _full(w, dims, B)
+    dt = dtype_of(*z.values(), *w.values())
+    z, w = _full(z, dims, B, dt), _full(w, dims, B, dt)
     so, srec = stage_offsets(nx, nu, nc)
     to, trec = term_offsets(nx, nct)
     x, u, v, l = z["xs"][:, :N], z["us"], z["vs"], z["lams"]
@@ -90,12 +114,12 @@ def grad_records(z, w, dims):
     blocks = dict(A=_cm(pair(l, x, L, X)), B=_cm(pair(l, u, L, U)), f=-L, Q=_cm(0.5 * pair(x, x, X, X)),
                   S=_cm(pair(x, u, X, U)), R=_cm(0.5 * pair(u, u, U, U)), q=-X, r=-U, C=_cm(pair(v, x, V, X)),
                   D=_cm(pair(v, u, V, U)), d=-V)
-    st = np.zeros((B, N, srec))
+    st = np.zeros((B, N, srec), dtype=dt)
     for k, (a, b) in so.items():
         st[..., a:b] = blocks[k]
     xN, XN = z["xs"][:, N], w["xs"][:, N]
     tb = dict(Q=_cm(0.5 * pair(xN, xN, XN, XN)), q=-XN, C=_cm(pair(z["vsT"], xN, w["vsT"], XN)), d=-w["vsT"])
-    tt = np.zeros((B, trec))
+    tt = np.zeros((B, trec), dtype=dt)
     for k, (a, b) in to.items():
         tt[:, a:b] = tb[k]
     G0 = _cm(pair(z["lam0"], z["xs"][:, 0], w["lam0"], w["xs"][:, 0]))

@@ -26,7 +26,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from lq_adjoint_ref import stage_offsets, term_offsets
+from lq_adjoint_ref import batched_solve, dtype_of, stage_offsets, term_offsets
 
 COT = ("ff", "fb", "vxx", "vx", "fft", "fbt")
 
@@ -38,8 +38,8 @@ def cot_shapes(dims, B):
                 fbt=(B, nct, nx))
 
 
-def full_cot(cot, dims, B):
-    return {k: np.zeros(s) if cot.get(k) is None else np.asarray(cot[k], dtype=np.float64).reshape(s)
+def full_cot(cot, dims, B, dt=np.float64):
+    return {k: np.zeros(s, dtype=dt) if cot.get(k) is None else np.asarray(cot[k], dtype=dt).reshape(s)
             for k, s in cot_shapes(dims, B).items()}
 
 
@@ -60,24 +60,26 @@ def _cm(M):
     return np.swapaxes(M, -1, -2).reshape(*M.shape[:-2], M.shape[-2] * M.shape[-1])
 
 
-def factor_adjoint(stage, term, ff, fb, Vxx, vx, ffT, fbT, cot, dims, mueq):
-    """Gradient records of <cot, factorisation>.  `mueq`: number or [B] array."""
+def factor_adjoint(stage, term, ff, fb, Vxx, vx, ffT, fbT, cot, dims, mueq, solve=None):
+    """Gradient records of <cot, factorisation>.  `mueq`: number or [B] array.  In the dtype of the inputs (see
+    lq_adjoint_ref); `solve`: the 2-D solver for object arrays (None: np.linalg.solve)."""
     nx, nu, nc, nct, nc0, N = dims
     n = nu + nc
     B = np.asarray(term).shape[0]
-    c = full_cot(cot, dims, B)
+    dt = dtype_of(stage, term, ff, fb, Vxx, vx, ffT, fbT, np.asarray(mueq), *cot.values())
+    c = full_cot(cot, dims, B, dt)
     so, srec = stage_offsets(nx, nu, nc)
     to, trec = term_offsets(nx, nct)
-    st = np.asarray(stage, dtype=np.float64).reshape(B, N, srec)
-    tt = np.asarray(term, dtype=np.float64).reshape(B, -1)
+    st = np.asarray(stage, dtype=dt).reshape(B, N, srec)
+    tt = np.asarray(term, dtype=dt).reshape(B, -1)
     blk = lambda rec, off, m, k: np.swapaxes(rec[..., off[0]:off[1]].reshape(*rec.shape[:-1], k, m), -1, -2)
-    mu = np.broadcast_to(np.asarray(mueq, dtype=np.float64), (B,))
-    V = _sym_lower(np.asarray(Vxx, dtype=np.float64))
-    ff = np.asarray(ff, dtype=np.float64).reshape(B, N, n + nx)
-    fb = np.asarray(fb, dtype=np.float64).reshape(B, N, n + nx, nx)
-    vx = np.asarray(vx, dtype=np.float64).reshape(B, N + 1, nx)
-    gs = np.zeros((B, N, srec))
-    gt = np.zeros((B, trec))
+    mu = np.broadcast_to(np.asarray(mueq, dtype=dt), (B,))
+    V = _sym_lower(np.asarray(Vxx, dtype=dt))
+    ff = np.asarray(ff, dtype=dt).reshape(B, N, n + nx)
+    fb = np.asarray(fb, dtype=dt).reshape(B, N, n + nx, nx)
+    vx = np.asarray(vx, dtype=dt).reshape(B, N + 1, nx)
+    gs = np.zeros((B, N, srec), dtype=dt)
+    gt = np.zeros((B, trec), dtype=dt)
     Vb = _sym(c["vxx"][:, 0])
     vb = c["vx"][:, 0].copy()
     mv = lambda M, x: np.einsum("bij,bj->bi", M, x)
@@ -109,13 +111,13 @@ def factor_adjoint(stage, term, ff, fb, Vxx, vx, ffT, fbT, cot, dims, mueq):
         Zb = c["fb"][:, t, nu:n] + C @ Vb
         zb = c["ff"][:, t, nu:n] + mv(C, vb)
         # solve
-        M = np.zeros((B, n, n))
+        M = np.zeros((B, n, n), dtype=dt)
         M[:, :nu, :nu] = _sym_lower(R + T(Bm) @ Vp @ Bm)
         M[:, nu:, :nu] = D
         M[:, :nu, nu:] = T(D)
         M[:, nu:, nu:] = -mu[:, None, None] * np.eye(nc)
         Xb = np.concatenate([np.concatenate([Kb, kb[..., None]], -1), np.concatenate([Zb, zb[..., None]], -1)], 1)
-        P = -np.linalg.solve(M, Xb)
+        P = -batched_solve(solve, M, Xb)
         Pu, Pc = P[:, :nu], P[:, nu:]
         Shb = Shb + T(Pu[..., :nx])
         rb = Pu[..., nx]
@@ -138,8 +140,8 @@ def factor_adjoint(stage, term, ff, fb, Vxx, vx, ffT, fbT, cot, dims, mueq):
         vb = c["vx"][:, t + 1] + vbp
     # terminal
     CN = blk(tt, to["C"], nct, nx)
-    ZN = np.asarray(fbT, dtype=np.float64).reshape(B, nct, nx)
-    zN = np.asarray(ffT, dtype=np.float64).reshape(B, nct)
+    ZN = np.asarray(fbT, dtype=dt).reshape(B, nct, nx)
+    zN = np.asarray(ffT, dtype=dt).reshape(B, nct)
     ZNb = c["fbt"] + CN @ Vb
     zNb = c["fft"] + mv(CN, vb)
     CNb = ZN @ Vb + outer(zN, vb) + ZNb / mu[:, None, None]
@@ -147,4 +149,4 @@ def factor_adjoint(stage, term, ff, fb, Vxx, vx, ffT, fbT, cot, dims, mueq):
     tb = dict(Q=_cm(Vb), q=vb, C=_cm(CNb), d=dNb)
     for key, (a0, a1) in to.items():
         gt[:, a0:a1] = tb[key]
-    return dict(stage=gs, term=gt, G0=np.zeros((B, nc0 * nx)), g0=np.zeros((B, nc0)))
+    return dict(stage=gs, term=gt, G0=np.zeros((B, nc0 * nx), dtype=dt), g0=np.zeros((B, nc0), dtype=dt))

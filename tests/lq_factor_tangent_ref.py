@@ -22,7 +22,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from lq_adjoint_ref import stage_offsets, term_offsets
+from lq_adjoint_ref import batched_solve, dtype_of, stage_offsets, term_offsets
 
 
 def _sym(M):
@@ -33,32 +33,35 @@ def _sym_lower(M):
     return np.tril(M) + np.swapaxes(np.tril(M, -1), -1, -2)
 
 
-def factor_tangent(stage, term, ff, fb, Vxx, vx, ffT, fbT, dot, dims, mueq):
-    """Tangents of the factorisation along `dot`.  `mueq`: number or [B] array."""
+def factor_tangent(stage, term, ff, fb, Vxx, vx, ffT, fbT, dot, dims, mueq, solve=None):
+    """Tangents of the factorisation along `dot`.  `mueq`: number or [B] array.  In the dtype of the inputs (see
+    lq_adjoint_ref); `solve`: the 2-D solver for object arrays (None: np.linalg.solve)."""
     nx, nu, nc, nct, nc0, N = dims
     n = nu + nc
     B = np.asarray(term).shape[0]
+    ty = dtype_of(stage, term, ff, fb, Vxx, vx, ffT, fbT, np.asarray(mueq), *dot.values())
     so, srec = stage_offsets(nx, nu, nc)
     to, trec = term_offsets(nx, nct)
-    st = np.asarray(stage, dtype=np.float64).reshape(B, N, srec)
-    tt = np.asarray(term, dtype=np.float64).reshape(B, -1)
-    ds = np.zeros((B, N, srec)) if dot.get("stage") is None else np.asarray(dot["stage"], np.float64).reshape(B, N, srec)
-    dt = np.zeros(tt.shape) if dot.get("term") is None else np.asarray(dot["term"], np.float64).reshape(tt.shape)
+    st = np.asarray(stage, dtype=ty).reshape(B, N, srec)
+    tt = np.asarray(term, dtype=ty).reshape(B, -1)
+    ds = np.zeros((B, N, srec), dtype=ty) if dot.get("stage") is None else \
+        np.asarray(dot["stage"], ty).reshape(B, N, srec)
+    dt = np.zeros(tt.shape, dtype=ty) if dot.get("term") is None else np.asarray(dot["term"], ty).reshape(tt.shape)
     blk = lambda rec, off, m, k: np.swapaxes(rec[..., off[0]:off[1]].reshape(*rec.shape[:-1], k, m), -1, -2)
     vec = lambda rec, off: rec[..., off[0]:off[1]]
-    mu = np.broadcast_to(np.asarray(mueq, dtype=np.float64), (B,))
-    V = _sym_lower(np.asarray(Vxx, dtype=np.float64))
-    ff = np.asarray(ff, dtype=np.float64).reshape(B, N, n + nx)
-    fb = np.asarray(fb, dtype=np.float64).reshape(B, N, n + nx, nx)
-    vx = np.asarray(vx, dtype=np.float64).reshape(B, N + 1, nx)
+    mu = np.broadcast_to(np.asarray(mueq, dtype=ty), (B,))
+    V = _sym_lower(np.asarray(Vxx, dtype=ty))
+    ff = np.asarray(ff, dtype=ty).reshape(B, N, n + nx)
+    fb = np.asarray(fb, dtype=ty).reshape(B, N, n + nx, nx)
+    vx = np.asarray(vx, dtype=ty).reshape(B, N + 1, nx)
     mv = lambda M, x: np.einsum("bij,bj->bi", M, x)
     T = lambda M: np.swapaxes(M, -1, -2)
-    out = dict(ff=np.zeros((B, N, n + nx)), fb=np.zeros((B, N, n + nx, nx)), vxx=np.zeros((B, N + 1, nx, nx)),
-               vx=np.zeros((B, N + 1, nx)))
+    out = dict(ff=np.zeros((B, N, n + nx), dtype=ty), fb=np.zeros((B, N, n + nx, nx), dtype=ty),
+               vxx=np.zeros((B, N + 1, nx, nx), dtype=ty), vx=np.zeros((B, N + 1, nx), dtype=ty))
     # terminal
     CN, dCN = blk(tt, to["C"], nct, nx), blk(dt, to["C"], nct, nx)
-    ZN = np.asarray(fbT, dtype=np.float64).reshape(B, nct, nx)
-    zN = np.asarray(ffT, dtype=np.float64).reshape(B, nct)
+    ZN = np.asarray(fbT, dtype=ty).reshape(B, nct, nx)
+    zN = np.asarray(ffT, dtype=ty).reshape(B, nct)
     dZN = dCN / mu[:, None, None]
     dzN = vec(dt, to["d"]) / mu[:, None]
     Vd = _sym(blk(dt, to["Q"], nx, nx) + T(dCN) @ ZN + T(CN) @ dZN)
@@ -85,14 +88,14 @@ def factor_tangent(stage, term, ff, fb, Vxx, vx, ffT, fbT, dot, dims, mueq):
         drh = dr + mv(T(dB), vplus) + mv(T(Bm), dvplus)
         dqh = dq + mv(T(dA), vplus) + mv(T(A), dvplus)
         # solve
-        M = np.zeros((B, n, n))
+        M = np.zeros((B, n, n), dtype=ty)
         M[:, :nu, :nu] = _sym_lower(R + T(Bm) @ Vp @ Bm)
         M[:, nu:, :nu] = D
         M[:, :nu, nu:] = T(D)
         M[:, nu:, nu:] = -mu[:, None, None] * np.eye(nc)
         Yu = np.concatenate([dRh @ K + T(dD) @ Z + T(dSh), (mv(dRh, k) + mv(T(dD), z) + drh)[..., None]], -1)
         Yc = np.concatenate([dD @ K + dC, (mv(dD, k) + dd)[..., None]], -1)
-        X = -np.linalg.solve(M, np.concatenate([Yu, Yc], 1))
+        X = -batched_solve(solve, M, np.concatenate([Yu, Yc], 1))
         dK, dk, dZ, dz = X[:, :nu, :nx], X[:, :nu, nx], X[:, nu:, :nx], X[:, nu:, nx]
         # closed loop
         dAh = dA + dB @ K + Bm @ dK

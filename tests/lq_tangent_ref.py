@@ -12,7 +12,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from lq_adjoint_ref import _full, adjoint_records, stage_offsets, term_offsets
+from lq_adjoint_ref import _full, adjoint_records, dtype_of, stage_offsets, term_offsets
 
 
 def _blk(rec, off, m, n):
@@ -37,10 +37,11 @@ def rho(dot, z, dims):
     """rho = Kdot z + hdot in the cotangent layout (xs, us, vs, vsT, lam0, lams) of lq_adjoint_ref."""
     nx, nu, nc, nct, nc0, N = dims
     B = np.asarray(z["xs"]).shape[0]
-    z = _full(z, dims, B)
+    dt = dtype_of(*z.values(), *dot.values())
+    z = _full(z, dims, B, dt)
     so, srec = stage_offsets(nx, nu, nc)
     to, trec = term_offsets(nx, nct)
-    get = lambda k, s: np.zeros(s) if dot.get(k) is None else np.asarray(dot[k], dtype=np.float64).reshape(s)
+    get = lambda k, s: np.zeros(s, dtype=dt) if dot.get(k) is None else np.asarray(dot[k], dtype=dt).reshape(s)
     st, tt = get("stage", (B, N, srec)), get("term", (B, trec))
     G0, g0 = np.swapaxes(get("G0", (B, nx, nc0)), -1, -2), get("g0", (B, nc0))
     x, u, v, l = z["xs"][:, :N], z["us"], z["vs"], z["lams"]
@@ -52,7 +53,7 @@ def rho(dot, z, dims):
         us=vec("r") + _mtv(S, x) + _mv(_sym(R), u) + _mtv(D, v) + _mtv(Bm, l),
         vs=vec("d") + _mv(C, x) + _mv(D, u),
         lams=vec("f") + _mv(A, x) + _mv(Bm, u))
-    xs = np.zeros((B, N + 1, nx))
+    xs = np.zeros((B, N + 1, nx), dtype=dt)
     xs[:, :N] = vec("q") + _mv(_sym(Q), x) + _mv(S, u) + _mtv(C, v) + _mtv(A, l)
     xN, vN = z["xs"][:, N], z["vsT"]
     QN, CN = _blk(tt, to["Q"], nx, nx), _blk(tt, to["C"], nct, nx)
