@@ -482,3 +482,66 @@ def solution_of(o):
 def factor_of(o):
     """hp_reference / oracle output keys -> the restatements' factor keys."""
     return dict(ff=o["ff"], fb=o["fb"], vxx=o["Vxx"], vx=o["vx"], fft=o["ffT"], fbt=o["fbT"])
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# FDDP backward pass
+# ---------------------------------------------------------------------------------------------------------------------
+FDDP_FAMILIES = ("K", "k", "Vxx", "Vx", "Quuks")
+
+
+def fddp_backward_pass(Jx, Ju, fs, Lxx, Lxu, Luu, Lx, Lu, Lxx_N, Lx_N, preg):
+    """oracle/fddp.py (SolverFDDPTpl::backwardPass, solver-fddp.hxx:204-277) restated in extended precision, statement by
+    statement, with the LLT solve of Quu replaced by plain Gaussian elimination.  Same arguments (one instance, fp64);
+    returns the same keys as object arrays: K, k, Quuks (N entries), Vxx, Vx (N + 1)."""
+    N = len(Jx)
+    nx = np.shape(Lxx_N)[0]
+    pr = MP.mpf(float(preg))
+    Vxx, Vx = [None] * (N + 1), [None] * (N + 1)
+    K, k, Quuks = [None] * N, [None] * N, [None] * N
+    V = mpa(Lxx_N)
+    for i in range(nx):
+        V[i, i] += pr                                                             # :217
+    Vxx[N] = V
+    Vx[N] = mpa(Lx_N) + V @ mpa(fs[N])                                            # :216, :219-220
+    for i in range(N - 1, -1, -1):
+        J = np.hstack([mpa(Jx[i]), mpa(Ju[i])])                                   # :236
+        nu = np.shape(Ju[i])[1]
+        grad = np.concatenate([mpa(Lx[i]), mpa(Lu[i])]) + J.T @ Vx[i + 1]         # :239-240
+        S = mpa(Lxu[i])
+        hess = np.block([[mpa(Lxx[i]), S], [S.T, mpa(Luu[i])]]) + (J.T @ Vxx[i + 1]) @ J   # :243-245
+        Qxx, Qxu, Quu = hess[:nx, :nx], hess[:nx, nx:], hess[nx:, nx:].copy()
+        for j in range(nu):
+            Quu[j, j] += pr                                                       # :246
+        Qx, Qu = grad[:nx], grad[nx:]
+        sol = lu_solve(Quu, np.column_stack([-Qu, -Qxu.T]))                       # :252-262
+        k[i], K[i] = sol[:, 0], sol[:, 1:]
+        Quuks[i] = Quu @ k[i]                                                     # :264
+        vx = Qx + K[i].T @ Qu                                                     # :268-269
+        v = Qxx + Qxu @ K[i]                                                      # :270-271
+        for r in range(nx):                                                       # :272 selfadjointView<Lower>
+            for c in range(r + 1, nx):
+                v[r, c] = v[c, r]
+        for r in range(nx):
+            v[r, r] += pr                                                         # :273
+        Vxx[i] = v
+        Vx[i] = vx + v @ mpa(fs[i])                                               # :274-276
+    return dict(K=K, k=k, Vxx=Vxx, Vx=Vx, Quuks=Quuks)
+
+
+def fddp_errors(got, ref):
+    """Per family of FDDP_FAMILIES: the worst relative error of any (instance, knot) block of ``got`` (lists over
+    instances of dicts of per-knot fp64 blocks, Vxx compared on its lower triangle) against ``ref`` (the same of
+    `fddp_backward_pass` outputs)."""
+    out = {}
+    for f in FDDP_FAMILIES:
+        errs = []
+        for g, r in zip(got, ref):
+            for a, b in zip(g[f], r[f]):
+                a, b = np.asarray(a, dtype=np.float64), to64(b)
+                if f == "Vxx":
+                    il = np.tril_indices(b.shape[0])
+                    a, b = a[il], b[il]
+                errs.append(_rel(a, b))
+        out[f] = max(errs)
+    return out
