@@ -32,6 +32,11 @@ schedule's sensitivity to a few parameters.
 right-hand sides in one call.  It is linear in the vectors and its own transpose, so its ``backward`` and ``jvp`` are
 ``lq_resolve`` calls again, and it has a vmap rule: ``torch.func.vmap``, ``jacrev``, ``jacfwd`` and higher orders work
 with respect to the vectors.
+
+:func:`lq_solve_higher` returns ``lq_solve``'s outputs, bit for bit, differentiable to any order (gradient penalties,
+Hessian-vector products, ``torch.func.hessian``): every derivative is resolve plus the two stateless streaming maps
+``ab2_gar_rho_many`` and ``ab2_gar_grad_many`` (DESIGN section 2p), through four Functions whose backward, jvp and vmap
+rules call each other.  ``lq_solve`` itself stays differentiable once.
 """
 from __future__ import annotations
 
@@ -569,3 +574,359 @@ def lq_factor_fwd(batch, stage, term, G0, g0, mueq):
     shape."""
     _check_inputs(batch, dict(stage=stage, term=term, G0=G0, g0=g0))
     return _LqFactorFwd.apply(batch, stage, term, G0, g0, mueq)
+
+
+# ---- higher derivatives of the solve: lq_solve_higher, from resolve and the two streaming maps (DESIGN section 2p) ----
+_NO_HIGHER_HANDLE = ("lq_solve_higher: plain serial handles only (warp and CTA kernels); dense, parametric and parallel "
+                     "handles are not served by resolve")
+
+
+class _Higher:
+    """The handle and mu of one lq_solve_higher call, and the factor epoch at which the handle's factorisation is that
+    call's data."""
+
+    def __init__(self, batch, mueq):
+        self.batch, self.mueq, self.epoch = batch, mueq, None
+        self.sol = tuple(tuple(batch.out_shape(w)) for w in _OUTS)
+        self.rec = tuple(_input_shapes(batch).values())
+
+    def stream(self, device):
+        return torch.cuda.current_stream(device).cuda_stream
+
+    def factor(self, P, stream):
+        """Make the handle's factorisation that of the data P = (stage, term, G0, g0), re-running set_problem and
+        backward when another call has moved the factor epoch since."""
+        if self.batch.factor_epoch() != self.epoch:
+            self.batch.set_problem(*P, memspace=_gar.AB2_DEVICE, stream=stream)
+            self.batch.backward(self.mueq, stream=stream)
+            self.epoch = self.batch.factor_epoch()
+
+
+def _none(ts):
+    return ts is None or all(t is None for t in ts)
+
+
+def _directions(ts, shapes):
+    """The number of directions of the operands ts (base shapes `shapes`): the leading size of those that carry one,
+    None when every operand has its base shape."""
+    for t, s in zip(ts, shapes):
+        if t is not None and t.dim() == len(s) + 1:
+            return t.shape[0]
+    return None
+
+
+def _device(h, ts):
+    for t in ts:
+        if t is not None:
+            return t.device
+    return torch.device("cuda", h.batch.dims.device)
+
+
+def _per(t, s, n, device):
+    """t as a contiguous float64 [n][...] tensor: broadcast when it has its base shape s, zeros when None."""
+    if t is None:
+        return torch.zeros((n,) + s, dtype=torch.float64, device=device)
+    if t.dim() == len(s):
+        t = t.unsqueeze(0).expand(n, *s)
+    return t.to(torch.float64).contiguous()
+
+
+def _vector(ts, shapes, n, device):
+    """A vector operand as the library's dict: shared ([batch][...]) when none of its fields carries directions, else
+    every field [n][...]; None fields are zeros."""
+    if _directions(ts, shapes) is None:
+        return {k: (torch.zeros(s, dtype=torch.float64, device=device) if t is None else t.to(torch.float64).contiguous())
+                for k, t, s in zip(_KEYS, ts, shapes)}
+    return {k: _per(t, s, n, device) for k, t, s in zip(_KEYS, ts, shapes)}
+
+
+def _records(ts, shapes, n):
+    return {k: None if t is None else _per(t, s, n, t.device) for k, t, s in zip(_INPUTS, ts, shapes)}
+
+
+def _results(outs, n):
+    return tuple(o if n else o[0] for o in outs)
+
+
+def _fold(info, in_dims, args, kinds, refuse):
+    """The vmap rule of the higher-order Functions: every vmapped dimension goes into the directions of one call.  An
+    operand of kind s (its base shape) that carries the level's dimension and directions of an inner level becomes
+    [V * n][...]; one without either is broadcast to them, or stays shared when no operand has inner directions.  Kind
+    "P" (the problem data) is refused when vmapped, kind None is passed as it is."""
+    V = info.batch_size
+    moved = []
+    for t, bd, k in zip(args, in_dims, kinds):
+        if k == "P" and bd is not None:
+            raise NotImplementedError(refuse)
+        moved.append(t.movedim(bd, 0) if bd is not None and isinstance(k, tuple) else t)
+    n = None
+    for t, bd, k in zip(moved, in_dims, kinds):
+        if isinstance(k, tuple) and t is not None and t.dim() - (bd is not None) > len(k):
+            n = t.shape[1 if bd is not None else 0]
+    flat = []
+    for t, bd, k in zip(moved, in_dims, kinds):
+        if isinstance(k, tuple) and t is not None:
+            inner = t.dim() - (bd is not None) > len(k)
+            if bd is not None and n is not None:
+                t = (t if inner else t.unsqueeze(1).expand(V, n, *k)).reshape(V * n, *k)
+            elif bd is None and inner:
+                t = t.unsqueeze(0).expand(V, *t.shape).reshape(V * n, *k)
+        flat.append(t)
+    return flat, n
+
+
+def _unfold(info, outs, n):
+    V = info.batch_size
+    return tuple(o.reshape(V, n, *o.shape[1:]) if n else o for o in outs), (0,) * len(outs)
+
+
+def _rho_sum(h, terms, e):
+    """sum of rho^(v)(P; a) over terms (v, P, a) plus e, by _Rho calls of at most two terms each (the term with
+    vectors first); terms with a zero P, or a zero a without vectors, are dropped.  None when nothing is left."""
+    terms = sorted([t for t in terms if not _none(t[1]) and not (_none(t[2]) and not t[0])], key=lambda t: not t[0])
+    none4, none6 = (None,) * 4, (None,) * 6
+    while terms:
+        first = terms.pop(0)
+        second = terms.pop(0) if terms else None
+        e = _Rho.apply(h, first[0], *first[1], *(first[2] or none6), *(second[1] if second else none4),
+                       *((second[2] or none6) if second else none6), *(e or none6))
+    return e
+
+
+def _grad_sum(h, pairs):
+    """sum of Gr^(v)(y; z) over pairs (v, y, z), by _Grad calls of at most two pairs each (the pair with vectors
+    first); pairs with a zero y, or a zero z without vectors, are dropped.  None when nothing is left."""
+    pairs = sorted([p for p in pairs if not _none(p[1]) and not (_none(p[2]) and not p[0])], key=lambda p: not p[0])
+    none6, total = (None,) * 6, None
+    while pairs:
+        first = pairs.pop(0)
+        second = pairs.pop(0) if pairs else None
+        g = _Grad.apply(h, first[0], *first[1], *(first[2] or none6), *(second[1] if second else none6),
+                        *((second[2] or none6) if second else none6))
+        total = g if total is None else tuple(a + b for a, b in zip(total, g))
+    return total
+
+
+def _pick(values, need):
+    return tuple(v if n else None for v, n in zip(values, need)) if values is not None else (None,) * len(need)
+
+
+class _Solve(torch.autograd.Function):
+    """z = solve(P): set_problem and sweep.  jvp: resolve(rho(Pdot; z)); vjp: Gr(resolve(c); z)."""
+
+    @staticmethod
+    def forward(h, stage, term, G0, g0):
+        stream = h.stream(stage.device)
+        h.batch.set_problem(stage, term, G0, g0, memspace=_gar.AB2_DEVICE, stream=stream)
+        h.batch.sweep(h.mueq, stream=stream)
+        h.epoch = h.batch.factor_epoch()
+        return _outputs(h.batch, stage.device, stream)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.h = inputs[0]
+        ctx.save_for_backward(*inputs[1:], *output)
+        ctx.save_for_forward(*inputs[1:], *output)
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *c):
+        if _none(c):
+            return (None,) * 5
+        saved = ctx.saved_tensors
+        P, z = saved[:4], saved[4:]
+        m = _Resolve.apply(ctx.h, *P, *c)
+        return (None,) + _pick(_grad_sum(ctx.h, [(True, m, z)]), ctx.needs_input_grad[1:5])
+
+    @staticmethod
+    def jvp(ctx, _h, *Pdot):
+        saved = ctx.saved_tensors
+        P, z = saved[:4], saved[4:]
+        if _none(Pdot):
+            return tuple(torch.zeros_like(t) for t in z)
+        return _Resolve.apply(ctx.h, *P, *_rho_sum(ctx.h, [(True, Pdot, z)], None))
+
+    @staticmethod
+    def vmap(info, in_dims, h, stage, term, G0, g0):
+        raise NotImplementedError(_NO_DATA_VMAP)
+
+
+class _Resolve(torch.autograd.Function):
+    """z = resolve_P(h) = -K(P)^-1 h, h in the solution's layouts.  jvp: resolve(hdot + rho_K(Pdot; z)); vjp: hbar =
+    m = resolve(c), Pbar = Gr_K(m; z)."""
+
+    @staticmethod
+    def forward(h, stage, term, G0, g0, *hv):
+        n = _directions(hv, h.sol)
+        device = stage.device
+        outs = [torch.empty((n or 1,) + s, dtype=torch.float64, device=device) for s in h.sol]
+        stream = h.stream(device)
+        if _none(hv):
+            return _results([o.zero_() for o in outs], n)
+        h.factor((stage, term, G0, g0), stream)
+        rhs = {k: None if t is None else _per(t, s, n or 1, device) for k, t, s in zip(_RHS, hv, h.sol)}
+        h.batch.resolve(rhs, dict(zip(_KEYS, outs)), h.mueq, stream=stream)
+        return _results(outs, n)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.h = inputs[0]
+        ctx.save_for_backward(*inputs[1:5], *output)
+        ctx.save_for_forward(*inputs[1:5], *output)
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *c):
+        if _none(c):
+            return (None,) * 11
+        saved = ctx.saved_tensors
+        P, z = saved[:4], saved[4:]
+        need = ctx.needs_input_grad
+        m = _Resolve.apply(ctx.h, *P, *c)
+        Pbar = _grad_sum(ctx.h, [(False, m, z)]) if any(need[1:5]) else None
+        return (None,) + _pick(Pbar, need[1:5]) + _pick(m, need[5:])
+
+    @staticmethod
+    def jvp(ctx, _h, *dots):
+        saved = ctx.saved_tensors
+        P, z = saved[:4], saved[4:]
+        r = _rho_sum(ctx.h, [(False, dots[:4], z)], None if _none(dots[4:]) else dots[4:])
+        if r is None:
+            return tuple(torch.zeros_like(t) for t in z)
+        return _Resolve.apply(ctx.h, *P, *r)
+
+    @staticmethod
+    def vmap(info, in_dims, h, *args):
+        flat, n = _fold(info, in_dims[1:], args, ("P",) * 4 + h.sol, _NO_DATA_VMAP)
+        return _unfold(info, _Resolve.apply(h, *flat), n)
+
+
+class _Rho(torch.autograd.Function):
+    """r = rho^(vec)(P1; a1) + rho_K(P2; a2) + e (ab2_gar_rho_many), in the solution's layouts.  jvp:
+    rho^(vec)(P1'; a1) + rho_K(P1; a1') + rho_K(P2'; a2) + rho_K(P2; a2') + e'; vjp: P1bar = Gr^(vec)(c; a1),
+    a1bar = rho_K(P1; c), P2bar = Gr_K(c; a2), a2bar = rho_K(P2; c), ebar = c."""
+
+    @staticmethod
+    def forward(h, vec, *args):
+        P1, a1, P2, a2, e = args[:4], args[4:10], args[10:14], args[14:20], args[20:26]
+        n = _directions(args, h.rec + h.sol + h.rec + h.sol + h.sol)
+        device = _device(h, args)
+        N = n or 1
+        out = {k: torch.empty((N,) + s, dtype=torch.float64, device=device) for k, s in zip(_KEYS, h.sol)}
+        two = not _none(P2)
+        h.batch.rho_many(_records(P1, h.rec, N), _vector(a1, h.sol, N, device), out, vectors=vec,
+                         dot2=_records(P2, h.rec, N) if two else None,
+                         a2=_vector(a2, h.sol, N, device) if two else None,
+                         e=None if _none(e) else {k: _per(t, s, N, device) for k, t, s in zip(_KEYS, e, h.sol)},
+                         stream=h.stream(device))
+        return _results(out.values(), n)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.h, ctx.vec = inputs[:2]
+        ctx.outs = [(o.shape, o.device) for o in output]
+        ctx.save_for_backward(*inputs[2:22])
+        ctx.save_for_forward(*inputs[2:22])
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *c):
+        if _none(c):
+            return (None,) * 28
+        saved = ctx.saved_tensors
+        P1, a1, P2, a2 = saved[:4], saved[4:10], saved[10:14], saved[14:20]
+        need, h = ctx.needs_input_grad[2:], ctx.h
+        P1bar = _grad_sum(h, [(ctx.vec, c, a1)]) if any(need[:4]) else None
+        a1bar = _rho_sum(h, [(False, P1, c)], None) if any(need[4:10]) else None
+        P2bar = _grad_sum(h, [(False, c, a2)]) if any(need[10:14]) else None
+        a2bar = _rho_sum(h, [(False, P2, c)], None) if any(need[14:20]) else None
+        return ((None, None) + _pick(P1bar, need[:4]) + _pick(a1bar, need[4:10]) + _pick(P2bar, need[10:14])
+                + _pick(a2bar, need[14:20]) + _pick(c, need[20:26]))
+
+    @staticmethod
+    def jvp(ctx, _h, _vec, *t):
+        saved = ctx.saved_tensors
+        P1, a1, P2, a2 = saved[:4], saved[4:10], saved[10:14], saved[14:20]
+        r = _rho_sum(ctx.h, [(ctx.vec, t[:4], a1), (False, P1, t[4:10]), (False, t[10:14], a2), (False, P2, t[14:20])],
+                     None if _none(t[20:26]) else t[20:26])
+        return r if r is not None else tuple(torch.zeros(sh, dtype=torch.float64, device=dv) for sh, dv in ctx.outs)
+
+    @staticmethod
+    def vmap(info, in_dims, h, vec, *args):
+        flat, n = _fold(info, in_dims[2:], args, h.rec + h.sol + h.rec + h.sol + h.sol, _NO_DATA_VMAP)
+        return _unfold(info, _Rho.apply(h, vec, *flat), n)
+
+
+class _Grad(torch.autograd.Function):
+    """g = Gr^(vec)(y1; z1) + Gr_K(y2; z2) (ab2_gar_grad_many), in the problem's record layouts.  jvp:
+    Gr^(vec)(y1'; z1) + Gr_K(y1; z1') + Gr_K(y2'; z2) + Gr_K(y2; z2'); vjp: y1bar = rho^(vec)(C; z1),
+    z1bar = rho_K(C; y1), y2bar = rho_K(C; z2), z2bar = rho_K(C; y2)."""
+
+    @staticmethod
+    def forward(h, vec, *args):
+        y1, z1, y2, z2 = args[:6], args[6:12], args[12:18], args[18:24]
+        n = _directions(args, h.sol * 4)
+        device = _device(h, args)
+        N = n or 1
+        grad = {k: torch.empty((N,) + s, dtype=torch.float64, device=device) for k, s in zip(_INPUTS, h.rec)}
+        two = not _none(y2)
+        h.batch.grad_many({k: _per(t, s, N, device) for k, t, s in zip(_KEYS, y1, h.sol)},
+                          _vector(z1, h.sol, N, device), grad, vectors=vec,
+                          y2={k: _per(t, s, N, device) for k, t, s in zip(_KEYS, y2, h.sol)} if two else None,
+                          z2=_vector(z2, h.sol, N, device) if two else None, stream=h.stream(device))
+        return _results(grad.values(), n)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.h, ctx.vec = inputs[:2]
+        ctx.outs = [(o.shape, o.device) for o in output]
+        ctx.save_for_backward(*inputs[2:])
+        ctx.save_for_forward(*inputs[2:])
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *C):
+        if _none(C):
+            return (None,) * 26
+        saved = ctx.saved_tensors
+        y1, z1, y2, z2 = saved[:6], saved[6:12], saved[12:18], saved[18:24]
+        need, h = ctx.needs_input_grad[2:], ctx.h
+        y1bar = _rho_sum(h, [(ctx.vec, C, z1)], None) if any(need[:6]) else None
+        z1bar = _rho_sum(h, [(False, C, y1)], None) if any(need[6:12]) else None
+        y2bar = _rho_sum(h, [(False, C, z2)], None) if any(need[12:18]) else None
+        z2bar = _rho_sum(h, [(False, C, y2)], None) if any(need[18:24]) else None
+        return ((None, None) + _pick(y1bar, need[:6]) + _pick(z1bar, need[6:12]) + _pick(y2bar, need[12:18])
+                + _pick(z2bar, need[18:24]))
+
+    @staticmethod
+    def jvp(ctx, _h, _vec, *t):
+        saved = ctx.saved_tensors
+        y1, z1, y2, z2 = saved[:6], saved[6:12], saved[12:18], saved[18:24]
+        g = _grad_sum(ctx.h, [(ctx.vec, t[:6], z1), (False, y1, t[6:12]), (False, t[12:18], z2), (False, y2, t[18:24])])
+        return g if g is not None else tuple(torch.zeros(sh, dtype=torch.float64, device=dv) for sh, dv in ctx.outs)
+
+    @staticmethod
+    def vmap(info, in_dims, h, vec, *args):
+        flat, n = _fold(info, in_dims[2:], args, h.sol * 4, _NO_DATA_VMAP)
+        return _unfold(info, _Grad.apply(h, vec, *flat), n)
+
+
+def lq_solve_higher(batch, stage, term, G0, g0, mueq):
+    """:func:`lq_solve`'s outputs ``(xs, us, vs, vsT, lam0, lams)``, bit for bit (the same set_problem and sweep),
+    differentiable to ANY order with respect to ``stage``, ``term``, ``G0`` and ``g0``: gradient penalties
+    (``create_graph=True``), Hessian-vector products (``torch.func.jvp`` of ``torch.func.grad``), ``torch.func.hessian``.
+    Every derivative is a composition of resolve (``ab2_gar_resolve``) and the two streaming maps rho and Gr
+    (``ab2_gar_rho_many``, ``ab2_gar_grad_many``); under vmap (``jacrev``, ``jacfwd``, ``hessian``) each op makes one
+    device call per vmap level, whatever the number of directions.  Its first derivatives equal lq_solve's vmapped ones
+    (``jacrev``, ``jacfwd``), and a single vjp or jvp equals ``adjoint_many`` / ``tangent_many`` at nrhs = 1.  A resolve
+    runs on the handle's factorisation of this call's data: when another call has refactored the handle since (its
+    ``factor_epoch`` moved), set_problem and backward are run again first.  ``mueq`` (a number or a [batch] tensor) is
+    not differentiated.  Plain serial handles only: dense, parametric and parallel handles raise ``ValueError`` before
+    any library call, as does a tensor that is not a contiguous float64 CUDA tensor of the handle's shape; vmap over the
+    problem data raises ``NotImplementedError``."""
+    if not isinstance(batch, _gar.CudaRiccatiBatch):
+        raise ValueError("lq_solve_higher: `batch` must be a CudaRiccatiBatch")
+    if batch.dense or batch.nth > 0 or batch.legs:
+        raise ValueError(_NO_HIGHER_HANDLE)
+    _check_inputs(batch, dict(stage=stage, term=term, G0=G0, g0=g0))
+    return _Solve.apply(_Higher(batch, mueq), stage, term, G0, g0)

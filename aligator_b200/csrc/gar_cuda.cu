@@ -1459,6 +1459,116 @@ int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, 
   return tangent_many_impl(s, 0.0, mueq, memspace, nrhs, primal, dot, work, out, stream);
 }
 
+// ---- the generalised streaming kernels (lq_jacobian.cu) as stateless calls: no factorisation, no mu ----
+static int check_stateless_handle(const ab2_gar_solver *s, int nrhs, const char *who) {
+  if (s->nth > 0 || s->legs > 1)
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": parametric (nth > 0) and parallel handles are not supported");
+  if (nrhs < 0)
+    return fail(AB2_ERR_INVALID, std::string(who) + ": nrhs < 0");
+  return AB2_OK;
+}
+// the output o may overlap none of the inputs, nor itself
+static int refuse_output_overlap(const Fields &o, std::initializer_list<const Fields *> in, const char *who) {
+  if (int rc = refuse_overlap(o, o, who))
+    return rc;
+  for (const Fields *f : in)
+    if (int rc = refuse_overlap(o, *f, who))
+      return rc;
+  return AB2_OK;
+}
+static ab2::SolVec sol_vec(const ab2_ls_iterate *v, bool each) {
+  return v ? ab2::SolVec{v->xs, v->us, v->vs, v->vsT, v->lam0, v->lams, each} : ab2::SolVec{};
+}
+
+int ab2_gar_rho_many(ab2_gar_solver *s, int nrhs, int with_vectors, const ab2_lq_tangent *dot1,
+                     const ab2_ls_iterate *a1, int a1_each, const ab2_lq_tangent *dot2, const ab2_ls_iterate *a2,
+                     int a2_each, const ab2_ls_iterate *e, const ab2_ls_trial *out, void *stream) {
+  const char *who = "rho_many";
+  if (!s || !dot1 || !a1 || !out || (dot2 && !a2))
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_stateless_handle(s, nrhs, who))
+    return rc;
+  const size_t B = s->d.batch, R = (size_t)nrhs * B;
+  const bool two = dot2 != nullptr;
+  const ab2_lq_tangent none{};
+  const ab2_ls_iterate zero{};
+  const Fields D1 = rec_fields(s, "dot1", *dot1, R), D2 = rec_fields(s, "dot2", two ? *dot2 : none, R),
+               A1 = sol_fields(s, "a1", *a1, a1_each ? R : B), A2 = sol_fields(s, "a2", two ? *a2 : zero, a2_each ? R : B),
+               E = sol_fields(s, "e", e ? *e : zero, R), O = sol_fields(s, "out", *out, R);
+  for (const Fields *f : {&A1, &O})
+    if (int rc = require(*f, who))
+      return rc;
+  if (two)
+    if (int rc = require(A2, who))
+      return rc;
+  if (e)
+    if (int rc = require(E, who))
+      return rc;
+  if (int rc = refuse_output_overlap(O, {&D1, &D2, &A1, &A2, &E}, who))
+    return rc;
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(s->d.device));
+  const bool plain = with_vectors && !a1_each && !two && !e;
+  ab2::JacobianRhsArgs ra{adjoint_dims(s), nrhs, dot1->stage, dot1->term, dot1->G0, dot1->g0,
+                          a1->xs, a1->us, a1->vs, a1->vsT, a1->lam0, a1->lams,
+                          out->xs, out->us, out->vs, out->vsT, out->lam0, out->lams};
+  if (!plain) {
+    ra.ext = true;
+    ra.vec = with_vectors != 0;
+    ra.z_each = a1_each != 0;
+    ra.two = two;
+    if (two) {
+      ra.stage2 = dot2->stage;
+      ra.term2 = dot2->term;
+      ra.G02 = dot2->G0;
+      ra.z2 = sol_vec(a2, a2_each != 0);
+    }
+    ra.e = sol_vec(e, true);
+  }
+  CUDA_TRY(ab2::launch_jacobian_rhs(ra, (cudaStream_t)stream));
+  s->launches += 1;
+  return AB2_OK;
+}
+
+int ab2_gar_grad_many(ab2_gar_solver *s, int nrhs, int with_vectors, const ab2_ls_iterate *y1,
+                      const ab2_ls_iterate *z1, int z1_each, const ab2_ls_iterate *y2, const ab2_ls_iterate *z2,
+                      int z2_each, const ab2_lq_grad *grad, void *stream) {
+  const char *who = "grad_many";
+  if (!s || !y1 || !z1 || !grad || (y2 && !z2))
+    return fail(AB2_ERR_INVALID, "null argument");
+  if (int rc = check_stateless_handle(s, nrhs, who))
+    return rc;
+  const size_t B = s->d.batch, R = (size_t)nrhs * B;
+  const bool two = y2 != nullptr;
+  const ab2_ls_iterate zero{};
+  const Fields Y1 = sol_fields(s, "y1", *y1, R), Z1 = sol_fields(s, "z1", *z1, z1_each ? R : B),
+               Y2 = sol_fields(s, "y2", two ? *y2 : zero, R), Z2 = sol_fields(s, "z2", two ? *z2 : zero, z2_each ? R : B),
+               G = rec_fields(s, "grad", *grad, R);
+  for (const Fields *f : {&Y1, &Z1, &Y2, &Z2})
+    if (int rc = (f == &Y1 || f == &Z1 || two) ? require(*f, who) : AB2_OK)
+      return rc;
+  if (int rc = refuse_output_overlap(G, {&Y1, &Z1, &Y2, &Z2}, who))
+    return rc;
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(s->d.device));
+  ab2::JacobianGradArgs ga{adjoint_dims(s), nrhs,
+                           z1->xs, z1->us, z1->vs, z1->vsT, z1->lam0, z1->lams,
+                           y1->xs, y1->us, y1->vs, y1->vsT, y1->lam0, y1->lams,
+                           grad->stage, grad->term, grad->G0, grad->g0, false};
+  if (!(with_vectors && !z1_each && !two)) {
+    ga.ext = true;
+    ga.vec = with_vectors != 0;
+    ga.z_each = z1_each != 0;
+    ga.y2 = sol_vec(y2, true);
+    ga.z2 = sol_vec(z2, z2_each != 0);
+  }
+  CUDA_TRY(ab2::launch_jacobian_grad(ga, (cudaStream_t)stream));
+  s->launches += 1;
+  return AB2_OK;
+}
+
 // ---- iterative refinement (lq_refine.cu): residual, resolve and update per step, on the last backward's factorisation ----
 static bool device_accessible(const void *p) {
   cudaPointerAttributes at{};

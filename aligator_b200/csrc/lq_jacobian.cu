@@ -21,6 +21,9 @@
 //    Each lane sums its rows in a fixed order (tile by tile, block by block, element by element); the tile boundaries
 //    depend on the record length only.
 // So right-hand side j's result is bit for bit independent of nrhs and of j's position, and of timing.
+// Both kernels have a generalised instantiation (EXT, ab2_gar_rho_many / ab2_gar_grad_many, DESIGN section 2p): the
+// vector blocks optional, a per-right-hand-side z staged once per (rhs, knot) beside the shared one, a second term or
+// pair without vector blocks, and an addend e, each element still summed in one fixed order.
 #include <cuda_runtime.h>
 
 #include "cp_async.cuh"
@@ -58,6 +61,37 @@ __device__ __forceinline__ double gvalue(unsigned ent, const double *p, const do
   }
   return sgn * s;
 }
+// The generalised mode's value of one element: Gr^(vec)(y; p) + Gr_K(y2; p2) (two), each pair rounded as the plain
+// mode's (sgn = +1, no swap); a vector element of a pair without vectors is 0.
+__device__ __forceinline__ double gvalue2(unsigned ent, const double *p, const double *y, bool vec, const double *p2,
+                                          const double *y2, bool two) {
+  const unsigned mode = ent >> 30;
+  double s = mode == G_SINGLE && !vec ? 0.0 : gvalue(ent, p, y, 1.0, false);
+  if (two)
+    s += mode == G_SINGLE ? 0.0 : gvalue(ent, p2, y2, 1.0, false);
+  return s;
+}
+// Entry k of knot `it`'s vector [x | u | v | l] (k < 2 nx + nu + nc) of the solution-layout vector z, whose row (the
+// instance, or j * batch + b) is `row`: x_t sits in row `row` of [.][N+1][nx], the others in [.][N][.].
+__device__ __forceinline__ double knot_entry(const double *xs, const double *us, const double *vs, const double *lams,
+                                             long it, long row, int k, int nx, int nu, int nc) {
+  const int U = nx, V = nx + nu, L = nx + nu + nc;
+  return k < U ? xs[(it + row) * nx + k] : k < V ? us[it * nu + k - U] : k < L ? vs[it * nc + k - V]
+                                                                             : lams[it * nx + k - L];
+}
+__device__ __forceinline__ double knot_entry(const SolVec &z, long it, long row, int k, int nx, int nu, int nc) {
+  return knot_entry(z.xs, z.us, z.vs, z.lams, it, row, k, nx, nu, nc);
+}
+// Entry k of row `row`'s terminal vector [x_N | v_N | x_0 | l_0] (k < 2 nx + nct + nc0) of z.
+__device__ __forceinline__ double term_entry(const SolVec &z, long row, int k, int nx, int nct, int nc0, int N) {
+  if (k < nx)
+    return z.xs[(row * (N + 1) + N) * nx + k];
+  if (k < nx + nct)
+    return z.vsT[row * nct + k - nx];
+  if (k < 2 * nx + nct)
+    return z.xs[row * (N + 1) * nx + k - nx - nct];
+  return z.lam0[row * nc0 + k - 2 * nx - nct];
+}
 
 // ---- rho rows from a staged tile holding record elements [e0, e1) ----
 // Part of row i of M y (col = false) or of M^T y (col = true) in the tile, for the m x n block M at record offset o.
@@ -89,40 +123,41 @@ __device__ __forceinline__ double ve(const double *tile, int e0, int e1, int o, 
 // stage rows [q (nx) | r (nu) | d (nc) | f (nx)]:
 //   rho_q = qdot + sym(Qdot) x + Sdot u + Cdot^T v + Adot^T l,  rho_r = rdot + Sdot^T x + sym(Rdot) u + Ddot^T v + Bdot^T l,
 //   rho_d = ddot + Cdot x + Ddot u,  rho_f = fdot + Adot x + Bdot u
+// vec = false: rho_K, the same rows without the tangent's vector blocks (qdot, rdot, ddot, fdot)
 __device__ __forceinline__ double stage_row(const double *tile, int e0, int e1, const StageOffsets &o, int nx, int nu,
                                             int nc, int row, const double *x, const double *u, const double *v,
-                                            const double *l) {
+                                            const double *l, bool vec = true) {
   if (row < nx) {
     const int i = row;
-    return ve(tile, e0, e1, o.q, i) +
+    return (vec ? ve(tile, e0, e1, o.q, i) : 0.0) +
            0.5 * (mv(tile, e0, e1, o.Q, nx, nx, i, false, x) + mv(tile, e0, e1, o.Q, nx, nx, i, true, x)) +
            mv(tile, e0, e1, o.S, nx, nu, i, false, u) + mv(tile, e0, e1, o.C, nc, nx, i, true, v) +
            mv(tile, e0, e1, o.A, nx, nx, i, true, l);
   }
   if (row < nx + nu) {
     const int i = row - nx;
-    return ve(tile, e0, e1, o.r, i) + mv(tile, e0, e1, o.S, nx, nu, i, true, x) +
+    return (vec ? ve(tile, e0, e1, o.r, i) : 0.0) + mv(tile, e0, e1, o.S, nx, nu, i, true, x) +
            0.5 * (mv(tile, e0, e1, o.R, nu, nu, i, false, u) + mv(tile, e0, e1, o.R, nu, nu, i, true, u)) +
            mv(tile, e0, e1, o.D, nc, nu, i, true, v) + mv(tile, e0, e1, o.B, nx, nu, i, true, l);
   }
   if (row < nx + nu + nc) {
     const int i = row - nx - nu;
-    return ve(tile, e0, e1, o.d, i) + mv(tile, e0, e1, o.C, nc, nx, i, false, x) +
+    return (vec ? ve(tile, e0, e1, o.d, i) : 0.0) + mv(tile, e0, e1, o.C, nc, nx, i, false, x) +
            mv(tile, e0, e1, o.D, nc, nu, i, false, u);
   }
   const int i = row - nx - nu - nc;
-  return ve(tile, e0, e1, o.f, i) + mv(tile, e0, e1, o.A, nx, nx, i, false, x) +
+  return (vec ? ve(tile, e0, e1, o.f, i) : 0.0) + mv(tile, e0, e1, o.A, nx, nx, i, false, x) +
          mv(tile, e0, e1, o.B, nx, nu, i, false, u);
 }
 // terminal rows [q_N (nx) | d_N (nct)]: rho_qN = qdot_N + sym(Qdot_N) x + C_Ndot^T v,  rho_dN = ddot_N + C_Ndot x
 __device__ __forceinline__ double term_row(const double *tile, int e0, int e1, const TermOffsets &o, int nx, int nct,
-                                           int row, const double *x, const double *v) {
+                                           int row, const double *x, const double *v, bool vec = true) {
   if (row < nx)
-    return ve(tile, e0, e1, o.q, row) +
+    return (vec ? ve(tile, e0, e1, o.q, row) : 0.0) +
            0.5 * (mv(tile, e0, e1, o.Q, nx, nx, row, false, x) + mv(tile, e0, e1, o.Q, nx, nx, row, true, x)) +
            mv(tile, e0, e1, o.C, nct, nx, row, true, v);
   const int i = row - nx;
-  return ve(tile, e0, e1, o.d, i) + mv(tile, e0, e1, o.C, nct, nx, i, false, x);
+  return (vec ? ve(tile, e0, e1, o.d, i) : 0.0) + mv(tile, e0, e1, o.C, nct, nx, i, false, x);
 }
 
 int sm_count() {
@@ -133,8 +168,9 @@ int sm_count() {
 }
 } // namespace
 
-// NEG: a.neg, as a template argument so that the flag costs no register
-template <bool NEG>
+// NEG: a.neg, as a template argument so that the flag costs no register.  EXT: a.ext, the generalised mode (per
+// right-hand-side z, a second pair, vector blocks optional); EXT = false is the plain mode's code unchanged.
+template <bool NEG, bool EXT>
 __global__ void __launch_bounds__(kWarps * 32) jacobian_grad_kernel(const JacobianGradArgs a, int chunk,
                                                                     int warp_doubles) {
   extern __shared__ __align__(16) double smem[];
@@ -180,80 +216,163 @@ __global__ void __launch_bounds__(kWarps * 32) jacobian_grad_kernel(const Jacobi
   double *pv = smem + (size_t)wid * warp_doubles;
   const long nS = a.stage ? (long)B * N : 0, nT = (a.term || a.G0 || a.g0) ? (long)B * a.nrhs : 0;
   const long w0 = (long)blockIdx.x * kWarps + wid, ws = (long)gridDim.x * kWarps;
-  for (long it = w0; it < nS + nT; it += ws) {
-    if (it < nS) { // stage knot (b, t) = record `it` of every right-hand side
-      const long b = it / N;
-      double *yv = pv + nrow;
-      for (int k = lane; k < nrow; k += 32)
-        pv[k] = k < U ? a.xs[(it + b) * nx + k] : k < V ? a.us[it * nu + k - U] : k < L ? a.vs[it * nc + k - V]
-                                                                                       : a.lams[it * nx + k - L];
-      for (int j0 = 0; j0 < a.nrhs; j0 += chunk) {
-        const int R = a.nrhs - j0 < chunk ? a.nrhs - j0 : chunk;
-        for (int p = lane; p < R * nrow; p += 32) {
-          const int g = p / nrow, k = p - g * nrow;
-          const long jit = (long)(j0 + g) * nS + it, jb = jit / N; // record and row (j * batch + b) of rhs j0 + g
-          yv[p] = k < U ? a.yxs[(jit + jb) * nx + k] : k < V ? a.yus[jit * nu + k - U]
-                                                 : k < L ? a.yvs[jit * nc + k - V] : a.ylams[jit * nx + k - L];
+  if constexpr (EXT) {
+    // stage buffer: [z (nrow) | z2 (nrow) | chunk slots]; the slot of one right-hand side holds y, then z (z_each),
+    // y2 and z2 (z2.each).  A shared z or z2 is staged once per knot, a per-right-hand-side one once per (rhs, knot).
+    const bool two = a.y2.xs != nullptr, e1 = a.z_each, e2 = two && a.z2.each, vec = a.vec;
+    const int slot = nrow * (1 + e1 + (two ? 1 + e2 : 0));
+    const SolVec Y{a.yxs, a.yus, a.yvs, a.yvsT, a.ylam0, a.ylams, true};
+    const SolVec Z{a.xs, a.us, a.vs, a.vsT, a.lam0, a.lams, e1};
+    double *zs = pv, *z2s = pv + nrow, *slots = pv + 2 * nrow;
+    for (long it = w0; it < nS + nT; it += ws) {
+      if (it < nS) { // stage knot (b, t) = record `it` of every right-hand side
+        const long b = it / N;
+        for (int k = lane; k < nrow; k += 32) {
+          if (!e1)
+            zs[k] = knot_entry(Z, it, b, k, nx, nu, nc);
+          if (two && !e2)
+            z2s[k] = knot_entry(a.z2, it, b, k, nx, nu, nc);
         }
-        __syncwarp();
-        double *out = a.stage + ((long)j0 * nS + it) * srec;
-        const long rstride = nS * srec;
-        int g = 0, e = lane;
-        while (e >= srec) {
-          e -= srec;
-          ++g;
-        }
-        for (int p = lane; p < R * srec; p += 32) {
-          out[g * rstride + e] = gvalue(map[e], pv, yv + g * nrow, sgn, NEG);
-          e += 32;
+        for (int j0 = 0; j0 < a.nrhs; j0 += chunk) {
+          const int R = a.nrhs - j0 < chunk ? a.nrhs - j0 : chunk;
+          for (int p = lane; p < R * nrow; p += 32) {
+            const int g = p / nrow, k = p - g * nrow;
+            const long jit = (long)(j0 + g) * nS + it, jb = jit / N; // record and row (j * batch + b) of rhs j0 + g
+            double *sl = slots + g * slot + k;
+            sl[0] = knot_entry(Y, jit, jb, k, nx, nu, nc);
+            if (e1)
+              sl[nrow] = knot_entry(Z, jit, jb, k, nx, nu, nc);
+            if (two)
+              sl[(1 + e1) * nrow] = knot_entry(a.y2, jit, jb, k, nx, nu, nc);
+            if (e2)
+              sl[(2 + e1) * nrow] = knot_entry(a.z2, jit, jb, k, nx, nu, nc);
+          }
+          __syncwarp();
+          double *out = a.stage + ((long)j0 * nS + it) * srec;
+          const long rstride = nS * srec;
+          int g = 0, e = lane;
           while (e >= srec) {
             e -= srec;
             ++g;
           }
+          for (int p = lane; p < R * srec; p += 32) {
+            const double *sl = slots + g * slot, *y2 = sl + (1 + e1) * nrow;
+            out[g * rstride + e] = gvalue2(map[e], e1 ? sl + nrow : zs, sl, vec, e2 ? y2 + nrow : z2s, y2, two);
+            e += 32;
+            while (e >= srec) {
+              e -= srec;
+              ++g;
+            }
+          }
+          __syncwarp(); // the slots are overwritten next
         }
-        __syncwarp(); // yv is overwritten next
+      } else { // (instance b, rhs j): terminal record, G0, g0; buffers [z | y | z2 | y2], each [x_N | v_N | x_0 | l_0]
+        const long jb = it - nS, b = jb % B, r1 = e1 ? jb : b, r2 = e2 ? jb : b;
+        double *yv = pv + tvec, *p2 = pv + 2 * tvec, *y2 = pv + 3 * tvec;
+        for (int k = lane; k < tvec; k += 32) {
+          pv[k] = term_entry(Z, r1, k, nx, nct, nc0, N);
+          yv[k] = term_entry(Y, jb, k, nx, nct, nc0, N);
+          if (two) {
+            p2[k] = term_entry(a.z2, r2, k, nx, nct, nc0, N);
+            y2[k] = term_entry(a.y2, jb, k, nx, nct, nc0, N);
+          }
+        }
+        __syncwarp();
+        if (a.term)
+          for (int e = lane; e < d.trec; e += 32)
+            a.term[jb * d.trec + e] = gvalue2(map[srec + e], pv, yv, vec, p2, y2, two);
+        if (a.G0)
+          for (int e = lane; e < nc0 * nx; e += 32) {
+            const int r = e % nc0, c = e / nc0;
+            double v = fma(yv[TL0 + r], pv[TX0 + c], pv[TL0 + r] * yv[TX0 + c]);
+            if (two)
+              v += fma(y2[TL0 + r], p2[TX0 + c], p2[TL0 + r] * y2[TX0 + c]);
+            a.G0[jb * nc0 * nx + e] = v;
+          }
+        if (a.g0)
+          for (int i = lane; i < nc0; i += 32)
+            a.g0[jb * nc0 + i] = vec ? yv[TL0 + i] : 0.0;
+        __syncwarp();
       }
-    } else { // (instance b, rhs j): terminal record, G0, g0
-      const long jb = it - nS, b = jb % B;
-      double *yv = pv + tvec;
-      for (int k = lane; k < tvec; k += 32) {
-        double p, y;
-        if (k < TV) {
-          p = a.xs[(b * (N + 1) + N) * nx + k];
-          y = a.yxs[(jb * (N + 1) + N) * nx + k];
-        } else if (k < TX0) {
-          p = a.vsT[b * nct + k - TV];
-          y = a.yvsT[jb * nct + k - TV];
-        } else if (k < TL0) {
-          p = a.xs[b * (N + 1) * nx + k - TX0];
-          y = a.yxs[jb * (N + 1) * nx + k - TX0];
-        } else {
-          p = a.lam0[b * nc0 + k - TL0];
-          y = a.ylam0[jb * nc0 + k - TL0];
+    }
+  } else {
+    for (long it = w0; it < nS + nT; it += ws) {
+      if (it < nS) { // stage knot (b, t) = record `it` of every right-hand side
+        const long b = it / N;
+        double *yv = pv + nrow;
+        for (int k = lane; k < nrow; k += 32)
+          pv[k] = k < U ? a.xs[(it + b) * nx + k] : k < V ? a.us[it * nu + k - U] : k < L ? a.vs[it * nc + k - V]
+                                                                                         : a.lams[it * nx + k - L];
+        for (int j0 = 0; j0 < a.nrhs; j0 += chunk) {
+          const int R = a.nrhs - j0 < chunk ? a.nrhs - j0 : chunk;
+          for (int p = lane; p < R * nrow; p += 32) {
+            const int g = p / nrow, k = p - g * nrow;
+            const long jit = (long)(j0 + g) * nS + it, jb = jit / N; // record and row (j * batch + b) of rhs j0 + g
+            yv[p] = k < U ? a.yxs[(jit + jb) * nx + k] : k < V ? a.yus[jit * nu + k - U]
+                                                   : k < L ? a.yvs[jit * nc + k - V] : a.ylams[jit * nx + k - L];
+          }
+          __syncwarp();
+          double *out = a.stage + ((long)j0 * nS + it) * srec;
+          const long rstride = nS * srec;
+          int g = 0, e = lane;
+          while (e >= srec) {
+            e -= srec;
+            ++g;
+          }
+          for (int p = lane; p < R * srec; p += 32) {
+            out[g * rstride + e] = gvalue(map[e], pv, yv + g * nrow, sgn, NEG);
+            e += 32;
+            while (e >= srec) {
+              e -= srec;
+              ++g;
+            }
+          }
+          __syncwarp(); // yv is overwritten next
         }
-        pv[k] = p;
-        yv[k] = y;
+      } else { // (instance b, rhs j): terminal record, G0, g0
+        const long jb = it - nS, b = jb % B;
+        double *yv = pv + tvec;
+        for (int k = lane; k < tvec; k += 32) {
+          double p, y;
+          if (k < TV) {
+            p = a.xs[(b * (N + 1) + N) * nx + k];
+            y = a.yxs[(jb * (N + 1) + N) * nx + k];
+          } else if (k < TX0) {
+            p = a.vsT[b * nct + k - TV];
+            y = a.yvsT[jb * nct + k - TV];
+          } else if (k < TL0) {
+            p = a.xs[b * (N + 1) * nx + k - TX0];
+            y = a.yxs[jb * (N + 1) * nx + k - TX0];
+          } else {
+            p = a.lam0[b * nc0 + k - TL0];
+            y = a.ylam0[jb * nc0 + k - TL0];
+          }
+          pv[k] = p;
+          yv[k] = y;
+        }
+        __syncwarp();
+        if (a.term)
+          for (int e = lane; e < d.trec; e += 32)
+            a.term[jb * d.trec + e] = gvalue(map[srec + e], pv, yv, sgn, false);
+        if (a.G0) // dG0 = y_l0 x_0^T + l_0 y_x0^T, column-major [nc0][nx]
+          for (int e = lane; e < nc0 * nx; e += 32) {
+            const int r = e % nc0, c = e / nc0;
+            const double v = fma(yv[TL0 + r], pv[TX0 + c], pv[TL0 + r] * yv[TX0 + c]);
+            a.G0[jb * nc0 * nx + e] = sgn * v;
+          }
+        if (a.g0)
+          for (int i = lane; i < nc0; i += 32)
+            a.g0[jb * nc0 + i] = sgn * yv[TL0 + i];
+        __syncwarp();
       }
-      __syncwarp();
-      if (a.term)
-        for (int e = lane; e < d.trec; e += 32)
-          a.term[jb * d.trec + e] = gvalue(map[srec + e], pv, yv, sgn, false);
-      if (a.G0) // dG0 = y_l0 x_0^T + l_0 y_x0^T, column-major [nc0][nx]
-        for (int e = lane; e < nc0 * nx; e += 32) {
-          const int r = e % nc0, c = e / nc0;
-          const double v = fma(yv[TL0 + r], pv[TX0 + c], pv[TL0 + r] * yv[TX0 + c]);
-          a.G0[jb * nc0 * nx + e] = sgn * v;
-        }
-      if (a.g0)
-        for (int i = lane; i < nc0; i += 32)
-          a.g0[jb * nc0 + i] = sgn * yv[TL0 + i];
-      __syncwarp();
     }
   }
 }
 
-// ONE: nrhs = 1 (ab2_gar_tangent), where the right-hand-side loop is a single pass and 4 CTAs per SM fit the registers
-template <bool ONE>
+// ONE: nrhs = 1 (ab2_gar_tangent), where the right-hand-side loop is a single pass and 4 CTAs per SM fit the registers.
+// EXT: a.ext, the generalised mode (per right-hand-side z, a second term, vector blocks optional, e); EXT = false is the
+// plain mode's code unchanged.
+template <bool ONE, bool EXT>
 __global__ void __launch_bounds__(kWarps * 32, ONE ? 4 : 3) jacobian_rhs_kernel(const JacobianRhsArgs a, int slice, int group,
                                                                       int warp_doubles) {
   extern __shared__ __align__(16) double smem[];
@@ -267,103 +386,264 @@ __global__ void __launch_bounds__(kWarps * 32, ONE ? 4 : 3) jacobian_rhs_kernel(
   const int nrow = 2 * nx + nu + nc;
   const long nS = (long)B * N, items = nS + (long)B * a.nrhs;
   const long w0 = (long)blockIdx.x * kWarps + wid, ws = (long)gridDim.x * kWarps;
-  for (long it = w0; it < items; it += ws) {
-    if (it < nS) { // stage knot (b, t) = record `it` of every right-hand side
-      const long b = it / N;
-      const int t = (int)(it - b * N);
-      double *x = vec, *u = x + nx, *v = u + nu, *l = v + nc, *acc = l + nx;
-      for (int k = lane; k < nrow; k += 32)
-        vec[k] = k < nx ? a.xs[(it + b) * nx + k] : k < nx + nu ? a.us[it * nu + k - nx]
-                 : k < nx + nu + nc ? a.vs[it * nc + k - nx - nu] : a.lams[it * nx + k - nx - nu - nc];
-      __syncwarp();
-      for (int j0 = 0; j0 < (ONE ? 1 : a.nrhs); j0 += group) {
-        const int R = ONE ? 1 : (a.nrhs - j0 < group ? a.nrhs - j0 : group);
-        for (int p = lane; p < R * nrow; p += 32)
-          acc[p] = 0.0;
-        if (a.stage) {
-          for (int e0 = 0; e0 < d.srec; e0 += slice) {
-            const int e1 = e0 + slice < d.srec ? e0 + slice : d.srec;
-            for (int g = 0; g < R; ++g)
-              stage_copy(tile + g * slice, a.stage + ((long)(j0 + g) * nS + it) * d.srec + e0, e1 - e0, lane);
+  if constexpr (EXT) {
+    // stage buffer: [z (nrow) | z2 (nrow) | the group's per-rhs z or z2 (group * nrow) | acc (group * nrow)].  A shared
+    // z or z2 is staged once per knot, a per-right-hand-side one once per (rhs, knot).  Each row sums the first term
+    // tile by tile, then the second term tile by tile, then the G0 products, then e: a fixed order.
+    const bool two = a.two, e1 = a.z_each, e2 = two && a.z2.each, vec1 = a.vec;
+    const SolVec Z{a.xs, a.us, a.vs, a.vsT, a.lam0, a.lams, e1};
+    const SolVec &Z2 = a.z2, &E = a.e;
+    const int nv = nx + nu + nc; // the offset of l in a knot vector
+    for (long it = w0; it < items; it += ws) {
+      if (it < nS) { // stage knot (b, t) = record `it` of every right-hand side
+        const long b = it / N;
+        const int t = (int)(it - b * N);
+        double *zs = vec, *z2s = zs + nrow, *pd = z2s + nrow, *acc = pd + group * nrow;
+        for (int k = lane; k < nrow; k += 32) {
+          if (!e1)
+            zs[k] = knot_entry(Z, it, b, k, nx, nu, nc);
+          if (two && !e2)
+            z2s[k] = knot_entry(Z2, it, b, k, nx, nu, nc);
+        }
+        __syncwarp();
+        for (int j0 = 0; j0 < a.nrhs; j0 += group) {
+          const int R = a.nrhs - j0 < group ? a.nrhs - j0 : group;
+          for (int p = lane; p < R * nrow; p += 32) {
+            acc[p] = 0.0;
+            if (e1) {
+              const int g = p / nrow;
+              const long jit = (long)(j0 + g) * nS + it;
+              pd[p] = knot_entry(Z, jit, jit / N, p - g * nrow, nx, nu, nc);
+            }
+          }
+          // term 1, then term 2: the tangent records of the group, tile by tile (the wait's __syncwarp also publishes pd)
+          for (int term = 0; term < (two ? 2 : 1); ++term) {
+            const double *rec = term ? a.stage2 : a.stage;
+            const bool each = term ? e2 : e1;
+            if (!rec)
+              continue;
+            if (term && e2) {
+              __syncwarp(); // term 1 has read pd
+              for (int p = lane; p < R * nrow; p += 32) {
+                const int g = p / nrow;
+                const long jit = (long)(j0 + g) * nS + it;
+                pd[p] = knot_entry(Z2, jit, jit / N, p - g * nrow, nx, nu, nc);
+              }
+            }
+            for (int e0 = 0; e0 < d.srec; e0 += slice) {
+              const int eh = e0 + slice < d.srec ? e0 + slice : d.srec;
+              for (int g = 0; g < R; ++g)
+                stage_copy(tile + g * slice, rec + ((long)(j0 + g) * nS + it) * d.srec + e0, eh - e0, lane);
+              cp_wait_all();
+              __syncwarp();
+              for (int p = lane; p < R * nrow; p += 32) {
+                const int g = p / nrow;
+                const double *z = each ? pd + g * nrow : term ? z2s : zs;
+                acc[p] += stage_row(tile + g * slice, e0, eh, so, nx, nu, nc, p - g * nrow, z, z + nx, z + nx + nu,
+                                    z + nv, term ? false : vec1);
+              }
+              __syncwarp(); // the tile is overwritten next
+            }
+          }
+          for (int p = lane; p < R * nrow; p += 32) {
+            const int g = p / nrow, r = p - g * nrow;
+            const long jit = (long)(j0 + g) * nS + it, jb = jit / N; // record and row (j * batch + b) of rhs j0 + g
+            double s = acc[p];
+            if (r < nx) {
+              if (t == 0) { // + G0dot^T lambda_0 of each term, G0dot column-major [nc0][nx]
+                for (int term = 0; term < (two ? 2 : 1); ++term) {
+                  const double *G = term ? a.G02 : a.G0;
+                  const SolVec &z = term ? Z2 : Z;
+                  if (!G)
+                    continue;
+                  const double *Gc = G + jb * nc0 * nx + (long)r * nc0, *l0 = z.lam0 + ((term ? e2 : e1) ? jb : b) * nc0;
+                  double gs = 0.0;
+                  for (int k = 0; k < nc0; ++k)
+                    gs = fma(Gc[k], l0[k], gs);
+                  s += gs;
+                }
+              }
+              const long o = (jit + jb) * nx + r;
+              a.q[o] = E.xs ? s + E.xs[o] : s;
+            } else if (r < nx + nu) {
+              const long o = jit * nu + r - nx;
+              a.r[o] = E.xs ? s + E.us[o] : s;
+            } else if (r < nv) {
+              const long o = jit * nc + r - nx - nu;
+              a.dv[o] = E.xs ? s + E.vs[o] : s;
+            } else {
+              const long o = jit * nx + r - nv;
+              a.f[o] = E.xs ? s + E.lams[o] : s;
+            }
+          }
+          __syncwarp(); // acc and pd are overwritten next
+        }
+      } else { // (instance b, rhs j): rows [q_N (nx) | d_N (nct) | g0 (nc0)]
+        const long jb = it - nS, b = jb % B, r1 = e1 ? jb : b, r2 = e2 ? jb : b;
+        const int trows = nx + nct + nc0;
+        double *x = vec, *v = x + nx, *x2 = v + nct, *v2 = x2 + nx, *acc = v2 + nct;
+        for (int k = lane; k < nx + nct; k += 32) {
+          vec[k] = k < nx ? Z.xs[(r1 * (N + 1) + N) * nx + k] : Z.vsT[r1 * nct + k - nx];
+          if (two)
+            x2[k] = k < nx ? Z2.xs[(r2 * (N + 1) + N) * nx + k] : Z2.vsT[r2 * nct + k - nx];
+        }
+        for (int r = lane; r < trows; r += 32)
+          acc[r] = 0.0;
+        __syncwarp();
+        for (int term = 0; term < (two ? 2 : 1); ++term) {
+          const double *rec = term ? a.term2 : a.term;
+          if (!rec)
+            continue;
+          for (int e0 = 0; e0 < d.trec; e0 += kTile) {
+            const int eh = e0 + kTile < d.trec ? e0 + kTile : d.trec;
+            stage_copy(tile, rec + jb * d.trec + e0, eh - e0, lane);
             cp_wait_all();
             __syncwarp();
-            for (int p = lane; p < R * nrow; p += 32) {
-              const int g = p / nrow;
-              acc[p] += stage_row(tile + g * slice, e0, e1, so, nx, nu, nc, p - g * nrow, x, u, v, l);
-            }
-            __syncwarp(); // the tile is overwritten next
+            for (int r = lane; r < nx + nct; r += 32)
+              acc[r] += term ? term_row(tile, e0, eh, to, nx, nct, r, x2, v2, false)
+                             : term_row(tile, e0, eh, to, nx, nct, r, x, v, vec1);
+            __syncwarp();
           }
         }
-        for (int p = lane; p < R * nrow; p += 32) {
-          const int g = p / nrow, r = p - g * nrow;
-          const long jit = (long)(j0 + g) * nS + it, jb = jit / N; // record and row (j * batch + b) of rhs j0 + g
-          double s = acc[p];
+        for (int r = lane; r < trows; r += 32) {
+          double s = acc[r];
           if (r < nx) {
-            if (t == 0 && a.G0) { // + G0dot^T lambda_0, G0dot column-major [nc0][nx]
-              const double *G = a.G0 + jb * nc0 * nx + (long)r * nc0, *l0 = a.lam0 + b * nc0;
+            if (N == 0) // x_0 = x_N: + G0dot^T lambda_0 of each term
+              for (int term = 0; term < (two ? 2 : 1); ++term) {
+                const double *G = term ? a.G02 : a.G0;
+                if (!G)
+                  continue;
+                const double *Gc = G + jb * nc0 * nx, *l0 = (term ? Z2 : Z).lam0 + (term ? r2 : r1) * nc0;
+                double gs = 0.0;
+                for (int k = 0; k < nc0; ++k)
+                  gs = fma(Gc[(long)r * nc0 + k], l0[k], gs);
+                s += gs;
+              }
+            const long o = (jb * (N + 1) + N) * nx + r;
+            a.q[o] = E.xs ? s + E.xs[o] : s;
+          } else if (r < nx + nct) {
+            const long o = jb * nct + r - nx;
+            a.dN[o] = E.xs ? s + E.vsT[o] : s;
+          } else { // rho_g0 = g0dot (with vectors) + G0dot x_0 of each term
+            const int i = r - nx - nct;
+            if (vec1 && a.g0)
+              s += a.g0[jb * nc0 + i];
+            for (int term = 0; term < (two ? 2 : 1); ++term) {
+              const double *G = term ? a.G02 : a.G0;
+              if (!G)
+                continue;
+              const double *Gc = G + jb * nc0 * nx, *x0 = (term ? Z2 : Z).xs + (term ? r2 : r1) * (N + 1) * nx;
               double gs = 0.0;
-              for (int k = 0; k < nc0; ++k)
-                gs = fma(G[k], l0[k], gs);
+              for (int c = 0; c < nx; ++c)
+                gs = fma(Gc[i + (long)c * nc0], x0[c], gs);
               s += gs;
             }
-            a.q[(jit + jb) * nx + r] = s;
-          } else if (r < nx + nu) {
-            a.r[jit * nu + r - nx] = s;
-          } else if (r < nx + nu + nc) {
-            a.dv[jit * nc + r - nx - nu] = s;
-          } else {
-            a.f[jit * nx + r - nx - nu - nc] = s;
+            const long o = jb * nc0 + i;
+            a.g0out[o] = E.xs ? s + E.lam0[o] : s;
           }
         }
+        __syncwarp();
       }
-      __syncwarp(); // the vectors are overwritten next
-    } else { // (instance b, rhs j): rows [q_N (nx) | d_N (nct) | g0 (nc0)]
-      const long jb = it - nS, b = jb % B;
-      const int trows = nx + nct + nc0;
-      double *x = vec, *v = x + nx, *acc = v + nct;
-      for (int k = lane; k < nx + nct; k += 32)
-        vec[k] = k < nx ? a.xs[(b * (N + 1) + N) * nx + k] : a.vsT[b * nct + k - nx];
-      for (int r = lane; r < trows; r += 32)
-        acc[r] = 0.0;
-      __syncwarp();
-      if (a.term) {
-        for (int e0 = 0; e0 < d.trec; e0 += kTile) {
-          const int e1 = e0 + kTile < d.trec ? e0 + kTile : d.trec;
-          stage_copy(tile, a.term + jb * d.trec + e0, e1 - e0, lane);
-          cp_wait_all();
-          __syncwarp();
-          for (int r = lane; r < nx + nct; r += 32)
-            acc[r] += term_row(tile, e0, e1, to, nx, nct, r, x, v);
-          __syncwarp();
-        }
-      }
-      const double *G = a.G0 ? a.G0 + jb * nc0 * nx : nullptr, *l0 = a.lam0 + b * nc0, *x0 = a.xs + b * (N + 1) * nx;
-      for (int r = lane; r < trows; r += 32) {
-        double s = acc[r];
-        if (r < nx) {
-          if (N == 0 && G) { // x_0 = x_N: + G0dot^T lambda_0
-            double gs = 0.0;
-            for (int k = 0; k < nc0; ++k)
-              gs = fma(G[(long)r * nc0 + k], l0[k], gs);
-            s += gs;
+    }
+  } else {
+    for (long it = w0; it < items; it += ws) {
+      if (it < nS) { // stage knot (b, t) = record `it` of every right-hand side
+        const long b = it / N;
+        const int t = (int)(it - b * N);
+        double *x = vec, *u = x + nx, *v = u + nu, *l = v + nc, *acc = l + nx;
+        for (int k = lane; k < nrow; k += 32)
+          vec[k] = k < nx ? a.xs[(it + b) * nx + k] : k < nx + nu ? a.us[it * nu + k - nx]
+                   : k < nx + nu + nc ? a.vs[it * nc + k - nx - nu] : a.lams[it * nx + k - nx - nu - nc];
+        __syncwarp();
+        for (int j0 = 0; j0 < (ONE ? 1 : a.nrhs); j0 += group) {
+          const int R = ONE ? 1 : (a.nrhs - j0 < group ? a.nrhs - j0 : group);
+          for (int p = lane; p < R * nrow; p += 32)
+            acc[p] = 0.0;
+          if (a.stage) {
+            for (int e0 = 0; e0 < d.srec; e0 += slice) {
+              const int e1 = e0 + slice < d.srec ? e0 + slice : d.srec;
+              for (int g = 0; g < R; ++g)
+                stage_copy(tile + g * slice, a.stage + ((long)(j0 + g) * nS + it) * d.srec + e0, e1 - e0, lane);
+              cp_wait_all();
+              __syncwarp();
+              for (int p = lane; p < R * nrow; p += 32) {
+                const int g = p / nrow;
+                acc[p] += stage_row(tile + g * slice, e0, e1, so, nx, nu, nc, p - g * nrow, x, u, v, l);
+              }
+              __syncwarp(); // the tile is overwritten next
+            }
           }
-          a.q[(jb * (N + 1) + N) * nx + r] = s;
-        } else if (r < nx + nct) {
-          a.dN[jb * nct + r - nx] = s;
-        } else { // rho_g0 = g0dot + G0dot x_0
-          const int i = r - nx - nct;
-          if (a.g0)
-            s += a.g0[jb * nc0 + i];
-          if (G) {
-            double gs = 0.0;
-            for (int c = 0; c < nx; ++c)
-              gs = fma(G[i + (long)c * nc0], x0[c], gs);
-            s += gs;
+          for (int p = lane; p < R * nrow; p += 32) {
+            const int g = p / nrow, r = p - g * nrow;
+            const long jit = (long)(j0 + g) * nS + it, jb = jit / N; // record and row (j * batch + b) of rhs j0 + g
+            double s = acc[p];
+            if (r < nx) {
+              if (t == 0 && a.G0) { // + G0dot^T lambda_0, G0dot column-major [nc0][nx]
+                const double *G = a.G0 + jb * nc0 * nx + (long)r * nc0, *l0 = a.lam0 + b * nc0;
+                double gs = 0.0;
+                for (int k = 0; k < nc0; ++k)
+                  gs = fma(G[k], l0[k], gs);
+                s += gs;
+              }
+              a.q[(jit + jb) * nx + r] = s;
+            } else if (r < nx + nu) {
+              a.r[jit * nu + r - nx] = s;
+            } else if (r < nx + nu + nc) {
+              a.dv[jit * nc + r - nx - nu] = s;
+            } else {
+              a.f[jit * nx + r - nx - nu - nc] = s;
+            }
           }
-          a.g0out[jb * nc0 + i] = s;
         }
+        __syncwarp(); // the vectors are overwritten next
+      } else { // (instance b, rhs j): rows [q_N (nx) | d_N (nct) | g0 (nc0)]
+        const long jb = it - nS, b = jb % B;
+        const int trows = nx + nct + nc0;
+        double *x = vec, *v = x + nx, *acc = v + nct;
+        for (int k = lane; k < nx + nct; k += 32)
+          vec[k] = k < nx ? a.xs[(b * (N + 1) + N) * nx + k] : a.vsT[b * nct + k - nx];
+        for (int r = lane; r < trows; r += 32)
+          acc[r] = 0.0;
+        __syncwarp();
+        if (a.term) {
+          for (int e0 = 0; e0 < d.trec; e0 += kTile) {
+            const int e1 = e0 + kTile < d.trec ? e0 + kTile : d.trec;
+            stage_copy(tile, a.term + jb * d.trec + e0, e1 - e0, lane);
+            cp_wait_all();
+            __syncwarp();
+            for (int r = lane; r < nx + nct; r += 32)
+              acc[r] += term_row(tile, e0, e1, to, nx, nct, r, x, v);
+            __syncwarp();
+          }
+        }
+        const double *G = a.G0 ? a.G0 + jb * nc0 * nx : nullptr, *l0 = a.lam0 + b * nc0, *x0 = a.xs + b * (N + 1) * nx;
+        for (int r = lane; r < trows; r += 32) {
+          double s = acc[r];
+          if (r < nx) {
+            if (N == 0 && G) { // x_0 = x_N: + G0dot^T lambda_0
+              double gs = 0.0;
+              for (int k = 0; k < nc0; ++k)
+                gs = fma(G[(long)r * nc0 + k], l0[k], gs);
+              s += gs;
+            }
+            a.q[(jb * (N + 1) + N) * nx + r] = s;
+          } else if (r < nx + nct) {
+            a.dN[jb * nct + r - nx] = s;
+          } else { // rho_g0 = g0dot + G0dot x_0
+            const int i = r - nx - nct;
+            if (a.g0)
+              s += a.g0[jb * nc0 + i];
+            if (G) {
+              double gs = 0.0;
+              for (int c = 0; c < nx; ++c)
+                gs = fma(G[i + (long)c * nc0], x0[c], gs);
+              s += gs;
+            }
+            a.g0out[jb * nc0 + i] = s;
+          }
+        }
+        __syncwarp();
       }
-      __syncwarp();
     }
   }
 }
@@ -374,13 +654,19 @@ cudaError_t launch_jacobian_grad(const JacobianGradArgs &a, cudaStream_t st) {
   if (a.nrhs <= 0 || items <= 0)
     return cudaSuccess;
   const int nrow = 2 * d.nx + d.nu + d.nc, tvec = 2 * d.nx + d.nct + d.nc0;
-  int chunk = (kVecDoubles - nrow) / nrow;
+  // plain: [z | chunk y]; generalised: [z | z2 | chunk slots of y, z (z_each), y2, z2 (z2.each)], terminal [z|y|z2|y2]
+  const bool two = a.ext && a.y2.xs;
+  const int shared = a.ext ? 2 * nrow : nrow, slot = nrow * (1 + (a.ext && a.z_each) + (two ? 1 + a.z2.each : 0));
+  int chunk = (kVecDoubles - shared) / slot;
   chunk = chunk < 1 ? 1 : (chunk > kMaxChunk ? kMaxChunk : chunk);
   chunk = chunk < a.nrhs ? chunk : a.nrhs;
-  int warp_doubles = nrow * (1 + chunk) > 2 * tvec ? nrow * (1 + chunk) : 2 * tvec;
+  const int tneed = (a.ext ? 4 : 2) * tvec;
+  int warp_doubles = shared + slot * chunk > tneed ? shared + slot * chunk : tneed;
   warp_doubles = (warp_doubles + 1) & ~1;
   const size_t smem = (size_t)warp_doubles * kWarps * sizeof(double) + (size_t)(d.srec + d.trec) * sizeof(unsigned);
-  void (*kernel)(const JacobianGradArgs, int, int) = a.neg ? jacobian_grad_kernel<true> : jacobian_grad_kernel<false>;
+  void (*kernel)(const JacobianGradArgs, int, int) = a.ext ? jacobian_grad_kernel<false, true>
+                                                     : a.neg ? jacobian_grad_kernel<true, false>
+                                                             : jacobian_grad_kernel<false, false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;
@@ -408,10 +694,15 @@ cudaError_t launch_jacobian_rhs(const JacobianRhsArgs &a, cudaStream_t st) {
   int group = d.srec <= kTile ? kTile / slice : 1;
   group = group < a.nrhs ? group : a.nrhs;
   const int nrow = 2 * d.nx + d.nu + d.nc, trows = d.nx + d.nct + d.nc0;
-  const int vecs = nrow + group * nrow > d.nx + d.nct + trows ? nrow + group * nrow : d.nx + d.nct + trows;
+  // plain: [z | acc], terminal [x_N | v_N | acc]; generalised: [z | z2 | pd | acc], terminal [x_N | v_N | x2_N | v2_N | acc]
+  const int svecs = a.ext ? 2 * nrow + 2 * group * nrow : nrow + group * nrow;
+  const int tvecs = (a.ext ? 2 : 1) * (d.nx + d.nct) + trows;
+  const int vecs = svecs > tvecs ? svecs : tvecs;
   const int warp_doubles = (kTile + vecs + 1) & ~1;
   const size_t smem = (size_t)warp_doubles * kWarps * sizeof(double);
-  void (*kernel)(const JacobianRhsArgs, int, int, int) = a.nrhs == 1 ? jacobian_rhs_kernel<true> : jacobian_rhs_kernel<false>;
+  void (*kernel)(const JacobianRhsArgs, int, int, int) = a.ext ? jacobian_rhs_kernel<false, true>
+                                                         : a.nrhs == 1 ? jacobian_rhs_kernel<true, false>
+                                                                       : jacobian_rhs_kernel<false, false>;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess)
     return e;

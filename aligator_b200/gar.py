@@ -214,6 +214,12 @@ def lib():
                                            C.POINTER(LsIterate), C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_tangent_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LsIterate), C.POINTER(LqTangent),
                                            C.POINTER(LsIterate), C.POINTER(LsIterate), C.c_void_p]
+        L.ab2_gar_rho_many.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(LqTangent), C.POINTER(LsIterate), C.c_int,
+                                       C.POINTER(LqTangent), C.POINTER(LsIterate), C.c_int, C.POINTER(LsIterate),
+                                       C.POINTER(LsIterate), C.c_void_p]
+        L.ab2_gar_grad_many.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(LsIterate), C.POINTER(LsIterate), C.c_int,
+                                        C.POINTER(LsIterate), C.POINTER(LsIterate), C.c_int, C.POINTER(LqGrad),
+                                        C.c_void_p]
         L.ab2_gar_refine.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p]
         L.ab2_gar_refine_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_int, C.POINTER(LqRhs),
                                           C.POINTER(LsIterate), C.POINTER(LqRefineWork), C.c_void_p, C.c_void_p]
@@ -721,6 +727,55 @@ class CudaRiccatiBatch:
         ot = _fill(LsIterate(), _LS_KEYS, out)
         self._mu_call("tangent_many", mueq, stream, (primal, tangent, work, out), int(nrhs), C.byref(pr), C.byref(dt),
                       C.byref(wk), C.byref(ot))
+
+    def _each(self, v):
+        """1 when the solution-layout dict ``v`` holds one vector per right-hand side ([nrhs][batch][...]), 0 when it is
+        shared ([batch][...]), read from ``v["xs"]`` (at nrhs = 1 the two layouts are one: shared)."""
+        d = self.dims
+        return int(v["xs"].numel() != d.batch * (d.horizon + 1) * d.nx)
+
+    def rho_many(self, dot, a, out, vectors=True, dot2=None, a2=None, e=None, stream=0):
+        """``ab2_gar_rho_many``: ``out`` receives, for every right-hand side j, rho^(v)(dot_j; a_j) + rho_K(dot2_j; a2_j)
+        + e_j in resolve's rhs layouts (rho^(v) = rho with the tangent's vector blocks when ``vectors``, rho_K without).
+        ``dot``, ``dot2``: dicts with any of stage, term, G0, g0 of device tensors [nrhs][batch][...] in the problem's
+        layouts (a key that is missing or None is zero; ``dot2`` None: no second term).  ``a``, ``a2``: dicts with keys
+        xs, us, vs, vsT, lam0, lams of device tensors, [nrhs][batch][...] (one per right-hand side) or [batch][...]
+        (shared), told apart by the size of ``xs``.  ``e`` (None: absent) and ``out``: the same keys, [nrhs][batch][...];
+        nrhs is read from ``out["xs"]``.  Reads no factorisation and touches none of the handle's outputs."""
+        d = self.dims
+        nrhs = out["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
+        d1 = _fill(LqTangent(), _GRAD_KEYS, dot)
+        a1 = _fill(LsIterate(), _LS_KEYS, a)
+        d2 = None if dot2 is None else _fill(LqTangent(), _GRAD_KEYS, dot2)
+        a2s = None if dot2 is None else _fill(LsIterate(), _LS_KEYS, a2)
+        es = None if e is None else _fill(LsIterate(), _LS_KEYS, e)
+        ot = _fill(LsIterate(), _LS_KEYS, out)
+        self._keep["rho_many"] = (dot, a, dot2, a2, e, out)
+        _check(lib().ab2_gar_rho_many(self.h, int(nrhs), int(bool(vectors)), C.byref(d1), C.byref(a1),
+                                      self._each(a), None if d2 is None else C.byref(d2),
+                                      None if a2s is None else C.byref(a2s),
+                                      0 if dot2 is None else self._each(a2), None if es is None else C.byref(es),
+                                      C.byref(ot), C.c_void_p(stream)))
+
+    def grad_many(self, y, z, grad, vectors=True, y2=None, z2=None, stream=0):
+        """``ab2_gar_grad_many``: ``grad`` receives, for every right-hand side j, Gr^(v)(y_j; z_j) + Gr_K(y2_j; z2_j):
+        adjoint_many's gradient records for y and the primal z (Gr^(v) = Gr with the vector blocks when ``vectors``,
+        Gr_K with them written 0).  ``y``, ``y2`` (None: no second pair): dicts with keys xs, us, vs, vsT, lam0, lams of
+        device tensors [nrhs][batch][...]; nrhs is read from ``y["xs"]``.  ``z``, ``z2``: the same keys, [nrhs][batch][...]
+        or [batch][...] (shared), told apart by the size of ``xs``.  ``grad``: dict with any of stage, term, G0, g0 of
+        device tensors [nrhs][batch][...] in the problem's layouts, overwritten (a missing key is not written).  Reads no
+        factorisation and touches none of the handle's outputs."""
+        d = self.dims
+        nrhs = y["xs"].numel() // (d.batch * (d.horizon + 1) * d.nx)
+        ys, zs = _fill(LsIterate(), _LS_KEYS, y), _fill(LsIterate(), _LS_KEYS, z)
+        y2s = None if y2 is None else _fill(LsIterate(), _LS_KEYS, y2)
+        z2s = None if y2 is None else _fill(LsIterate(), _LS_KEYS, z2)
+        gr = _fill(LqGrad(), _GRAD_KEYS, grad)
+        self._keep["grad_many"] = (y, z, y2, z2, grad)
+        _check(lib().ab2_gar_grad_many(self.h, int(nrhs), int(bool(vectors)), C.byref(ys), C.byref(zs),
+                                       self._each(z), None if y2s is None else C.byref(y2s),
+                                       None if z2s is None else C.byref(z2s),
+                                       0 if y2 is None else self._each(z2), C.byref(gr), C.c_void_p(stream)))
 
     def refine(self, mueq, steps=1, norms=False, stream=0):
         """Iterative refinement of the handle's own trajectory outputs (OUT_XS .. OUT_LBDAS) against the current

@@ -525,6 +525,46 @@ int ab2_gar_tangent_many_v(ab2_gar_solver *s, const double *mueq, int memspace, 
                            const ab2_ls_iterate *primal, const ab2_lq_tangent *dot,
                            const ab2_ls_trial *work, const ab2_ls_trial *out, void *stream);
 
+/* The two streaming kernels of adjoint_many / tangent_many as stateless calls, generalised for higher derivatives of
+ * the solve (every derivative of z = solve(P), of resolve and of these two maps is made of resolve and these two maps;
+ * DESIGN section 2p).  K is affine in the data P, so for a data direction Pdot and a vector a in the solution's layout:
+ *   rho(Pdot; a)   = Kdot(Pdot) a + hdot(Pdot): ab2_gar_tangent's right-hand side with z replaced by a (sym(Qdot),
+ *                    sym(Rdot) included); rho_K(Pdot; a) = Kdot(Pdot) a, the same without the tangent's vector blocks
+ *                    (qdot, rdot, ddot, fdot, qdot_N, ddot_N, g0dot);
+ *   Gr(y; z)       = adjoint_many's gradient records for y and the primal z: dh = y, dK = y z^T read out of K's blocks
+ *                    (symmetric part for Q and R, pad = +0.0); Gr_K(y; z) the same with every vector block written 0.
+ * They pair as <Gr(y; z), Pdot> = <y, rho(Pdot; z)> and <Gr_K(y; z), Pdot> = <y, rho_K(Pdot; z)> = <z, rho_K(Pdot; y)>,
+ * so Gr_K(y; z) = Gr_K(z; y) and the derivatives of each map are the other map again.
+ *   rho_many,  for each right-hand side j:  out_j = rho^(v)(dot1_j; a1_j) + rho_K(dot2_j; a2_j) + e_j,
+ *     rho^(v) = rho when with_vectors != 0, else rho_K.  out is in resolve's rhs layouts (q like xs with q_N last, r like
+ *     us, d like vs, dN like vsT, g0 like lam0, f like lams).  dot2 == NULL: no second term (a2 is ignored);
+ *     e == NULL: no e.
+ *   grad_many, for each right-hand side j:  grad_j = Gr^(v)(y1_j; z1_j) + Gr_K(y2_j; z2_j),
+ *     Gr^(v) = Gr when with_vectors != 0, else Gr_K.  y2 == NULL: no second pair (z2 is ignored).
+ * Layouts: dot1, dot2, e, y1, y2, out and grad are [nrhs][batch][...] in DEVICE memory (block j * batch + b is
+ * right-hand side j of instance b); dot and grad use the problem's record layouts (stage records' pad double written as
+ * 0, never read).  A vector operand a1, a2, z1, z2 is [nrhs][batch][...] when its flag (*_each) is nonzero and
+ * [batch][...] shared by every right-hand side when it is 0; a shared operand is staged once per knot, a per-direction one
+ * read once per (direction, knot).  A NULL dot field is zero; every field of nonzero size of a1, y1, z1, e and out (and
+ * of a2 with dot2, of z2 with y2) is required; a NULL grad field is not written.
+ * At with_vectors != 0, shared a1 / z1 and no second term or e, the calls run adjoint_many's and tangent_many's kernels,
+ * with their bits; every other mode runs the generalised instantiation, whose one-term results equal those bits.
+ * Right-hand side j's results are bit for bit independent of nrhs and of j's position (each element is summed in a fixed
+ * order: term 1, term 2, then e).
+ * The calls read no factorisation and no mu: no state precondition, one launch on `stream`, and every handle output,
+ * the status and ab2_gar_factor_epoch are unchanged.  Dense handles are served (their records have the same layout).
+ * Errors (nothing is launched): AB2_ERR_UNSUPPORTED for parametric (nth > 0) and parallel handles, whose records have
+ * another layout; AB2_ERR_INVALID for nrhs < 0, a NULL required argument or field, or an output field overlapping any
+ * input field or another output field.  nrhs == 0 launches and writes nothing. */
+int ab2_gar_rho_many (ab2_gar_solver *s, int nrhs, int with_vectors,
+                      const ab2_lq_tangent *dot1, const ab2_ls_iterate *a1, int a1_each,
+                      const ab2_lq_tangent *dot2, const ab2_ls_iterate *a2, int a2_each,
+                      const ab2_ls_iterate *e, const ab2_ls_trial *out, void *stream);
+int ab2_gar_grad_many(ab2_gar_solver *s, int nrhs, int with_vectors,
+                      const ab2_ls_iterate *y1, const ab2_ls_iterate *z1, int z1_each,
+                      const ab2_ls_iterate *y2, const ab2_ls_iterate *z2, int z2_each,
+                      const ab2_lq_grad *grad, void *stream);
+
 /* Iterative refinement of the LQ solution on the last backward's factorisation (what ParallelRiccatiSolver does to its
  * condensed system, parallel-solver.hxx:185-202, here for the whole serial solve).  At small penalties (mu = 1e-8 and
  * below) the fp64 recursion loses digits to the conditioning of the stage KKT systems; a step or two of refinement
