@@ -14,6 +14,39 @@
 #include "group_emu.cpp"
 #include "resolve_emu.cpp"
 
+// Every shape `supported` (the library's ab2_gar_supported) accepts with nx, nu, nc < lim and nc0 in {0, 1, nx/2, nx},
+// for the factorisation's derivative program whose item size is `item_bytes` (emu_factor_adjoint_item_bytes or
+// emu_factor_tangent_item_bytes): how many are accepted (*accepted), how many of those need more than 227 KB of shared
+// memory (the return value; the first one in *bad = nx, nu, nc, nc0), and the largest item that fits, in bytes
+// (*largest).
+extern "C" long emu_factor_size_scan(long (*item_bytes)(int, int, int), int (*supported)(int, int, int, int), int lim,
+                                     int *bad, long *largest, long *accepted) {
+  long over = 0;
+  *largest = 0;
+  *accepted = 0;
+  for (int nx = 1; nx < lim; ++nx)
+    for (int nu = 1; nu < lim; ++nu)
+      for (int nc = 0; nc < lim; ++nc) {
+        const int nc0s[4] = {0, 1, nx / 2, nx};
+        for (int i = 0; i < 4; ++i) {
+          const int nc0 = nc0s[i];
+          if (i && nc0 == nc0s[i - 1])
+            continue;
+          if (!supported(nx, nu, nc, nc0))
+            continue;
+          ++*accepted;
+          const long bytes = item_bytes(nx, nu, nc);
+          if (bytes > 227 * 1024) {
+            if (over++ == 0)
+              bad[0] = nx, bad[1] = nu, bad[2] = nc, bad[3] = nc0;
+          } else if (bytes > *largest) {
+            *largest = bytes;
+          }
+        }
+      }
+  return over;
+}
+
 extern "C" int emu_sweep_params_size() { return (int)sizeof(ab2::SweepParams); }
 
 // offsetof(ab2::SweepParams, name), or -1 for a name that is not a field

@@ -15,6 +15,10 @@ import numpy as np
 
 import gen
 import lq_adjoint_ref
+import lq_cases
+import lq_factor_adjoint_ref
+import lq_resolve_ref
+from oracle import gar_oracle as orc
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 EMU_DIR = os.path.join(HERE, "emu")
@@ -74,6 +78,14 @@ def lib():
                 os.remove(tmp)
     h = C.CDLL(LIB)
     h.emu_sweep_params_offset.argtypes = [C.c_char_p]
+    for name in ("emu_factor_adjoint", "emu_factor_tangent", "emu_resolve"):
+        getattr(h, name).argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
+    for name in ("emu_factor_adjoint_item_bytes", "emu_factor_tangent_item_bytes"):
+        getattr(h, name).restype = C.c_long
+        getattr(h, name).argtypes = [C.c_int, C.c_int, C.c_int]
+    h.emu_factor_size_scan.restype = h.emu_resolve_size_scan.restype = C.c_long
+    h.emu_factor_size_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+    h.emu_resolve_size_scan.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     bad = layout_mismatches(h)
     assert not bad, "tests/emu_harness.py SweepParams does not match ab2::SweepParams: %s" % bad
     return h
@@ -180,3 +192,141 @@ def emulate(kind, probs, dims, mueq, arg=0, packed=False, legs=0, collapse=False
     assert rc == 0, (kind, rc)
     out["status"], out["pivstat"] = status, pivstat
     return out
+
+
+def pack_vxx(Vxx):
+    """[B][N+1][nx][nx] (row index first) -> the packed layout of vxx_layout.h: packed lower triangles, and the full
+    column-major slot-0 blocks."""
+    B, K, nx, _ = Vxx.shape
+    P = (nx * (nx + 1) // 2 + 1) & ~1
+    pk = np.zeros((B, K, P))
+    for j in range(nx):
+        c0 = j * nx - j * (j - 1) // 2
+        pk[:, :, c0:c0 + nx - j] = Vxx[:, :, j:, j]
+    return pk, np.ascontiguousarray(np.swapaxes(Vxx[:, 0], -1, -2)).reshape(B, nx * nx)
+
+
+def from_device(out):
+    """Device-layout tangents -> the restatement's shapes: vxx blocks back from column-major."""
+    return {k: (np.swapaxes(v, -1, -2) if k == "vxx" and v is not None else v) for k, v in out.items()}
+
+
+def run_factor_adjoint(recs, fac, cot, case, mu, lanes, packed=True, head=0):
+    """Run the ab2_gar_factor_adjoint program (tests/emu/factor_adjoint_emu.cpp) on `lanes` emulated lanes per instance:
+    the gradient records of the cotangent `cot` of the factorisation `fac` (the restatement\'s shapes).  packed: Vxx
+    in the warp kernel\'s packed layout; head: the stage ring\'s head."""
+    nx, nu, nc, nct, nc0, N = case
+    stage, term, _, _ = recs
+    B = term.shape[0]
+    head = head % N if N else 0
+    if head:
+        stage = np.roll(stage, head, axis=1)  # knot t in slot (t + head) mod N
+    Vxx = np.asarray(fac["vxx"])
+    V, V0 = pack_vxx(Vxx) if packed else (np.ascontiguousarray(np.swapaxes(Vxx, -1, -2)), None)
+    dc = lq_cases.device_cot(cot, case, B)
+    keep = [np.ascontiguousarray(a, dtype=np.float64) for a in
+            (stage, term, fac["fb"], fac["fbt"], V)] + [V0] + \
+           [np.ascontiguousarray(fac[k], dtype=np.float64) for k in ("ff", "vx", "fft")] + [dc.get(k) for k in lq_factor_adjoint_ref.COT]
+    _, srec = lq_adjoint_ref.stage_offsets(nx, nu, nc)
+    out = dict(stage=np.full((B, N, srec), np.nan), term=np.full(term.shape, np.nan), G0=np.full((B, nc0 * nx), np.nan),
+               g0=np.full((B, nc0), np.nan))
+    ptr = lambda a: None if a is None or a.size == 0 else a.ctypes.data
+    ins = (C.c_void_p * 15)(*[ptr(a) for a in keep])
+    outs = (C.c_void_p * 4)(*[ptr(out[k]) for k in ("stage", "term", "G0", "g0")])
+    dims = np.array([B, N, nx, nu, nc, nct, nc0, srec, term.shape[1], head, lanes], dtype=np.int32)
+    mub = None if np.ndim(mu) == 0 else np.ascontiguousarray(mu, dtype=np.float64)
+    lib().emu_factor_adjoint(dims.ctypes.data, float(mu) if mub is None else 0.0, ptr(mub), ins, outs)
+    return out
+
+
+def run_factor_tangent(recs, fac, dot, case, mu, lanes, packed=True, head=0, want=lq_factor_adjoint_ref.COT):
+    """Run the ab2_gar_factor_tangent program (tests/emu/factor_tangent_emu.cpp) like run_factor_adjoint: the tangents
+    of the factorisation along the record tangent `dot`, only the families in `want` written."""
+    nx, nu, nc, nct, nc0, N = case
+    stage, term, _, _ = recs
+    B = term.shape[0]
+    head = head % N if N else 0
+    if head:
+        stage = np.roll(stage, head, axis=1)  # knot t in slot (t + head) mod N
+    Vxx = np.asarray(fac["vxx"])
+    V, V0 = pack_vxx(Vxx) if packed else (np.ascontiguousarray(np.swapaxes(Vxx, -1, -2)), None)
+    keep = [np.ascontiguousarray(a, dtype=np.float64) for a in (stage, term, fac["fb"], fac["fbt"], V)] + [V0] + \
+           [np.ascontiguousarray(fac[k], dtype=np.float64) for k in ("ff", "vx", "fft")] + \
+           [None if dot.get(k) is None else np.ascontiguousarray(dot[k], dtype=np.float64) for k in ("stage", "term")]
+    out = {k: np.full(s, np.nan) for k, s in lq_cases.out_shapes(case, B).items()}
+    ptr = lambda a: None if a is None or a.size == 0 else a.ctypes.data
+    ins = (C.c_void_p * 11)(*[ptr(a) for a in keep])
+    outs = (C.c_void_p * 6)(*[ptr(out[k]) if k in want else None for k in lq_factor_adjoint_ref.COT])
+    _, srec = lq_adjoint_ref.stage_offsets(nx, nu, nc)
+    dims = np.array([B, N, nx, nu, nc, nct, nc0, srec, term.shape[1], head, lanes], dtype=np.int32)
+    mub = None if np.ndim(mu) == 0 else np.ascontiguousarray(mu, dtype=np.float64)
+    lib().emu_factor_tangent(dims.ctypes.data, float(mu) if mub is None else 0.0, ptr(mub), ins, outs)
+    return from_device(out)
+
+
+def run_resolve(recs, o, h, case, nrhs, mu, lanes, chunk, packed, head):
+    """Run the ab2_gar_resolve program (tests/emu/resolve_emu.cpp): the solutions of the nrhs right-hand sides h on
+    the oracle\'s factorisation o, `chunk` right-hand sides per item on `lanes` emulated lanes."""
+    nx, nu, nc, nct, nc0, N = case
+    stage, term, G0, _ = recs
+    B = term.shape[0]
+    if head and N:
+        stage = np.roll(stage, head, axis=1)  # knot t in slot (t + head) mod N
+    Vxx = np.asarray(o["Vxx"])
+    if packed:
+        V, V0 = pack_vxx(Vxx)
+    else:
+        V, V0 = np.ascontiguousarray(np.swapaxes(Vxx, -1, -2)), None
+    keep = [np.ascontiguousarray(a, dtype=np.float64) for a in (stage, term, G0, o["fb"], o["fbT"], V)]
+    keep.append(None if V0 is None else np.ascontiguousarray(V0))
+    hf = lq_resolve_ref.full_rhs(h, case, B, nrhs)
+    keep += [np.ascontiguousarray(hf[k]) for k in lq_resolve_ref.RHS]
+    out = {k: np.full((nrhs,) + s, np.nan) for k, s in zip(lq_resolve_ref.SOL, lq_resolve_ref.rhs_shapes(case, B).values())}
+    ptr = lambda a: None if a is None or a.size == 0 else a.ctypes.data
+    ins = (C.c_void_p * 13)(*[ptr(a) for a in keep])
+    outs = (C.c_void_p * 6)(*[ptr(out[k]) for k in lq_resolve_ref.SOL])
+    _, srec = lq_adjoint_ref.stage_offsets(nx, nu, nc)
+    dims = np.array([B, N, nx, nu, nc, nct, nc0, srec, term.shape[1], head if N else 0, nrhs, chunk, lanes],
+                    dtype=np.int32)
+    mub = None if np.ndim(mu) == 0 else np.ascontiguousarray(mu, dtype=np.float64)
+    lib().emu_resolve(dims.ctypes.data, float(mu) if mub is None else 0.0, ptr(mub), ins, outs)
+    return out
+
+
+def check_against_oracle(nx, nu, nc, nct, N, B, mueq, seed, tol=1e-10, style="conditioned", db=0,
+                         pivoting=False, block=0):
+    probs = gen.generate_batch(seed, B, N, nx, nu, nc, nct, style=style)
+    if pivoting:
+        gen.make_pivoting(probs)
+    # block = 0: the warp-per-instance group program; block = NW > 0: the CTA-per-instance program of
+    # riccati_block.cuh with NW emulated warps; block = -NW: its compile-time specialisation (StaticBlockDims)
+    kind = "group" if block == 0 else ("block" if block > 0 else "static")
+    got = emulate(kind, probs, (nx, nu, nc, nct, N), mueq, db if block == 0 else abs(block))
+    got["Vxx"] = got["Vxx"].reshape(B, N + 1, nx, nx).transpose(0, 1, 3, 2)
+    assert np.all(got["status"] == 0)
+    stage, term, G0, g0 = gen.pack_problems(probs)
+    bo = orc.BatchedOracle(nx, nu, nc, nct, probs[0].nc0, N, B, stage, term, G0, g0)
+    bo.sweep(mueq, nthreads=1)
+    ref = bo.get()
+    worst = {}
+    for b in range(B):
+        for t in range(N):
+            worst["K"] = max(worst.get("K", 0), gen.rel_fro(got["fb"][b, t, :nu], ref["fb"][b, t, :nu]))
+            worst["k"] = max(worst.get("k", 0), gen.rel_fro(got["ff"][b, t, :nu], ref["ff"][b, t, :nu]))
+            worst["fb"] = max(worst.get("fb", 0), gen.rel_fro(got["fb"][b, t], ref["fb"][b, t]))
+            worst["ff"] = max(worst.get("ff", 0), gen.rel_fro(got["ff"][b, t], ref["ff"][b, t]))
+        for t in range(N + 1):
+            worst["Vxx"] = max(worst.get("Vxx", 0), gen.rel_fro(got["Vxx"][b, t], ref["Vxx"][b, t]))
+            worst["vx"] = max(worst.get("vx", 0), gen.rel_fro(got["vx"][b, t], ref["vx"][b, t]))
+        for key in ("xs", "us", "vs", "lbdas", "lbd0", "vsT"):
+            if ref[key].size:
+                worst[key] = max(worst.get(key, 0), gen.rel_fro(got[key][b], ref[key][b]))
+    # K alone on control-constrained knots is limited by eps*cond(KKT) ~ 6e-17/mueq between
+    # any two correct fp64 solvers (SURVEY Appendix C); everything else is gated at `tol`.
+    tolk = max(tol, 2.4e-16 / mueq) if nc > 0 else tol
+    bad = {k: v for k, v in worst.items() if not v <= (tolk if k in ("K", "k") else tol)}
+    assert not bad, (bad, worst)
+    # structural semantics (A1): Vxx_t symmetric for t >= 1 when N > 0
+    for t in range(1, N + 1):
+        assert np.array_equal(got["Vxx"][0, t], got["Vxx"][0, t].T)
+    return worst

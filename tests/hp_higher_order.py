@@ -16,8 +16,8 @@ import hp_reference as hp
 import lq_adjoint_ref as aref
 import lq_resolve_ref as rref
 import lq_tangent_ref as tref
-from test_higher_order_oracle import grad_modes, rho_modes
-from test_hp_derivatives import oracle_solution
+from lq_cases import oracle_solution
+from lq_higher_ref import grad_modes, rho_modes
 
 KEYS = aref.KEYS
 RECS = ("stage", "term", "G0", "g0")

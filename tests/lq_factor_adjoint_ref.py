@@ -150,3 +150,60 @@ def factor_adjoint(stage, term, ff, fb, Vxx, vx, ffT, fbT, cot, dims, mueq, solv
     for key, (a0, a1) in to.items():
         gt[:, a0:a1] = tb[key]
     return dict(stage=gs, term=gt, G0=np.zeros((B, nc0 * nx), dtype=dt), g0=np.zeros((B, nc0), dtype=dt))
+
+
+def torch_factor(stage, term, case, mu):
+    """The backward recursion in float64 CPU torch: (ff, fb, vxx, vx, fft, fbt) in the restatement's shapes.  Stage
+    KKT systems by torch.linalg.solve, Q and R as (P + P^T) / 2 of the stored blocks."""
+    import torch
+    nx, nu, nc, nct, nc0, N = case
+    B = term.shape[0]
+    so, _ = stage_offsets(nx, nu, nc)
+    to, _ = term_offsets(nx, nct)
+    blk = lambda rec, off, m, n: rec[..., off[0]:off[1]].reshape(*rec.shape[:-1], n, m).transpose(-1, -2)
+    sym = lambda P: 0.5 * (P + P.transpose(-1, -2))
+    T = lambda M: M.transpose(-1, -2)
+    mv = lambda M, x: (M @ x[..., None])[..., 0]
+    QN, qN = sym(blk(term, to["Q"], nx, nx)), term[:, to["q"][0]:to["q"][1]]
+    CN, dN = blk(term, to["C"], nct, nx), term[:, to["d"][0]:to["d"][1]]
+    fbt, fft = CN / mu, dN / mu
+    V = QN + T(CN) @ fbt
+    v = qN + mv(T(CN), fft)
+    Vs, vs, ffs, fbs = [V], [v], [], []
+    for t in range(N - 1, -1, -1):
+        r = stage[:, t]
+        A, Bm, f = blk(r, so["A"], nx, nx), blk(r, so["B"], nx, nu), r[:, so["f"][0]:so["f"][1]]
+        Q, S, R = sym(blk(r, so["Q"], nx, nx)), blk(r, so["S"], nx, nu), sym(blk(r, so["R"], nu, nu))
+        q, rr = r[:, so["q"][0]:so["q"][1]], r[:, so["r"][0]:so["r"][1]]
+        Cm, D, d = blk(r, so["C"], nc, nx), blk(r, so["D"], nc, nu), r[:, so["d"][0]:so["d"][1]]
+        vplus = v + mv(V, f)
+        Sh, Qh = S + T(A) @ V @ Bm, Q + T(A) @ V @ A
+        top = torch.cat([R + T(Bm) @ V @ Bm, T(D)], -1)
+        bot = torch.cat([D, -mu * torch.eye(nc, dtype=torch.float64).expand(B, nc, nc)], -1)
+        M = torch.cat([top, bot], -2)
+        Y = torch.cat([torch.cat([T(Sh), (rr + mv(T(Bm), vplus))[..., None]], -1),
+                       torch.cat([Cm, d[..., None]], -1)], -2)
+        X = -torch.linalg.solve(M, Y)
+        K, k, Z, z = X[:, :nu, :nx], X[:, :nu, nx], X[:, nu:, :nx], X[:, nu:, nx]
+        fbs.append(torch.cat([K, Z, A + Bm @ K], -2))
+        ffs.append(torch.cat([k, z, f + mv(Bm, k)], -1))
+        V = Qh + Sh @ K + T(Cm) @ Z
+        v = q + mv(T(A), vplus) + mv(Sh, k) + mv(T(Cm), z)
+        Vs.append(V)
+        vs.append(v)
+    st = lambda xs, shape: torch.stack(xs[::-1], 1) if xs else torch.zeros(shape, dtype=torch.float64)
+    nr = nu + nc + nx
+    return dict(ff=st(ffs, (B, 0, nr)), fb=st(fbs, (B, 0, nr, nx)), vxx=torch.stack(Vs[::-1], 1),
+                vx=torch.stack(vs[::-1], 1), fft=fft, fbt=fbt)
+
+
+def autograd(stage, term, case, mu, cot):
+    """(factorisation, gradient records of <factorisation, cot>) by torch.autograd through torch_factor."""
+    import torch
+    s = torch.tensor(stage, requires_grad=True)
+    t = torch.tensor(term, requires_grad=True)
+    out = torch_factor(s, t, case, mu)
+    loss = sum((out[k] * torch.tensor(cot[k])).sum() for k in COT)
+    gs, gt = torch.autograd.grad(loss, (s, t), allow_unused=True)
+    zero = lambda g, x: np.zeros(x.shape) if g is None else g.numpy()
+    return {k: v.detach().numpy() for k, v in out.items()}, dict(stage=zero(gs, stage), term=zero(gt, term))

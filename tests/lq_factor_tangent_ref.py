@@ -23,6 +23,7 @@ from __future__ import annotations
 import numpy as np
 
 from lq_adjoint_ref import batched_solve, dtype_of, stage_offsets, term_offsets
+from lq_factor_adjoint_ref import torch_factor
 
 
 def _sym(M):
@@ -107,3 +108,12 @@ def factor_tangent(stage, term, ff, fb, Vxx, vx, ffT, fbT, dot, dims, mueq, solv
         vd = dqh + mv(dSh, k) + mv(Sh, dk) + mv(T(dC), z) + mv(T(C), dz)
         out["vxx"][:, t], out["vx"][:, t] = Vd, vd
     return out
+
+
+def jvp(stage, term, case, mu, dot):
+    """(factorisation, its tangent) by torch.func.jvp through torch_factor."""
+    import torch
+    f = lambda s, t: torch_factor(s, t, case, mu)
+    fac, tan = torch.func.jvp(f, (torch.tensor(stage), torch.tensor(term)),
+                              (torch.tensor(dot["stage"]), torch.tensor(dot["term"])))
+    return {k: v.numpy() for k, v in fac.items()}, {k: v.numpy() for k, v in tan.items()}

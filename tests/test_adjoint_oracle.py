@@ -6,6 +6,7 @@ import pytest
 
 import gen
 import lq_adjoint_ref as ref
+from lq_cases import batch_records
 
 MU = 1e-2
 STAGE_BLOCKS = ("A", "B", "f", "Q", "S", "R", "q", "r", "C", "D", "d")
@@ -30,14 +31,7 @@ def _cotangent(case, seed):
 
 def _records(p, case):
     """Packed (padded) single-instance records of problem p."""
-    nx, nu, nc, nct, nc0, N = case
-    _, srec = ref.stage_offsets(nx, nu, nc)
-    stage = np.zeros((1, N, srec))
-    for t in range(N):
-        r = gen.stage_record(p.stages[t])
-        stage[0, t, :r.size] = r
-    return (stage, gen.term_record(p.stages[N])[None], np.asarray(p.G0).ravel(order="F")[None],
-            np.asarray(p.g0)[None])
+    return batch_records([p], case)
 
 
 def _dims(p):

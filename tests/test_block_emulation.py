@@ -2,7 +2,7 @@
 (riccati_block.cuh) through tests/emu/block_emu.cpp, compared with the oracle."""
 import pytest
 
-from test_group_emulation import check_against_oracle
+from emu_harness import check_against_oracle
 
 
 @pytest.mark.parametrize("shape,nw", [

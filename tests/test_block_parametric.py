@@ -5,22 +5,8 @@ import pytest
 
 import gen
 from emu_harness import emulate
+from lq_cases import make_problem
 from oracle import gar_oracle as orc
-
-
-def make_problem(seed, N, nx, nu, nc, nct, nth):
-    rng = np.random.default_rng(seed)
-    x0 = rng.standard_normal(nx)
-    p = gen.generate_lq_problem(rng, x0, N, nx, nu, nth, nc, singular=False, conditioned=True,
-                                control_rows=nc > 0, term_nc=nct)
-    for k in p.stages:  # non-trivial parametric blocks everywhere
-        k.Gx[...] = 0.3 * rng.standard_normal(k.Gx.shape)
-        k.Gu[...] = 0.3 * rng.standard_normal(k.Gu.shape)
-        k.Gv[...] = 0.0  # (the reference's Vxt formula drops Z^T Gv; legs always have Gv = 0)
-        g = rng.standard_normal((nth, nth))
-        k.Gth[...] = g @ g.T / max(nth, 1) + np.eye(nth)
-        k.gamma[...] = rng.standard_normal(nth)
-    return p
 
 
 @pytest.mark.parametrize("shape", [(5, 2, 0, 0, 3, 6, 1e-8, 1), (4, 3, 2, 0, 2, 5, 1e-3, 1), (7, 3, 0, 2, 7, 4, 1e-2, 2),

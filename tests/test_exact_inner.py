@@ -20,9 +20,7 @@ from oracle import fddp as of
 from oracle import linesearch as ols
 from oracle import lq_assemble as olq
 from oracle import proxddp_inner as pin
-from test_fddp import _random_fddp
-from test_lq_assemble import random_inputs
-from test_proxddp_inner import _hand_case, _hand_gradient_inputs
+from inner_cases import fddp_args, fddp_case, hand_case, hand_gradient_inputs, random_inputs
 
 INF = np.inf
 
@@ -84,7 +82,7 @@ def _exact(w):
 
 
 def test_multipliers_reference_reproduces_the_hand_case():
-    h = _hand_case()
+    h = hand_case()
     m = pin.compute_multipliers(**h)
     got = _restated_outputs(m, 1, 2, 3)
     w = xr.multipliers(_hand_mult_inputs(h), got, h["lo"], h["hi"], h["loN"], h["hiN"], h["mu"], h["mu_dyn"])
@@ -101,7 +99,7 @@ def test_multipliers_reference_reproduces_the_hand_case():
 
 
 def test_gradient_and_criterion_references_reproduce_the_hand_case():
-    h, g = _hand_case(), _hand_gradient_inputs()
+    h, g = hand_case(), hand_gradient_inputs()
     inp = dict(lx=np.array(g["lx"]), lu=np.array(g["lu"]), lx_N=g["lx_N"], Jx=np.array(g["Jx"]), Ju=np.array(g["Ju"]),
                cJx=np.array(g["cJx"]), cJu=np.array(g["cJu"]), cJx_N=g["cJx_N"], G0=g["G0"], lam0=h["lams"][0],
                lams=np.array(h["lams"][1:]), vs=np.array(h["vs"][:1]), vsT=h["vs"][1])
@@ -294,31 +292,6 @@ def test_bar_rejects_the_neighbours_alpha_on_an_instance_boundary():
     assert got[4, 0] != want[4, 0]
     assert gen.rel_fro(got, x + alpha[:, None] * dx) <= 1e-15
     assert xr.failures(got, want)
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# FDDP: the extended-precision backward pass
-# ---------------------------------------------------------------------------------------------------------------------
-def fddp_case(name, rng, B, N, nx, nu):
-    """test_fddp's random problems, and the variants of the level-2 FDDP tests: 'singular' (the last control direction
-    scaled by 1e-5 in Ju, Lxu, Luu: Quu's smallest eigenvalue ~1e-10, preg 1e-10), 'defects' (fs ~ 1e3)."""
-    d = _random_fddp(rng, B, N, nx, nu)
-    preg = 1e-4
-    if name == "singular":
-        s = np.ones(nu)
-        s[-1] = 1e-5
-        d["Ju"] = d["Ju"] * s
-        d["Lxu"] = d["Lxu"] * s
-        d["Luu"] = d["Luu"] * s[:, None] * s
-        preg = 1e-10
-    elif name == "defects":
-        d["fs"] = 1e3 * rng.standard_normal(d["fs"].shape)
-    return d, preg
-
-
-def fddp_args(d, b):
-    return ([list(d[k][b]) for k in ("Jx", "Ju")] + [list(d["fs"][b])]
-            + [list(d[k][b]) for k in ("Lxx", "Lxu", "Luu", "Lx", "Lu")] + [d["Lxx_N"][b], d["Lx_N"][b]])
 
 
 def test_fddp_reference_satisfies_the_recursion():

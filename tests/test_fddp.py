@@ -4,28 +4,14 @@ import numpy as np
 import pytest
 
 import gen
+from inner_cases import random_fddp
 from oracle import fddp as of
-
-
-def _random_fddp(rng, B, N, nx, nu):
-    w = lambda n, p: (lambda r: r @ r.T)(rng.standard_normal((n, p)))
-    d = dict(Jx=np.zeros((B, N, nx, nx)), Ju=rng.uniform(-1, 1, (B, N, nx, nu)), fs=0.1 * rng.standard_normal((B, N + 1, nx)),
-             Lxx=np.zeros((B, N, nx, nx)), Lxu=np.zeros((B, N, nx, nu)), Luu=np.zeros((B, N, nu, nu)),
-             Lx=rng.uniform(-1, 1, (B, N, nx)), Lu=rng.uniform(-1, 1, (B, N, nu)), Lxx_N=np.zeros((B, nx, nx)),
-             Lx_N=rng.uniform(-1, 1, (B, nx)))
-    for b in range(B):
-        for t in range(N):
-            H = w(nx + nu, nx + nu + 1) / max(nx, nu)
-            d["Lxx"][b, t], d["Lxu"][b, t], d["Luu"][b, t] = H[:nx, :nx], H[:nx, nx:], H[nx:, nx:]
-            d["Jx"][b, t] = np.eye(nx) + 0.1 * rng.standard_normal((nx, nx)) / np.sqrt(nx)
-        d["Lxx_N"][b] = w(nx, nx + 1) / nx
-    return d
 
 
 def test_restatement_satisfies_the_recursion():
     rng = np.random.default_rng(0)
     B, N, nx, nu, preg = 1, 6, 4, 2, 1e-3
-    d = _random_fddp(rng, B, N, nx, nu)
+    d = random_fddp(rng, B, N, nx, nu)
     r = of.backward_pass(*[list(d[k][0]) for k in ("Jx", "Ju")], list(d["fs"][0]), *[list(d[k][0]) for k in
                          ("Lxx", "Lxu", "Luu", "Lx", "Lu")], d["Lxx_N"][0], d["Lx_N"][0], preg)
     for i in range(N):  # Quu k = -Qu and Quu K = -Qux (the LLT solve), Quuks = Quu k
@@ -50,7 +36,7 @@ def test_device_fddp_backward_pass(shape):
     nx, nu, N, B = shape
     preg = 1e-4
     rng = np.random.default_rng(nx)
-    d = _random_fddp(rng, B, N, nx, nu)
+    d = random_fddp(rng, B, N, nx, nu)
     dev = torch.device("cuda:0")
     cm = lambda a: np.ascontiguousarray(np.swapaxes(a, -1, -2))  # column-major blocks
     arr = {k: torch.tensor(cm(d[k]) if d[k].ndim >= 3 and k not in ("fs", "Lx", "Lu", "Lx_N") else d[k], device=dev)

@@ -14,7 +14,7 @@ import gen
 import hp_reference as hp
 from exact_bounds import same_bits
 from oracle import fddp as of
-from test_exact_inner import fddp_args, fddp_case
+from inner_cases import fddp_args, fddp_case
 
 pytestmark = pytest.mark.gpu
 

@@ -9,44 +9,17 @@ import pytest
 import gen
 import lq_adjoint_ref as aref
 import lq_factor_adjoint_ref as ref
-from test_factor_adjoint_oracle import block_errors, device_cot, torch_factor
-from test_gpu_adjoint import _block_inputs, _outputs, env  # noqa: F401  (env is the module fixture)
+import lq_gpu
+from lq_cases import block_errors, device_cot
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-10
 FAMS = ref.COT
 
 
-def _records(gar, probs):
-    stage, term, G0, g0 = [np.ascontiguousarray(a) for a in gar.pack_problems(probs)]
-    B, N = len(probs), probs[0].horizon
-    return stage.reshape(B, N, stage.size // max(B * N, 1)), term.reshape(B, -1), G0.reshape(B, -1), g0.reshape(B, -1)
-
-
-def _factor(gar, s):
-    """The handle's own factorisation in the restatement's shapes."""
-    return dict(ff=s.get(gar.OUT_FF), fb=s.get(gar.OUT_FB), vxx=s.get(gar.OUT_VXX), vx=s.get(gar.OUT_VX),
-                fft=s.get(gar.OUT_FFT), fbt=s.get(gar.OUT_FBT))
-
-
-def _dev(torch, a):
-    return None if a is None else torch.tensor(np.ascontiguousarray(a, dtype=np.float64), device="cuda")
-
-
-def _grads(torch, s):
-    d = s.dims
-    shapes = dict(stage=(d.batch, d.horizon, s.srec), term=(d.batch, s.trec), G0=(d.batch, d.nc0 * d.nx),
-                  g0=(d.batch, d.nc0))
-    return {k: torch.full(v, float("nan"), dtype=torch.float64, device="cuda") for k, v in shapes.items()}
-
-
-def _run(env, s, cot, mu, d6):
-    _, _, torch = env
-    dc = {k: _dev(torch, v) for k, v in device_cot(cot, d6, s.dims.batch).items()}
-    g = _grads(torch, s)
-    s.factor_adjoint(dc, g, mu if np.ndim(mu) == 0 else _dev(torch, mu))
-    s.synchronize()
-    return {k: v.cpu().numpy() for k, v in g.items()}
+@pytest.fixture(scope="module")
+def env():
+    return lq_gpu.gpu_env()
 
 
 def _check(got, want, d6, tol, what):
@@ -61,35 +34,23 @@ def _restate(recs, fac, cot, d6, mu):
                               cot, d6, mu)
 
 
-# (name, CudaRiccatiBatch keyword arguments, (nx, nu, nc, nct, nc0, N, B), mu)
-CASES = [("warp_c3", {}, (4, 2, 2, 2, 4, 6, 9), 1e-3),
-         ("cta_v9", dict(variant=9), (4, 2, 2, 2, 4, 6, 9), 1e-3),
-         ("mma_12", {}, (12, 6, 0, 3, 12, 6, 9), 1e-3),
-         ("lane_c1", {}, (6, 3, 0, 2, 3, 5, 5), 1e-3),
-         ("cta_runtime", {}, (7, 3, 2, 2, 7, 5, 8), 1e-2),
-         ("N0", {}, (4, 2, 2, 2, 4, 0, 3), 1e-3),
-         ("N1", {}, (6, 3, 0, 2, 3, 1, 3), 1e-3),
-         ("small_mu", {}, (4, 2, 2, 2, 4, 5, 4), 1e-8),
-         ("small_mu_v9", dict(variant=9), (12, 6, 0, 3, 12, 4, 3), 1e-8)]
-
-
-@pytest.mark.parametrize("name,kw,dims,mu", CASES, ids=[c[0] for c in CASES])
+@pytest.mark.parametrize("name,kw,dims,mu", lq_gpu.FACTOR_HANDLES, ids=[c[0] for c in lq_gpu.FACTOR_HANDLES])
 def test_matches_restatement(env, name, kw, dims, mu):
     gar, _, _ = env
     d6 = dims[:6]
     B = dims[6]
     probs = gen.generate_batch(41, B, dims[5], *dims[:3], dims[3])
-    recs = _records(gar, probs)
+    recs = lq_gpu.handle_records(gar, probs)
     s = gar.CudaRiccatiBatch(*dims, **kw)
     s.set_problem(*recs)
     s.backward(mu)
     cot = ref.random_cot(np.random.default_rng(2), d6, B)
-    got = _run(env, s, cot, mu, d6)
-    _check(got, _restate(recs, _factor(gar, s), cot, d6, mu), d6, max(TOL, 2.4e-16 / mu), name)
+    got = lq_gpu.device_factor_adjoint(env, s, cot, mu, d6)
+    _check(got, _restate(recs, lq_gpu.factor(gar, s), cot, d6, mu), d6, max(TOL, 2.4e-16 / mu), name)
     # NULL fields are zero cotangents; FB alone
     for part in (dict(fb=cot["fb"]), dict(cot, vxx=None, fft=None), dict(vxx=cot["vxx"], vx=cot["vx"])):
-        got = _run(env, s, part, mu, d6)
-        _check(got, _restate(recs, _factor(gar, s), part, d6, mu), d6, max(TOL, 2.4e-16 / mu), (name, list(part)))
+        got = lq_gpu.device_factor_adjoint(env, s, part, mu, d6)
+        _check(got, _restate(recs, lq_gpu.factor(gar, s), part, d6, mu), d6, max(TOL, 2.4e-16 / mu), (name, list(part)))
     s.close()
 
 
@@ -100,14 +61,14 @@ def test_forced_2x2_pivots_cycle_append_and_per_instance_mu(env):
     d6 = dims[:6]
     probs = gen.generate_batch(42, B, N, nx, nu, nc, nct)
     gen.make_2x2_pivots(probs)
-    recs = _records(gar, probs)
+    recs = lq_gpu.handle_records(gar, probs)
     s = gar.CudaRiccatiBatch(*dims)
     s.set_problem(*recs)
     mu = np.array([1e-3, 1e-2, 1e-3, 1e-1, 1e-3, 1e-2])
     s.backward(mu)
     assert s.pivot_stats()[0].sum() > 0  # the 2x2 pivot path ran
     cot = ref.random_cot(np.random.default_rng(3), d6, B)
-    _check(_run(env, s, cot, mu, d6), _restate(recs, _factor(gar, s), cot, d6, mu), d6, TOL, "2x2 _v")
+    _check(lq_gpu.device_factor_adjoint(env, s, cot, mu, d6), _restate(recs, lq_gpu.factor(gar, s), cot, d6, mu), d6, TOL, "2x2 _v")
     # cycle_append, then a backward: records are read through the ring head
     _, srec = aref.stage_offsets(nx, nu, nc)
     new = gen.generate_batch(43, B, 1, nx, nu, nc, nct)
@@ -115,11 +76,11 @@ def test_forced_2x2_pivots_cycle_append_and_per_instance_mu(env):
                    for p in new])
     s.cycle_append(np.ascontiguousarray(nl))
     with pytest.raises(gar.GarError, match="error 4"):
-        _run(env, s, cot, 1e-3, d6)
+        lq_gpu.device_factor_adjoint(env, s, cot, 1e-3, d6)
     s.backward(1e-3)
     stage = s.get_problem(0).reshape(B, N, -1)
     term = s.get_problem(1).reshape(B, -1)
-    _check(_run(env, s, cot, 1e-3, d6), _restate((stage, term), _factor(gar, s), cot, d6, 1e-3), d6, TOL, "cycle")
+    _check(lq_gpu.device_factor_adjoint(env, s, cot, 1e-3, d6), _restate((stage, term), lq_gpu.factor(gar, s), cot, d6, 1e-3), d6, TOL, "cycle")
     s.close()
 
 
@@ -129,25 +90,25 @@ def test_state_untouched_deterministic_and_errors(env):
     nx, nu, nc, nct, nc0, N, B = dims
     d6 = dims[:6]
     mu = 1e-3
-    recs = _records(gar, gen.generate_batch(44, B, N, nx, nu, nc, nct))
+    recs = lq_gpu.handle_records(gar, gen.generate_batch(44, B, N, nx, nu, nc, nct))
     s = gar.CudaRiccatiBatch(*dims)
     s.set_problem(*recs)
     cot = ref.random_cot(np.random.default_rng(4), d6, B)
     with pytest.raises(gar.GarError, match="error 4"):  # no backward since set_problem
-        _run(env, s, cot, mu, d6)
+        lq_gpu.device_factor_adjoint(env, s, cot, mu, d6)
     s.sweep(mu)
-    before, e0 = _outputs(gar, s), s.factor_epoch()
-    a1 = _run(env, s, cot, mu, d6)
-    a2 = _run(env, s, cot, mu, d6)
+    before, e0 = lq_gpu.outputs(gar, s), s.factor_epoch()
+    a1 = lq_gpu.device_factor_adjoint(env, s, cot, mu, d6)
+    a2 = lq_gpu.device_factor_adjoint(env, s, cot, mu, d6)
     for k in a1:
         assert np.array_equal(a1[k], a2[k]), k  # two calls, identical bits
-    after = _outputs(gar, s)
+    after = lq_gpu.outputs(gar, s)
     for k, v in before.items():
         assert np.array_equal(v, after[k], equal_nan=True), k
     assert s.factor_epoch() == e0
     # errors: nothing is launched
-    g = _grads(torch, s)
-    dc = {k: _dev(torch, v) for k, v in device_cot(cot, d6, B).items()}
+    g = lq_gpu.grads(torch, s)
+    dc = {k: lq_gpu.dev(torch, v) for k, v in device_cot(cot, d6, B).items()}
     n0 = s.launch_count()
     with pytest.raises(gar.GarError, match="error 1"):
         s.factor_adjoint(dc, g, 0.0)
@@ -192,7 +153,7 @@ def test_full_size(env, cfg):
     shapes = ref.cot_shapes(d6, B)
     cot = {k: torch.randn(v, dtype=torch.float64, device="cuda", generator=gen_t) for k, v in shapes.items()}
     dc = {k: (v.transpose(-1, -2).contiguous() if k == "vxx" else v) for k, v in cot.items()}
-    g = _grads(torch, s)
+    g = lq_gpu.grads(torch, s)
     s.factor_adjoint(dc, g, mu)
     s.synchronize()
     # the first wave, a wave boundary and the ragged tail (C5: a few instances)
@@ -222,7 +183,7 @@ def test_gradcheck_lq_factor(env):
     nx, nu, nc, nct, nc0, N, B = 4, 2, 2, 2, 4, 3, 2
     probs = gen.generate_batch(21, B, N, nx, nu, nc, nct)
     s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B)
-    blocks, term, init = _block_inputs(torch, probs)
+    blocks, term, init = lq_gpu.block_inputs(torch, probs)
     names = list(blocks) + ["t" + n for n in term]
     leaves = list(blocks.values()) + list(term.values())
     sym = lambda P: 0.5 * (P + P.transpose(-1, -2))
@@ -240,7 +201,7 @@ def test_gradcheck_lq_factor(env):
 
 
 def _torch_solution(fac, G0, g0, case):
-    """The LQ solution from a torch factorisation (torch_factor) and the initial condition, differentiably."""
+    """The LQ solution from a torch factorisation (ref.torch_factor) and the initial condition, differentiably."""
     import torch
     nx, nu, nc, nct, nc0, N = case
     B = G0.shape[0]
@@ -269,7 +230,7 @@ def test_mixed_loss_jacrev_and_jvp(env):
     case = (4, 2, 2, 2, 4, 4)
     nx, nu, nc, nct, nc0, N = case
     B, mu = 2, 1e-2
-    recs = _records(gar, gen.general_initial_condition(gen.generate_batch(45, B, N, nx, nu, nc, nct), nc0, 45))
+    recs = lq_gpu.handle_records(gar, gen.general_initial_condition(gen.generate_batch(45, B, N, nx, nu, nc, nct), nc0, 45))
     s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B)
     rng = np.random.default_rng(6)
     dev = [torch.tensor(np.ascontiguousarray(a), device="cuda", requires_grad=True) for a in recs]
@@ -283,7 +244,7 @@ def test_mixed_loss_jacrev_and_jvp(env):
         sum((o * torch.tensor(cs[k], device="cuda")).sum() for k, o in zip(aref.KEYS, so))
     gd = torch.autograd.grad(loss, dev)
     cpu = [torch.tensor(a, requires_grad=True) for a in recs]
-    fac = torch_factor(cpu[0], cpu[1], case, mu)
+    fac = ref.torch_factor(cpu[0], cpu[1], case, mu)
     sol = _torch_solution(fac, cpu[2], cpu[3], case)
     lc = sum((fac[k] * torch.tensor(cf[k])).sum() for k in FAMS) + \
         sum((sol[k] * torch.tensor(cs[k])).sum() for k in aref.KEYS)
@@ -296,7 +257,7 @@ def test_mixed_loss_jacrev_and_jvp(env):
     K0 = lambda st: ag.lq_factor(s, st, *rest, mu)[1][:, 0, :nu, :]
     J = torch.func.jacrev(K0)(st0).cpu().numpy()
     Jc = torch.autograd.functional.jacobian(
-        lambda st: torch_factor(st, torch.tensor(recs[1]), case, mu)["fb"][:, 0, :nu, :], torch.tensor(recs[0]))
+        lambda st: ref.torch_factor(st, torch.tensor(recs[1]), case, mu)["fb"][:, 0, :nu, :], torch.tensor(recs[0]))
     # the oracle's gradient is the symmetric-argument one for Q and R: compare on a symmetric direction
     so_, _ = aref.stage_offsets(nx, nu, nc)
     d = rng.standard_normal(recs[0].shape)

@@ -11,28 +11,17 @@ import gen
 import lq_adjoint_ref as aref
 import lq_factor_adjoint_ref as adj
 import lq_factor_tangent_ref as ref
-from test_factor_adjoint_oracle import device_cot, torch_factor
-from test_factor_tangent_oracle import FAMS, family_errors, out_shapes, random_dot
-from test_gpu_adjoint import _block_inputs, _outputs, env  # noqa: F401  (env is the module fixture)
-from test_gpu_factor_adjoint import CASES, _dev, _factor, _grads, _records
+import lq_gpu
+from lq_cases import device_cot, family_errors, random_dot
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-10
+FAMS = adj.COT
 
 
-def _outs(torch, case, B):
-    """NaN-filled out tensors in the device layouts (vxx as column-major blocks: same shape)."""
-    return {k: torch.full(s, float("nan"), dtype=torch.float64, device="cuda") for k, s in out_shapes(case, B).items()}
-
-
-def _run(env, s, dot, mu, d6, want=FAMS):
-    _, _, torch = env
-    B = s.dims.batch
-    o = _outs(torch, d6, B)
-    s.factor_tangent({k: _dev(torch, v) for k, v in dot.items()}, {k: v for k, v in o.items() if k in want},
-                     mu if np.ndim(mu) == 0 else _dev(torch, mu))
-    s.synchronize()
-    return {k: (np.swapaxes(v.cpu().numpy(), -1, -2) if k == "vxx" else v.cpu().numpy()) for k, v in o.items()}
+@pytest.fixture(scope="module")
+def env():
+    return lq_gpu.gpu_env()
 
 
 def _restate(recs, fac, dot, d6, mu):
@@ -46,25 +35,25 @@ def _check(got, want, tol, what, fams=FAMS):
     assert np.array_equal(got["vxx"], np.swapaxes(got["vxx"], -1, -2)) or "vxx" not in fams, what
 
 
-@pytest.mark.parametrize("name,kw,dims,mu", CASES, ids=[c[0] for c in CASES])
+@pytest.mark.parametrize("name,kw,dims,mu", lq_gpu.FACTOR_HANDLES, ids=[c[0] for c in lq_gpu.FACTOR_HANDLES])
 def test_matches_restatement(env, name, kw, dims, mu):
     gar, _, _ = env
     d6 = dims[:6]
     B = dims[6]
     probs = gen.generate_batch(61, B, dims[5], *dims[:3], dims[3])
-    recs = _records(gar, probs)
+    recs = lq_gpu.handle_records(gar, probs)
     s = gar.CudaRiccatiBatch(*dims, **kw)
     s.set_problem(*recs)
     s.backward(mu)
     dot = random_dot(np.random.default_rng(21), d6, B)
     tol = max(TOL, 2.4e-16 / mu)
-    fac = _factor(gar, s)
-    _check(_run(env, s, dot, mu, d6), _restate(recs, fac, dot, d6, mu), tol, name)
+    fac = lq_gpu.factor(gar, s)
+    _check(lq_gpu.device_factor_tangent(env, s, dot, mu, d6), _restate(recs, fac, dot, d6, mu), tol, name)
     # NULL tangent fields are zero: stage only, term only
     for part in (dict(stage=dot["stage"]), dict(term=dot["term"])):
-        _check(_run(env, s, part, mu, d6), _restate(recs, fac, part, d6, mu), tol, (name, list(part)))
+        _check(lq_gpu.device_factor_tangent(env, s, part, mu, d6), _restate(recs, fac, part, d6, mu), tol, (name, list(part)))
     # NULL out fields are not written
-    got = _run(env, s, dot, mu, d6, want=("fb", "vx"))
+    got = lq_gpu.device_factor_tangent(env, s, dot, mu, d6, want=("fb", "vx"))
     _check(got, _restate(recs, fac, dot, d6, mu), tol, (name, "fb vx"), fams=("fb", "vx"))
     for k in ("ff", "vxx", "fft", "fbt"):
         assert np.isnan(got[k]).all(), (name, k)
@@ -78,14 +67,14 @@ def test_forced_2x2_pivots_cycle_append_and_per_instance_mu(env):
     d6 = dims[:6]
     probs = gen.generate_batch(62, B, N, nx, nu, nc, nct)
     gen.make_2x2_pivots(probs)
-    recs = _records(gar, probs)
+    recs = lq_gpu.handle_records(gar, probs)
     s = gar.CudaRiccatiBatch(*dims)
     s.set_problem(*recs)
     mu = np.array([1e-3, 1e-2, 1e-3, 1e-1, 1e-3, 1e-2])
     s.backward(mu)
     assert s.pivot_stats()[0].sum() > 0  # the 2x2 pivot path ran
     dot = random_dot(np.random.default_rng(22), d6, B)
-    _check(_run(env, s, dot, mu, d6), _restate(recs, _factor(gar, s), dot, d6, mu), TOL, "2x2 _v")
+    _check(lq_gpu.device_factor_tangent(env, s, dot, mu, d6), _restate(recs, lq_gpu.factor(gar, s), dot, d6, mu), TOL, "2x2 _v")
     # cycle_append, then a backward: records are read through the ring head
     _, srec = aref.stage_offsets(nx, nu, nc)
     new = gen.generate_batch(63, B, 1, nx, nu, nc, nct)
@@ -93,11 +82,11 @@ def test_forced_2x2_pivots_cycle_append_and_per_instance_mu(env):
                    for p in new])
     s.cycle_append(np.ascontiguousarray(nl))
     with pytest.raises(gar.GarError, match="error 4"):
-        _run(env, s, dot, 1e-3, d6)
+        lq_gpu.device_factor_tangent(env, s, dot, 1e-3, d6)
     s.backward(1e-3)
     stage = s.get_problem(0).reshape(B, N, -1)
     term = s.get_problem(1).reshape(B, -1)
-    _check(_run(env, s, dot, 1e-3, d6), _restate((stage, term), _factor(gar, s), dot, d6, 1e-3), TOL, "cycle")
+    _check(lq_gpu.device_factor_tangent(env, s, dot, 1e-3, d6), _restate((stage, term), lq_gpu.factor(gar, s), dot, d6, 1e-3), TOL, "cycle")
     s.close()
 
 
@@ -107,25 +96,25 @@ def test_state_untouched_deterministic_and_errors(env):
     nx, nu, nc, nct, nc0, N, B = dims
     d6 = dims[:6]
     mu = 1e-3
-    recs = _records(gar, gen.generate_batch(64, B, N, nx, nu, nc, nct))
+    recs = lq_gpu.handle_records(gar, gen.generate_batch(64, B, N, nx, nu, nc, nct))
     s = gar.CudaRiccatiBatch(*dims)
     s.set_problem(*recs)
     dot = random_dot(np.random.default_rng(23), d6, B)
     with pytest.raises(gar.GarError, match="error 4"):  # no backward since set_problem
-        _run(env, s, dot, mu, d6)
+        lq_gpu.device_factor_tangent(env, s, dot, mu, d6)
     s.sweep(mu)
-    before, e0 = _outputs(gar, s), s.factor_epoch()
-    a1 = _run(env, s, dot, mu, d6)
-    a2 = _run(env, s, dot, mu, d6)
+    before, e0 = lq_gpu.outputs(gar, s), s.factor_epoch()
+    a1 = lq_gpu.device_factor_tangent(env, s, dot, mu, d6)
+    a2 = lq_gpu.device_factor_tangent(env, s, dot, mu, d6)
     for k in a1:
         assert np.array_equal(a1[k], a2[k]), k  # two calls, identical bits
-    after = _outputs(gar, s)
+    after = lq_gpu.outputs(gar, s)
     for k, v in before.items():
         assert np.array_equal(v, after[k], equal_nan=True), k
     assert s.factor_epoch() == e0
     # errors: nothing is launched
-    o = _outs(torch, d6, B)
-    dd = {k: _dev(torch, v) for k, v in dot.items()}
+    o = lq_gpu.outs(torch, d6, B)
+    dd = {k: lq_gpu.dev(torch, v) for k, v in dot.items()}
     n0 = s.launch_count()
     with pytest.raises(gar.GarError, match="error 1"):
         s.factor_tangent(dd, o, 0.0)
@@ -156,8 +145,8 @@ def test_state_untouched_deterministic_and_errors(env):
         u.close()
 
 
-@pytest.mark.parametrize("name,kw,dims,mu", [CASES[0], CASES[1], CASES[4], CASES[7]],
-                         ids=[CASES[i][0] for i in (0, 1, 4, 7)])
+@pytest.mark.parametrize("name,kw,dims,mu", [lq_gpu.FACTOR_HANDLES[0], lq_gpu.FACTOR_HANDLES[1], lq_gpu.FACTOR_HANDLES[4], lq_gpu.FACTOR_HANDLES[7]],
+                         ids=[lq_gpu.FACTOR_HANDLES[i][0] for i in (0, 1, 4, 7)])
 def test_duality_with_factor_adjoint(env, name, kw, dims, mu):
     """<cbar, ydot> from factor_tangent = <factor_adjoint(cbar), pdot>, both on the device: within 1e-10 relative, or
     at small mu within the conditioning bar max(1e-10, 2.4e-16 / mu) of the two calls' own results (the pairings grow
@@ -165,7 +154,7 @@ def test_duality_with_factor_adjoint(env, name, kw, dims, mu):
     gar, _, torch = env
     d6 = dims[:6]
     B = dims[6]
-    recs = _records(gar, gen.generate_batch(65, B, dims[5], *dims[:3], dims[3]))
+    recs = lq_gpu.handle_records(gar, gen.generate_batch(65, B, dims[5], *dims[:3], dims[3]))
     s = gar.CudaRiccatiBatch(*dims, **kw)
     s.set_problem(*recs)
     s.backward(mu)
@@ -173,9 +162,9 @@ def test_duality_with_factor_adjoint(env, name, kw, dims, mu):
     for _ in range(2):
         dot = random_dot(rng, d6, B)
         cot = adj.random_cot(rng, d6, B)
-        tan = _run(env, s, dot, mu, d6)
-        dc = {k: _dev(torch, v) for k, v in device_cot(cot, d6, B).items()}
-        g = _grads(torch, s)
+        tan = lq_gpu.device_factor_tangent(env, s, dot, mu, d6)
+        dc = {k: lq_gpu.dev(torch, v) for k, v in device_cot(cot, d6, B).items()}
+        g = lq_gpu.grads(torch, s)
         s.factor_adjoint(dc, g, mu)
         s.synchronize()
         lhs = sum(float((tan[k] * cot[k]).sum()) for k in FAMS)
@@ -199,7 +188,7 @@ def test_full_size(env, cfg):
     gen_t = torch.Generator(device="cuda").manual_seed(6)
     dot = dict(stage=torch.randn(stage.shape, dtype=torch.float64, device="cuda", generator=gen_t),
                term=torch.randn(term.shape, dtype=torch.float64, device="cuda", generator=gen_t))
-    o = _outs(torch, d6, B)
+    o = lq_gpu.outs(torch, d6, B)
     s.factor_tangent(dot, o, mu)
     s.synchronize()
     # the first wave, a wave boundary and the ragged tail (C5: a few instances)
@@ -228,7 +217,7 @@ def test_full_size(env, cfg):
 def _torch_case(env, seed, case=(4, 2, 2, 2, 4, 4), B=2):
     gar, ag, torch = env
     nx, nu, nc, nct, nc0, N = case
-    recs = _records(gar, gen.general_initial_condition(gen.generate_batch(seed, B, N, nx, nu, nc, nct), nc0, seed))
+    recs = lq_gpu.handle_records(gar, gen.general_initial_condition(gen.generate_batch(seed, B, N, nx, nu, nc, nct), nc0, seed))
     s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B)
     dev = [torch.tensor(np.ascontiguousarray(a), device="cuda") for a in recs]
     return s, recs, dev
@@ -269,7 +258,7 @@ def test_gradcheck_forward_mode(env):
     nx, nu, nc, nct, nc0, N, B = 4, 2, 2, 2, 4, 3, 2
     probs = gen.generate_batch(67, B, N, nx, nu, nc, nct)
     s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B)
-    blocks, term, init = _block_inputs(torch, probs)
+    blocks, term, init = lq_gpu.block_inputs(torch, probs)
     names = list(blocks) + ["t" + n for n in term]
     leaves = list(blocks.values()) + list(term.values())
     sym = lambda P: 0.5 * (P + P.transpose(-1, -2))  # the sweep reads Q and R as symmetric
@@ -322,7 +311,7 @@ def test_jacfwd_matches_jacrev_and_refusals(env):
     cpu_st = torch.tensor(recs[0])
     e = torch.zeros_like(cpu_st)
     e[idx[0]] = 1.0
-    _, tK = torch.func.jvp(lambda x: torch_factor(x, torch.tensor(recs[1]), case, mu)["fb"][:, 0, :nu, :], (cpu_st,),
+    _, tK = torch.func.jvp(lambda x: adj.torch_factor(x, torch.tensor(recs[1]), case, mu)["fb"][:, 0, :nu, :], (cpu_st,),
                            (e,))
     assert gen.rel_fro(Jf[..., 0].cpu().numpy(), tK.numpy()) <= 1e-9
     s.close()

@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 
 import gen
-from test_fddp import _random_fddp
+from inner_cases import random_fddp
 
 pytestmark = pytest.mark.gpu
 
@@ -52,7 +52,7 @@ def test_transition_table(kind):
     zeros = lambda *shape: torch.zeros(shape, dtype=torch.float64, device="cuda")
     sol = dict(xs=(B, N + 1, nx), us=(B, N, nu), vs=(B, N, 0), vsT=(B, 0), lam0=(B, nx), lams=(B, N, nx))
     cm = lambda a: np.ascontiguousarray(np.swapaxes(a, -1, -2))
-    fd = _random_fddp(np.random.default_rng(2), B, N, nx, nu)
+    fd = random_fddp(np.random.default_rng(2), B, N, nx, nu)
     fddp = {k: dev(cm(v) if v.ndim >= 3 and k not in ("fs", "Lx", "Lu", "Lx_N") else v) for k, v in fd.items()}
     lq = {k: fddp[k] for k in ("Jx", "Ju", "Lxx", "Lxu", "Luu", "Lx", "Lu", "Lxx_N", "Lx_N")}
     lq.update(slack=fddp["fs"][:, 1:].contiguous(), G0=dev(np.tile(-np.eye(nx).ravel(), (B, 1))),

@@ -13,11 +13,10 @@ import gen
 import hp_higher_order as hho
 import hp_reference as hp
 import lq_adjoint_ref as aref
-from test_gpu_adjoint import _outputs, _primal, env  # noqa: F401  (env is the module fixture)
-from test_gpu_jacobian import _cots, _dots, _grad_bufs, _np, _rec_shapes, _sol_bufs
-from test_gpu_resolve import SERIAL, _setup
-from test_higher_order_oracle import grad_modes, rho_modes
-from test_hp_derivatives import check_bar, symmetric_dot
+import lq_gpu
+from lq_cases import check_bar, symmetric_dot
+from lq_gpu import SERIAL
+from lq_higher_ref import grad_modes, rho_modes
 
 pytestmark = pytest.mark.gpu
 KEYS = aref.KEYS
@@ -34,6 +33,11 @@ MODES = [(True, False), (True, True), (False, True)]
 MODE_IDS = ["each1", "each12", "each2"]
 
 
+@pytest.fixture(scope="module")
+def env():
+    return lq_gpu.gpu_env()
+
+
 def _rel(got, want):
     return max(gen.rel_fro(got[k], want[k]) for k in want if np.asarray(want[k]).size)
 
@@ -44,39 +48,39 @@ def _d6(s):
 
 
 def _shared(env, primal, seed):
-    return {k: v[0] for k, v in _cots(env, None, primal, 1, seed).items()}
+    return {k: v[0] for k, v in lq_gpu.cots(env, None, primal, 1, seed).items()}
 
 
 @pytest.mark.parametrize("each1,each2", MODES, ids=MODE_IDS)
 @pytest.mark.parametrize("name,kw,dims", CASES, ids=IDS)
 def test_kernels_against_numpy_and_bits(env, name, kw, dims, each1, each2):
     gar, _, torch = env
-    s, _ = _setup(env, kw, dims, 5, MU)
-    d6, primal = _d6(s), _primal(env, s)
-    before, epoch, launches = _outputs(gar, s), s.factor_epoch(), s.launch_count()
-    dot1, dot2 = _dots(env, s, NRHS, 11), _dots(env, s, NRHS, 21)
-    e, y1, y2 = (_cots(env, s, primal, NRHS, seed) for seed in (41, 51, 61))
-    a1 = _cots(env, s, primal, NRHS, 31) if each1 else _shared(env, primal, 31)
-    a2 = _cots(env, s, primal, NRHS, 71) if each2 else _shared(env, primal, 71)
-    vecs = lambda d, each: _np(d) if each else _np(d) | {"each": False}
+    s, _ = lq_gpu.setup(env, kw, dims, 5, MU)
+    d6, primal = _d6(s), lq_gpu.primal(env, s)
+    before, epoch, launches = lq_gpu.outputs(gar, s), s.factor_epoch(), s.launch_count()
+    dot1, dot2 = lq_gpu.dots(env, s, NRHS, 11), lq_gpu.dots(env, s, NRHS, 21)
+    e, y1, y2 = (lq_gpu.cots(env, s, primal, NRHS, seed) for seed in (41, 51, 61))
+    a1 = lq_gpu.cots(env, s, primal, NRHS, 31) if each1 else _shared(env, primal, 31)
+    a2 = lq_gpu.cots(env, s, primal, NRHS, 71) if each2 else _shared(env, primal, 71)
+    vecs = lambda d, each: lq_gpu.to_np(d) if each else lq_gpu.to_np(d) | {"each": False}
     pick = lambda d, each, j: {k: v[j:j + 1] for k, v in d.items()} if each else d
     for vec in (True, False):
-        out = _sol_bufs(env, primal, NRHS)
+        out = lq_gpu.sol_bufs(env, primal, NRHS)
         s.rho_many(dot1, a1, out, vec, dot2, a2, e)
-        want = rho_modes(NRHS, d6, _np(dot1), vecs(a1, each1), vec, _np(dot2), vecs(a2, each2), _np(e))
-        assert _rel(_np(out), want) <= 1e-12, vec
-        grad = _grad_bufs(env, s, NRHS)
+        want = rho_modes(NRHS, d6, lq_gpu.to_np(dot1), vecs(a1, each1), vec, lq_gpu.to_np(dot2), vecs(a2, each2), lq_gpu.to_np(e))
+        assert _rel(lq_gpu.to_np(out), want) <= 1e-12, vec
+        grad = lq_gpu.grad_bufs_many(env, s, NRHS)
         s.grad_many(y1, a1, grad, vec, y2, a2)
-        want = grad_modes(NRHS, d6, _np(y1), vecs(a1, each1), vec, _np(y2), vecs(a2, each2))
-        assert _rel(_np(grad), want) <= 1e-12, vec
+        want = grad_modes(NRHS, d6, lq_gpu.to_np(y1), vecs(a1, each1), vec, lq_gpu.to_np(y2), vecs(a2, each2))
+        assert _rel(lq_gpu.to_np(grad), want) <= 1e-12, vec
         # right-hand side j alone gives the bits it had among NRHS
         for j in (0, 17, NRHS - 1):
-            one = _sol_bufs(env, primal, 1)
+            one = lq_gpu.sol_bufs(env, primal, 1)
             s.rho_many({k: v[j:j + 1] for k, v in dot1.items()}, pick(a1, each1, j), one, vec,
                        {k: v[j:j + 1] for k, v in dot2.items()}, pick(a2, each2, j),
                        {k: v[j:j + 1] for k, v in e.items()})
             assert all(torch.equal(one[k][0], out[k][j]) for k in KEYS), (vec, j)
-            g1 = _grad_bufs(env, s, 1)
+            g1 = lq_gpu.grad_bufs_many(env, s, 1)
             s.grad_many({k: v[j:j + 1] for k, v in y1.items()}, pick(a1, each1, j), g1, vec,
                         {k: v[j:j + 1] for k, v in y2.items()}, pick(a2, each2, j))
             assert all(torch.equal(g1[k][0], grad[k][j]) for k in RECS), (vec, j)
@@ -85,20 +89,20 @@ def test_kernels_against_numpy_and_bits(env, name, kw, dims, each1, each2):
         return
     # one term with the vector blocks and a shared primal: tangent_many's work and adjoint_many's gradient, bit for bit;
     # the same primal given per direction runs the generalised instantiation and gives the same bits
-    work, zd = _sol_bufs(env, primal, NRHS), _sol_bufs(env, primal, NRHS)
+    work, zd = lq_gpu.sol_bufs(env, primal, NRHS), lq_gpu.sol_bufs(env, primal, NRHS)
     s.tangent_many(primal, dot1, work, zd, MU)
-    rho, rho_each = _sol_bufs(env, primal, NRHS), _sol_bufs(env, primal, NRHS)
+    rho, rho_each = lq_gpu.sol_bufs(env, primal, NRHS), lq_gpu.sol_bufs(env, primal, NRHS)
     s.rho_many(dot1, primal, rho)
     s.rho_many(dot1, {k: v.expand(NRHS, *v.shape).contiguous() for k, v in primal.items()}, rho_each)
     assert all(torch.equal(rho[k], work[k]) and torch.equal(rho_each[k], work[k]) for k in KEYS)
-    y, g_adj = _sol_bufs(env, primal, NRHS), _grad_bufs(env, s, NRHS)
+    y, g_adj = lq_gpu.sol_bufs(env, primal, NRHS), lq_gpu.grad_bufs_many(env, s, NRHS)
     s.adjoint_many(primal, y1, y, g_adj, MU)
-    g, g_each = _grad_bufs(env, s, NRHS), _grad_bufs(env, s, NRHS)
+    g, g_each = lq_gpu.grad_bufs_many(env, s, NRHS), lq_gpu.grad_bufs_many(env, s, NRHS)
     s.grad_many(y, primal, g)
     s.grad_many(y, {k: v.expand(NRHS, *v.shape).contiguous() for k, v in primal.items()}, g_each)
     assert all(torch.equal(g[k], g_adj[k]) and torch.equal(g_each[k], g_adj[k]) for k in RECS)
     # the calls read and write nothing of the handle's
-    after = _outputs(gar, s)
+    after = lq_gpu.outputs(gar, s)
     assert all(np.array_equal(before[k], after[k]) for k in before) and s.factor_epoch() == epoch
     assert s.launch_count() > launches
     s.close()
@@ -106,10 +110,10 @@ def test_kernels_against_numpy_and_bits(env, name, kw, dims, each1, each2):
 
 def test_errors_launch_nothing(env):
     gar, _, torch = env
-    s, _ = _setup(env, {}, (4, 2, 2, 2, 4, 6, 9), 3, MU)
-    primal = _primal(env, s)
-    dot, a = _dots(env, s, 2, 1), _cots(env, s, primal, 2, 2)
-    out, grad = _sol_bufs(env, primal, 2), _grad_bufs(env, s, 2)
+    s, _ = lq_gpu.setup(env, {}, (4, 2, 2, 2, 4, 6, 9), 3, MU)
+    primal = lq_gpu.primal(env, s)
+    dot, a = lq_gpu.dots(env, s, 2, 1), lq_gpu.cots(env, s, primal, 2, 2)
+    out, grad = lq_gpu.sol_bufs(env, primal, 2), lq_gpu.grad_bufs_many(env, s, 2)
     n0 = s.launch_count()
     fill = lambda d, T: C.byref(gar._fill(T(), [f for f, _ in T._fields_], d))
     assert gar.lib().ab2_gar_rho_many(s.h, -1, 1, fill(dot, gar.LqTangent), fill(a, gar.LsIterate), 1, None, None, 0,
@@ -131,13 +135,13 @@ def test_errors_launch_nothing(env):
 def _torch_recs(env, s, recs):
     torch = env[2]
     return [torch.tensor(np.ascontiguousarray(a), device="cuda").reshape(sh)
-            for a, sh in zip(recs, _rec_shapes(s).values())]
+            for a, sh in zip(recs, lq_gpu.rec_shapes(s).values())]
 
 
 @pytest.mark.parametrize("kw", [{}, dict(variant=9)], ids=["warp", "cta_v9"])
 def test_first_derivatives_bit_equal_lq_solve(env, kw):
     _, ag, torch = env
-    s, recs = _setup(env, kw, (4, 2, 2, 2, 4, 5, 6), 7, MU)
+    s, recs = lq_gpu.setup(env, kw, (4, 2, 2, 2, 4, 5, 6), 7, MU)
     P = _torch_recs(env, s, recs)
     for k in (0, 1, 5):
         for i in (0, 1, 2, 3):
@@ -206,7 +210,7 @@ def test_full_size_hvp(env):
     instances sampled across the launch."""
     _, ag, torch = env
     dims, mu, V = (12, 6, 0, 0, 12, 100, 4096), 1e-2, 8
-    s, recs = _setup(env, {}, dims, 2, mu)
+    s, recs = lq_gpu.setup(env, {}, dims, 2, mu)
     P = _torch_recs(env, s, recs)
     outs = ag.lq_solve(s, *P, mu)
     g = torch.Generator(device="cuda").manual_seed(6)

@@ -13,17 +13,20 @@ import pytest
 import gen
 import hp_reference as hp
 import lq_adjoint_ref as aref
-import test_gpu_factor_adjoint as gfa
-import test_gpu_factor_tangent as gft
+import lq_factor_adjoint_ref as fadj
+import lq_gpu
 from aligator_b200.lqr import LqrKnot, LqrProblem
-from test_gpu_adjoint import _grad_bufs, _np, _primal, env  # noqa: F401  (env is the module fixture)
-from test_hp_derivatives import Case, check_bar, symmetric_dot
-from test_hp_emulation import run_oracle as run_solver
+from lq_cases import Case, check_bar, run_solver, symmetric_dot
 
 pytestmark = pytest.mark.gpu
 
 DEFAULT, CTA, DENSE = {}, dict(variant=9), dict(dense=True)
 WARP = [dict(variant=v) for v in (0, 1, 2, 3, 4, 5, 6, 7, 8, 10)]
+
+
+@pytest.fixture(scope="module")
+def env():
+    return lq_gpu.gpu_env()
 
 
 def kw_id(kw):
@@ -136,14 +139,14 @@ def run_adjoint_tangent(env, c, kw):
     """(gradient records of adjoint, zdot of tangent) of one handle on the case's cotangent and tangent."""
     _, _, torch = env
     s = _handle(env, c, kw)
-    primal = {k: v.clone() for k, v in _primal(env, s).items()}
-    g = _grad_bufs(env, s)
+    primal = {k: v.clone() for k, v in lq_gpu.primal(env, s).items()}
+    g = lq_gpu.grad_bufs(env, s)
     s.adjoint(primal, _devs(torch, c.cot), g, _mu_arg(torch, c.mu))
     s.synchronize()
-    g = _np(g)
+    g = lq_gpu.to_np(g)
     s.tangent(primal, _devs(torch, c.dot), _mu_arg(torch, c.mu))
     s.synchronize()
-    zd = _np(_primal(env, s))
+    zd = lq_gpu.to_np(lq_gpu.primal(env, s))
     s.close()
     return g, zd
 
@@ -215,17 +218,17 @@ def test_many_rhs_meet_the_bar(env, name, kw):
         nx, nu, nc = c0.d6[:3]
         assert gar.stage_record_doubles(nx, nu, nc) == int(name[3:])
     s = _handle(env, c0, kw)
-    primal = {k: v.clone() for k, v in _primal(env, s).items()}
+    primal = {k: v.clone() for k, v in lq_gpu.primal(env, s).items()}
     stack = lambda ds: {k: _dev(torch, np.stack([d[k] for d in ds])) for k in ds[0]}
     nan = lambda shape: torch.full(shape, float("nan"), dtype=torch.float64, device="cuda")
     work = {k: nan((nrhs,) + tuple(v.shape)) for k, v in primal.items()}
-    grad = {k: nan((nrhs,) + tuple(v.shape)) for k, v in _grad_bufs(env, s).items()}
+    grad = {k: nan((nrhs,) + tuple(v.shape)) for k, v in lq_gpu.grad_bufs(env, s).items()}
     s.adjoint_many(primal, stack(cots), work, grad, mu)
     twork = {k: nan((nrhs,) + tuple(v.shape)) for k, v in primal.items()}
     out = {k: nan((nrhs,) + tuple(v.shape)) for k, v in primal.items()}
     s.tangent_many(primal, stack(dots), twork, out, mu)
     s.synchronize()
-    G, Z = _np(grad), _np(out)
+    G, Z = lq_gpu.to_np(grad), lq_gpu.to_np(out)
     s.close()
     for j, c in cases.items():
         e_ref = c.e_refs()
@@ -247,8 +250,8 @@ def run_factor(env, c, kw, recs=None):
     s.set_problem(*[np.ascontiguousarray(a) for a in c.recs])
     s.backward(_mu_arg(torch, c.mu))
     assert np.all(s.status() == 0)
-    g = gfa._run(env, s, c.fcot, c.mu, d6)
-    t = gft._run(env, s, dict(stage=c.dot["stage"], term=c.dot["term"]), c.mu, d6)
+    g = lq_gpu.device_factor_adjoint(env, s, c.fcot, c.mu, d6)
+    t = lq_gpu.device_factor_tangent(env, s, dict(stage=c.dot["stage"], term=c.dot["term"]), c.mu, d6)
     s.close()
     return g, t
 
@@ -323,8 +326,8 @@ def test_factor_derivatives_after_cycle_append(env):
     rotated = Case(problems_from_records(*recs, d6), c.mu, inputs=dict(cot=c.cot, fcot=c.fcot, dot=c.dot))
     rotated.hdims = d6
     assert np.array_equal(rotated.recs[0], recs[0]) and np.array_equal(rotated.recs[1], recs[1])
-    g = gfa._run(env, s, c.fcot, c.mu, d6)
-    t = gft._run(env, s, dict(stage=c.dot["stage"], term=c.dot["term"]), c.mu, d6)
+    g = lq_gpu.device_factor_adjoint(env, s, c.fcot, c.mu, d6)
+    t = lq_gpu.device_factor_tangent(env, s, dict(stage=c.dot["stage"], term=c.dot["term"]), c.mu, d6)
     s.close()
     check_factor(rotated, g, t, "cycle_append")
 
@@ -353,23 +356,23 @@ def test_full_size_sampled_instances(env, cfg):
     recs = [a.cpu().numpy() for a in (stage.view(B, N, -1), term, G0, g0)]
     rng = np.random.default_rng(12)
     cot = {k: rng.standard_normal(sh) for k, sh in aref._shapes(d6, B).items()}
-    fcot = {k: rng.standard_normal(sh) for k, sh in gfa.ref.cot_shapes(d6, B).items()}
+    fcot = {k: rng.standard_normal(sh) for k, sh in fadj.cot_shapes(d6, B).items()}
     dot = symmetric_dot(rng, d6, B)
     s = gar.CudaRiccatiBatch(*d6, B)
     s.set_problem(stage, term, G0, g0, memspace=gar.AB2_DEVICE)
     s.sweep(mu)
     assert np.all(s.status() == 0)
-    primal = {k: v.clone() for k, v in _primal(env, s).items()}
-    g = _grad_bufs(env, s)
+    primal = {k: v.clone() for k, v in lq_gpu.primal(env, s).items()}
+    g = lq_gpu.grad_bufs(env, s)
     s.adjoint(primal, {k: _dev(torch, v) for k, v in cot.items()}, g, mu)
     s.synchronize()
-    g = _np(g)
+    g = lq_gpu.to_np(g)
     s.tangent(primal, {k: _dev(torch, v) for k, v in dot.items()}, mu)
     s.synchronize()
-    zd = _np(_primal(env, s))
+    zd = lq_gpu.to_np(lq_gpu.primal(env, s))
     s.backward(mu)
-    gf = gfa._run(env, s, fcot, mu, d6)
-    ft = gft._run(env, s, dict(stage=dot["stage"], term=dot["term"]), mu, d6)
+    gf = lq_gpu.device_factor_adjoint(env, s, fcot, mu, d6)
+    ft = lq_gpu.device_factor_tangent(env, s, dict(stage=dot["stage"], term=dot["term"]), mu, d6)
     s.close()
     pick = lambda d: {k: np.asarray(v)[idx] for k, v in d.items()}
     c = Case(problems_from_records(*[a[idx] for a in recs], d6), mu,

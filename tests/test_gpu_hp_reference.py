@@ -10,7 +10,7 @@ import pytest
 
 import gen
 import hp_reference as hp
-from test_hp_emulation import families, run_oracle
+from lq_cases import families, run_solver
 
 pytestmark = pytest.mark.gpu
 
@@ -84,7 +84,7 @@ def case(name):
     dims, B, mueq, _, _ = CASES[name]
     probs = make_problems(name)
     ref, _ = hp.solve(probs, mueq)
-    return probs, ref, hp.error_families(run_oracle(probs, dims, mueq), ref, dims[1], dims[2], dims[4])
+    return probs, ref, hp.error_families(run_solver(probs, dims, mueq), ref, dims[1], dims[2], dims[4])
 
 
 @functools.lru_cache(maxsize=None)
@@ -95,7 +95,7 @@ def oracle_errors(name, algorithm):
     probs, ref, e = case(name)
     if algorithm == "serial":
         return e
-    own = hp.error_families(run_oracle(probs, dims, mueq, algorithm), ref, dims[1], dims[2], dims[4])
+    own = hp.error_families(run_solver(probs, dims, mueq, algorithm), ref, dims[1], dims[2], dims[4])
     return {f: max(v, e[f]) for f, v in own.items()}
 
 
@@ -157,7 +157,7 @@ def test_full_size_c2_sampled_instances(gar):
     st, tm, g0m, g0v = (a.cpu().numpy() for a in (stage, term, G0, g0))
     probs = [unpack(st[b].reshape(N, -1), tm[b], g0m[b], g0v[b], nx, nu) for b in idx]
     ref, _ = hp.solve(probs, mueq)
-    e_oracle = hp.error_families(run_oracle(probs, (nx, nu, 0, 0, N), mueq), ref, nu, 0, N)
+    e_oracle = hp.error_families(run_solver(probs, (nx, nu, 0, 0, N), mueq), ref, nu, 0, N)
     e_kernel = hp.error_families(got, ref, nu, 0, N)
     print("\n" + hp.table("C2 full size, 16 sampled instances", e_oracle, e_kernel))
     assert not hp.violations(e_kernel, e_oracle), hp.table("C2", e_oracle, e_kernel)

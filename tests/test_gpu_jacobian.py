@@ -10,10 +10,10 @@ import pytest
 
 import gen
 import lq_adjoint_ref as aref
+import lq_gpu
 import lq_tangent_ref as tref
 from oracle import gar_oracle as orc
-from test_gpu_adjoint import HANDLES, MUS, _outputs, _primal, _setup, env  # noqa: F401  (env is the module fixture)
-from test_gpu_resolve import SERIAL
+from lq_gpu import MUS, SERIAL
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-10
@@ -21,46 +21,15 @@ KEYS = aref.KEYS
 RECS = ("stage", "term", "G0", "g0")
 
 
-def _rec_shapes(s):
-    d = s.dims
-    return dict(stage=(d.batch, d.horizon, s.srec), term=(d.batch, s.trec), G0=(d.batch, d.nc0 * d.nx),
-                g0=(d.batch, d.nc0))
-
-
-def _randn(torch, shape, seed):
-    g = torch.Generator(device="cuda")
-    g.manual_seed(seed)
-    return torch.randn(shape, generator=g, dtype=torch.float64, device="cuda")
-
-
-def _cots(env, s, primal, nrhs, seed):
-    return {k: _randn(env[2], (nrhs,) + tuple(v.shape), seed + i) for i, (k, v) in enumerate(primal.items())}
-
-
-def _dots(env, s, nrhs, seed):
-    return {k: _randn(env[2], (nrhs,) + sh, seed + i) for i, (k, sh) in enumerate(_rec_shapes(s).items())}
-
-
-def _nan(torch, shape):
-    return torch.full(shape, float("nan"), dtype=torch.float64, device="cuda")
-
-
-def _sol_bufs(env, primal, nrhs):
-    return {k: _nan(env[2], (nrhs,) + tuple(v.shape)) for k, v in primal.items()}
-
-
-def _grad_bufs(env, s, nrhs):
-    return {k: _nan(env[2], (nrhs,) + sh) for k, sh in _rec_shapes(s).items()}
+@pytest.fixture(scope="module")
+def env():
+    return lq_gpu.gpu_env()
 
 
 def _trajectory(env, s):
     gar = env[0]
     return {k: s.get(w) for k, w in zip(KEYS, (gar.OUT_XS, gar.OUT_US, gar.OUT_VS, gar.OUT_VST, gar.OUT_LBD0,
                                                gar.OUT_LBDAS))}
-
-
-def _np(d):
-    return {k: v.cpu().numpy() for k, v in d.items()}
 
 
 def _oracle(dims, recs, mu):
@@ -91,24 +60,24 @@ def test_parity_with_single_calls_and_oracle(env, name, kw, dims, mu):
     nx, nu, nc, nct, nc0, N, B = dims
     d6 = dims[:6]
     tol = _tols(mu)
-    s, recs = _setup(env, kw, dims, 3, mu)
-    primal = _primal(env, s)
+    s, recs = lq_gpu.setup(env, kw, dims, 3, mu)
+    primal = lq_gpu.primal(env, s)
     nrhs = 3
-    cot, dot = _cots(env, s, primal, nrhs, 11), _dots(env, s, nrhs, 21)
-    work, grad = _sol_bufs(env, primal, nrhs), _grad_bufs(env, s, nrhs)
-    twork, out = _sol_bufs(env, primal, nrhs), _sol_bufs(env, primal, nrhs)
-    before, e0 = _outputs(gar, s), s.factor_epoch()
+    cot, dot = lq_gpu.cots(env, s, primal, nrhs, 11), lq_gpu.dots(env, s, nrhs, 21)
+    work, grad = lq_gpu.sol_bufs(env, primal, nrhs), lq_gpu.grad_bufs_many(env, s, nrhs)
+    twork, out = lq_gpu.sol_bufs(env, primal, nrhs), lq_gpu.sol_bufs(env, primal, nrhs)
+    before, e0 = lq_gpu.outputs(gar, s), s.factor_epoch()
     s.adjoint_many(primal, cot, work, grad, mu)
     s.tangent_many(primal, dot, twork, out, mu)
     s.synchronize()
-    after = _outputs(gar, s)
+    after = lq_gpu.outputs(gar, s)
     for k, a in before.items():  # every handle output is bit-equal before and after, and the epoch does not move
         assert np.array_equal(a, after[k], equal_nan=True), (name, k)
     assert s.factor_epoch() == e0
-    G, Y, Z = _np(grad), _np(work), _np(out)
+    G, Y, Z = lq_gpu.to_np(grad), lq_gpu.to_np(work), lq_gpu.to_np(out)
     assert np.all(G["stage"][..., aref.stage_offsets(nx, nu, nc)[0]["d"][1]:] == 0.0)  # the pad double
     zo = _oracle(dims, recs, mu)
-    pn = _np(primal)
+    pn = lq_gpu.to_np(primal)
     for j in range(nrhs):
         cj = {k: v[j].cpu().numpy() for k, v in cot.items()}
         dj = {k: v[j].cpu().numpy() for k, v in dot.items()}
@@ -119,9 +88,9 @@ def test_parity_with_single_calls_and_oracle(env, name, kw, dims, mu):
         zd = _oracle(dims, tref.tangent_records(*recs, dj, zo, d6), mu)
         _close({k: v[j] for k, v in Z.items()}, zd, tol, (name, mu, j, "zdot/oracle"))
         # against separate single calls
-        g1 = {k: torch.empty(sh, dtype=torch.float64, device="cuda") for k, sh in _rec_shapes(s).items()}
+        g1 = {k: torch.empty(sh, dtype=torch.float64, device="cuda") for k, sh in lq_gpu.rec_shapes(s).items()}
         s.adjoint(primal, {k: v[j] for k, v in cot.items()}, g1, mu)
-        _close({k: v[j] for k, v in G.items()}, _np(g1), tol, (name, mu, j, "grad/adjoint"))
+        _close({k: v[j] for k, v in G.items()}, lq_gpu.to_np(g1), tol, (name, mu, j, "grad/adjoint"))
         s.tangent(primal, {k: v[j] for k, v in dot.items()}, mu)
         _close({k: v[j] for k, v in Z.items()}, _trajectory(env, s), tol, (name, mu, j, "zdot/tangent"))
     s.close()
@@ -133,18 +102,18 @@ def test_bits_null_fields_and_v_twins(env, name, kw, dims):
     gar, _, torch = env
     B = dims[-1]
     mu = 1e-2
-    s, _ = _setup(env, kw, dims, 7, mu)
-    primal = _primal(env, s)
-    cot, dot = _cots(env, s, primal, 5, 31), _dots(env, s, 5, 41)
-    work, grad = _sol_bufs(env, primal, 5), _grad_bufs(env, s, 5)
-    twork, out = _sol_bufs(env, primal, 5), _sol_bufs(env, primal, 5)
+    s, _ = lq_gpu.setup(env, kw, dims, 7, mu)
+    primal = lq_gpu.primal(env, s)
+    cot, dot = lq_gpu.cots(env, s, primal, 5, 31), lq_gpu.dots(env, s, 5, 41)
+    work, grad = lq_gpu.sol_bufs(env, primal, 5), lq_gpu.grad_bufs_many(env, s, 5)
+    twork, out = lq_gpu.sol_bufs(env, primal, 5), lq_gpu.sol_bufs(env, primal, 5)
     s.adjoint_many(primal, cot, work, grad, mu)
     s.tangent_many(primal, dot, twork, out, mu)
     # right-hand side j's results do not depend on nrhs or on j's position
     for j in (0, 2, 4):
-        w1, g1 = _sol_bufs(env, primal, 1), _grad_bufs(env, s, 1)
+        w1, g1 = lq_gpu.sol_bufs(env, primal, 1), lq_gpu.grad_bufs_many(env, s, 1)
         s.adjoint_many(primal, {k: v[j:j + 1].contiguous() for k, v in cot.items()}, w1, g1, mu)
-        tw1, o1 = _sol_bufs(env, primal, 1), _sol_bufs(env, primal, 1)
+        tw1, o1 = lq_gpu.sol_bufs(env, primal, 1), lq_gpu.sol_bufs(env, primal, 1)
         s.tangent_many(primal, {k: v[j:j + 1].contiguous() for k, v in dot.items()}, tw1, o1, mu)
         for k in RECS:
             assert torch.equal(g1[k][0], grad[k][j]), (name, j, k)
@@ -154,23 +123,23 @@ def test_bits_null_fields_and_v_twins(env, name, kw, dims):
     # NULL grad fields are not written; NULL cotangent and tangent fields are zeros
     part = {k: v[:2].contiguous() if k in ("xs", "lam0") else None for k, v in cot.items()}
     zeros = {k: v if v is not None else torch.zeros_like(cot[k][:2]) for k, v in part.items()}
-    ga, gb = _grad_bufs(env, s, 2), _grad_bufs(env, s, 2)
-    s.adjoint_many(primal, part, _sol_bufs(env, primal, 2), dict(stage=ga["stage"], g0=ga["g0"]), mu)
-    s.adjoint_many(primal, zeros, _sol_bufs(env, primal, 2), gb, mu)
+    ga, gb = lq_gpu.grad_bufs_many(env, s, 2), lq_gpu.grad_bufs_many(env, s, 2)
+    s.adjoint_many(primal, part, lq_gpu.sol_bufs(env, primal, 2), dict(stage=ga["stage"], g0=ga["g0"]), mu)
+    s.adjoint_many(primal, zeros, lq_gpu.sol_bufs(env, primal, 2), gb, mu)
     assert torch.equal(ga["stage"], gb["stage"]) and torch.equal(ga["g0"], gb["g0"])
     assert torch.isnan(ga["term"]).all() and torch.isnan(ga["G0"]).all()
     tpart = {k: v[:2].contiguous() if k in ("term", "G0") else None for k, v in dot.items()}
     tzeros = {k: v if v is not None else torch.zeros_like(dot[k][:2]) for k, v in tpart.items()}
-    oa, ob = _sol_bufs(env, primal, 2), _sol_bufs(env, primal, 2)
-    s.tangent_many(primal, tpart, _sol_bufs(env, primal, 2), oa, mu)
-    s.tangent_many(primal, tzeros, _sol_bufs(env, primal, 2), ob, mu)
+    oa, ob = lq_gpu.sol_bufs(env, primal, 2), lq_gpu.sol_bufs(env, primal, 2)
+    s.tangent_many(primal, tpart, lq_gpu.sol_bufs(env, primal, 2), oa, mu)
+    s.tangent_many(primal, tzeros, lq_gpu.sol_bufs(env, primal, 2), ob, mu)
     for k in KEYS:
         assert torch.equal(oa[k], ob[k]), (name, k)
     # the _v twins equal the scalar calls, with mu in host and in device memory
     for m in (np.full(B, mu), torch.full((B,), mu, dtype=torch.float64, device="cuda")):
-        wv, gv = _sol_bufs(env, primal, 5), _grad_bufs(env, s, 5)
+        wv, gv = lq_gpu.sol_bufs(env, primal, 5), lq_gpu.grad_bufs_many(env, s, 5)
         s.adjoint_many(primal, cot, wv, gv, m)
-        tv, ov = _sol_bufs(env, primal, 5), _sol_bufs(env, primal, 5)
+        tv, ov = lq_gpu.sol_bufs(env, primal, 5), lq_gpu.sol_bufs(env, primal, 5)
         s.tangent_many(primal, dot, tv, ov, m)
         for k in RECS:
             assert torch.equal(gv[k], grad[k]), (name, k)
@@ -185,11 +154,11 @@ def test_duality_on_device(env, name, kw, dims):
     """<zbar_i, zdot_j> = <grad_i, pdot_j> for 3 x 3 pairs."""
     gar, _, torch = env
     mu = 1e-2
-    s, _ = _setup(env, kw, dims, 9, mu)
-    primal = _primal(env, s)
-    cot, dot = _cots(env, s, primal, 3, 51), _dots(env, s, 3, 61)
-    work, grad = _sol_bufs(env, primal, 3), _grad_bufs(env, s, 3)
-    twork, out = _sol_bufs(env, primal, 3), _sol_bufs(env, primal, 3)
+    s, _ = lq_gpu.setup(env, kw, dims, 9, mu)
+    primal = lq_gpu.primal(env, s)
+    cot, dot = lq_gpu.cots(env, s, primal, 3, 51), lq_gpu.dots(env, s, 3, 61)
+    work, grad = lq_gpu.sol_bufs(env, primal, 3), lq_gpu.grad_bufs_many(env, s, 3)
+    twork, out = lq_gpu.sol_bufs(env, primal, 3), lq_gpu.sol_bufs(env, primal, 3)
     s.adjoint_many(primal, cot, work, grad, mu)
     s.tangent_many(primal, dot, twork, out, mu)
     for i in range(3):
@@ -207,27 +176,27 @@ def test_cycle_append(env):
     dims = (4, 2, 2, 2, 4, 6, 9)
     nx, nu, nc, nct, nc0, N, B = dims
     mu = 1e-2
-    s, _ = _setup(env, {}, dims, 1, mu)
+    s, _ = lq_gpu.setup(env, {}, dims, 1, mu)
     new_last = np.ascontiguousarray(gen.stage_record(gen.generate_batch(9, 1, 1, nx, nu, nc, nct)[0].stages[0]))
     nl = np.zeros((B, s.srec))
     nl[:, :new_last.size] = new_last
     s.cycle_append(nl)
-    primal = _primal(env, s)
-    cot, dot = _cots(env, s, primal, 2, 71), _dots(env, s, 2, 81)
+    primal = lq_gpu.primal(env, s)
+    cot, dot = lq_gpu.cots(env, s, primal, 2, 71), lq_gpu.dots(env, s, 2, 81)
     with pytest.raises(gar.GarError):  # no backward since cycle_append
-        s.adjoint_many(primal, cot, _sol_bufs(env, primal, 2), _grad_bufs(env, s, 2), mu)
+        s.adjoint_many(primal, cot, lq_gpu.sol_bufs(env, primal, 2), lq_gpu.grad_bufs_many(env, s, 2), mu)
     s.sweep(mu)
-    primal = _primal(env, s)
-    work, grad = _sol_bufs(env, primal, 2), _grad_bufs(env, s, 2)
-    twork, out = _sol_bufs(env, primal, 2), _sol_bufs(env, primal, 2)
+    primal = lq_gpu.primal(env, s)
+    work, grad = lq_gpu.sol_bufs(env, primal, 2), lq_gpu.grad_bufs_many(env, s, 2)
+    twork, out = lq_gpu.sol_bufs(env, primal, 2), lq_gpu.sol_bufs(env, primal, 2)
     s.adjoint_many(primal, cot, work, grad, mu)
     s.tangent_many(primal, dot, twork, out, mu)
     for j in range(2):
-        g1 = {k: torch.empty(sh, dtype=torch.float64, device="cuda") for k, sh in _rec_shapes(s).items()}
+        g1 = {k: torch.empty(sh, dtype=torch.float64, device="cuda") for k, sh in lq_gpu.rec_shapes(s).items()}
         s.adjoint(primal, {k: v[j] for k, v in cot.items()}, g1, mu)
-        _close({k: v[j] for k, v in _np(grad).items()}, _np(g1), _tols(mu), j)
+        _close({k: v[j] for k, v in lq_gpu.to_np(grad).items()}, lq_gpu.to_np(g1), _tols(mu), j)
         s.tangent(primal, {k: v[j] for k, v in dot.items()}, mu)
-        _close({k: v[j] for k, v in _np(out).items()}, _trajectory(env, s), _tols(mu), j)
+        _close({k: v[j] for k, v in lq_gpu.to_np(out).items()}, _trajectory(env, s), _tols(mu), j)
     s.close()
 
 
@@ -260,8 +229,8 @@ def test_state_and_errors(env):
     cot = {k: torch.zeros((2,) + sh, dtype=torch.float64, device="cuda") for k, sh in shapes.items()}
     work = {k: torch.zeros((2,) + sh, dtype=torch.float64, device="cuda") for k, sh in shapes.items()}
     out = {k: torch.zeros((2,) + sh, dtype=torch.float64, device="cuda") for k, sh in shapes.items()}
-    grad = {k: torch.zeros((2,) + sh, dtype=torch.float64, device="cuda") for k, sh in _rec_shapes(s).items()}
-    dot = {k: torch.zeros((2,) + sh, dtype=torch.float64, device="cuda") for k, sh in _rec_shapes(s).items()}
+    grad = {k: torch.zeros((2,) + sh, dtype=torch.float64, device="cuda") for k, sh in lq_gpu.rec_shapes(s).items()}
+    dot = {k: torch.zeros((2,) + sh, dtype=torch.float64, device="cuda") for k, sh in lq_gpu.rec_shapes(s).items()}
     adj = lambda **kw: _rc_adj(gar, s, kw.get("mu", mu), kw.get("nrhs", 2), kw.get("primal", primal), kw.get("cot", cot),
                                kw.get("work", work), kw.get("grad", grad))
     tan = lambda **kw: _rc_tan(gar, s, kw.get("mu", mu), kw.get("nrhs", 2), kw.get("primal", primal), kw.get("dot", dot),
@@ -318,12 +287,12 @@ def test_torch_func(env, dense):
     dims = (4, 2, 2, 2, 4, 3, 2)
     nx, nu, nc, nct, nc0, N, B = dims
     mu = 1e-2
-    s, recs = _setup(env, dict(dense=dense), dims, 13, mu)
+    s, recs = lq_gpu.setup(env, dict(dense=dense), dims, 13, mu)
     calls = {}
     for n in ("adjoint", "tangent", "adjoint_many", "tangent_many"):
         _counting(s, n, calls)
     stage, term, G0, g0 = [torch.tensor(np.ascontiguousarray(a), device="cuda").reshape(sh)
-                           for a, sh in zip(recs, _rec_shapes(s).values())]
+                           for a, sh in zip(recs, lq_gpu.rec_shapes(s).values())]
     for k in (0, 1, 5):  # xs, us, lams
         f = lambda st: ag.lq_solve(s, st, term, G0, g0, mu)[k]
         calls.clear()
@@ -400,23 +369,23 @@ def test_full_size(env, dims):
     nx, nu, nc, nct, nc0, N, B = dims
     mu = 1e-2
     nrhs = 4
-    s, _ = _setup(env, {}, dims, 2, mu)
-    primal = _primal(env, s)
+    s, _ = lq_gpu.setup(env, {}, dims, 2, mu)
+    primal = lq_gpu.primal(env, s)
     idx = torch.tensor(np.r_[0:3, B // 2 - 2:B // 2 + 2, B - 5:B], device="cuda")  # first wave, a wave boundary, the tail
-    cot = _cots(env, s, primal, nrhs, 91)
-    work, grad = _sol_bufs(env, primal, nrhs), _grad_bufs(env, s, nrhs)
+    cot = lq_gpu.cots(env, s, primal, nrhs, 91)
+    work, grad = lq_gpu.sol_bufs(env, primal, nrhs), lq_gpu.grad_bufs_many(env, s, nrhs)
     s.adjoint_many(primal, cot, work, grad, mu)
     sub = {k: v[:, idx].cpu().numpy() for k, v in grad.items()}
     del work, grad
     for j in (0, nrhs - 1):
-        g1 = {k: torch.empty(sh, dtype=torch.float64, device="cuda") for k, sh in _rec_shapes(s).items()}
+        g1 = {k: torch.empty(sh, dtype=torch.float64, device="cuda") for k, sh in lq_gpu.rec_shapes(s).items()}
         s.adjoint(primal, {k: v[j] for k, v in cot.items()}, g1, mu)
         _close({k: v[j] for k, v in sub.items()}, {k: v[idx].cpu().numpy() for k, v in g1.items()}, _tols(mu), j)
         del g1
     del cot
     torch.cuda.empty_cache()
-    dot = _dots(env, s, nrhs, 93)
-    work, out = _sol_bufs(env, primal, nrhs), _sol_bufs(env, primal, nrhs)
+    dot = lq_gpu.dots(env, s, nrhs, 93)
+    work, out = lq_gpu.sol_bufs(env, primal, nrhs), lq_gpu.sol_bufs(env, primal, nrhs)
     s.tangent_many(primal, dot, work, out, mu)
     for j in (0, nrhs - 1):
         s.tangent(primal, {k: v[j] for k, v in dot.items()}, mu)

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import gen
+import lq_gpu
 from oracle import gar_oracle as orc
 from oracle import fddp as of
 
@@ -29,13 +30,6 @@ def _problem(gar, nx, nu, N, B, seed):
     bo = orc.BatchedOracle(nx, nu, 0, 0, nx, N, B, *packed)
     bo.sweep(1e-8)
     return probs, packed, bo.get()
-
-
-class _DeviceArray:
-    """A raw device pointer of n doubles, readable by torch.as_tensor."""
-
-    def __init__(self, ptr, n):
-        self.__cuda_array_interface__ = dict(shape=(n,), typestr="<f8", data=(ptr, False), version=2)
 
 
 def _expand(raw, B, N, nx):
@@ -76,7 +70,7 @@ def test_getters_and_raw_layout(gar, shape):
         assert np.array_equal(a.reshape(nb, nt, nx, nx).transpose(0, 1, 3, 2), V[b0:b0 + nb, t0:t0 + nt])
     P = (nx * (nx + 1) // 2 + 1) & ~1
     n = B * (N + 1) * P + B * nx * nx
-    raw = torch.as_tensor(_DeviceArray(s.device_ptr(gar.OUT_VXX), n), device="cuda:0")
+    raw = torch.as_tensor(lq_gpu.DeviceArray(s.device_ptr(gar.OUT_VXX), n), device="cuda:0")
     torch.cuda.synchronize()
     assert np.array_equal(_expand(raw.cpu().numpy(), B, N, nx), V)  # the documented raw layout, by hand
     s.close()
@@ -140,9 +134,9 @@ def test_variant_switch_between_backward_and_forward(gar, first, second):
 
 def test_fddp_vx_reads_either_layout(gar):
     import torch
-    from test_fddp import _random_fddp
+    from inner_cases import random_fddp
     nx, nu, N, B = 12, 6, 15, 4
-    d = _random_fddp(np.random.default_rng(3), B, N, nx, nu)
+    d = random_fddp(np.random.default_rng(3), B, N, nx, nu)
     dev = torch.device("cuda:0")
     cm = lambda a: np.ascontiguousarray(np.swapaxes(a, -1, -2))
     arr = {k: torch.tensor(cm(d[k]) if d[k].ndim >= 3 and k not in ("fs", "Lx", "Lu", "Lx_N") else d[k], device=dev)

@@ -596,9 +596,9 @@ def test_kkt_error_of_every_instance_at_full_size(gar):
 def test_parametric_problems(gar, shape):
     """nth > 0 (riccati-kernel.hxx:185-192, 278-311; proximal-riccati.hxx:50-59; forward with theta)
     through the Python mirror of ProximalRiccatiSolver, against the oracle."""
-    import test_block_parametric as tp
+    import lq_cases
     nx, nu, nc, nct, nth, N, mueq = shape
-    probs = [tp.make_problem(50 + b, N, nx, nu, nc, nct, nth) for b in range(3)]
+    probs = [lq_cases.make_problem(50 + b, N, nx, nu, nc, nct, nth) for b in range(3)]
     solver = gar.ProximalRiccatiSolver(probs)
     assert solver.backward(mueq)
     thetas = np.random.default_rng(1).standard_normal((3, nth))

@@ -12,15 +12,19 @@ import hp_reference as hp
 import lq_adjoint_ref as aref
 import lq_refine_ref as fref
 import lq_resolve_ref as rref
-from test_gpu_adjoint import HANDLES, _outputs, env  # noqa: F401  (env is the module fixture)
-from test_gpu_packed_vxx import _DeviceArray
-from test_refine_oracle import errors, refine_case, refined_on_oracle
-from test_resolve_oracle import _records
+import lq_gpu
+from lq_cases import batch_records, errors, refine_case, refined_on_oracle
+from lq_gpu import HANDLES
 
 pytestmark = pytest.mark.gpu
 # every kernel kind resolve serves: warp variants (packed Vxx), the CTA kernel, a run-time shape, C5 dims
 KINDS = [h for h in HANDLES if not h[1].get("dense")] + [("c5_dims", {}, (57, 28, 0, 0, 57, 3, 2))]
 KIND_IDS = [h[0] for h in KINDS]
+
+
+@pytest.fixture(scope="module")
+def env():
+    return lq_gpu.gpu_env()
 
 
 def _slack(z):
@@ -97,7 +101,7 @@ def test_norms_state_and_kernel_kinds(env, name, kw, dims):
     nx, nu, nc, nct, nc0, N, B = dims
     mu = 1e-5
     s, recs = _handle(env, kw, dims, 31, mu)
-    before = _outputs(gar, s)
+    before = lq_gpu.outputs(gar, s)
     e0 = s.factor_epoch()
     # steps = 0: the first norm only, the trajectory bit-identical; it equals max(kkt_error) within rounding
     z0 = _traj(gar, s)
@@ -105,7 +109,7 @@ def test_norms_state_and_kernel_kinds(env, name, kw, dims):
     k0 = s.kkt_error(mu).max(axis=1)
     assert n0.shape == (B, 1)
     assert np.allclose(n0[:, 0], k0, rtol=0, atol=_slack(z0)), (n0[:, 0], k0)
-    after0 = _outputs(gar, s)
+    after0 = lq_gpu.outputs(gar, s)
     for k, a in before.items():
         assert np.array_equal(a, after0[k], equal_nan=True), (name, k)
     # two steps: the first column repeats, the last equals the kkt error of the refined trajectory
@@ -115,7 +119,7 @@ def test_norms_state_and_kernel_kinds(env, name, kw, dims):
     assert np.allclose(norms[:, -1], s.kkt_error(mu).max(axis=1), rtol=0, atol=_slack(z))
     assert _not_worse(norms[:, -1], norms[:, 0], z), norms
     # every other output bit-identical, the epoch unchanged; the refined trajectory is close to the unrefined one
-    after = _outputs(gar, s)
+    after = lq_gpu.outputs(gar, s)
     for k, a in before.items():
         if k not in range(gar.OUT_XS, gar.OUT_LBDAS + 1):
             assert np.array_equal(a, after[k], equal_nan=True), (name, k)
@@ -150,7 +154,7 @@ def test_kkt_error_is_the_residual_norm(env, dims, general_g0):
             n = s.refine(mu, 0, norms=True)[:, 0]
             assert np.all(np.isfinite(k)) and np.any(k > 0)
             assert np.array_equal(k.max(axis=1).view(np.uint64), n.view(np.uint64)), (ring, k.max(axis=1), n)
-        xs = torch.as_tensor(_DeviceArray(s.device_ptr(gar.OUT_XS), B * (N + 1) * nx), device="cuda")
+        xs = torch.as_tensor(lq_gpu.DeviceArray(s.device_ptr(gar.OUT_XS), B * (N + 1) * nx), device="cuda")
         xs[(1 * (N + 1) + N // 2) * nx] = float("nan")  # instance 1, knot N / 2, x[0]
         torch.cuda.synchronize()
         kn = s.kkt_error(mu)
@@ -228,7 +232,7 @@ def test_refine_many_on_resolve_outputs_meets_the_bar(env, name):
     s.refine_many(hd, z, _work(env, case, B, 2), mu, steps=2)
     for j in range(2):
         rp = rref.replaced_problems(probs, {k: v[j] for k, v in h.items()})
-        rr = [np.ascontiguousarray(a) for a in _records(rp, case)]
+        rr = [np.ascontiguousarray(a) for a in batch_records(rp, case)]
         zc, _, _, want, _ = refined_on_oracle(rp, rr, case, mu)
         e_ref = errors(zc, want, case)
         e = errors({k: v[j:j + 1].cpu().numpy() for k, v in z.items()}, want, case)

@@ -10,25 +10,19 @@ import pytest
 
 import gen
 import lq_adjoint_ref as aref
+import lq_gpu
 import lq_resolve_ref as ref
 from oracle import gar_oracle as orc
-from test_gpu_adjoint import HANDLES, MUS, _outputs, env  # noqa: F401  (env is the module fixture)
-from test_resolve_oracle import BAR_CASES, bar_case, bar_violations
+from lq_cases import BAR_CASES, bar_case, bar_violations
+from lq_gpu import MUS, SERIAL
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-10
-SERIAL = [h for h in HANDLES if not h[1].get("dense")]
 
 
-def _setup(env, kw, dims, seed, mu):
-    gar, _, _ = env
-    nx, nu, nc, nct, nc0, N, B = dims
-    probs = gen.generate_batch(seed, B, N, nx, nu, nc, nct)
-    recs = [np.ascontiguousarray(a) for a in gar.pack_problems(probs)]
-    s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B, **kw)
-    s.set_problem(*recs)
-    s.sweep(mu)
-    return s, recs
+@pytest.fixture(scope="module")
+def env():
+    return lq_gpu.gpu_env()
 
 
 def _dev_rhs(env, h):
@@ -40,10 +34,6 @@ def _out(env, d6, B, nrhs):
     _, _, torch = env
     return {k: torch.full((nrhs,) + s, float("nan"), dtype=torch.float64, device="cuda")
             for k, s in zip(ref.SOL, ref.rhs_shapes(d6, B).values())}
-
-
-def _np(z):
-    return {k: v.cpu().numpy() for k, v in z.items()}
 
 
 def _oracle_replaced(recs, hj, d6, B, mu):
@@ -65,17 +55,17 @@ def _close(z, want, tol, what, tol_vsT=None):
 def test_parity_with_oracle(env, name, kw, dims, mu):
     nx, nu, nc, nct, nc0, N, B = dims
     d6 = dims[:6]
-    s, recs = _setup(env, kw, dims, 3, mu)
-    before = _outputs(env[0], s)
+    s, recs = lq_gpu.setup(env, kw, dims, 3, mu)
+    before = lq_gpu.outputs(env[0], s)
     h = ref.random_rhs(np.random.default_rng(4), d6, B, 3)
     out = _out(env, d6, B, 3)
     s.resolve(_dev_rhs(env, h), out, mu)
-    z = _np(out)
+    z = lq_gpu.to_np(out)
     # v_N = (d_N + C_N x_N) / mu: x_N's rounding error reaches the terminal multipliers amplified by 1 / mu
     for j in range(3):
         _close({k: v[j] for k, v in z.items()}, _oracle_replaced(recs, {k: v[j] for k, v in h.items()}, d6, B, mu),
                TOL, (name, mu, j), tol_vsT=max(TOL, 1e-13 / mu))
-    after = _outputs(env[0], s)
+    after = lq_gpu.outputs(env[0], s)
     for k, a in before.items():  # every handle output is bit-equal before and after
         assert np.array_equal(a, after[k], equal_nan=True), (name, k)
     s.close()
@@ -88,7 +78,7 @@ def test_consistency_with_sweep_adjoint_tangent(env, name, kw, dims):
     nx, nu, nc, nct, nc0, N, B = dims
     d6 = dims[:6]
     mu = 1e-2
-    s, recs = _setup(env, kw, dims, 5, mu)
+    s, recs = lq_gpu.setup(env, kw, dims, 5, mu)
     primal = {k: torch.tensor(s.get(w), device="cuda") for k, w in zip(
         aref.KEYS, (gar.OUT_XS, gar.OUT_US, gar.OUT_VS, gar.OUT_VST, gar.OUT_LBD0, gar.OUT_LBDAS))}
     stage, term, G0, g0 = recs
@@ -100,7 +90,7 @@ def test_consistency_with_sweep_adjoint_tangent(env, name, kw, dims):
                dN=term[:, to["d"][0]:to["d"][1]], g0=g0, f=vec("f"))
     out = _out(env, d6, B, 1)
     s.resolve(_dev_rhs(env, {k: v[None] for k, v in own.items()}), out, mu)
-    _close({k: v[0] for k, v in _np(out).items()}, {k: v.cpu().numpy() for k, v in primal.items()}, 1e-12, "primal")
+    _close({k: v[0] for k, v in lq_gpu.to_np(out).items()}, {k: v.cpu().numpy() for k, v in primal.items()}, 1e-12, "primal")
     # -zbar gives the adjoint's trajectory
     rng = np.random.default_rng(6)
     zbar = {k: torch.tensor(rng.standard_normal(tuple(v.shape)), device="cuda") for k, v in primal.items()}
@@ -112,7 +102,7 @@ def test_consistency_with_sweep_adjoint_tangent(env, name, kw, dims):
     s.adjoint(primal, zbar, grad, mu)
     w = {k: s.get(wh) for k, wh in zip(ref.SOL, (gar.OUT_XS, gar.OUT_US, gar.OUT_VS, gar.OUT_VST, gar.OUT_LBD0,
                                                 gar.OUT_LBDAS))}
-    _close({k: v[0] for k, v in _np(out).items()}, w, TOL, "adjoint")
+    _close({k: v[0] for k, v in lq_gpu.to_np(out).items()}, w, TOL, "adjoint")
     # rho gives the tangent's trajectory (the handle is refactored by the adjoint: same matrices)
     import lq_tangent_ref as tref
     dot = dict(stage=rng.standard_normal((B, N, s.srec)), term=rng.standard_normal((B, s.trec)),
@@ -125,7 +115,7 @@ def test_consistency_with_sweep_adjoint_tangent(env, name, kw, dims):
     s.tangent(primal, _dev_rhs(env, dot), mu)
     zd = {k: s.get(wh) for k, wh in zip(ref.SOL, (gar.OUT_XS, gar.OUT_US, gar.OUT_VS, gar.OUT_VST, gar.OUT_LBD0,
                                                  gar.OUT_LBDAS))}
-    _close({k: v[0] for k, v in _np(out).items()}, zd, TOL, "tangent")
+    _close({k: v[0] for k, v in lq_gpu.to_np(out).items()}, zd, TOL, "tangent")
     s.close()
 
 
@@ -135,7 +125,7 @@ def test_bit_equal_across_nrhs_and_v_twin(env, name, kw, dims):
     nx, nu, nc, nct, nc0, N, B = dims
     d6 = dims[:6]
     mu = 1e-2
-    s, _ = _setup(env, kw, dims, 7, mu)
+    s, _ = lq_gpu.setup(env, kw, dims, 7, mu)
     for nrhs in (3, 32):
         h = _dev_rhs(env, ref.random_rhs(np.random.default_rng(nrhs), d6, B, nrhs))
         out = _out(env, d6, B, nrhs)
@@ -212,7 +202,7 @@ def test_state_and_errors(env):
     term, G0, g0 = [s.get_problem(w).reshape(B, -1) for w in (1, 2, 3)]
     h = ref.random_rhs(np.random.default_rng(2), d6, B, 2)
     s.resolve(_dev_rhs(env, h), out, mu)
-    z = _np(out)
+    z = lq_gpu.to_np(out)
     for j in range(2):
         _close({k: v[j] for k, v in z.items()},
                _oracle_replaced((stage, term, G0, g0), {k: v[j] for k, v in h.items()}, d6, B, mu), TOL, j)
@@ -233,12 +223,12 @@ def test_full_size(env, dims):
     mu = 1e-2
     rng = np.random.default_rng(1)
     nrhs = 4
-    s, recs = _setup(env, {}, dims, 2, mu)
+    s, recs = lq_gpu.setup(env, {}, dims, 2, mu)
     h = ref.random_rhs(rng, d6, B, nrhs)
     out = _out(env, d6, B, nrhs)
     s.resolve(_dev_rhs(env, h), out, mu)
     idx = np.r_[0:3, B // 2 - 2:B // 2 + 2, B - 5:B]  # first wave, a wave boundary, the ragged tail
-    z = _np(out)
+    z = lq_gpu.to_np(out)
     st = recs[0].reshape(B, N, -1)
     sub = [np.ascontiguousarray(a[idx]) for a in (st, recs[1], recs[2].reshape(B, -1), recs[3].reshape(B, -1))]
     for j in (0, nrhs - 1):
@@ -260,7 +250,7 @@ def test_device_meets_the_conditioning_bar(env, name):
     s.sweep(mu)
     out = _out(env, case, B, 2)
     s.resolve(_dev_rhs(env, h), out, mu)
-    z = _np(out)
+    z = lq_gpu.to_np(out)
     for j in range(2):
         bad, tab = bar_violations(probs, recs, case, mu, {k: v[j] for k, v in h.items()}, {k: v[j] for k, v in z.items()})
         assert not bad, "%s rhs %d\n%s" % (name, j, tab)
@@ -273,7 +263,7 @@ def test_torch_entry_point(env):
     nx, nu, nc, nct, nc0, N, B = dims
     d6 = dims[:6]
     mu = 1e-2
-    s, recs = _setup(env, {}, dims, 9, mu)
+    s, recs = lq_gpu.setup(env, {}, dims, 9, mu)
     h = _dev_rhs(env, ref.random_rhs(np.random.default_rng(10), d6, B, 3))
     out = _out(env, d6, B, 3)
     s.resolve(h, out, mu)

@@ -12,8 +12,8 @@ import pytest
 
 import gen
 import lq_adjoint_ref as aref
+import lq_gpu
 import lq_tangent_ref as ref
-import test_gpu_adjoint as ga
 from oracle import gar_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -23,20 +23,14 @@ MUS = (1.0, 1e-2, 1e-5)
 TOL = 1e-10
 KEYS = aref.KEYS
 DOTS = ("stage", "term", "G0", "g0")
-HANDLES = ga.HANDLES
+HANDLES = lq_gpu.HANDLES
 FEW = [HANDLES[0], HANDLES[9], HANDLES[-3], HANDLES[-2], HANDLES[-1]]
 FEW_IDS = ["lane_v0", "mma_12_v7", "cta_v9", "cta_runtime", "dense"]
 
 
 @pytest.fixture(scope="module")
 def env():
-    import torch
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    import __graft_entry__ as g
-    g.build()
-    import aligator_b200.gar as gar
-    import aligator_b200.autograd as ag
-    return gar, ag, torch
+    return lq_gpu.gpu_env()
 
 
 def _tangent(env, s, seed, scale=1.0):
@@ -55,7 +49,7 @@ def _np(d):
 
 
 def _zdot(env, s):
-    return _np(ga._primal(env, s))
+    return _np(lq_gpu.primal(env, s))
 
 
 def _oracle_solve(recs, dims, mu):
@@ -87,10 +81,10 @@ def _equal(a, b):
 @pytest.mark.parametrize("name,kw,dims", HANDLES, ids=[h[0] for h in HANDLES])
 def test_tangent_matches_oracle_and_state_afterwards(env, name, kw, dims, mu):
     gar, _, torch = env
-    s, recs = ga._setup(env, kw, dims, seed=dims[0] * 31 + dims[-1], mu=mu)
-    before = ga._outputs(gar, s)
+    s, recs = lq_gpu.setup(env, kw, dims, seed=dims[0] * 31 + dims[-1], mu=mu)
+    before = lq_gpu.outputs(gar, s)
     problem = [s.get_problem(w).copy() for w in range(4)]
-    primal = ga._primal(env, s)
+    primal = lq_gpu.primal(env, s)
     dot = _tangent(env, s, 1)
     n0 = s.launch_count()
     s.tangent(primal, dot, mu)
@@ -98,14 +92,14 @@ def test_tangent_matches_oracle_and_state_afterwards(env, name, kw, dims, mu):
     assert s.launch_count() - n0 == 3
     _check_against_oracle(_zdot(env, s), _oracle_tangent(recs, _np(dot), dims, mu), (name, mu))
     # the matrix recursion never reads the vectors: FB, VXX and the pivot statistics are the primal sweep's
-    after = ga._outputs(gar, s)
+    after = lq_gpu.outputs(gar, s)
     for k in (gar.OUT_FB, gar.OUT_VXX, gar.OUT_FBT, "pivots", "status"):
         if k in before:
             assert np.array_equal(after[k], before[k]), (name, k)
     for w in range(4):
         assert np.array_equal(s.get_problem(w), problem[w]), (name, "problem", w)
     s.sweep(mu)
-    again = ga._outputs(gar, s)
+    again = lq_gpu.outputs(gar, s)
     for k in before:
         assert np.array_equal(again[k], before[k], equal_nan=True), (name, "sweep after tangent", k)
     s.close()
@@ -114,8 +108,8 @@ def test_tangent_matches_oracle_and_state_afterwards(env, name, kw, dims, mu):
 @pytest.mark.parametrize("name,kw,dims", FEW, ids=FEW_IDS)
 def test_exactness(env, name, kw, dims):
     gar, _, torch = env
-    s, _ = ga._setup(env, kw, dims, seed=5)
-    primal = ga._primal(env, s)
+    s, _ = lq_gpu.setup(env, kw, dims, seed=5)
+    primal = lq_gpu.primal(env, s)
     dot = _tangent(env, s, 2)
     s.tangent(primal, dot, MU)
     base = _zdot(env, s)
@@ -141,7 +135,7 @@ def test_exactness(env, name, kw, dims):
         assert _equal(a, _zdot(env, s)), (name, drop)
     # the primal passed as the handle's own outputs: the same bits as a copy
     s.sweep(MU)
-    own = {k: s.device_ptr(w) for k, w in ga._out_of(gar).items()}
+    own = {k: s.device_ptr(w) for k, w in lq_gpu.out_of(gar).items()}
     s.tangent(own, dot, MU)
     assert _equal(_zdot(env, s), base), (name, "aliased primal")
     s.close()
@@ -151,10 +145,10 @@ def test_exactness(env, name, kw, dims):
 def test_tangent_v_matches_scalar_calls(env, name, kw, dims):
     gar, _, torch = env
     nx, nu, nc, nct, nc0, N, B = dims
-    s, _ = ga._setup(env, kw, dims, seed=9)
+    s, _ = lq_gpu.setup(env, kw, dims, seed=9)
     dot = _tangent(env, s, 3)
     # a constant array: the scalar call's bits
-    primal = ga._primal(env, s)
+    primal = lq_gpu.primal(env, s)
     s.tangent(primal, dot, MU)
     want = _zdot(env, s)
     for mu_arg in (np.full(B, MU), torch.full((B,), MU, dtype=torch.float64, device="cuda")):
@@ -169,17 +163,17 @@ def test_tangent_v_matches_scalar_calls(env, name, kw, dims):
     want_out = {}
     for v in MUS:
         s.sweep(v)
-        s.tangent(ga._primal(env, s), dot, v)
+        s.tangent(lq_gpu.primal(env, s), dot, v)
         sel = mu_b == v
         for k, a in _zdot(env, s).items():
             want[k][sel] = a[sel]
-        for k, a in ga._outputs(gar, s).items():
+        for k, a in lq_gpu.outputs(gar, s).items():
             want_out.setdefault(k, np.empty_like(a))[sel] = a[sel]
     for mu_arg in (mu_b, torch.tensor(mu_b, device="cuda")):
         s.sweep(mu_arg)
-        s.tangent(ga._primal(env, s), dot, mu_arg)
+        s.tangent(lq_gpu.primal(env, s), dot, mu_arg)
         assert _equal(_zdot(env, s), want), (name, type(mu_arg))
-        got_out = ga._outputs(gar, s)
+        got_out = lq_gpu.outputs(gar, s)
         for k in want_out:
             assert np.array_equal(got_out[k], want_out[k], equal_nan=True), (name, type(mu_arg), k)
     s.close()
@@ -190,21 +184,21 @@ def test_tangent_v_matches_scalar_calls(env, name, kw, dims):
 def test_cycle_append_then_tangent(env, name, kw, dims):
     gar, _, torch = env
     nx, nu, nc, nct, nc0, N, B = dims
-    s, recs = ga._setup(env, kw, dims, seed=13)
+    s, recs = lq_gpu.setup(env, kw, dims, seed=13)
     new_last = np.ascontiguousarray(gar.pack_problems(gen.generate_batch(99, B, 1, nx, nu, nc, nct))[0].reshape(B, -1))
     s.cycle_append(new_last)
     s.sweep(MU)
-    primal = ga._primal(env, s)
+    primal = lq_gpu.primal(env, s)
     dot = _tangent(env, s, 4)
     s.tangent(primal, dot, MU)
-    got, got_out = _zdot(env, s), ga._outputs(gar, s)
+    got, got_out = _zdot(env, s), lq_gpu.outputs(gar, s)
     rot = np.ascontiguousarray(np.concatenate([recs[0].reshape(B, N, -1)[:, 1:], new_last[:, None]], axis=1))
     f = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B, **kw)
     f.set_problem(rot, recs[1], recs[2], recs[3])
     f.sweep(MU)
-    f.tangent(ga._primal(env, f), dot, MU)
+    f.tangent(lq_gpu.primal(env, f), dot, MU)
     assert _equal(got, _zdot(env, f)), name
-    for k, a in ga._outputs(gar, f).items():
+    for k, a in lq_gpu.outputs(gar, f).items():
         assert np.array_equal(got_out[k], a, equal_nan=True), (name, k)
     s.close()
     f.close()
@@ -232,14 +226,14 @@ def test_errors(env):
         s.sweep(MU)
         s.synchronize()
         n0 = s.launch_count()
-        z = ga._zeros_like_outputs(env, s)
+        z = lq_gpu.zeros_like_outputs(env, s)
         assert _rc(gar, s, z, {}) == 2, kw  # AB2_ERR_UNSUPPORTED
         with pytest.raises(gar.GarError):
             s.tangent(z, {}, MU)
         assert s.launch_count() == n0
         s.close()
     s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B)
-    z = ga._zeros_like_outputs(env, s)
+    z = lq_gpu.zeros_like_outputs(env, s)
     assert _rc(gar, s, z, {}) == 4  # AB2_ERR_STATE: no problem set
     assert s.launch_count() == 0
     s.set_problem(*gar.pack_problems(gen.generate_batch(1, B, N, nx, nu, nc, nct)))
@@ -259,14 +253,14 @@ def test_errors(env):
 def test_duality_with_the_adjoint(env, name, kw, dims):
     """<zbar, tangent(pdot)> = <adjoint(zbar), pdot> on the device."""
     gar, _, torch = env
-    s, _ = ga._setup(env, kw, dims, seed=17)
-    primal = ga._primal(env, s)
-    zbar = ga._cotangent(env, s, 6)
+    s, _ = lq_gpu.setup(env, kw, dims, seed=17)
+    primal = lq_gpu.primal(env, s)
+    zbar = lq_gpu.cotangent(env, s, 6)
     dot = _tangent(env, s, 7)
-    grad = ga._grad_bufs(env, s)
+    grad = lq_gpu.grad_bufs(env, s)
     s.adjoint(primal, zbar, grad, MU)
     s.tangent(primal, dot, MU)
-    zdot = ga._primal(env, s)
+    zdot = lq_gpu.primal(env, s)
     lhs = sum(float(torch.sum(zbar[k] * zdot[k])) for k in KEYS)
     rhs = sum(float(torch.sum(grad[k] * dot[k])) for k in DOTS)
     assert abs(lhs - rhs) <= 1e-12 * max(abs(lhs), abs(rhs)), (name, lhs, rhs)
@@ -277,18 +271,18 @@ def test_func_jvp_is_the_tangent_call(env):
     gar, ag, torch = env
     name, kw, dims = HANDLES[0]
     nx, nu, nc, nct, nc0, N, B = dims
-    s, recs = ga._setup(env, kw, dims, seed=23)
+    s, recs = lq_gpu.setup(env, kw, dims, seed=23)
     prim = tuple(torch.tensor(np.ascontiguousarray(a), device="cuda") for a in recs)
     dot = _tangent(env, s, 8)
     tans = tuple(dot[k] for k in DOTS)
     outs, jv = torch.func.jvp(lambda *a: ag.lq_solve(s, *a, MU), prim, tans)
     s.set_problem(*prim, memspace=gar.AB2_DEVICE)
     s.sweep(MU)
-    primal = ga._primal(env, s)
+    primal = lq_gpu.primal(env, s)
     for k, o in zip(KEYS, outs):
         assert torch.equal(o, primal[k]), k
     s.tangent(primal, dot, MU)
-    want = ga._primal(env, s)
+    want = lq_gpu.primal(env, s)
     for k, t in zip(KEYS, jv):
         assert torch.equal(t, want[k]), k
     # torch.autograd.forward_ad gives the same bits
@@ -307,7 +301,7 @@ def test_gradcheck_forward_mode(env, dims, kw):
     nx, nu, nc, nct, nc0, N, B = dims
     probs = gen.generate_batch(21, B, N, nx, nu, nc, nct)
     s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B, **kw)
-    blocks, term, init = ga._block_inputs(torch, probs)
+    blocks, term, init = lq_gpu.block_inputs(torch, probs)
     names = list(blocks) + ["t" + n for n in term] + list(init)
     leaves = list(blocks.values()) + list(term.values()) + list(init.values())
     sym = lambda P: 0.5 * (P + P.transpose(-1, -2))
@@ -335,7 +329,7 @@ def test_full_size(env, cfg):
     s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nx, N, B)
     s.set_problem(stage, term, G0, g0, memspace=gar.AB2_DEVICE)
     s.sweep(mu)
-    primal = ga._primal(env, s)
+    primal = lq_gpu.primal(env, s)
     dot = _tangent(env, s, 5)
     s.tangent(primal, dot, mu)
     s.synchronize()

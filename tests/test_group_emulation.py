@@ -6,47 +6,8 @@ import numpy as np
 import pytest
 
 import gen
-from emu_harness import emulate
+from emu_harness import check_against_oracle, emulate
 from oracle import gar_oracle as orc
-
-
-def check_against_oracle(nx, nu, nc, nct, N, B, mueq, seed, tol=1e-10, style="conditioned", db=0,
-                         pivoting=False, block=0):
-    probs = gen.generate_batch(seed, B, N, nx, nu, nc, nct, style=style)
-    if pivoting:
-        gen.make_pivoting(probs)
-    # block = 0: the warp-per-instance group program; block = NW > 0: the CTA-per-instance program of
-    # riccati_block.cuh with NW emulated warps; block = -NW: its compile-time specialisation (StaticBlockDims)
-    kind = "group" if block == 0 else ("block" if block > 0 else "static")
-    got = emulate(kind, probs, (nx, nu, nc, nct, N), mueq, db if block == 0 else abs(block))
-    got["Vxx"] = got["Vxx"].reshape(B, N + 1, nx, nx).transpose(0, 1, 3, 2)
-    assert np.all(got["status"] == 0)
-    stage, term, G0, g0 = gen.pack_problems(probs)
-    bo = orc.BatchedOracle(nx, nu, nc, nct, probs[0].nc0, N, B, stage, term, G0, g0)
-    bo.sweep(mueq, nthreads=1)
-    ref = bo.get()
-    worst = {}
-    for b in range(B):
-        for t in range(N):
-            worst["K"] = max(worst.get("K", 0), gen.rel_fro(got["fb"][b, t, :nu], ref["fb"][b, t, :nu]))
-            worst["k"] = max(worst.get("k", 0), gen.rel_fro(got["ff"][b, t, :nu], ref["ff"][b, t, :nu]))
-            worst["fb"] = max(worst.get("fb", 0), gen.rel_fro(got["fb"][b, t], ref["fb"][b, t]))
-            worst["ff"] = max(worst.get("ff", 0), gen.rel_fro(got["ff"][b, t], ref["ff"][b, t]))
-        for t in range(N + 1):
-            worst["Vxx"] = max(worst.get("Vxx", 0), gen.rel_fro(got["Vxx"][b, t], ref["Vxx"][b, t]))
-            worst["vx"] = max(worst.get("vx", 0), gen.rel_fro(got["vx"][b, t], ref["vx"][b, t]))
-        for key in ("xs", "us", "vs", "lbdas", "lbd0", "vsT"):
-            if ref[key].size:
-                worst[key] = max(worst.get(key, 0), gen.rel_fro(got[key][b], ref[key][b]))
-    # K alone on control-constrained knots is limited by eps*cond(KKT) ~ 6e-17/mueq between
-    # any two correct fp64 solvers (SURVEY Appendix C); everything else is gated at `tol`.
-    tolk = max(tol, 2.4e-16 / mueq) if nc > 0 else tol
-    bad = {k: v for k, v in worst.items() if not v <= (tolk if k in ("K", "k") else tol)}
-    assert not bad, (bad, worst)
-    # structural semantics (A1): Vxx_t symmetric for t >= 1 when N > 0
-    for t in range(1, N + 1):
-        assert np.array_equal(got["Vxx"][0, t], got["Vxx"][0, t].T)
-    return worst
 
 
 @pytest.mark.parametrize("db", [0, 1])

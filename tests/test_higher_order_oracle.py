@@ -2,7 +2,7 @@
 DESIGN section 2p).
 
 * The two kernel modes restated in numpy (per-direction vectors, two terms, with and without the vector blocks, e), on
-  top of lq_tangent_ref.rho and test_jacobian_oracle.grad_many, against a dense Kdot: K is affine in the data P, so
+  top of lq_tangent_ref.rho and lq_higher_ref.grad_many, against a dense Kdot: K is affine in the data P, so
   Kdot = K(P + Pdot) - K(P) of the dense KKT matrix (gen.lqr_dense_kkt); and the pairing identities.
 * The torch plumbing of lq_solve_higher against a CPU stand-in for the handle that solves the dense KKT systems in
   float64 and runs the numpy restatements for rho_many / grad_many, checked against a pure-torch differentiable dense
@@ -17,8 +17,8 @@ import pytest
 
 import gen
 import lq_adjoint_ref as aref
-import lq_tangent_ref as tref
-from test_jacobian_oracle import _records, grad_many
+from lq_cases import jacobian_records
+from lq_higher_ref import grad_modes, rho_modes
 
 MU = 0.1
 # (nx, nu, nc, nct, nc0, N, B)
@@ -27,64 +27,6 @@ IDS = ["nx%d_nu%d_nc%d_nct%d_nc0%d_N%d_B%d" % c for c in CASES]
 KEYS = aref.KEYS
 RECS = ("stage", "term", "G0", "g0")
 HVP_CALLS = dict(backward=1, resolve=3, grad_many=2, rho_many=2)  # device calls of a hessian or a batch of HVPs
-
-
-# ---- numpy restatements of the two kernel modes ----
-def _no_vectors(dot, d6):
-    """The tangent records with their vector blocks (q, r, d, f, q_N, d_N, g0) zero: rho(., a) of it is rho_K."""
-    nx, nu, nc, nct, nc0, N = d6
-    so, _ = aref.stage_offsets(nx, nu, nc)
-    to, _ = aref.term_offsets(nx, nct)
-    out = {k: None if dot.get(k) is None else np.array(dot[k], dtype=np.float64) for k in RECS}
-    if out["stage"] is not None:
-        for k in ("f", "q", "r", "d"):
-            out["stage"][..., so[k][0]:so[k][1]] = 0.0
-    if out["term"] is not None:
-        for k in ("q", "d"):
-            out["term"][..., to[k][0]:to[k][1]] = 0.0
-    out["g0"] = None
-    return out
-
-
-def _zero_vector_blocks(g, d6):
-    """Gradient records with their vector blocks written 0: Gr_K from Gr."""
-    return _no_vectors(g, d6) | {"g0": np.zeros_like(g["g0"])}
-
-
-def _at(v, j):
-    """Direction j of a dict of [nrhs][batch][...] arrays, or the dict itself when it is shared ([batch][...])."""
-    return v if v.get("each") is False else {k: None if v.get(k) is None else v[k][j] for k in v if k != "each"}
-
-
-def rho_modes(nrhs, d6, dot1, a1, vec=True, dot2=None, a2=None, e=None):
-    """out_j = rho^(vec)(dot1_j; a1_j) + rho_K(dot2_j; a2_j) + e_j, per direction (the kernel's sum order: term 1,
-    term 2, e).  A vector dict with each=False is shared."""
-    outs = []
-    for j in range(nrhs):
-        d1 = {k: None if dot1.get(k) is None else dot1[k][j] for k in RECS}
-        r = tref.rho(d1 if vec else _no_vectors(d1, d6), {k: _at(a1, j)[k] for k in KEYS}, d6)
-        if dot2 is not None:
-            d2 = _no_vectors({k: None if dot2.get(k) is None else dot2[k][j] for k in RECS}, d6)
-            r2 = tref.rho(d2, {k: _at(a2, j)[k] for k in KEYS}, d6)
-            r = {k: r[k] + r2[k] for k in KEYS}
-        if e is not None:
-            r = {k: r[k] + e[k][j] for k in KEYS}
-        outs.append(r)
-    return {k: np.stack([o[k] for o in outs]) for k in KEYS}
-
-
-def grad_modes(nrhs, d6, y1, z1, vec=True, y2=None, z2=None):
-    """out_j = Gr^(vec)(y1_j; z1_j) + Gr_K(y2_j; z2_j), per direction."""
-    outs = []
-    for j in range(nrhs):
-        g = grad_many({k: _at(z1, j)[k] for k in KEYS}, {k: y1[k][j] for k in KEYS}, d6)
-        if not vec:
-            g = _zero_vector_blocks(g, d6)
-        if y2 is not None:
-            g2 = _zero_vector_blocks(grad_many({k: _at(z2, j)[k] for k in KEYS}, {k: y2[k][j] for k in KEYS}, d6), d6)
-            g = {k: g[k] + g2[k] for k in RECS}
-        outs.append(g)
-    return {k: np.stack([o[k] for o in outs]) for k in RECS}
 
 
 # ---- the dense KKT system of one instance, from the records ----
@@ -176,7 +118,7 @@ def _scale(a, b):
 def test_rho_modes_against_dense_kdot(case):
     d6, B, nrhs = case[:6], case[6], 3
     rng = np.random.default_rng(1)
-    recs = _records(case, 3)
+    recs = jacobian_records(case, 3)
     dot1, dot2 = _random_recs(case, rng, nrhs), _random_recs(case, rng, nrhs)
     a1, a2, e = _random_vec(case, rng, (nrhs,)), _random_vec(case, rng, ()), _random_vec(case, rng, (nrhs,))
     a2["each"] = False
@@ -342,7 +284,7 @@ def _setup(monkeypatch, case):
     import aligator_b200.autograd as ag
     monkeypatch.setattr(torch.cuda, "current_stream", lambda device=None: types.SimpleNamespace(cuda_stream=0))
     s = _DenseHandle(torch, case)
-    recs = [torch.from_numpy(np.ascontiguousarray(r)) for r in _records(case, 11)]
+    recs = [torch.from_numpy(np.ascontiguousarray(r)) for r in jacobian_records(case, 11)]
     solve = lambda *P: ag._Solve.apply(ag._Higher(s, MU), *P)
     ref = _torch_reference(torch, case, [r.numpy() for r in recs])
     g = torch.Generator().manual_seed(3)
@@ -441,7 +383,7 @@ def test_hvp_references_agree(d6, B, mu):
     like 1 / mu: that is what the GPU bar's e_ref measures)."""
     import hp_higher_order as hho
     import hp_reference as hp
-    from test_hp_derivatives import symmetric_dot
+    from lq_cases import symmetric_dot
     nx, nu, nc, nct, nc0, N = d6
     probs = gen.general_initial_condition(gen.generate_batch(3, B, N, nx, nu, nc, nct), nc0, 3)
     rng = np.random.default_rng(1)

@@ -7,7 +7,7 @@ tests/lq_adjoint_ref.py and tests/lq_factor_adjoint_ref.py evaluated on object a
   <g, pdot> = <cbar, ydot(pdot)> on every case, to 1e-25;
 - the fp64 restatements, fed with the oracle's factorisation and solution, are measured against the references: their
   error e_ref is the bar of every implementation, and it is set beside the error of the fp64 torch derivation of the
-  factorisation's derivatives (test_factor_adjoint_oracle.torch_factor);
+  factorisation's derivatives (lq_factor_adjoint_ref.torch_factor);
 - the device programs compiled for the host (factor_adjoint_emu, factor_tangent_emu; resolve_emu followed by the
   restatements' streaming step, the CPU stand-in for adjoint_many / tangent_many) meet the bar of DESIGN §5:
   e_kernel <= max(16 e_ref, 64 u) family by family, each family's error the worst per-(instance, knot) relative error;
@@ -21,13 +21,10 @@ import gen
 import hp_reference as hp
 import lq_adjoint_ref as aref
 import lq_factor_adjoint_ref as fadj
-import lq_factor_tangent_ref as ftan
 import lq_tangent_ref as tref
-import test_factor_adjoint_oracle as tfa
-import test_factor_tangent_oracle as tft
-import test_resolve_oracle as tro
-from oracle import gar_oracle as orc
-from test_jacobian_oracle import _cot_rhs, grad_many
+from emu_harness import run_factor_adjoint, run_factor_tangent, run_resolve
+from lq_cases import Case, block_errors, check_bar, cot_rhs, family_errors, symmetric_dot
+from lq_higher_ref import grad_many
 
 PIN = 1e-25  # the closed forms against the central differences
 
@@ -56,113 +53,9 @@ def make_problems(name, seed=4000):
     return probs
 
 
-def symmetric_dot(rng, d6, B):
-    """A data tangent in the records' layouts with symmetric Q, R and Q_N (the pad double random too)."""
-    nx, nu, nc, nct, nc0, N = d6
-    so, srec = aref.stage_offsets(nx, nu, nc)
-    to, trec = aref.term_offsets(nx, nct)
-    dot = dict(stage=rng.standard_normal((B, N, srec)), term=rng.standard_normal((B, trec)),
-               G0=rng.standard_normal((B, nc0 * nx)), g0=rng.standard_normal((B, nc0)))
-    for key, off, k in (("stage", so["Q"], nx), ("stage", so["R"], nu), ("term", to["Q"], nx)):
-        x = dot[key]
-        M = x[..., off[0]:off[1]].reshape(*x.shape[:-1], k, k)
-        x[..., off[0]:off[1]] = (M + np.swapaxes(M, -1, -2)).reshape(*x.shape[:-1], k * k)
-    return dot
-
-
-def run_oracle(recs, d6, mu):
-    """The oracle's batched sweep: its outputs in hp_reference's keys.  mu: a number, or one per instance (one oracle
-    sweep per instance)."""
-    nx, nu, nc, nct, nc0, N = d6
-    B = recs[1].shape[0]
-    if np.ndim(mu):
-        per = [run_oracle([a[b:b + 1] for a in recs], d6, m) for b, m in enumerate(mu)]
-        return {k: np.concatenate([o[k] for o in per]) for k in per[0]}
-    bo = orc.BatchedOracle(nx, nu, nc, nct, nc0, N, B, *[np.ascontiguousarray(a) for a in recs])
-    bo.sweep(mu, nthreads=1)
-    assert np.all(bo.status == 1)  # the oracle reports 1 = ok
-    return bo.get()
-
-
-def oracle_solution(recs, d6, mu):
-    return aref.oracle_dict(run_oracle(recs, d6, mu))
-
-
-class Case:
-    """One case's problems, the oracle's outputs, the inputs of every derivative call, the extended-precision
-    references (fp64-rounded) and the fp64 restatements' results fed by the oracle."""
-
-    def __init__(self, probs, mu, seed=1, inputs=None):
-        """inputs: the cotangents and the tangent (cot, fcot, dot) to use instead of random ones."""
-        self.probs, self.mu = probs, mu
-        self.d6 = hp.dims_of(probs[0])
-        B = len(probs)
-        self.recs = hp.records(probs)
-        rng = np.random.default_rng(seed)
-        if inputs is None:
-            inputs = dict(cot={k: rng.standard_normal(s) for k, s in aref._shapes(self.d6, B).items()},
-                          fcot=fadj.random_cot(rng, self.d6, B), dot=symmetric_dot(rng, self.d6, B))
-        self.cot, self.fcot, self.dot = inputs["cot"], inputs["fcot"], inputs["dot"]
-        # extended precision
-        _, self.hps = hp.solve(probs, mu)
-        self.g_hp = hp.grads64(hp.grad_solution(probs, mu, self.cot, self.hps))
-        self.gf_hp = hp.grads64(hp.grad_factor(probs, mu, self.fcot, self.hps))
-        td, _ = hp.tangents(probs, mu, self.dot)
-        self.zd_hp, self.fd_hp = hp.solution_of(td), hp.factor_of(td)
-        # the oracle and the fp64 restatements fed by it
-        self.out = run_oracle(self.recs, self.d6, mu)
-        self.z, self.fac = aref.oracle_dict(self.out), hp.factor_of(self.out)
-        w = oracle_solution(aref.adjoint_records(*self.recs, self.cot, self.d6), self.d6, mu)
-        self.g_ref = aref.grad_records(self.z, w, self.d6)
-        self.zd_ref = oracle_solution(tref.tangent_records(*self.recs, self.dot, self.z, self.d6), self.d6, mu)
-        f = self.fac
-        self.gf_ref = fadj.factor_adjoint(self.recs[0], self.recs[1], f["ff"], f["fb"], f["vxx"], f["vx"], f["fft"],
-                                          f["fbt"], self.fcot, self.d6, mu)
-        self.fd_ref = ftan.factor_tangent(self.recs[0], self.recs[1], f["ff"], f["fb"], f["vxx"], f["vx"], f["fft"],
-                                          f["fbt"], self.dot, self.d6, mu)
-
-    # the error families of each call's output against the reference
-    def e_adjoint(self, g):
-        return hp.grad_errors(g, self.g_hp, self.d6)
-
-    def e_tangent(self, zd):
-        return hp.solution_errors(zd, self.zd_hp, self.d6)
-
-    def e_factor_adjoint(self, g):
-        return hp.grad_errors(g, self.gf_hp, self.d6, hp.GRAD_FAMILIES[:-2])
-
-    def e_factor_tangent(self, fd):
-        return hp.factor_errors(fd, self.fd_hp, self.d6)
-
-    def e_refs(self):
-        return dict(adjoint=self.e_adjoint(self.g_ref), tangent=self.e_tangent(self.zd_ref),
-                    factor_adjoint=self.e_factor_adjoint(self.gf_ref),
-                    factor_tangent=self.e_factor_tangent(self.fd_ref))
-
-    def e_torch(self):
-        """The fp64 torch derivation's errors on the factorisation's derivatives (autograd and jvp through
-        test_factor_adjoint_oracle.torch_factor)."""
-        st, tt = self.recs[0], self.recs[1]
-        B = tt.shape[0]
-        mus = np.broadcast_to(np.asarray(self.mu, dtype=np.float64), (B,))
-        one = lambda d, b: {k: v[b:b + 1] for k, v in d.items()}
-        per = [(tfa._autograd(st[b:b + 1], tt[b:b + 1], self.d6, mus[b], one(self.fcot, b))[1],
-                tft._jvp(st[b:b + 1], tt[b:b + 1], self.d6, mus[b],
-                         dict(stage=self.dot["stage"][b:b + 1], term=self.dot["term"][b:b + 1]))[1]) for b in range(B)]
-        ga, jv = ({k: np.concatenate([p[i][k] for p in per]) for k in per[0][i]} for i in (0, 1))
-        ga.update(G0=np.zeros((B, self.d6[4] * self.d6[0])), g0=np.zeros((B, self.d6[4])))
-        return dict(factor_adjoint=self.e_factor_adjoint(ga), factor_tangent=self.e_factor_tangent(jv))
-
-
 @functools.lru_cache(maxsize=None)
 def case(name):
     return Case(make_problems(name), CASES[name][2])
-
-
-def check_bar(e_kernel, e_ref, title, e_torch=None):
-    """e_kernel <= max(16 e_ref, 64 u) family by family; the table of the case on failure."""
-    bad = hp.violations(e_kernel, e_ref)
-    assert not bad, hp.table(title, e_ref, e_kernel, e_torch)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -276,11 +169,11 @@ def test_emulated_factor_programs_meet_the_bar(name):
     e_ref = c.e_refs()
     recs, fac, d6, mu = c.recs, c.fac, c.d6, c.mu
     for lanes, packed, head in GEOMETRIES:
-        g = tfa.run_emu(recs, fac, c.fcot, d6, mu, lanes, packed, head)
+        g = run_factor_adjoint(recs, fac, c.fcot, d6, mu, lanes, packed, head)
         assert np.isfinite(g["stage"]).all() and not g["G0"].any() and not g["g0"].any()
         geo = (lanes, packed, head)
         check_bar(c.e_factor_adjoint(g), e_ref["factor_adjoint"], "%s factor_adjoint %s" % (name, geo))
-        t = tft.run_emu(recs, fac, dict(stage=c.dot["stage"], term=c.dot["term"]), d6, mu, lanes, packed, head)
+        t = run_factor_tangent(recs, fac, dict(stage=c.dot["stage"], term=c.dot["term"]), d6, mu, lanes, packed, head)
         check_bar(c.e_factor_tangent(t), e_ref["factor_tangent"], "%s factor_tangent %s" % (name, geo))
 
 
@@ -291,27 +184,27 @@ def test_emulated_factor_programs_per_instance_mu():
     c = Case(probs, mus)
     e_ref = c.e_refs()
     for lanes, packed, head in GEOMETRIES[:2]:
-        g = tfa.run_emu(c.recs, c.fac, c.fcot, c.d6, mus, lanes, packed, head)
+        g = run_factor_adjoint(c.recs, c.fac, c.fcot, c.d6, mus, lanes, packed, head)
         check_bar(c.e_factor_adjoint(g), e_ref["factor_adjoint"], "factor_adjoint per-instance mu")
-        t = tft.run_emu(c.recs, c.fac, dict(stage=c.dot["stage"], term=c.dot["term"]), c.d6, mus, lanes, packed, head)
+        t = run_factor_tangent(c.recs, c.fac, dict(stage=c.dot["stage"], term=c.dot["term"]), c.d6, mus, lanes, packed, head)
         check_bar(c.e_factor_tangent(t), e_ref["factor_tangent"], "factor_tangent per-instance mu")
 
 
 @pytest.mark.parametrize("name", ["c3_mu1e-3", "c3_mu1e-8", "c2_nct3_mu1e-8", "pad_nc0_1", "pivots_2x2", "N0", "N1"])
 def test_emulated_many_rhs_meets_the_bar(name):
     """adjoint_many and tangent_many on the host: resolve_emu on the oracle's factorisation for the cotangent (resp.
-    rho = Kdot z + hdot), then the streaming kernels' formulas (test_jacobian_oracle.grad_many)."""
+    rho = Kdot z + hdot), then the streaming kernels' formulas (lq_higher_ref.grad_many)."""
     c = case(name)
     e_ref = c.e_refs()
     B = len(c.probs)
     rho = tref.rho(c.dot, c.z, c.d6)
     for lanes, chunk, packed, head in ((32, 2, True, 0), (5, 1, False, 1)):
-        y = tro._run_emu(c.recs, c.out, {k: v[None] for k, v in _cot_rhs(c.cot).items()}, c.d6, 1, c.mu, lanes, chunk,
+        y = run_resolve(c.recs, c.out, {k: v[None] for k, v in cot_rhs(c.cot).items()}, c.d6, 1, c.mu, lanes, chunk,
                          packed, head)
         g = grad_many(c.z, {k: v[0] for k, v in y.items()}, c.d6)
         g["G0"], g["g0"] = g["G0"].reshape(B, -1), g["g0"].reshape(B, -1)
         check_bar(c.e_adjoint(g), e_ref["adjoint"], "%s adjoint_many (host) %s" % (name, (lanes, chunk)))
-        zd = tro._run_emu(c.recs, c.out, {k: v[None] for k, v in _cot_rhs(rho).items()}, c.d6, 1, c.mu, lanes, chunk,
+        zd = run_resolve(c.recs, c.out, {k: v[None] for k, v in cot_rhs(rho).items()}, c.d6, 1, c.mu, lanes, chunk,
                           packed, head)
         check_bar(c.e_tangent({k: v[0] for k, v in zd.items()}), e_ref["tangent"],
                   "%s tangent_many (host) %s" % (name, (lanes, chunk)))
@@ -340,14 +233,14 @@ def test_bar_rejects_a_1e12_error_that_1e10_accepts(name):
     nx, nu, nc, nct, nc0, N = c.d6
     so, _ = aref.stage_offsets(nx, nu, nc)
     t = N // 2
-    g = tfa.run_emu(c.recs, c.fac, c.fcot, c.d6, c.mu, 32)
+    g = run_factor_adjoint(c.recs, c.fac, c.fcot, c.d6, c.mu, 32)
     assert not hp.violations(c.e_factor_adjoint(g), e_ref["factor_adjoint"])
     for fam in ("A", "Q"):
         bad = dict(g, stage=_bump(g["stage"], np.s_[0, t, so[fam][0]:so[fam][1]]))
-        assert max(tfa.block_errors(bad, c.gf_ref, c.d6).values()) <= 1e-10
+        assert max(block_errors(bad, c.gf_ref, c.d6).values()) <= 1e-10
         assert fam in hp.violations(c.e_factor_adjoint(bad), e_ref["factor_adjoint"]), fam
-    ft = tft.run_emu(c.recs, c.fac, dict(stage=c.dot["stage"], term=c.dot["term"]), c.d6, c.mu, 32)
+    ft = run_factor_tangent(c.recs, c.fac, dict(stage=c.dot["stage"], term=c.dot["term"]), c.d6, c.mu, 32)
     assert not hp.violations(c.e_factor_tangent(ft), e_ref["factor_tangent"])
     bad = dict(ft, fb=_bump(ft["fb"], np.s_[0, t, :nu]))
-    assert max(tft.family_errors(bad, c.fd_ref).values()) <= 1e-10
+    assert max(family_errors(bad, c.fd_ref).values()) <= 1e-10
     assert "K" in hp.violations(c.e_factor_tangent(bad), e_ref["factor_tangent"])

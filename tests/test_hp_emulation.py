@@ -12,11 +12,9 @@ import pytest
 
 import gen
 import hp_reference as hp
-from aligator_b200.lqr import LqrKnot
 from emu_harness import emulate, lib
-from oracle import gar_oracle as orc
+from lq_cases import families, run_solver
 
-TRAJ = ("xs", "us", "vs", "lbd")
 
 # name: ((nx, nu, nc, nct, N), batch, mueq, problem transform, well conditioned)
 CASES = {
@@ -54,7 +52,7 @@ def case(name):
     nx, nu, nc, nct, N = dims
     probs = make_problems(name)
     ref, _ = hp.solve(probs, mueq)
-    ora = run_oracle(probs, dims, mueq)
+    ora = run_solver(probs, dims, mueq)
     return probs, ref, ora, hp.error_families(ora, ref, nu, nc, N)
 
 
@@ -68,49 +66,8 @@ def oracle_errors(name, algorithm):
     probs, ref, ora, e = case(name)
     if algorithm == "serial":
         return e
-    own = hp.error_families(run_oracle(probs, dims, mueq, algorithm), ref, dims[1], dims[2], dims[4])
+    own = hp.error_families(run_solver(probs, dims, mueq, algorithm), ref, dims[1], dims[2], dims[4])
     return {f: max(v, e[f]) for f, v in own.items()}
-
-
-def run_oracle(probs, dims, mueq, algorithm="serial"):
-    """The oracle's outputs in the product's layouts: the batched serial solver, or per instance its restatement of
-    the dense solver ('dense') or of the parallel solver with T legs ('legsT')."""
-    nx, nu, nc, nct, N = dims
-    if algorithm == "serial":
-        stage, term, G0, g0 = gen.pack_problems(probs)
-        bo = orc.BatchedOracle(nx, nu, nc, nct, probs[0].nc0, N, len(probs), stage, term, G0, g0)
-        bo.sweep(mueq, nthreads=1)
-        assert np.all(bo.status == 1)
-        return bo.get()
-    return hp.stack_solutions([oracle_instance(p, mueq, algorithm) for p in probs])
-
-
-def oracle_instance(p, mueq, algorithm):
-    N = p.horizon
-    nu, nc = p.stages[0].nu, p.stages[0].nc
-    if algorithm == "dense":
-        q = p.copy()
-        kt = q.stages[-1]
-        k0 = LqrKnot(kt.nx, 0, kt.nc, 0)  # the dense solver's terminal knot has nx2 = 0 (tests/test_oracle_dense.py)
-        k0.Q[:], k0.q[:], k0.C[:], k0.d[:] = kt.Q, kt.q, kt.C, kt.d
-        q.stages[-1] = k0
-        op = orc.OracleProblem(q)
-        s = orc.RiccatiSolverDense(op)
-    else:
-        op = orc.OracleProblem(p.copy())
-        s = orc.ParallelRiccatiSolver(op, int(algorithm[4:]), threaded=False)
-    assert s.backward(mueq)
-    sol = orc.OracleSolution(op)
-    assert s.forward(sol)
-    xs, us, vs, lb = sol.get()
-    o = dict(xs=np.stack(xs), us=np.stack(us[:N]).reshape(N, nu), vs=np.stack(vs[:N]).reshape(N, nc), vsT=vs[N],
-             lbd0=lb[0], lbdas=np.stack(lb[1:]))
-    if algorithm == "dense":
-        fs = [s.factor(t) for t in range(N + 1)]
-        o.update(fb=np.stack([f["fb"][:nu + nc] for f in fs[:N]]), ff=np.stack([f["ff"][:nu + nc] for f in fs[:N]]),
-                 Vxx=np.stack([f["Pxx"] for f in fs]), vx=np.stack([f["px"] for f in fs]),
-                 fbT=fs[N]["fb"][:p.stages[N].nc], ffT=fs[N]["ff"][:p.stages[N].nc])
-    return o
 
 
 def expand_packed(out, nx, N):
@@ -160,16 +117,6 @@ def programs(dims, nc0):
 def algorithm(prog):
     """The oracle's restatement of the algorithm a program runs: the bar is that implementation's own error."""
     return {"dense": "dense", "legs": "legs%d" % prog[3]}.get(prog[0], "serial")
-
-
-def families(prog):
-    """The families a program is measured on: leg mode's gains are parametric in the next leg's head and the dense
-    program's rows after Z are its own (co-state, then closed loop), so those are measured on what they share."""
-    if prog[0] == "legs":
-        return TRAJ
-    if prog[0] == "dense":
-        return ("K", "k", "Z", "z", "Vxx", "vx") + TRAJ
-    return hp.FAMILIES
 
 
 def prog_id(p):

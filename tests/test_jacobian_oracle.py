@@ -13,6 +13,8 @@ import gen
 import lq_adjoint_ref as aref
 import lq_resolve_ref as rref
 import lq_tangent_ref as tref
+from lq_cases import cot_rhs, jacobian_records
+from lq_higher_ref import grad_many
 from oracle import gar_oracle as orc
 
 MU = 1e-2
@@ -21,21 +23,6 @@ CASES = [(3, 2, 1, 1, 3, 4, 2), (4, 2, 1, 0, 0, 4, 1), (4, 3, 0, 1, 4, 0, 2), (5
          (4, 2, 0, 1, 1, 1, 3)]
 IDS = ["nx%d_nu%d_nc%d_nct%d_nc0%d_N%d_B%d" % c for c in CASES]
 NRHS = 3
-
-
-def _records(case, seed):
-    nx, nu, nc, nct, nc0, N, B = case
-    probs = gen.general_initial_condition(gen.generate_batch(seed, B, N, nx, nu, nc, nct), nc0, seed)
-    _, srec = aref.stage_offsets(nx, nu, nc)
-    stage = np.zeros((B, N, srec))
-    for b, p in enumerate(probs):
-        for t in range(N):
-            r = gen.stage_record(p.stages[t])
-            stage[b, t, :r.size] = r
-    term = np.stack([gen.term_record(p.stages[N]) for p in probs])
-    G0 = np.stack([np.asarray(p.G0).ravel(order="F") for p in probs]).reshape(B, nc0 * nx)
-    g0 = np.stack([np.asarray(p.g0) for p in probs]).reshape(B, nc0)
-    return stage, term, G0, g0
 
 
 def _solve(case, recs):
@@ -49,37 +36,6 @@ def _solve(case, recs):
 def _resolve(case, recs, h):
     """resolve(h) = -K^-1 h for ONE right-hand side: the oracle's solve of the problem with its vectors replaced."""
     return _solve(case, rref.replaced_records(*recs, h, case[:6]))
-
-
-def grad_many(z, y, d6):
-    """Gradient records from z and y = resolve(zbar) (the kernel's formulas: dh = y, dK = y z^T, symmetric part of
-    Q and R)."""
-    nx, nu, nc, nct, nc0, N = d6
-    so, srec = aref.stage_offsets(nx, nu, nc)
-    to, trec = aref.term_offsets(nx, nct)
-    B = z["xs"].shape[0]
-    o, cm = aref._outer, aref._cm
-    pair = lambda a, b, ya, yb: o(ya, b) + o(a, yb)  # y_a b^T + a y_b^T
-    x, u, v, l = z["xs"][:, :N], z["us"], z["vs"], z["lams"]
-    X, U, V, L = y["xs"][:, :N], y["us"], y["vs"], y["lams"]
-    blocks = dict(A=cm(pair(l, x, L, X)), B=cm(pair(l, u, L, U)), f=L, Q=cm(0.5 * pair(x, x, X, X)),
-                  S=cm(pair(x, u, X, U)), R=cm(0.5 * pair(u, u, U, U)), q=X, r=U, C=cm(pair(v, x, V, X)),
-                  D=cm(pair(v, u, V, U)), d=V)
-    st = np.zeros((B, N, srec))
-    for k, (a, b) in so.items():
-        st[..., a:b] = blocks[k]
-    xN, XN = z["xs"][:, N], y["xs"][:, N]
-    tb = dict(Q=cm(0.5 * pair(xN, xN, XN, XN)), q=XN, C=cm(pair(z["vsT"], xN, y["vsT"], XN)), d=y["vsT"])
-    tt = np.zeros((B, trec))
-    for k, (a, b) in to.items():
-        tt[:, a:b] = tb[k]
-    G0 = cm(pair(z["lam0"], z["xs"][:, 0], y["lam0"], y["xs"][:, 0]))
-    return dict(stage=st, term=tt, G0=G0, g0=y["lam0"])
-
-
-def _cot_rhs(c):
-    """A cotangent as resolve's right-hand side: xs -> q, us -> r, vs -> d, vsT -> dN, lam0 -> g0, lams -> f."""
-    return dict(q=c["xs"], r=c["us"], d=c["vs"], dN=c["vsT"], g0=c["lam0"], f=c["lams"])
 
 
 def _random(case, seed):
@@ -100,17 +56,17 @@ def _rel(a, b):
 @pytest.mark.parametrize("case", CASES, ids=IDS)
 def test_reverse_and_forward_formulas_match_single_references(case):
     d6 = case[:6]
-    recs = _records(case, 5)
+    recs = jacobian_records(case, 5)
     z = _solve(case, recs)
     cots, dots = _random(case, 6)
     for j in range(NRHS):
         # reverse: y = resolve(zbar), then y z^T, against the adjoint reference (w = K^-1 zbar, dK = -w z^T)
-        y = _resolve(case, recs, _cot_rhs(cots[j]))
+        y = _resolve(case, recs, cot_rhs(cots[j]))
         w = _solve(case, aref.adjoint_records(*recs, cots[j], d6))
         assert _rel(grad_many(z, y, d6), aref.grad_records(z, w, d6)) <= 1e-12, j
         # forward: resolve(rho), against the tangent reference (the tangent problem's solve)
         rho = tref.rho(dots[j], z, d6)
-        zd = _resolve(case, recs, _cot_rhs(rho))
+        zd = _resolve(case, recs, cot_rhs(rho))
         assert _rel(zd, _solve(case, tref.tangent_records(*recs, dots[j], z, d6))) <= 1e-12, j
 
 
@@ -118,11 +74,11 @@ def test_reverse_and_forward_formulas_match_single_references(case):
 def test_duality_for_every_pair(case):
     """<zbar_i, zdot_j> = <grad_i, pdot_j> for every (i, j), asymmetric Q and R tangents included."""
     d6 = case[:6]
-    recs = _records(case, 8)
+    recs = jacobian_records(case, 8)
     z = _solve(case, recs)
     cots, dots = _random(case, 9)
-    grads = [grad_many(z, _resolve(case, recs, _cot_rhs(c)), d6) for c in cots]
-    zdots = [_resolve(case, recs, _cot_rhs(tref.rho(p, z, d6))) for p in dots]
+    grads = [grad_many(z, _resolve(case, recs, cot_rhs(c)), d6) for c in cots]
+    zdots = [_resolve(case, recs, cot_rhs(tref.rho(p, z, d6))) for p in dots]
     for i in range(NRHS):
         for j in range(NRHS):
             lhs = [cots[i][k] * zdots[j][k] for k in aref.KEYS]

@@ -4,31 +4,8 @@ oracle (GPU)."""
 import numpy as np
 import pytest
 
+from inner_cases import random_inputs
 from oracle import lq_assemble as orc
-
-
-def random_inputs(rng, N, nx, nu, nc, nct, nc0, exact=True, init_hess=True):
-    r = lambda *s: rng.standard_normal(s)
-    sym = lambda a: 0.5 * (a + np.swapaxes(a, -1, -2))
-    spd = lambda a: a @ np.swapaxes(a, -1, -2) / a.shape[-1] + np.eye(a.shape[-1])  # well-posed sweeps
-    inp = dict(Jx=np.eye(nx) + 0.1 * r(N, nx, nx), Ju=r(N, nx, nu), slack=r(N, nx), Lxx=spd(r(N, nx, nx)),
-               Lxu=0.1 * r(N, nx, nu), Luu=spd(r(N, nu, nu)), Lx=r(N, nx), Lu=r(N, nu), Lxx_N=spd(r(nx, nx)),
-               Lx_N=r(nx), preg=1e-3 * (1 + rng.random()), mu_inv=10.0 ** rng.integers(1, 4))
-    if exact:
-        inp.update(Hxx=0.01 * sym(r(N, nx, nx)), Hxu=0.01 * r(N, nx, nu), Huu=0.01 * sym(r(N, nu, nu)))
-    if nc:
-        # mixed product set: equality rows (always active), negative-orthant rows, box rows
-        kinds = rng.integers(0, 3, nc)
-        lo = np.where(kinds == 0, np.inf, np.where(kinds == 1, -np.inf, -0.5))
-        hi = np.where(kinds == 0, np.inf, np.where(kinds == 1, 0.0, 0.5))
-        inp.update(cJx=r(N, nc, nx), cJu=r(N, nc, nu), Lv=r(N, nc), shifted=r(N, nc), lo=lo, hi=hi)
-    if nct:
-        inp.update(cJx_N=r(nct, nx), Lv_N=r(nct), shifted_N=r(nct), loN=np.full(nct, -np.inf), hiN=np.zeros(nct))
-    if nc0:
-        inp.update(G0=r(nc0, nx), g0=r(nc0))
-    if init_hess:
-        inp["Hxx0"] = 0.01 * sym(r(nx, nx))
-    return inp
 
 
 def test_oracle_hand_case():

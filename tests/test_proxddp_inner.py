@@ -8,30 +8,14 @@ import numpy as np
 import pytest
 
 import gen
+from inner_cases import hand_case, hand_gradient_inputs
 from oracle import proxddp_inner as pin
 
 INF = np.inf
 
 
-# ---------------------------------------------------------------------------------------------------------------
-# CPU: the restatement
-# ---------------------------------------------------------------------------------------------------------------
-def _hand_case():
-    """nx = 2, nu = 1, nc = 3 (equality, negative orthant, box [-1, 1]), nct = 1 (negative orthant), nc0 = 2, N = 1.
-    Every number is dyadic, so each expected value below is exact."""
-    return dict(
-        xs=[np.array([1.0, 2.0]), np.array([3.0, -1.0])],
-        lams=[np.array([1.0, -1.0]), np.array([2.0, 0.0])],
-        vs=[np.array([1.0, 2.0, -1.0]), np.array([3.0])],
-        prev_vs=[np.array([0.5, 1.0, 1.0]), np.array([0.5])],
-        init_value=np.array([0.5, -0.5]),
-        cvals=[np.array([0.25, 0.0, 0.5]), np.array([-1.0])],
-        lo=np.array([INF, -INF, -1.0]), hi=np.array([INF, 0.0, 1.0]), loN=np.array([-INF]), hiN=np.array([0.0]),
-        mu=0.5, mu_dyn=0.25, xnext=[np.array([13.0, 9.0])])
-
-
 def test_multipliers_hand_case():
-    h = _hand_case()
+    h = hand_case()
     m = pin.compute_multipliers(**h)
     assert np.array_equal(m["fs"][0], [0.5, -0.5]) and np.array_equal(m["fs"][1], [10.0, 10.0])  # xnext - x1
     # lam0_plus = lam0 + fs0 / mu (mu = 0.5; with mu_dyn it would be [3, -3])
@@ -57,16 +41,9 @@ def test_multipliers_hand_case():
     assert not pin.compute_multipliers(**h3)["ok"]
 
 
-def _hand_gradient_inputs():
-    return dict(lx=[np.array([0.5, 0.5])], lu=[np.array([1.0])], lx_N=np.array([1.0, 1.0]),
-                Jx=[np.array([[1.0, 2.0], [3.0, 4.0]])], Ju=[np.array([[1.0], [5.0]])],
-                cJx=[np.array([[1.0, 0.0], [0.0, 1.0], [1.0, 1.0]])], cJu=[np.array([[0.0], [1.0], [2.0]])],
-                cJx_N=np.array([[2.0, -1.0]]), G0=np.array([[1.0, 0.0], [0.0, 2.0]]))
-
-
 def test_gradient_and_criterion_hand_case():
-    h = _hand_case()
-    g = _hand_gradient_inputs()
+    h = hand_case()
+    g = hand_gradient_inputs()
     Lxs, Lus = pin.lagrangian_gradient(**g, lams=h["lams"], vs=h["vs"])
     # Lx_0 = G0^T lam0 (1, -2) + lx (0.5, 0.5) + Jx^T lam1 (2, 4) + cJx^T v0 (0, 1)
     assert np.array_equal(Lxs[0], [3.5, 3.5])

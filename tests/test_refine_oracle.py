@@ -6,10 +6,9 @@ import pytest
 
 import gen
 import hp_reference as hp
-import lq_adjoint_ref as aref
 import lq_refine_ref as fref
 import lq_resolve_ref as rref
-from test_resolve_oracle import BAR_CASES, _oracle, _records
+from lq_cases import BAR_CASES, batch_records, errors, refine_case, refined_on_oracle, run_oracle
 
 # (nx, nu, nc, nct, nc0, N): C1, C2 and C3 dims, nct in {0, 2}, nc0 in {0, 1, nx/2, nx}, N in {0, 1, 5, 100}
 CASES = [(6, 3, 0, 0, 6, 5), (6, 3, 0, 2, 1, 1), (12, 6, 0, 0, 12, 1), (12, 6, 0, 2, 6, 0), (12, 6, 0, 0, 0, 5),
@@ -47,7 +46,7 @@ def test_residual_matches_dense_kkt(case, own):
     nx, nu, nc, nct, nc0, N = case
     probs = _probs(case, 21)
     B, nrhs = len(probs), (1 if own else 2)
-    stage, term, G0, g0 = _records(probs, case)
+    stage, term, G0, g0 = batch_records(probs, case)
     rng = np.random.default_rng(22)
     z = {k: rng.standard_normal((nrhs,) + s) for k, s in zip(rref.SOL, rref.rhs_shapes(case, B).values())}
     h = None if own else rref.random_rhs(rng, case, B, nrhs)
@@ -66,44 +65,7 @@ def test_residual_matches_dense_kkt(case, own):
     assert norms.shape == (nrhs, B) and np.all(norms > 0)
 
 
-def refine_case(name):
-    """(problems, records, dims, mu) of a refinement case: the conditioning-bar cases of the resolve tests and a
-    general G0."""
-    if name == "general_G0":
-        probs = gen.general_initial_condition(gen.generate_batch(4100, 3, 20, 4, 2, 2, 0), 2, 4100)
-        case, mu = (4, 2, 2, 0, 2, 20), 1e-8
-    else:
-        (nx, nu, nc, nct, N), B, mu, transform = BAR_CASES[name]
-        probs = gen.generate_batch(3000 + sum(map(ord, name)), B, N, nx, nu, nc, nct)
-        if transform is not None:
-            transform(probs)
-        case = (nx, nu, nc, nct, nx, N)
-    return probs, _records(probs, case), case, mu
-
-
 REFINE_CASES = list(BAR_CASES) + ["general_G0"]
-
-
-def errors(z, want, case):
-    """Error families (xs, us, vs, lbd) of right-hand side 0 of the solution dict z against hp_reference's `want`."""
-    nx, nu, nc, nct, nc0, N = case
-    got = {k: v[0] for k, v in z.items()}
-    return hp.error_families(dict(got, lbd0=got["lam0"], lbdas=got["lams"]), want, nu, nc, N, ("xs", "us", "vs", "lbd"))
-
-
-def refined_on_oracle(probs, recs, case, mu, steps=2):
-    """(refined z, unrefined z, norms, extended-precision solution, floor) for the primal of `probs`, refined on the
-    oracle's factorisation.  floor: per family, the larger error after one and after two steps started from the
-    correctly rounded solution -- the noise level of a refinement whose residual is computed in fp64."""
-    o = _oracle(recs, case, mu)
-    fac = (o["fb"], o["fbT"], o["Vxx"])
-    z0 = {k: v[None] for k, v in aref.oracle_dict(o).items()}
-    z, norms = fref.refine(*recs, *fac, z0, None, case, mu, steps)
-    want, _ = hp.solve(probs, mu)
-    exact = {k: want[w][None] for k, w in zip(aref.KEYS, ("xs", "us", "vs", "vsT", "lbd0", "lbdas"))}
-    e1 = errors(fref.refine(*recs, *fac, exact, None, case, mu, 1)[0], want, case)
-    e2 = errors(fref.refine(*recs, *fac, exact, None, case, mu, 2)[0], want, case)
-    return z, z0, norms, want, {f: max(e1[f], e2[f]) for f in e1}
 
 
 @pytest.mark.parametrize("name", REFINE_CASES)
@@ -134,8 +96,8 @@ def test_zero_steps_and_resolve_outputs():
     ulps of the solution (resolve is already accurate at mu = 1e-2)."""
     case = (4, 2, 2, 2, 4, 5)
     probs = _probs(case, 23)
-    recs = _records(probs, case)
-    o = _oracle(recs, case, MU)
+    recs = batch_records(probs, case)
+    o = run_oracle(recs, case, MU)
     h = rref.random_rhs(np.random.default_rng(24), case, 2, 3)
     z0 = rref.resolve(recs[0], recs[1], recs[2], o["fb"], o["fbT"], o["Vxx"], h, case, MU, 3)
     z, norms = fref.refine(*recs, o["fb"], o["fbT"], o["Vxx"], z0, h, case, MU, 0)

@@ -8,6 +8,7 @@ import pytest
 import gen
 import lq_adjoint_ref as aref
 import lq_tangent_ref as ref
+from lq_cases import batch_records
 from oracle import gar_oracle as orc
 
 MU = 1e-2
@@ -28,14 +29,7 @@ def _problem(case, seed):
 
 def _records(p, case):
     """Packed (padded) single-instance records of problem p."""
-    nx, nu, nc, nct, nc0, N = case
-    _, srec = aref.stage_offsets(nx, nu, nc)
-    stage = np.zeros((1, N, srec))
-    for t in range(N):
-        r = gen.stage_record(p.stages[t])
-        stage[0, t, :r.size] = r
-    return (stage, gen.term_record(p.stages[N])[None], np.asarray(p.G0).ravel(order="F")[None],
-            np.asarray(p.g0)[None])
+    return batch_records([p], case)
 
 
 def _symmetrize(rec, off, n):

@@ -36,7 +36,7 @@ def transcript(gar, torch, kw, dims):
     """One line per call of the script: name, return code and message, launch-count delta, factor_epoch, ring heads."""
     import ctypes as C
     import gen
-    from test_fddp import _random_fddp
+    from inner_cases import random_fddp
     nx, nu, N, B = dims
     rng = np.random.default_rng(11)
     s = gar.CudaRiccatiBatch(nx, nu, 0, 0, nx, N, B, **kw)
@@ -49,7 +49,7 @@ def transcript(gar, torch, kw, dims):
     sol = dict(xs=(B, N + 1, nx), us=(B, N, nu), vs=(B, N, 0), vsT=(B, 0), lam0=(B, nx), lams=(B, N, nx))
     rec = dict(stage=(B, N, s.srec), term=(B, s.trec), G0=(B, nx * nx), g0=(B, nx))
     cm = lambda a: np.ascontiguousarray(np.swapaxes(a, -1, -2))
-    fd = _random_fddp(rng, B, N, nx, nu)
+    fd = random_fddp(rng, B, N, nx, nu)
     fddp = {k: dev(cm(v) if v.ndim >= 3 and k not in ("fs", "Lx", "Lu", "Lx_N") else v) for k, v in fd.items()}
     lq = {k: fddp[k] for k in ("Jx", "Ju", "Lxx", "Lxu", "Luu", "Lx", "Lu", "Lxx_N", "Lx_N")}
     lq.update(slack=fddp["fs"][:, 1:].contiguous(), G0=dev(np.tile(-np.eye(nx).ravel(), (B, 1))),
