@@ -249,15 +249,15 @@ def make_homogeneous(probs):
 
 
 def scale_instances(probs, exponents, mueq):
-    """Instance b times c_b = 2**exponents[b]: Q, S, R, q, r, C, D, d, G0 and g0 scaled (A, B, f kept), and
-    mu_b = c_b * mueq.  Every saddle-point system of instance b is then exactly c_b times the original one.
-    Returns (scaled copies, [batch] per-instance mu)."""
+    """Instance b times c_b = 2**exponents[b]: Q, S, R, q, r, C, D, d, the parametric blocks Gx, Gu, Gv, Gth,
+    gamma (empty when nth = 0), G0 and g0 scaled (A, B, f kept), and mu_b = c_b * mueq.  Every saddle-point system
+    of instance b is then exactly c_b times the original one.  Returns (scaled copies, [batch] per-instance mu)."""
     out = []
     for p, s in zip(probs, exponents):
         q = p.copy()
         c = 2.0 ** int(s)
         for k in q.stages:
-            for name in ("Q", "S", "R", "q", "r", "C", "D", "d"):
+            for name in ("Q", "S", "R", "q", "r", "C", "D", "d", "Gx", "Gu", "Gv", "Gth", "gamma"):
                 getattr(k, name)[...] *= c
         q.G0 *= c
         q.g0 *= c

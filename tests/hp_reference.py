@@ -7,7 +7,9 @@ nothing depends on Bunch-Kaufman pivot decisions.  The fp64 inputs are exact in 
 computes from them is accurate to ~cond * 1e-50, far below anything fp64 can resolve.
 
 `solve` returns the outputs in the product's layouts (fp64, rounded from the extended-precision values);
-`error_families` measures an implementation against them, family by family.
+`error_families` measures an implementation against them, family by family.  `solve_parametric` is the recursion of
+parametric problems (nth > 0) as the reference states it, `solve_legs` the parallel solver's legs and condensed system
+on top of it (tests/test_hp_parametric.py pins both).
 
 Derivatives of the solve, exact to far below fp64, without any derivative formula or with the closed forms evaluated in
 extended precision: `tangent_problem` is the forward mode of every output of the sweep by central differences of the
@@ -185,6 +187,232 @@ def solve(probs, mueq):
     return {k: np.stack([to64(h[k]) for h in hp]) for k in hp[0]}, hp
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Parametric problems (nth > 0) and leg mode
+# ---------------------------------------------------------------------------------------------------------------------
+# The reference's recursion with theta, statement by statement.  With nc > 0 it is not the exact theta-derivative of
+# the value function: Vxt leaves out Z^T Gv, vt leaves out Gv^T z and Vtt leaves out Gv^T Zth
+# (riccati-kernel.hxx:298-310), and a terminal knot with nu = 0 ignores its Gv (:146-149).  The restatement follows
+# the reference there too; where Gv = 0 the recursion is exact (tests/test_hp_parametric.py pins it).
+PARAM_BLOCKS = ("Gx", "Gu", "Gv", "Gth", "gamma")
+
+
+def _mp_pknot(k):
+    d = _mp_knot(k)
+    d.update({n: mpa(getattr(k, n)) for n in PARAM_BLOCKS})
+    return d
+
+
+def _kkt(m, Rh, mu):
+    nc = m["C"].shape[0]
+    return np.block([[Rh, m["D"].T], [m["D"], -mu * eye(nc)]]) if nc else Rh
+
+
+def _terminal_solve(m, mu):
+    """terminalSolve (riccati-kernel.hxx:131-193), both branches.  -> dict of the knot's factors: fb, ff, fth (rows
+    [K; Z] only: a terminal knot has no closed loop), Vxx, vx and, with nth > 0, Vxt, Vtt, vt."""
+    nu, nc, nth = m["R"].shape[0], m["C"].shape[0], m["Gth"].shape[0]
+    if nu == 0:                                                                   # :146-149
+        fb, ff, fth = m["C"] / mu, m["d"] / mu, zeros(nc, nth)
+    else:                                                                         # :150-173
+        rhs = np.concatenate([np.concatenate([m["S"].T, m["r"][:, None], m["Gu"]], axis=1),
+                              np.concatenate([m["C"], m["d"][:, None], zeros(nc, nth)], axis=1)], axis=0)
+        sol = -lu_solve(_kkt(m, m["R"], mu), rhs)
+        fb, ff, fth = sol[:, :m["Q"].shape[0]], sol[:, m["Q"].shape[0]], sol[:, m["Q"].shape[0] + 1:]
+    K, k, Z, z = fb[:nu], ff[:nu], fb[nu:], ff[nu:]
+    o = dict(fb=fb, ff=ff, fth=fth, Vxx=m["Q"] + m["C"].T @ Z + m["S"] @ K, vx=m["q"] + m["C"].T @ z + m["S"] @ k)
+    if nth:                                                                       # :185-192
+        o.update(Vxt=m["Gx"] + K.T @ m["Gu"], Vtt=m["Gth"] + m["Gu"].T @ fth[:nu], vt=m["gamma"] + m["Gu"].T @ k)
+    return o
+
+
+def _stage_solve(m, n, mu):
+    """stageKernelSolve (riccati-kernel.hxx:210-312) of knot m given the next knot's factors n; the theta columns
+    are extra right-hand sides of the stage KKT system."""
+    nx, nu, nc, nth = m["Q"].shape[0], m["R"].shape[0], m["C"].shape[0], m["Gth"].shape[0]
+    V, v = n["Vxx"], n["vx"]
+    vp = v + V @ m["f"]
+    Qh = m["Q"] + m["A"].T @ V @ m["A"]
+    Sh = m["S"] + m["A"].T @ V @ m["B"]
+    Rh = m["R"] + m["B"].T @ V @ m["B"]
+    qh = m["q"] + m["A"].T @ vp
+    rh = m["r"] + m["B"].T @ vp
+    top = [Sh.T, rh[:, None]] + ([m["Gu"] + m["B"].T @ n["Vxt"]] if nth else [])   # Guhat, :286-287
+    bot = [m["C"], m["d"][:, None]] + ([m["Gv"]] if nth else [])
+    sol = -lu_solve(_kkt(m, Rh, mu), np.concatenate([np.concatenate(top, axis=1), np.concatenate(bot, axis=1)]))
+    KZ, kz = sol[:, :nx], sol[:, nx]
+    K, k = KZ[:nu], kz[:nu]
+    Ah, a = m["A"] + m["B"] @ K, m["f"] + m["B"] @ k
+    o = dict(fb=np.concatenate([KZ, Ah], axis=0), ff=np.concatenate([kz, a]),
+             Vxx=Qh + Sh @ K + m["C"].T @ KZ[nu:], vx=qh + Sh @ k + m["C"].T @ kz[nu:])
+    if nth:
+        KZth = sol[:, nx + 1:]
+        Yth = m["B"] @ KZth[:nu]                                                  # :295
+        o.update(fth=np.concatenate([KZth, Yth], axis=0),
+                 vt=m["gamma"] + n["vt"] + m["Gu"].T @ k + n["Vxt"].T @ a,       # :298-301
+                 Vxt=m["Gx"] + K.T @ m["Gu"] + Ah.T @ n["Vxt"],                   # :304-306
+                 Vtt=m["Gth"] + n["Vtt"] + m["Gu"].T @ KZth[:nu] + n["Vxt"].T @ Yth)  # :308-310
+    return o
+
+
+def _backward(st, mu):
+    """backwardImpl (riccati-kernel.hxx:105-129) over the knot dicts st: the last one by terminalSolve."""
+    fac = [None] * len(st)
+    fac[-1] = _terminal_solve(st[-1], mu)
+    for t in range(len(st) - 2, -1, -1):
+        fac[t] = _stage_solve(st[t], fac[t + 1], mu)
+    return fac
+
+
+def _rollout(st, fac, x0, theta):
+    """forwardImpl (riccati-kernel.hxx:315-377) from x0 over the knots st; theta None or an object vector.  -> xs,
+    us (one per knot with nu > 0), vs (one per knot), lbdas (the co-states of knots 1 .. n)."""
+    xs, us, vs, lbdas = [x0], [], [], []
+    n = len(st) - 1
+    for t in range(n + 1):
+        m, f, x = st[t], fac[t], xs[t]
+        nu, nc = m["R"].shape[0], m["C"].shape[0]
+        th = theta is not None and m["Gth"].shape[0] > 0
+        if nu:
+            us.append(f["fb"][:nu] @ x + f["ff"][:nu] + (f["fth"][:nu] @ theta if th else 0))
+        vs.append(f["fb"][nu:nu + nc] @ x + f["ff"][nu:nu + nc] + (f["fth"][nu:nu + nc] @ theta if th else 0))
+        if t == n:
+            break
+        xs.append(f["fb"][nu + nc:] @ x + f["ff"][nu + nc:] + (f["fth"][nu + nc:] @ theta if th else 0))
+        g = fac[t + 1]
+        lbdas.append(g["Vxx"] @ xs[t + 1] + g["vx"] + (g["Vxt"] @ theta if th else 0))
+    return xs, us, vs, lbdas
+
+
+def solve_parametric(p, mueq, theta=None):
+    """One parametric LqrProblem (uniform stage dims, terminal nu = 0) at penalty mueq: the reference's backward pass
+    with theta (riccati-kernel.hxx), the initial system with thGrad and thHess (proximal-riccati.hxx:39-60) and the
+    rollout at theta (computeInitial, :196-207, then forwardImpl) -> dict of extended-precision outputs in the
+    product's layouts: solve_problem's keys, and fth [N][nu+nc+nx][nth], Vxt [N+1][nx][nth], Vtt [N+1][nth][nth],
+    vt [N+1][nth], kkt0 [nx+nc0], kkt0fth [nx+nc0][nth], thGrad [nth], thHess [nth][nth].  theta None: the
+    theta-free rollout."""
+    N, nx, nc0 = p.horizon, p.stages[0].nx, p.nc0
+    nth = p.stages[0].Gth.shape[0]
+    st = [_mp_pknot(k) for k in p.stages]
+    mu = MP.mpf(float(mueq))
+    fac = _backward(st, mu)
+    G0, g0 = mpa(p.G0), mpa(p.g0)
+    f0 = fac[0]
+    M0 = np.block([[f0["Vxx"], G0.T], [G0, zeros(nc0, nc0)]]) if nc0 else f0["Vxx"]
+    s0 = -lu_solve(M0, np.concatenate([np.concatenate([f0["vx"], g0])[:, None],
+                                       np.concatenate([f0["Vxt"], zeros(nc0, nth)])], axis=1))   # :50-55
+    kkt0, kkt0fth = s0[:, 0], s0[:, 1:]
+    th = None if theta is None else mpa(theta)
+    init = kkt0 + (kkt0fth @ th if th is not None else 0)                                           # :196-207
+    xs, us, vs, lbdas = _rollout(st, fac, init[:nx], th)
+    stack = lambda lst, *shape: np.stack(lst) if lst else zeros(*shape)
+    nu, nc = (p.stages[0].nu, p.stages[0].nc) if N else (0, 0)
+    return dict(fb=stack([f["fb"] for f in fac[:N]], 0, nu + nc + nx, nx),
+                ff=stack([f["ff"] for f in fac[:N]], 0, nu + nc + nx),
+                fth=stack([f["fth"] for f in fac[:N]], 0, nu + nc + nx, nth),
+                Vxx=np.stack([f["Vxx"] for f in fac]), vx=np.stack([f["vx"] for f in fac]),
+                Vxt=np.stack([f["Vxt"] for f in fac]), Vtt=np.stack([f["Vtt"] for f in fac]),
+                vt=np.stack([f["vt"] for f in fac]), fbT=fac[N]["fb"], ffT=fac[N]["ff"],
+                kkt0=kkt0, kkt0fth=kkt0fth,
+                thGrad=f0["vt"] + f0["Vxt"].T @ kkt0[:nx], thHess=f0["Vtt"] + f0["Vxt"].T @ kkt0fth[:nx],  # :57-59
+                xs=np.stack(xs), us=stack(us, 0, nu), vs=stack(vs[:N], 0, nc), vsT=vs[N], lbd0=init[nx:],
+                lbdas=stack(lbdas, 0, nx))
+
+
+def solve_parametric_batch(probs, mueq, thetas=None):
+    """solve_parametric over a batch (thetas: None or [B][nth]) -> (fp64 outputs [B, ...], extended-precision dicts)."""
+    mus = np.broadcast_to(np.asarray(mueq, dtype=np.float64), (len(probs),))
+    hp = [solve_parametric(p, m, None if thetas is None else thetas[b]) for b, (p, m) in enumerate(zip(probs, mus))]
+    return {k: np.stack([to64(h[k]) for h in hp]) for k in hp[0]}, hp
+
+
+def get_work(N, i, T):
+    """parallel-solver.hxx:23-28: the knots [beg, end) of leg i of T."""
+    return i * (N + 1) // T, (i + 1) * (N + 1) // T
+
+
+def solve_legs(p, mueq, T):
+    """ParallelRiccatiSolver (parallel-solver.hxx:51-243) with T legs restated in extended precision: every knot of a
+    leg but the last leg parameterised by nth = nx (addParameterization, :52-60), each leg's last knot configured as
+    Gx = A^T, Gu = B^T, Gth = 0, gamma = f (:136-147) and solved by terminalSolve's nu > 0 branch, the condensed
+    system as assembleCondensedSystem(0) builds it (:85-129) solved by Gaussian elimination (no refinement), and
+    the legs' rollouts, each at theta = the next leg head's co-state (:209-243).  Also collapseFeedback as the
+    reference states it (parallel-solver.hpp:41-51): K_0 - Kth_0 Vxt_0^T.
+
+    -> dict of extended-precision outputs in the product's layouts (leg mode: nth = nx): solve_problem's keys, fth,
+    Vxt, Vtt, vt (zero on the last leg's knots, which carry no parameters), `param` [N+1] (True on the knots that
+    carry them) and `collapse` [nu][nx].  A leg's last knot has no closed loop: its Ahat, a and Yth rows are zero."""
+    N, nx, nc0 = p.horizon, p.stages[0].nx, p.nc0
+    nu, nc = p.stages[0].nu, p.stages[0].nc
+    assert N > 0 and T >= 2
+    mu = MP.mpf(float(mueq))
+    legs = [get_work(N, i, T) for i in range(T)]
+    st, fac = [None] * (N + 1), [None] * (N + 1)
+    for i, (beg, end) in enumerate(legs):
+        for t in range(beg, end):
+            k = p.stages[t].copy()
+            if i + 1 < T:
+                k.addParameterization(nx)
+                if t == end - 1:                                                  # configure_knot
+                    k.Gx[...], k.Gu[...], k.Gth[...], k.gamma[...] = k.A.T, k.B.T, 0.0, k.f
+            st[t] = _mp_pknot(k)
+        fac[beg:end] = _backward(st[beg:end], mu)
+    # the condensed system, blocks [lbd0 | x0 | theta_0 | x_h1 | theta_1 | ...]
+    dims = [nc0, nx] + [nx] * (2 * (T - 1))
+    off = np.concatenate([[0], np.cumsum(dims)])
+    M, rhs = zeros(off[-1], off[-1]), zeros(off[-1])
+    put = lambda i, j, blk: M.__setitem__((slice(off[i], off[i + 1]), slice(off[j], off[j + 1])), blk)
+    put(0, 1, mpa(p.G0))
+    put(1, 0, mpa(p.G0).T)
+    put(1, 1, fac[0]["Vxx"])
+    rhs[off[0]:off[1]], rhs[off[1]:off[2]] = -mpa(p.g0), -fac[0]["vx"]
+    put(1, 2, fac[0]["Vxt"])
+    put(2, 1, fac[0]["Vxt"].T)
+    for i in range(T - 1):
+        i0, i1 = legs[i]
+        j = 2 * (i + 1)
+        put(j, j, fac[i0]["Vtt"])
+        put(j + 1, j + 1, fac[i1]["Vxx"])
+        put(j, j + 1, -eye(nx))
+        put(j + 1, j, -eye(nx))
+        if i + 2 < T:
+            put(j + 1, j + 2, fac[i1]["Vxt"])
+            put(j + 2, j + 1, fac[i1]["Vxt"].T)
+        rhs[off[j]:off[j + 1]], rhs[off[j + 1]:off[j + 2]] = -fac[i0]["vt"], -fac[i1]["vx"]
+    sol = lu_solve(M, rhs[:, None])[:, 0]
+    seg = lambda j: sol[off[j]:off[j + 1]]
+    xs, us, vs, lbdas = [None] * (N + 1), [None] * N, [None] * (N + 1), [None] * N
+    for i, (beg, end) in enumerate(legs):
+        th = seg(2 * (i + 1)) if i + 1 < T else None
+        x, u, v, lb = _rollout(st[beg:end], fac[beg:end], seg(2 * i + 1), th)
+        xs[beg:end], vs[beg:end] = x, v
+        us[beg:beg + len(u)] = u
+        lbdas[beg:end - 1] = lb
+        if i:
+            lbdas[beg - 1] = seg(2 * i)
+    nr = nu + nc + nx
+    pad = lambda a, rows: np.concatenate([a, zeros(rows - a.shape[0], *a.shape[1:])]) if a.shape[0] < rows else a
+    param = np.array([t < legs[-1][0] for t in range(N + 1)])
+    par = lambda f, key, *shape: f[key] if key in f else zeros(*shape)
+    fb0 = fac[0]["fb"]
+    return dict(fb=np.stack([pad(f["fb"], nr) for f in fac[:N]]), ff=np.stack([pad(f["ff"], nr) for f in fac[:N]]),
+                fth=np.stack([pad(par(f, "fth", nr, nx), nr) for f in fac[:N]]),
+                Vxx=np.stack([f["Vxx"] for f in fac]), vx=np.stack([f["vx"] for f in fac]),
+                Vxt=np.stack([par(f, "Vxt", nx, nx) for f in fac]), Vtt=np.stack([par(f, "Vtt", nx, nx) for f in fac]),
+                vt=np.stack([par(f, "vt", nx) for f in fac]), fbT=fac[N]["fb"], ffT=fac[N]["ff"], param=param,
+                xs=np.stack(xs), us=np.stack(us), vs=np.stack(vs[:N]).reshape(N, nc), vsT=vs[N], lbd0=seg(0),
+                lbdas=np.stack(lbdas), collapse=fb0[:nu] - fac[0]["fth"][:nu] @ fac[0]["Vxt"].T)
+
+
+def solve_legs_batch(probs, mueq, T):
+    """solve_legs over a batch -> (fp64 outputs [B, ...], extended-precision dicts)."""
+    mus = np.broadcast_to(np.asarray(mueq, dtype=np.float64), (len(probs),))
+    hp = [solve_legs(p, m, T) for p, m in zip(probs, mus)]
+    out = {k: np.stack([to64(h[k]) for h in hp]) for k in hp[0] if k != "param"}
+    out["param"] = np.stack([h["param"] for h in hp])
+    return out, hp
+
+
 def kkt_residual(p, mueq, h):
     """Relative residual of the whole-problem KKT system (gen.lqr_dense_kkt), evaluated in extended precision at the
     extended-precision solution h: ||K z + rhs||_inf / (||K||_inf ||z||_inf + ||rhs||_inf)."""
@@ -234,7 +462,8 @@ def stage_equation_residual(p, mueq, h):
 # ---------------------------------------------------------------------------------------------------------------------
 # Error families and the conditioning-aware tolerance
 # ---------------------------------------------------------------------------------------------------------------------
-FAMILIES = ("K", "k", "Z", "z", "Ahat", "a", "Vxx", "vx", "xs", "us", "vs", "lbd")
+FAMILIES = ("K", "k", "Z", "z", "Ahat", "a", "Vxx", "vx", "xs", "us", "vs", "lbd",
+            "Kth", "Zth", "Yth", "Vxt", "Vtt", "vt", "kkt0fth", "thGrad", "thHess", "collapse")
 FLOOR = 64 * U   # below this two correct fp64 implementations are indistinguishable
 FACTOR = 16      # how much worse than the oracle the kernel may be on the same inputs
 
@@ -249,10 +478,14 @@ def _rel(a, b):
 def _pieces(o, nu, nc, N):
     """family -> list of per-(instance, knot) blocks of output dict o (fp64, product layouts); families whose
     outputs o does not have are left out (an implementation that computes only the trajectory, or only the
-    factorisation)."""
+    factorisation).  The parametric families: Kth, Zth, Yth (the row blocks of fth [b, t]), Vxt, Vtt, vt per knot,
+    kkt0fth, thGrad, thHess per instance, each in the product's layout ([nx][nth] for Vxt); where o has `param`
+    [B][N+1] (leg mode) only on the knots it marks.  collapse: collapse_feedback's first gain [b] ([nu][nx])."""
     traj = "xs" in o
     B = o["xs" if traj else "fb"].shape[0]
     P = {f: [] for f in FAMILIES}
+    param = o.get("param")
+    has = lambda b, t: param is None or param[b, t]
     for b in range(B):
         for t in range(N):
             if "fb" in o:
@@ -262,6 +495,11 @@ def _pieces(o, nu, nc, N):
                     P["Z"].append(fb[nu:nu + nc]); P["z"].append(ff[nu:nu + nc])
                 if fb.shape[0] > nu + nc:
                     P["Ahat"].append(fb[nu + nc:]); P["a"].append(ff[nu + nc:])
+            if "fth" in o and has(b, t):
+                fth = o["fth"][b, t]
+                P["Kth"].append(fth[:nu]); P["Yth"].append(fth[nu + nc:])
+                if nc:
+                    P["Zth"].append(fth[nu:nu + nc])
             if traj:
                 if nc:
                     P["vs"].append(o["vs"][b, t])
@@ -276,14 +514,22 @@ def _pieces(o, nu, nc, N):
         for t in range(N + 1):
             if "Vxx" in o:
                 P["Vxx"].append(o["Vxx"][b, t]); P["vx"].append(o["vx"][b, t])
+            if "Vxt" in o and has(b, t):
+                P["Vxt"].append(o["Vxt"][b, t]); P["Vtt"].append(o["Vtt"][b, t]); P["vt"].append(o["vt"][b, t])
             if traj:
                 P["xs"].append(o["xs"][b, t])
+        for f in ("kkt0fth", "thGrad", "thHess", "collapse"):
+            if f in o:
+                P[f].append(o[f][b])
     return P
 
 
 def error_families(got, ref, nu, nc, N, families=FAMILIES):
     """Max over instances and knots of the relative error of `got` against the fp64-rounded extended-precision
-    outputs `ref`, per family (families without entries on either side are left out)."""
+    outputs `ref`, per family (families without entries on either side are left out).  The knots that carry
+    parameters are those `ref` marks (leg mode)."""
+    if "param" in ref:
+        got = dict(got, param=ref["param"])
     g, r = _pieces(got, nu, nc, N), _pieces(ref, nu, nc, N)
     return {f: max(_rel(a, b) for a, b in zip(g[f], r[f])) for f in families
             if g[f] and len(g[f]) == len(r[f]) and sum(np.size(b) for b in r[f])}
@@ -307,11 +553,11 @@ def table(title, e_oracle, e_kernel, e_torch=None):
     """One row per family: the oracle's error, the kernel's and their ratio; with `e_torch`, the error of the fp64
     torch.autograd derivation beside them."""
     extra = lambda f: "" if e_torch is None else " %10.2e" % e_torch.get(f, float("nan"))
-    rows = ["%s\n  %-5s %10s %10s %7s%s" % (title, "family", "e_oracle", "e_kernel", "ratio",
+    rows = ["%s\n  %-8s %10s %10s %7s%s" % (title, "family", "e_oracle", "e_kernel", "ratio",
                                            "" if e_torch is None else " %10s" % "e_torch")]
     for f in e_kernel:
         ratio = e_kernel[f] / e_oracle[f] if e_oracle[f] > 0 else float("inf") if e_kernel[f] > 0 else 0.0
-        rows.append("  %-5s %10.2e %10.2e %7.2f%s" % (f, e_oracle[f], e_kernel[f], ratio, extra(f)))
+        rows.append("  %-8s %10.2e %10.2e %7.2f%s" % (f, e_oracle[f], e_kernel[f], ratio, extra(f)))
     return "\n".join(rows)
 
 

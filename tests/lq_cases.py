@@ -122,7 +122,11 @@ def families(prog):
     return hp.FAMILIES
 
 
-def make_problem(seed, N, nx, nu, nc, nct, nth):
+def make_problem(seed, N, nx, nu, nc, nct, nth, gv=False):
+    """A seeded parametric problem with non-trivial Gx, Gu, Gth and gamma on every knot.  Gv is zero unless `gv`:
+    then Gaussian on every knot with rows (the terminal one included), drawn after everything else so the other
+    blocks are those of gv=False.  (The reference's recursion is the exact theta-derivative only where Gv = 0,
+    DESIGN §4; legs always have Gv = 0.)"""
     rng = np.random.default_rng(seed)
     x0 = rng.standard_normal(nx)
     p = gen.generate_lq_problem(rng, x0, N, nx, nu, nth, nc, singular=False, conditioned=True,
@@ -130,11 +134,129 @@ def make_problem(seed, N, nx, nu, nc, nct, nth):
     for k in p.stages:  # non-trivial parametric blocks everywhere
         k.Gx[...] = 0.3 * rng.standard_normal(k.Gx.shape)
         k.Gu[...] = 0.3 * rng.standard_normal(k.Gu.shape)
-        k.Gv[...] = 0.0  # (the reference's Vxt formula drops Z^T Gv; legs always have Gv = 0)
+        k.Gv[...] = 0.0
         g = rng.standard_normal((nth, nth))
         k.Gth[...] = g @ g.T / max(nth, 1) + np.eye(nth)
         k.gamma[...] = rng.standard_normal(nth)
+    if gv:
+        for k in p.stages:
+            k.Gv[...] = rng.standard_normal(k.Gv.shape)
     return p
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Parametric problems and leg mode at the level-2 bar
+# ---------------------------------------------------------------------------------------------------------------------
+# name: ((nx, nu, nc, nct, nth, N), batch, mueq, Gv != 0, nc0 of a Gaussian G0 (None: G0 = -I), theta scale)
+PARAM_CASES = {
+    "c3_mu1e-3": ((4, 2, 2, 0, 4, 20), 3, 1e-3, False, None, 1.0),
+    "c3_mu1e-8": ((4, 2, 2, 0, 4, 20), 3, 1e-8, False, None, 1.0),
+    "c3_gv": ((4, 2, 2, 0, 3, 12), 3, 1e-3, True, None, 1.0),
+    "nct_gv": ((4, 2, 2, 2, 3, 10), 2, 1e-3, True, None, 1.0),
+    "nth1": ((6, 3, 0, 0, 1, 8), 2, 1e-8, False, None, 1.0),
+    "nth_nx": ((6, 3, 0, 0, 6, 8), 2, 1e-8, False, None, 1.0),
+    "nth33": ((5, 2, 1, 0, 33, 4), 2, 1e-3, True, None, 1.0),
+    "N0": ((4, 2, 2, 2, 3, 0), 2, 1e-3, True, None, 1.0),
+    "N1": ((5, 2, 1, 0, 3, 1), 2, 1e-3, True, None, 1.0),
+    "theta1e6": ((6, 3, 1, 0, 4, 8), 2, 1e-3, True, None, 1e6),
+}
+for _nc0 in (0, 1, 3, 6):
+    PARAM_CASES["G0_nc0_%d" % _nc0] = ((6, 3, 1, 0, 3, 6), 2, 1e-3, True, _nc0, 1.0)
+
+
+def param_problems(name, B=None, seed=0):
+    """The problems and thetas [B][nth] of a parametric case (B instances, each its own problem and theta)."""
+    (nx, nu, nc, nct, nth, N), B0, mueq, gv, nc0, scale = PARAM_CASES[name]
+    B = B0 if B is None else B
+    base = 5000 + 100 * seed + sum(map(ord, name))
+    probs = [make_problem([base, b], N, nx, nu, nc, nct, nth, gv) for b in range(B)]
+    if nc0 is not None:
+        gen.general_initial_condition(probs, nc0, base)
+    thetas = scale * np.random.default_rng(base).standard_normal((B, nth))
+    return probs, thetas
+
+
+def oracle_parametric(probs, mueq, thetas):
+    """The oracle's ProximalRiccatiSolver on each problem, forward at its theta -> the outputs in hp_reference's
+    keys and the product's layouts (those of hp_reference.solve_parametric).  mueq: a number or one per instance."""
+    mus = np.broadcast_to(np.asarray(mueq, dtype=np.float64), (len(probs),))
+    per = []
+    for p, mu, th in zip(probs, mus, thetas):
+        N = p.horizon
+        nu, ncs = (p.stages[0].nu, p.stages[0].nc) if N else (0, 0)
+        op = orc.OracleProblem(p)
+        s = orc.ProximalRiccatiSolver(op)
+        assert s.backward(mu)
+        sol = orc.OracleSolution(op)
+        assert s.forward(sol, th)
+        fs = [s.factor(t) for t in range(N + 1)]
+        k0 = s.kkt0()
+        xs, us, vs, lb = sol.get()
+        nr, nc, nth = fs[0]["fb"].shape[0], len(vs[0]), len(th)
+        nct = fs[N]["fb"].shape[0] - fs[N]["dims"][1] - fs[N]["dims"][3]
+        stk = lambda lst, *shape: np.stack(lst) if lst else np.zeros(shape)
+        per.append(dict(fb=stk([f["fb"] for f in fs[:N]], 0, nr, len(xs[0])), ff=stk([f["ff"] for f in fs[:N]], 0, nr),
+                        fth=stk([f["fth"] for f in fs[:N]], 0, nr, nth),
+                        Vxx=np.stack([f["Vxx"] for f in fs]), vx=np.stack([f["vx"] for f in fs]),
+                        Vxt=np.stack([f["Vxt"] for f in fs]), Vtt=np.stack([f["Vtt"] for f in fs]),
+                        vt=np.stack([f["vt"] for f in fs]), fbT=fs[N]["fb"][:nct], ffT=fs[N]["ff"][:nct],
+                        kkt0=k0["ff"], kkt0fth=k0["fth"], thGrad=k0["thGrad"], thHess=k0["thHess"],
+                        xs=np.stack(xs), us=stk(us[:N], 0, nu).reshape(N, nu),
+                        vs=stk(vs[:N], 0, ncs).reshape(N, ncs), vsT=vs[N], lbd0=lb[0],
+                        lbdas=stk(lb[1:], 0, len(xs[0]))))
+    return hp.stack_solutions(per)
+
+
+def oracle_legs(probs, mueq, T):
+    """The oracle's ParallelRiccatiSolver with T legs on each problem -> its factors in the product's layouts (leg
+    mode: nth = nx, zero on the knots without parameters), its rollout, and `collapse`: the first gain after
+    collapseFeedback."""
+    per = []
+    for p in probs:
+        N, nx, nu = p.horizon, p.stages[0].nx, p.stages[0].nu
+        op = orc.OracleProblem(p.copy())
+        s = orc.ParallelRiccatiSolver(op, T, threaded=False)
+        assert s.backward(mueq)
+        sol = orc.OracleSolution(op)
+        assert s.forward(sol)
+        fs = [s.factor(t) for t in range(N + 1)]
+        par = lambda f, k, *shape: f[k] if f["dims"][4] else np.zeros(shape)
+        xs, us, vs, lb = sol.get()
+        nr = fs[0]["fb"].shape[0]
+        s.collapseFeedback()
+        per.append(dict(fb=np.stack([f["fb"] for f in fs[:N]]), ff=np.stack([f["ff"] for f in fs[:N]]),
+                        fth=np.stack([par(f, "fth", nr, nx) for f in fs[:N]]),
+                        Vxx=np.stack([f["Vxx"] for f in fs]), vx=np.stack([f["vx"] for f in fs]),
+                        Vxt=np.stack([par(f, "Vxt", nx, nx) for f in fs]),
+                        Vtt=np.stack([par(f, "Vtt", nx, nx) for f in fs]), vt=np.stack([par(f, "vt", nx) for f in fs]),
+                        fbT=fs[N]["fb"][:p.stages[N].nc], ffT=fs[N]["ff"][:p.stages[N].nc], xs=np.stack(xs), us=np.stack(us[:N]).reshape(N, nu),
+                        vs=np.stack(vs[:N]).reshape(N, p.stages[0].nc), vsT=vs[N], lbd0=lb[0],
+                        lbdas=np.stack(lb[1:]), collapse=s.factor(0)["fb"][:nu]))
+    return hp.stack_solutions(per)
+
+
+def param_oracle_errors(probs, mueq, thetas, ref):
+    """e_oracle of parametric problems against the restatement's fp64 outputs `ref`: the error families of the oracle's
+    ProximalRiccatiSolver, and on the theta-free factor families (K, k, Z, z, Vxx, vx) the larger of that and the
+    oracle's dense solver's on the same problems without parameters.  Both are correct fp64 solvers; where a quantity
+    comes out of a cancellation (z = (d + D k) / mu on an active row, say) one of them alone can land unrepresentatively
+    close, as in tests/test_hp_emulation.py's bar for the dense and leg programs."""
+    nx, nu, nc, nct, nc0, N = hp.dims_of(probs[0])
+    e = hp.error_families(oracle_parametric(probs, mueq, thetas), ref, nu, nc, N)
+    if N == 0:
+        return e
+    plain = []
+    for p in probs:
+        q = p.copy()
+        q.addParameterization(0)
+        plain.append(q)
+    dense = hp.error_families(run_solver(plain, (nx, nu, nc, nct, N), mueq, "dense"), ref, nu, nc, N,
+                              ("K", "k", "Z", "z", "Vxx", "vx"))
+    return {f: max(v, dense.get(f, 0.0)) for f, v in e.items()}
+
+
+PARAM_KEYS = ("fth", "Vxt", "Vtt", "vt", "kkt0fth", "thGrad", "thHess")
+LEG_FAMILIES = ("K", "k", "Z", "z", "Ahat", "a", "Vxx", "vx", "Kth", "Zth", "Yth", "Vxt", "Vtt", "vt", "collapse")
 
 
 def symmetric_dot(rng, d6, B):

@@ -9,11 +9,13 @@ from lq_cases import make_problem
 from oracle import gar_oracle as orc
 
 
+# (nx, nu, nc, nct, nth, N, mueq, warps[, Gv != 0])
 @pytest.mark.parametrize("shape", [(5, 2, 0, 0, 3, 6, 1e-8, 1), (4, 3, 2, 0, 2, 5, 1e-3, 1), (7, 3, 0, 2, 7, 4, 1e-2, 2),
-                                   (6, 2, 1, 0, 1, 3, 1e-3, 1)])
+                                   (6, 2, 1, 0, 1, 3, 1e-3, 1), (4, 3, 2, 0, 2, 5, 1e-3, 1, True),
+                                   (5, 2, 2, 2, 3, 4, 1e-2, 1, True)])
 def test_parametric_block_sweep(shape):
-    nx, nu, nc, nct, nth, N, mueq, nw = shape
-    p = make_problem(sum(shape[:6]), N, nx, nu, nc, nct, nth)
+    nx, nu, nc, nct, nth, N, mueq, nw = shape[:8]
+    p = make_problem(sum(shape[:6]), N, nx, nu, nc, nct, nth, gv=len(shape) > 8 and shape[8])
     theta = np.random.default_rng(3).standard_normal(nth)
     got = emulate("parametric", [p], (nx, nu, nc, nct, N), mueq, nw, nth=nth, theta=theta)
     assert got["status"][0] == 0

@@ -592,13 +592,14 @@ def test_kkt_error_of_every_instance_at_full_size(gar):
     s.close()
 
 
-@pytest.mark.parametrize("shape", [(5, 2, 0, 0, 3, 6, 1e-8), (4, 3, 2, 0, 2, 5, 1e-3), (7, 3, 0, 2, 7, 4, 1e-2)])
+@pytest.mark.parametrize("shape", [(5, 2, 0, 0, 3, 6, 1e-8), (4, 3, 2, 0, 2, 5, 1e-3), (7, 3, 0, 2, 7, 4, 1e-2),
+                                   (4, 3, 2, 0, 2, 5, 1e-3, True), (5, 2, 2, 2, 3, 4, 1e-2, True)])
 def test_parametric_problems(gar, shape):
     """nth > 0 (riccati-kernel.hxx:185-192, 278-311; proximal-riccati.hxx:50-59; forward with theta)
-    through the Python mirror of ProximalRiccatiSolver, against the oracle."""
+    through the Python mirror of ProximalRiccatiSolver, against the oracle.  shape[7]: Gv != 0."""
     import lq_cases
-    nx, nu, nc, nct, nth, N, mueq = shape
-    probs = [lq_cases.make_problem(50 + b, N, nx, nu, nc, nct, nth) for b in range(3)]
+    nx, nu, nc, nct, nth, N, mueq = shape[:7]
+    probs = [lq_cases.make_problem(50 + b, N, nx, nu, nc, nct, nth, gv=len(shape) > 7) for b in range(3)]
     solver = gar.ProximalRiccatiSolver(probs)
     assert solver.backward(mueq)
     thetas = np.random.default_rng(1).standard_normal((3, nth))
