@@ -37,6 +37,10 @@ with respect to the vectors.
 Hessian-vector products, ``torch.func.hessian``): every derivative is resolve plus the two stateless streaming maps
 ``ab2_gar_rho_many`` and ``ab2_gar_grad_many`` (DESIGN section 2p), through four Functions whose backward, jvp and vmap
 rules call each other.  ``lq_solve`` itself stays differentiable once.
+
+:func:`lq_solve_theta` solves a parametric problem (nth > 0) at ``theta`` and is differentiable with respect to theta,
+in both modes and to any order: the solution is affine in theta, and its Jacobian J is applied from the stored factors
+by ``ab2_gar_theta_tangent`` (J d) and ``ab2_gar_theta_adjoint`` (J^T zbar), one launch per vmap level.
 """
 from __future__ import annotations
 
@@ -930,3 +934,192 @@ def lq_solve_higher(batch, stage, term, G0, g0, mueq):
         raise ValueError(_NO_HIGHER_HANDLE)
     _check_inputs(batch, dict(stage=stage, term=term, G0=G0, g0=g0))
     return _Solve.apply(_Higher(batch, mueq), stage, term, G0, g0)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Derivatives of a parametric solution with respect to theta
+# ---------------------------------------------------------------------------------------------------------------------
+_NO_THETA_HANDLE = ("lq_solve_theta: parametric handles only (nth > 0); plain, dense and parallel handles have no theta "
+                    "to differentiate")
+_NO_THETA_VMAP = ("lq_solve_theta: vmap over theta or the problem data is not supported; vmap over cotangents and "
+                  "tangents is (torch.func.jacrev, jacfwd, hessian, vmap of a vjp or jvp function)")
+
+
+class _Theta(_Higher):
+    """The handle, mu and data of one lq_solve_theta call: its factorisation is re-made from the data P when another
+    call has moved the factor epoch (_Higher.factor)."""
+
+    def __init__(self, batch, mueq):
+        super().__init__(batch, mueq)
+        self.P = None
+        self.th = (batch.dims.batch, batch.nth)
+
+
+def _lead(ts, shapes):
+    """The broadcast leading dimensions of the operands ts over their base shapes (None operands left out)."""
+    leads = [tuple(t.shape[:t.dim() - len(s)]) for t, s in zip(ts, shapes) if t is not None]
+    return tuple(torch.broadcast_shapes(*leads)) if leads else ()
+
+
+def _count(lead):
+    n = 1
+    for m in lead:
+        n *= m
+    return n
+
+
+def _moved(info, t, bd):
+    """A vmapped operand with the level's dimension first (broadcast to it when unbatched)."""
+    if t is None:
+        return None
+    return t.movedim(bd, 0) if bd is not None else t.unsqueeze(0).expand(info.batch_size, *t.shape)
+
+
+class _LqSolveTheta(torch.autograd.Function):
+    """z = solve(P, theta): set_problem, backward, forward_theta.  jvp: J thetadot; vjp: J^T zbar."""
+
+    @staticmethod
+    def forward(h, stage, term, G0, g0, theta):
+        theta = _plain(theta)
+        stream = h.stream(theta.device)
+        h.P = tuple(_plain(t) for t in (stage, term, G0, g0))
+        h.batch.set_problem(*h.P, memspace=_gar.AB2_DEVICE, stream=stream)
+        h.batch.backward(h.mueq, stream=stream)
+        h.epoch = h.batch.factor_epoch()
+        h.batch.forward(stream=stream, theta=theta)
+        return _outputs(h.batch, theta.device, stream)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.h = inputs[0]
+        ctx.outs = [(o.shape, o.device) for o in output]
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *zbar):
+        if _none(zbar):
+            return (None,) * 6
+        return (None,) * 5 + (_ThetaAdjoint.apply(ctx.h, *zbar),)
+
+    @staticmethod
+    def jvp(ctx, _h, _stage, _term, _G0, _g0, dtheta):
+        if dtheta is None:
+            return tuple(torch.zeros(s, dtype=torch.float64, device=d) for s, d in ctx.outs)
+        return _ThetaTangent.apply(ctx.h, dtheta)
+
+    @staticmethod
+    def vmap(info, in_dims, h, stage, term, G0, g0, theta):
+        # torch runs the forward unbatched when no input is batched (jacfwd, vmap over cotangents); it needs this rule
+        # to exist all the same
+        raise NotImplementedError(_NO_THETA_VMAP)
+
+
+class _ThetaTangent(torch.autograd.Function):
+    """J d for directions d [..., batch, nth] (ab2_gar_theta_tangent, every leading index one direction).  Linear:
+    jvp J ddot, vjp J^T zbar."""
+
+    @staticmethod
+    def forward(h, d):
+        d = _plain(d)
+        lead = tuple(d.shape[:-2])
+        n = _count(lead)
+        outs = [torch.empty((n,) + s, dtype=torch.float64, device=d.device) for s in h.sol]
+        if n:
+            stream = h.stream(d.device)
+            h.factor(h.P, stream)
+            h.batch.theta_tangent(d.reshape(n, *h.th).to(torch.float64).contiguous(), dict(zip(_KEYS, outs)),
+                                  stream=stream)
+        return tuple(o.reshape(*lead, *o.shape[1:]) for o in outs)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.h = inputs[0]
+        ctx.outs = [(o.shape, o.device) for o in output]
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, *zbar):
+        if _none(zbar):
+            return None, None
+        return None, _ThetaAdjoint.apply(ctx.h, *zbar)
+
+    @staticmethod
+    def jvp(ctx, _h, ddot):
+        if ddot is None:
+            return tuple(torch.zeros(s, dtype=torch.float64, device=dv) for s, dv in ctx.outs)
+        return _ThetaTangent.apply(ctx.h, ddot)
+
+    @staticmethod
+    def vmap(info, in_dims, h, d):
+        return _ThetaTangent.apply(h, _moved(info, d, in_dims[1])), (0,) * 6
+
+
+class _ThetaAdjoint(torch.autograd.Function):
+    """J^T zbar for cotangents zbar in the solution's layouts behind any leading dimensions (ab2_gar_theta_adjoint;
+    None is zero).  Linear: jvp J^T zdot, vjp J thbar."""
+
+    @staticmethod
+    def forward(h, *zbar):
+        zbar = [None if t is None else _plain(t) for t in zbar]
+        lead = _lead(zbar, h.sol)
+        n = _count(lead)
+        device = _device(h, zbar)
+        tb = torch.empty((n,) + h.th, dtype=torch.float64, device=device)
+        if n:
+            stream = h.stream(device)
+            h.factor(h.P, stream)
+            cot = {k: None if t is None else t.expand(*lead, *s).reshape(n, *s).to(torch.float64).contiguous()
+                   for k, t, s in zip(_KEYS, zbar, h.sol)}
+            h.batch.theta_adjoint(cot, tb, stream=stream)
+        return tb.reshape(*lead, *h.th)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        ctx.h = inputs[0]
+        ctx.out = (output.shape, output.device)
+        ctx.set_materialize_grads(False)
+
+    @staticmethod
+    def backward(ctx, thbar):
+        if thbar is None:
+            return (None,) * 7
+        return (None,) + _pick(_ThetaTangent.apply(ctx.h, thbar), ctx.needs_input_grad[1:])
+
+    @staticmethod
+    def jvp(ctx, _h, *zdot):
+        if _none(zdot):
+            return torch.zeros(ctx.out[0], dtype=torch.float64, device=ctx.out[1])
+        return _ThetaAdjoint.apply(ctx.h, *zdot)
+
+    @staticmethod
+    def vmap(info, in_dims, h, *zbar):
+        return _ThetaAdjoint.apply(h, *[_moved(info, t, bd) for t, bd in zip(zbar, in_dims[1:])]), 0
+
+
+def lq_solve_theta(batch, stage, term, G0, g0, mueq, theta):
+    """Solve the parametric LQ problems of ``batch`` (a handle with nth > 0) at ``theta`` [batch][nth] on
+    ``torch.cuda.current_stream()``: set_problem, backward and the parametric forward pass.  Returns ``(xs, us, vs, vsT,
+    lam0, lams)`` in the solver's output layouts, differentiable with respect to ``theta`` in both modes and to any
+    order.  The solution is affine in theta, z = z_0 + J theta, and J comes from the stored factors without a new
+    factorisation: a vjp is one ``theta_adjoint`` launch (J^T zbar), a jvp one ``theta_tangent`` launch (J d), and under
+    vmap (``jacrev``, ``jacfwd``, ``hessian``) all the cotangents or tangents of a level go to one launch.  ``jacfwd`` is
+    the cheap direction: nth tangents.  When another call has refactored the handle since (its ``factor_epoch``
+    moved), set_problem and backward are run again before a derivative.  ``mueq`` (a number or a [batch] tensor) is not
+    differentiated, nor is the problem data: ``stage``, ``term``, ``G0`` and ``g0`` that require grad raise
+    ``ValueError``, as do handles without parameters (plain, dense, parallel) and a tensor that is not a contiguous
+    float64 CUDA tensor of the handle's shape, all before any library call.  vmap over ``theta`` or the data raises
+    ``NotImplementedError``."""
+    if not isinstance(batch, _gar.CudaRiccatiBatch):
+        raise ValueError("lq_solve_theta: `batch` must be a CudaRiccatiBatch")
+    if batch.nth == 0 or batch.dense or batch.legs:
+        raise ValueError(_NO_THETA_HANDLE)
+    _check_inputs(batch, dict(stage=stage, term=term, G0=G0, g0=g0))
+    for name, t in dict(stage=stage, term=term, G0=G0, g0=g0).items():
+        if t.requires_grad:
+            raise ValueError("lq_solve_theta: %s requires grad; derivatives with respect to the data of a parametric "
+                             "problem are not served, only with respect to theta" % name)
+    shape = (batch.dims.batch, batch.nth)
+    if (not isinstance(theta, torch.Tensor) or theta.dtype != torch.float64 or not theta.is_cuda
+            or not theta.is_contiguous() or tuple(theta.shape) != shape):
+        raise ValueError("lq_solve_theta: theta must be a contiguous float64 CUDA tensor of shape %s" % (shape,))
+    return _LqSolveTheta.apply(_Theta(batch, mueq), stage, term, G0, g0, theta)

@@ -75,7 +75,8 @@ def build(verbose=False, force=False, ptxas_v=False):
     for name, src in (("capi", "gar_cuda.cu"), ("block", "block_kernel.cu"),
                       ("assemble", "lq_assemble.cu"), ("adjoint", "lq_adjoint.cu"), ("resolve", "lq_resolve.cu"),
                       ("factor_adjoint", "lq_factor_adjoint.cu"), ("factor_tangent", "lq_factor_tangent.cu"),
-                      ("jacobian", "lq_jacobian.cu"), ("refine", "lq_refine.cu"), ("linesearch", "linesearch.cu"),
+                      ("jacobian", "lq_jacobian.cu"), ("refine", "lq_refine.cu"), ("theta", "lq_theta.cu"),
+                      ("linesearch", "linesearch.cu"),
                       ("inner", "proxddp_inner.cu")):
         obj(name, src)
     todo =[(o, c) for (o, c) in jobs if force or not os.path.exists(o)]

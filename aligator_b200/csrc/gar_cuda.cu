@@ -20,6 +20,7 @@
 #include "linesearch.h"
 #include "lq_adjoint.h"
 #include "lq_resolve.h"
+#include "lq_theta.h"
 #include "lq_factor_adjoint.h"
 #include "lq_factor_tangent.h"
 #include "lq_jacobian.h"
@@ -1223,6 +1224,116 @@ int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int n
   if (!mueq)
     return fail(AB2_ERR_INVALID, "null mueq array");
   return resolve_impl(s, 0.0, mueq, memspace, nrhs, rhs, out, stream);
+}
+
+// ---- derivatives of a parametric solution with respect to theta (lq_theta.cu): J d and J^T zbar from the stored
+//      factors, one launch each ----
+static const char *const kThetaNames[1] = {"theta"};
+// a [blocks][nth] theta array as one field
+static Fields theta_fields(const ab2_gar_solver *s, const char *what, const double *p, size_t blocks) {
+  const size_t per[1] = {(size_t)s->nth};
+  return make_fields(what, kThetaNames, {p}, per, blocks);
+}
+// The checks both calls share, in this order: handle kind, factorisation current, nrhs, then that one direction fits.
+static int check_theta_handle(const ab2_gar_solver *s, int nrhs, const char *who) {
+  if (s->nth == 0 || s->legs > 1 || s->dense)
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": handles without parameters (nth = 0, dense) and parallel handles are not supported");
+  if (!s->have_problem || !s->factor_current)
+    return fail(AB2_ERR_STATE, std::string(who) + ": no backward since the last set_problem or assemble");
+  if (nrhs < 0)
+    return fail(AB2_ERR_INVALID, std::string(who) + ": nrhs < 0");
+  return AB2_OK;
+}
+static int check_theta_fits(const ab2_gar_solver *s, const char *who) {
+  const ab2_gar_dims &d = s->d;
+  if ((size_t)ab2::theta_item_doubles(d.nx, d.nu, d.nc, d.nct, d.nc0, s->nth, 1) * sizeof(double) > ab2::kThetaSmemMax)
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one direction of this shape does not fit 227 KB of shared memory");
+  return AB2_OK;
+}
+// The stored factorisation as the theta programs read it (parametric handles run the CTA kernel: full VXX blocks).
+static ab2::ThetaArgs theta_view(const ab2_gar_solver *s, int nrhs) {
+  const ab2_gar_dims &d = s->d;
+  ab2::ThetaArgs a{};
+  a.batch = d.batch;
+  a.N = d.horizon;
+  a.nx = d.nx;
+  a.nu = d.nu;
+  a.nc = d.nc;
+  a.nct = d.nct;
+  a.nc0 = d.nc0;
+  a.nth = s->nth;
+  a.nrhs = nrhs;
+  a.fb = s->out[AB2_OUT_FB];
+  a.fth = s->out[AB2_OUT_FTH];
+  a.fbT = s->out[AB2_OUT_FBT];
+  a.Vxx = s->out[AB2_OUT_VXX];
+  a.Vxt = s->out[AB2_OUT_VXT];
+  a.kkt0fth = s->out[AB2_OUT_KKT0FTH];
+  return a;
+}
+int ab2_gar_theta_tangent(ab2_gar_solver *s, int nrhs, const double *dtheta, const ab2_ls_trial *out, void *stream) {
+  if (!s || !out)
+    return fail(AB2_ERR_INVALID, "null argument");
+  const char *who = "theta_tangent";
+  if (int rc = check_theta_handle(s, nrhs, who))
+    return rc;
+  const size_t R = (size_t)nrhs * s->d.batch;
+  const Fields O = sol_fields(s, "out", *out, R), T = theta_fields(s, "dtheta", dtheta, R);
+  if (int rc = require(sol_fields(s, "out", *out, 1), who)) // (refused even at nrhs = 0)
+    return rc;
+  if (int rc = require(theta_fields(s, "dtheta", dtheta, 1), who))
+    return rc;
+  if (int rc = refuse_overlap(T, O, who))
+    return rc;
+  if (int rc = refuse_overlap(O, out_fields(s), who))
+    return rc;
+  if (int rc = check_theta_fits(s, who))
+    return rc;
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(s->d.device));
+  ab2::ThetaArgs a = theta_view(s, nrhs);
+  a.dtheta = dtheta;
+  a.xs = out->xs;
+  a.us = out->us;
+  a.vs = out->vs;
+  a.vsT = out->vsT;
+  a.lam0 = out->lam0;
+  a.lams = out->lams;
+  CUDA_TRY(ab2::launch_theta_tangent(a, (cudaStream_t)stream));
+  s->launches += 1;
+  return AB2_OK;
+}
+int ab2_gar_theta_adjoint(ab2_gar_solver *s, int nrhs, const ab2_ls_iterate *cot, double *theta_bar, void *stream) {
+  if (!s || !cot)
+    return fail(AB2_ERR_INVALID, "null argument");
+  const char *who = "theta_adjoint";
+  if (int rc = check_theta_handle(s, nrhs, who))
+    return rc;
+  const size_t R = (size_t)nrhs * s->d.batch;
+  const Fields T = theta_fields(s, "theta_bar", theta_bar, R);
+  if (int rc = require(theta_fields(s, "theta_bar", theta_bar, 1), who)) // (refused even at nrhs = 0)
+    return rc;
+  if (int rc = refuse_overlap(sol_fields(s, "cot", *cot, R), T, who))
+    return rc;
+  if (int rc = refuse_overlap(T, out_fields(s), who))
+    return rc;
+  if (int rc = check_theta_fits(s, who))
+    return rc;
+  if (nrhs == 0)
+    return AB2_OK;
+  CUDA_TRY(cudaSetDevice(s->d.device));
+  ab2::ThetaArgs a = theta_view(s, nrhs);
+  a.cxs = cot->xs;
+  a.cus = cot->us;
+  a.cvs = cot->vs;
+  a.cvsT = cot->vsT;
+  a.clam0 = cot->lam0;
+  a.clams = cot->lams;
+  a.theta_bar = theta_bar;
+  CUDA_TRY(ab2::launch_theta_adjoint(a, (cudaStream_t)stream));
+  s->launches += 1;
+  return AB2_OK;
 }
 // ---- derivatives of the backward recursion (lq_factor_adjoint.cu, lq_factor_tangent.cu) ----
 // The handle checks ab2_gar_factor_adjoint and ab2_gar_factor_tangent share: handle kind, and a backward on the

@@ -210,6 +210,8 @@ def lib():
         L.ab2_gar_resolve.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LqRhs), C.POINTER(LsIterate),
                                       C.c_void_p]
         L.ab2_gar_factor_epoch.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
+        L.ab2_gar_theta_tangent.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(LsIterate), C.c_void_p]
+        L.ab2_gar_theta_adjoint.argtypes = [C.c_void_p, C.c_int, C.POINTER(LsIterate), C.c_void_p, C.c_void_p]
         L.ab2_gar_adjoint_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LsIterate), C.POINTER(LsIterate),
                                            C.POINTER(LsIterate), C.POINTER(LqGrad), C.c_void_p]
         L.ab2_gar_tangent_many.argtypes = [C.c_void_p, C.c_double, C.c_int, C.POINTER(LsIterate), C.POINTER(LqTangent),
@@ -409,9 +411,17 @@ class CudaRiccatiBatch:
         self._mu_call("backward", mueq, stream, None)
 
     def forward(self, stream=0, theta=None):
-        """forward(); with ``theta`` ([batch][nth] host array) the parametric rollout."""
+        """forward(); with ``theta`` ([batch][nth]) the parametric rollout.  A CUDA tensor is read on the device,
+        stream-ordered (no synchronisation); anything else is copied from the host and the call synchronises."""
         if theta is None:
             _check(lib().ab2_gar_forward(self.h, C.c_void_p(stream)))
+        elif hasattr(theta, "is_cuda") and theta.is_cuda:
+            import torch
+            if theta.dtype != torch.float64 or theta.numel() != self.dims.batch * self.nth:
+                raise ValueError("theta: expected %d float64 values ([batch][nth])" % (self.dims.batch * self.nth))
+            th = theta.contiguous()
+            self._keep["forward"] = th
+            _check(lib().ab2_gar_forward_theta(self.h, _ptr(th), AB2_DEVICE, C.c_void_p(stream)))
         else:
             th = np.ascontiguousarray(theta, dtype=np.float64)
             assert th.size == self.dims.batch * self.nth
@@ -691,6 +701,29 @@ class CudaRiccatiBatch:
         rh = _fill(LqRhs(), _RHS_KEYS, rhs)
         ot = _fill(LsIterate(), _LS_KEYS, out)
         self._mu_call("resolve", mueq, stream, (rhs, out), int(nrhs), C.byref(rh), C.byref(ot))
+
+    def theta_tangent(self, dtheta, out, stream=0):
+        """J d for a parametric handle (``ab2_gar_theta_tangent``): the derivative of ``forward(theta=...)``'s
+        solution along each direction d.  ``dtheta``: device tensor [nrhs][batch][nth]; ``out``: dict with keys xs, us,
+        vs, vsT, lam0, lams of device tensors [nrhs][batch][...] in the solution's layouts, overwritten.  nrhs is read
+        from ``dtheta``.  Reads only the last backward's factors; the handle's outputs are not touched."""
+        d = self.dims
+        nrhs = dtheta.numel() // (d.batch * self.nth)
+        ot = _fill(LsIterate(), _LS_KEYS, out)
+        self._keep["theta_tangent"] = (dtheta, out)
+        _check(lib().ab2_gar_theta_tangent(self.h, int(nrhs), _ptr(dtheta), C.byref(ot), C.c_void_p(stream)))
+
+    def theta_adjoint(self, cot, theta_bar, stream=0):
+        """J^T zbar for a parametric handle (``ab2_gar_theta_adjoint``): the gradient with respect to theta of a loss
+        whose cotangents with respect to the solution are ``cot``, a dict with any of xs, us, vs, vsT, lam0, lams of
+        device tensors [nrhs][batch][...] (a key that is missing or None is zero).  ``theta_bar``: device tensor
+        [nrhs][batch][nth], overwritten; nrhs is read from it.  Reads only the last backward's factors; the handle's
+        outputs are not touched."""
+        d = self.dims
+        nrhs = theta_bar.numel() // (d.batch * self.nth)
+        ct = _fill(LsIterate(), _LS_KEYS, cot)
+        self._keep["theta_adjoint"] = (cot, theta_bar)
+        _check(lib().ab2_gar_theta_adjoint(self.h, int(nrhs), C.byref(ct), _ptr(theta_bar), C.c_void_p(stream)))
 
     def adjoint_many(self, primal, cotangent, work, grad, mueq, stream=0):
         """Many cotangents on the last backward's factorisation (``ab2_gar_adjoint_many``): ``grad`` receives, for every

@@ -481,6 +481,37 @@ int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int n
  * belong to is still the handle's.  A host-side increment; it changes nothing those calls compute. */
 int ab2_gar_factor_epoch(const ab2_gar_solver *s, long long *epoch);
 
+/* Derivatives of a parametric solution with respect to theta (handles of ab2_gar_create_parametric, nth > 0).  The
+ * matrices do not depend on theta, so forward_theta's solution is affine in it, z(theta) = z_0 + J theta, and J is
+ * made of the factors the last backward stored: FB = [K; Z; Ahat], FTH = [Kth; Zth; Yth], VXX, VXT, FBT (Z_N) and
+ * F0 = KKT0FTH (rows x_0, then lam_0).  theta_tangent returns J d for directions d, theta_adjoint J^T zbar for
+ * cotangents zbar (the gradient of a loss with respect to theta); neither refactors or sweeps.
+ *   theta_tangent (the theta terms of forward_theta, without its feed-forward terms):
+ *     x_0 = F0_x d,  lam_0 = F0_lam d
+ *     t = 0..N-1:  u_t = K_t x_t + Kth_t d,  v_t = Z_t x_t + Zth_t d,  x_{t+1} = Ahat_t x_t + Yth_t d,
+ *                  lam_{t+1} = Vxx_{t+1} x_{t+1} + Vxt_{t+1} d
+ *     v_N = Z_N x_N   (the terminal knot has no theta term, as in forward_theta)
+ *   theta_adjoint (its exact transpose), cotangents (xbar, ubar, vbar, vbar_N, lambar_0, lambar) and c_t the
+ *   cotangent of x_t:
+ *     c_N = xbar_N + Z_N^T vbar_N + Vxx_N lambar_N,  thbar = Vxt_N^T lambar_N        (the Vxx and Vxt terms for N >= 1)
+ *     t = N-1..0:  thbar += Kth_t^T ubar_t + Zth_t^T vbar_t + Yth_t^T c_{t+1}  (+ Vxt_t^T lambar_t for t >= 1)
+ *                  c_t = xbar_t + K_t^T ubar_t + Z_t^T vbar_t + Ahat_t^T c_{t+1}  (+ Vxx_t lambar_t for t >= 1)
+ *     thbar += F0_x^T c_0 + F0_lam^T lambar_0
+ * Layouts: dtheta and theta_bar are [nrhs][batch][nth]; out and cot are [nrhs][batch][...] in the solution's layouts
+ * (ab2_ls_trial / ab2_ls_iterate, lams[t] = lambda_{t+1}); block j * batch + b is direction j of instance b.  Every
+ * array is DEVICE memory.  A NULL cot field is zero; dtheta, theta_bar and every out field of nonzero size are
+ * required.  No mu argument: only the stored factorisation is read.  The calls write the caller's arrays and nothing
+ * else: every handle output (FF .. THHESS), the status words, the pivot statistics and ab2_gar_factor_epoch are
+ * unchanged.  One launch each on `stream`; direction j's result is bit for bit independent of nrhs and of j's
+ * position (one warp per instance and chunk of directions, no atomics).
+ * Errors (nothing is launched), checked in this order: AB2_ERR_UNSUPPORTED for handles without parameters (nth = 0,
+ * dense) and parallel handles (their theta is implicit); AB2_ERR_STATE when no backward has run since the last
+ * set_problem or assemble; AB2_ERR_INVALID for nrhs < 0, a NULL required field, dtheta or cot overlapping out or
+ * theta_bar, or out or theta_bar overlapping an output of the handle.  A shape whose one direction needs more than
+ * 227 KB of shared memory returns AB2_ERR_UNSUPPORTED.  nrhs == 0 launches nothing. */
+int ab2_gar_theta_tangent(ab2_gar_solver *s, int nrhs, const double *dtheta, const ab2_ls_trial *out, void *stream);
+int ab2_gar_theta_adjoint(ab2_gar_solver *s, int nrhs, const ab2_ls_iterate *cot, double *theta_bar, void *stream);
+
 /* Jacobians of the LQ solution with respect to the problem data: many cotangents (reverse mode) or many tangents
  * (forward mode) on the last backward's factorisation, through ab2_gar_resolve's program (resolve(h) = -K^-1 h), without
  * re-running the matrix recursion per right-hand side.
