@@ -73,10 +73,8 @@ def build(verbose=False, force=False, ptxas_v=False):
         obj("k_%d_%d_%d" % (nx, nu, nc), "kernel_inst.cu",
             ["-DAB2_NX=%d" % nx, "-DAB2_NU=%d" % nu, "-DAB2_NC=%d" % nc, "-DAB2_G=%d" % g], "%d_%d_%d_%d" % (nx, nu, nc, g))
     for name, src in (("capi", "gar_cuda.cu"), ("block", "block_kernel.cu"),
-                      ("assemble", "lq_assemble.cu"), ("adjoint", "lq_adjoint.cu"), ("resolve", "lq_resolve.cu"),
-                      ("factor_adjoint", "lq_factor_adjoint.cu"), ("factor_tangent", "lq_factor_tangent.cu"),
-                      ("jacobian", "lq_jacobian.cu"), ("refine", "lq_refine.cu"), ("theta", "lq_theta.cu"),
-                      ("linesearch", "linesearch.cu"),
+                      ("assemble", "lq_assemble.cu"), ("adjoint", "lq_adjoint.cu"), ("lq_items", "lq_items.cu"),
+                      ("jacobian", "lq_jacobian.cu"), ("refine", "lq_refine.cu"), ("linesearch", "linesearch.cu"),
                       ("inner", "proxddp_inner.cu")):
         obj(name, src)
     todo =[(o, c) for (o, c) in jobs if force or not os.path.exists(o)]

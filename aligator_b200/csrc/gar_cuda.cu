@@ -19,10 +19,7 @@
 #include "../../include/aligator_b200/gar.h"
 #include "linesearch.h"
 #include "lq_adjoint.h"
-#include "lq_resolve.h"
-#include "lq_theta.h"
-#include "lq_factor_adjoint.h"
-#include "lq_factor_tangent.h"
+#include "lq_items.h"
 #include "lq_jacobian.h"
 #include "lq_refine.h"
 #include "lq_assemble.h"
@@ -1125,7 +1122,7 @@ int ab2_gar_tangent_v(ab2_gar_solver *s, const double *mueq, int memspace, const
   return tangent_impl(s, 0.0, mueq, memspace, primal, dot, stream);
 }
 
-// ---- re-solve for new vectors (lq_resolve.cu): the vector half of the recursion on the last backward's factorisation ----
+// ---- re-solve for new vectors (lq_resolve.cuh): the vector half of the recursion on the last backward's factorisation ----
 // The first checks of every call that runs resolve's program, in this order: handle kind, factorisation current, nrhs.
 static int check_resolve_handle(const ab2_gar_solver *s, int nrhs, const char *who) {
   if (s->nth > 0 || s->legs > 1 || s->dense)
@@ -1136,11 +1133,16 @@ static int check_resolve_handle(const ab2_gar_solver *s, int nrhs, const char *w
     return fail(AB2_ERR_INVALID, std::string(who) + ": nrhs < 0");
   return AB2_OK;
 }
-static int check_resolve_fits(const ab2_gar_solver *s, const char *who) {
-  const ab2_gar_dims &d = s->d;
-  if ((size_t)ab2::resolve_item_doubles(d.nx, d.nu, d.nc, d.nc0, 1) * sizeof(double) > ab2::kResolveSmemMax)
-    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one right-hand side of this shape does not fit 227 KB of shared memory");
+// AB2_ERR_UNSUPPORTED when one column or instance of an item program (lq_items.h), `bytes` of shared memory, does not
+// fit one CTA; unit: "right-hand side", "direction" or "instance".
+static int check_item_fits(size_t bytes, const char *unit, const char *who) {
+  if (bytes > (size_t)ab2::kItemSmemMax)
+    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one " + unit + " of this shape does not fit 227 KB of shared memory");
   return AB2_OK;
+}
+// shared memory of one right-hand side of resolve's program
+static size_t resolve_column_bytes(const ab2_gar_dims &d) {
+  return (size_t)ab2::resolve_item_doubles(d.nx, d.nu, d.nc, d.nc0, 1) * sizeof(double);
 }
 // The records and the last backward's factorisation as resolve's program reads them (no right-hand sides).
 static ab2::ResolveArgs factor_view(const ab2_gar_solver *s, double mueq, const double *mu_dev) {
@@ -1205,7 +1207,7 @@ static int resolve_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, 
   // that overlaps an rhs array would be read after it was overwritten
   if (int rc = refuse_overlap(rhs_fields(s, "rhs", *rhs, R), sol_fields(s, "out", *out, R), who))
     return rc;
-  if (int rc = check_resolve_fits(s, who))
+  if (int rc = check_item_fits(resolve_column_bytes(s->d), "right-hand side", who))
     return rc;
   if (nrhs == 0)
     return AB2_OK;
@@ -1226,7 +1228,7 @@ int ab2_gar_resolve_v(ab2_gar_solver *s, const double *mueq, int memspace, int n
   return resolve_impl(s, 0.0, mueq, memspace, nrhs, rhs, out, stream);
 }
 
-// ---- derivatives of a parametric solution with respect to theta (lq_theta.cu): J d and J^T zbar from the stored
+// ---- derivatives of a parametric solution with respect to theta (lq_theta.cuh): J d and J^T zbar from the stored
 //      factors, one launch each ----
 static const char *const kThetaNames[1] = {"theta"};
 // a [blocks][nth] theta array as one field
@@ -1244,11 +1246,10 @@ static int check_theta_handle(const ab2_gar_solver *s, int nrhs, const char *who
     return fail(AB2_ERR_INVALID, std::string(who) + ": nrhs < 0");
   return AB2_OK;
 }
-static int check_theta_fits(const ab2_gar_solver *s, const char *who) {
+// shared memory of one direction of the theta programs
+static size_t theta_column_bytes(const ab2_gar_solver *s) {
   const ab2_gar_dims &d = s->d;
-  if ((size_t)ab2::theta_item_doubles(d.nx, d.nu, d.nc, d.nct, d.nc0, s->nth, 1) * sizeof(double) > ab2::kThetaSmemMax)
-    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one direction of this shape does not fit 227 KB of shared memory");
-  return AB2_OK;
+  return (size_t)ab2::theta_item_doubles(d.nx, d.nu, d.nc, d.nct, d.nc0, s->nth, 1) * sizeof(double);
 }
 // The stored factorisation as the theta programs read it (parametric handles run the CTA kernel: full VXX blocks).
 static ab2::ThetaArgs theta_view(const ab2_gar_solver *s, int nrhs) {
@@ -1287,7 +1288,7 @@ int ab2_gar_theta_tangent(ab2_gar_solver *s, int nrhs, const double *dtheta, con
     return rc;
   if (int rc = refuse_overlap(O, out_fields(s), who))
     return rc;
-  if (int rc = check_theta_fits(s, who))
+  if (int rc = check_item_fits(theta_column_bytes(s), "direction", who))
     return rc;
   if (nrhs == 0)
     return AB2_OK;
@@ -1318,7 +1319,7 @@ int ab2_gar_theta_adjoint(ab2_gar_solver *s, int nrhs, const ab2_ls_iterate *cot
     return rc;
   if (int rc = refuse_overlap(T, out_fields(s), who))
     return rc;
-  if (int rc = check_theta_fits(s, who))
+  if (int rc = check_item_fits(theta_column_bytes(s), "direction", who))
     return rc;
   if (nrhs == 0)
     return AB2_OK;
@@ -1335,7 +1336,7 @@ int ab2_gar_theta_adjoint(ab2_gar_solver *s, int nrhs, const ab2_ls_iterate *cot
   s->launches += 1;
   return AB2_OK;
 }
-// ---- derivatives of the backward recursion (lq_factor_adjoint.cu, lq_factor_tangent.cu) ----
+// ---- derivatives of the backward recursion (lq_factor_adjoint.cuh, lq_factor_tangent.cuh) ----
 // The handle checks ab2_gar_factor_adjoint and ab2_gar_factor_tangent share: handle kind, and a backward on the
 // problem's own vectors.
 static int check_factor_handle(const ab2_gar_solver *s, const char *who) {
@@ -1346,7 +1347,7 @@ static int check_factor_handle(const ab2_gar_solver *s, const char *who) {
   return AB2_OK;
 }
 
-// ---- reverse mode of the backward recursion (lq_factor_adjoint.cu): cotangents of the factorisation -> gradients ----
+// ---- reverse mode of the backward recursion (lq_factor_adjoint.cuh): cotangents of the factorisation -> gradients ----
 static int factor_adjoint_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
                                const ab2_factor_cotangent *cot, const ab2_lq_grad *grad, void *stream) {
   if (!s || !cot || !grad)
@@ -1363,8 +1364,8 @@ static int factor_adjoint_impl(ab2_gar_solver *s, double mueq, const double *mue
     return rc;
   if (int rc = refuse_overlap(G, out_fields(s), who))
     return rc;
-  if ((size_t)ab2::factor_adjoint_item_doubles(d.nx, d.nu, d.nc) * sizeof(double) > ab2::kFactorAdjointSmemMax)
-    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one instance of this shape does not fit 227 KB of shared memory");
+  if (int rc = check_item_fits((size_t)ab2::factor_adjoint_item_doubles(d.nx, d.nu, d.nc) * sizeof(double), "instance", who))
+    return rc;
   cudaStream_t st;
   const double *mu_dev;
   if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
@@ -1399,7 +1400,7 @@ int ab2_gar_factor_adjoint_v(ab2_gar_solver *s, const double *mueq, int memspace
   return factor_adjoint_impl(s, 0.0, mueq, memspace, cot, grad, stream);
 }
 
-// ---- forward mode of the backward recursion (lq_factor_tangent.cu): tangent records -> tangents of the factorisation ----
+// ---- forward mode of the backward recursion (lq_factor_tangent.cuh): tangent records -> tangents of the factorisation ----
 static int factor_tangent_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace,
                                const ab2_lq_tangent *dot, const ab2_factor_tangent *out, void *stream) {
   if (!s || !dot || !out)
@@ -1416,8 +1417,8 @@ static int factor_tangent_impl(ab2_gar_solver *s, double mueq, const double *mue
     return rc;
   if (int rc = refuse_overlap(O, out_fields(s), who))
     return rc;
-  if ((size_t)ab2::factor_tangent_item_doubles(d.nx, d.nu, d.nc) * sizeof(double) > ab2::kFactorTangentSmemMax)
-    return fail(AB2_ERR_UNSUPPORTED, std::string(who) + ": one instance of this shape does not fit 227 KB of shared memory");
+  if (int rc = check_item_fits((size_t)ab2::factor_tangent_item_doubles(d.nx, d.nu, d.nc) * sizeof(double), "instance", who))
+    return rc;
   cudaStream_t st;
   const double *mu_dev;
   if (int rc = begin_launch(s, mueq_arr, memspace, stream, &st, &mu_dev))
@@ -1482,7 +1483,7 @@ static int adjoint_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
                               FieldPair{&G, &G}})
     if (int rc = refuse_overlap(*ab.first, *ab.second, who))
       return rc;
-  if (int rc = check_resolve_fits(s, who))
+  if (int rc = check_item_fits(resolve_column_bytes(s->d), "right-hand side", who))
     return rc;
   if (nrhs == 0)
     return AB2_OK;
@@ -1541,7 +1542,7 @@ static int tangent_many_impl(ab2_gar_solver *s, double mueq, const double *mueq_
                               FieldPair{&O, &O}})
     if (int rc = refuse_overlap(*ab.first, *ab.second, who))
       return rc;
-  if (int rc = check_resolve_fits(s, who))
+  if (int rc = check_item_fits(resolve_column_bytes(s->d), "right-hand side", who))
     return rc;
   if (nrhs == 0)
     return AB2_OK;
@@ -1774,7 +1775,7 @@ static int check_refine_args(const ab2_gar_solver *s, double mueq, const double 
     return fail(AB2_ERR_INVALID, std::string(who) + ": steps < 0");
   if (int rc = check_mu(s, mueq, mueq_arr, who))
     return rc;
-  return check_resolve_fits(s, who);
+  return check_item_fits(resolve_column_bytes(s->d), "right-hand side", who);
 }
 
 static int refine_impl(ab2_gar_solver *s, double mueq, const double *mueq_arr, int memspace, int steps, double *norms,

@@ -1,5 +1,5 @@
 // lq_jacobian.cu -- the two streaming kernels of ab2_gar_adjoint_many and ab2_gar_tangent_many: many cotangents or
-// tangents per factorisation, around ab2_gar_resolve's program (lq_resolve.cu), which solves z = resolve(h) = -K^-1 h.
+// tangents per factorisation, around ab2_gar_resolve's program (lq_resolve.cuh), which solves z = resolve(h) = -K^-1 h.
 // ab2_gar_adjoint and ab2_gar_tangent run the same kernels at nrhs = 1 around their own sweep (gar_cuda.cu).
 //  * jacobian_grad_kernel: reverse mode.  For cotangent j, y_j = resolve(zbar_j) = -K^-1 zbar_j, so the gradients of
 //    ab2_gar_adjoint (dh = -w, dK = -w z^T with w = K^-1 zbar) are dh = y_j and dK = y_j z^T read out of K's blocks:

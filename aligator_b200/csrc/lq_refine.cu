@@ -1,6 +1,6 @@
 // lq_refine.cu -- the residual kernel of ab2_gar_refine, ab2_gar_refine_many and ab2_gar_kkt_error.  Refinement
 // improves a solution estimate z of K z = -h on the last backward's factorisation, with resolve(r) = -K^-1 r
-// (lq_resolve.cu) as the correction solver and linear_step_kernel (linesearch.cu) as the update z += delta.  The update
+// (lq_resolve.cuh) as the correction solver and linear_step_kernel (linesearch.cu) as the update z += delta.  The update
 // cannot be fused into the next residual launch: the residual of knot t reads x_{t+1} and lambda_t, which other warps
 // would be updating.
 //  * refine_residual_kernel: r = K z + h in resolve's rhs layouts, row by row (lambda_{t+1} = lams[t], lambda_t =

@@ -1,7 +1,7 @@
 // The host emulation library of the device programs: the warp-per-instance group program (group_emu.cpp), the
 // CTA-per-instance program with its leg mode, and the stage-dense program (block_emu.cpp), and the per-item programs of
-// resolve and the factorisation's derivatives (resolve_emu.cpp, factor_adjoint_emu.cpp, factor_tangent_emu.cpp), in one
-// translation unit.
+// resolve, the θ derivatives and the factorisation's derivatives (resolve_emu.cpp, theta_emu.cpp,
+// factor_adjoint_emu.cpp, factor_tangent_emu.cpp), in one translation unit.
 // TEST INFRASTRUCTURE.  Every entry point takes a complete ab2::SweepParams; the layout exports below let the
 // caller's mirror of that struct check itself against this build.
 #include <cstddef>
@@ -13,14 +13,16 @@
 #include "factor_tangent_emu.cpp"
 #include "group_emu.cpp"
 #include "resolve_emu.cpp"
+#include "theta_emu.cpp"
 
 // Every shape `supported` (the library's ab2_gar_supported) accepts with nx, nu, nc < lim and nc0 in {0, 1, nx/2, nx},
-// for the factorisation's derivative program whose item size is `item_bytes` (emu_factor_adjoint_item_bytes or
-// emu_factor_tangent_item_bytes): how many are accepted (*accepted), how many of those need more than 227 KB of shared
-// memory (the return value; the first one in *bad = nx, nu, nc, nc0), and the largest item that fits, in bytes
-// (*largest).
-extern "C" long emu_factor_size_scan(long (*item_bytes)(int, int, int), int (*supported)(int, int, int, int), int lim,
-                                     int *bad, long *largest, long *accepted) {
+// and with nct in {0, nx} and nth in {1, nx, 33} when `parametric` (nct = nth = 0 otherwise), for the item program
+// whose item of one column or instance takes item_bytes(nx, nu, nc, nct, nc0, nth, 1) bytes of shared memory (one of
+// the emu_*_item_bytes): how many are accepted (*accepted), how many of those need more than 227 KB (the return
+// value; the first one in *bad = nx, nu, nc, nc0, nct, nth), and the largest item that fits, in bytes (*largest).
+extern "C" long emu_item_size_scan(long (*item_bytes)(int, int, int, int, int, int, int), int parametric,
+                                   int (*supported)(int, int, int, int), int lim, int *bad, long *largest,
+                                   long *accepted) {
   long over = 0;
   *largest = 0;
   *accepted = 0;
@@ -34,14 +36,19 @@ extern "C" long emu_factor_size_scan(long (*item_bytes)(int, int, int), int (*su
             continue;
           if (!supported(nx, nu, nc, nc0))
             continue;
-          ++*accepted;
-          const long bytes = item_bytes(nx, nu, nc);
-          if (bytes > 227 * 1024) {
-            if (over++ == 0)
-              bad[0] = nx, bad[1] = nu, bad[2] = nc, bad[3] = nc0;
-          } else if (bytes > *largest) {
-            *largest = bytes;
-          }
+          const int ncts[2] = {0, nx}, nths[3] = {1, nx, 33};
+          for (int t = 0; t < (parametric ? 2 : 1); ++t)
+            for (int h = 0; h < (parametric ? 3 : 1); ++h) {
+              const int nct = ncts[t], nth = parametric ? nths[h] : 0;
+              ++*accepted;
+              const long bytes = item_bytes(nx, nu, nc, nct, nc0, nth, 1);
+              if (bytes > 227 * 1024) {
+                if (over++ == 0)
+                  bad[0] = nx, bad[1] = nu, bad[2] = nc, bad[3] = nc0, bad[4] = nct, bad[5] = nth;
+              } else if (bytes > *largest) {
+                *largest = bytes;
+              }
+            }
         }
       }
   return over;

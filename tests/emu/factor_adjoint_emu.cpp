@@ -19,13 +19,12 @@ extern "C" int emu_factor_adjoint(const int *dims, double mueq, const double *mu
   a.g_stage = out[0], a.g_term = out[1], a.g_G0 = out[2], a.g_g0 = out[3];
   r.mueq = mueq;
   r.mueq_b = mueq_b;
-  std::vector<double> sm(ab2::factor_adjoint_item_doubles(r.nx, r.nu, r.nc));
-  for (long b = 0; b < r.batch; ++b) {
-    run_lanes(nl, [&](const EmuCtx &ctx) { ab2::factor_adjoint_item(a, ctx, sm.data(), b); });
-  }
+  run_instances(r.batch, nl, ab2::factor_adjoint_item_doubles(r.nx, r.nu, r.nc),
+                [&](const EmuCtx &ctx, double *sm, long b) { ab2::factor_adjoint_item(a, ctx, sm, b); });
   return 0;
 }
 
-extern "C" long emu_factor_adjoint_item_bytes(int nx, int nu, int nc) {
+// bytes of shared memory one instance uses (nct, nc0, nth, chunk: not read)
+extern "C" long emu_factor_adjoint_item_bytes(int nx, int nu, int nc, int nct, int nc0, int nth, int chunk) {
   return (long)ab2::factor_adjoint_item_doubles(nx, nu, nc) * (long)sizeof(double);
 }

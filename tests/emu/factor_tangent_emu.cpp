@@ -19,13 +19,12 @@ extern "C" int emu_factor_tangent(const int *dims, double mueq, const double *mu
   a.o_ff = out[0], a.o_fb = out[1], a.o_vxx = out[2], a.o_vx = out[3], a.o_fft = out[4], a.o_fbt = out[5];
   r.mueq = mueq;
   r.mueq_b = mueq_b;
-  std::vector<double> sm(ab2::factor_tangent_item_doubles(r.nx, r.nu, r.nc));
-  for (long b = 0; b < r.batch; ++b) {
-    run_lanes(nl, [&](const EmuCtx &ctx) { ab2::factor_tangent_item(a, ctx, sm.data(), b); });
-  }
+  run_instances(r.batch, nl, ab2::factor_tangent_item_doubles(r.nx, r.nu, r.nc),
+                [&](const EmuCtx &ctx, double *sm, long b) { ab2::factor_tangent_item(a, ctx, sm, b); });
   return 0;
 }
 
-extern "C" long emu_factor_tangent_item_bytes(int nx, int nu, int nc) {
+// bytes of shared memory one instance uses (nct, nc0, nth, chunk: not read)
+extern "C" long emu_factor_tangent_item_bytes(int nx, int nu, int nc, int nct, int nc0, int nth, int chunk) {
   return (long)ab2::factor_tangent_item_doubles(nx, nu, nc) * (long)sizeof(double);
 }

@@ -16,37 +16,12 @@ extern "C" int emu_resolve(const int *dims, double mueq, const double *mueq_b, c
   a.xs = out[0], a.us = out[1], a.vs = out[2], a.vsT = out[3], a.lam0 = out[4], a.lams = out[5];
   a.mueq = mueq;
   a.mueq_b = mueq_b;
-  const int chunks = (a.nrhs + a.chunk - 1) / a.chunk;
-  std::vector<double> sm(ab2::resolve_item_doubles(a.nx, a.nu, a.nc, a.nc0, a.chunk));
-  for (long b = 0; b < a.batch; ++b)
-    for (int c = 0; c < chunks; ++c) {
-      const int j0 = c * a.chunk, R = a.nrhs - j0 < a.chunk ? a.nrhs - j0 : a.chunk;
-      run_lanes(nl, [&](const EmuCtx &ctx) { ab2::resolve_item(a, ctx, sm.data(), b, j0, R); });
-    }
+  run_chunks(a.batch, a.nrhs, a.chunk, nl, ab2::resolve_item_doubles(a.nx, a.nu, a.nc, a.nc0, a.chunk),
+             [&](const EmuCtx &ctx, double *sm, long b, int j0, int R) { ab2::resolve_item(a, ctx, sm, b, j0, R); });
   return 0;
 }
 
-// Every shape `supported` (the library's ab2_gar_supported) accepts with nx, nu, nc < lim and nc0 in {0, 1, nx/2, nx}:
-// how many need more than 227 KB of shared memory for one right-hand side (the first one in *bad = nx, nu, nc, nc0),
-// and the largest item in bytes (*largest).
-extern "C" long emu_resolve_size_scan(int (*supported)(int, int, int, int), int lim, int *bad, long *largest) {
-  long over = 0;
-  *largest = 0;
-  for (int nx = 1; nx < lim; ++nx)
-    for (int nu = 1; nu < lim; ++nu)
-      for (int nc = 0; nc < lim; ++nc) {
-        const int nc0s[4] = {0, 1, nx / 2, nx};
-        for (int i = 0; i < 4; ++i) {
-          const int nc0 = nc0s[i];
-          if (i && nc0 == nc0s[i - 1])
-            continue;
-          if (!supported(nx, nu, nc, nc0))
-            continue;
-          const long bytes = (long)ab2::resolve_item_doubles(nx, nu, nc, nc0, 1) * (long)sizeof(double);
-          *largest = bytes > *largest ? bytes : *largest;
-          if (bytes > 227 * 1024 && over++ == 0)
-            bad[0] = nx, bad[1] = nu, bad[2] = nc, bad[3] = nc0;
-        }
-      }
-  return over;
+// bytes of shared memory one item of `chunk` right-hand sides uses (nct, nth: not read)
+extern "C" long emu_resolve_item_bytes(int nx, int nu, int nc, int nct, int nc0, int nth, int chunk) {
+  return (long)ab2::resolve_item_doubles(nx, nu, nc, nc0, chunk) * (long)sizeof(double);
 }

@@ -1,7 +1,9 @@
-"""The host emulation of the sweep programs (tests/emu/, one shared library) and the one way the CPU suite runs it.
+"""The host emulation of the sweep programs and the per-item programs (tests/emu/, one shared library) and the one way
+the CPU suite runs them.
 
 The library compiles riccati_group.cuh, riccati_block.cuh and riccati_dense.cuh with g++: a group is G std::threads, a
-CTA 32*W, sync() a std::barrier, mma.sync a fragment exchange, a TMA copy a memcpy.  `SweepParams` below mirrors
+CTA 32*W, sync() a std::barrier, mma.sync a fragment exchange, a TMA copy a memcpy.  The item programs (lq_resolve.cuh,
+lq_theta.cuh, lq_factor_adjoint.cuh, lq_factor_tangent.cuh) run the same way, one item after another.  `SweepParams` below mirrors
 ab2::SweepParams field for field; the library checks the mirror when it loads."""
 import ctypes as C
 import functools
@@ -28,6 +30,7 @@ LIB = os.path.join(tempfile.gettempdir(), "ab2_emu_%d_%s" % (os.getuid(), hashli
                    "libsweep_emu.so")
 _dp = C.POINTER(C.c_double)
 _ip = C.POINTER(C.c_int)
+SOL = lq_resolve_ref.SOL  # the fields of a solution, as resolve and the theta tangent write them
 
 
 class SweepParams(C.Structure):
@@ -80,12 +83,12 @@ def lib():
     h.emu_sweep_params_offset.argtypes = [C.c_char_p]
     for name in ("emu_factor_adjoint", "emu_factor_tangent", "emu_resolve"):
         getattr(h, name).argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]
-    for name in ("emu_factor_adjoint_item_bytes", "emu_factor_tangent_item_bytes"):
-        getattr(h, name).restype = C.c_long
-        getattr(h, name).argtypes = [C.c_int, C.c_int, C.c_int]
-    h.emu_factor_size_scan.restype = h.emu_resolve_size_scan.restype = C.c_long
-    h.emu_factor_size_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    h.emu_resolve_size_scan.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    h.emu_theta.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    for name in ("emu_resolve", "emu_theta", "emu_factor_adjoint", "emu_factor_tangent"):
+        getattr(h, name + "_item_bytes").restype = C.c_long
+        getattr(h, name + "_item_bytes").argtypes = [C.c_int] * 7  # nx, nu, nc, nct, nc0, nth, chunk
+    h.emu_item_size_scan.restype = C.c_long
+    h.emu_item_size_scan.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     bad = layout_mismatches(h)
     assert not bad, "tests/emu_harness.py SweepParams does not match ab2::SweepParams: %s" % bad
     return h
@@ -281,15 +284,45 @@ def run_resolve(recs, o, h, case, nrhs, mu, lanes, chunk, packed, head):
     keep.append(None if V0 is None else np.ascontiguousarray(V0))
     hf = lq_resolve_ref.full_rhs(h, case, B, nrhs)
     keep += [np.ascontiguousarray(hf[k]) for k in lq_resolve_ref.RHS]
-    out = {k: np.full((nrhs,) + s, np.nan) for k, s in zip(lq_resolve_ref.SOL, lq_resolve_ref.rhs_shapes(case, B).values())}
+    out = {k: np.full((nrhs,) + s, np.nan) for k, s in zip(SOL, lq_resolve_ref.rhs_shapes(case, B).values())}
     ptr = lambda a: None if a is None or a.size == 0 else a.ctypes.data
     ins = (C.c_void_p * 13)(*[ptr(a) for a in keep])
-    outs = (C.c_void_p * 6)(*[ptr(out[k]) for k in lq_resolve_ref.SOL])
+    outs = (C.c_void_p * 6)(*[ptr(out[k]) for k in SOL])
     _, srec = lq_adjoint_ref.stage_offsets(nx, nu, nc)
     dims = np.array([B, N, nx, nu, nc, nct, nc0, srec, term.shape[1], head if N else 0, nrhs, chunk, lanes],
                     dtype=np.int32)
     mub = None if np.ndim(mu) == 0 else np.ascontiguousarray(mu, dtype=np.float64)
     lib().emu_resolve(dims.ctypes.data, float(mu) if mub is None else 0.0, ptr(mub), ins, outs)
+    return out
+
+
+def shapes(d7, B):
+    """Per-direction shapes of the solution's fields; d7 = (nx, nu, nc, nct, nc0, nth, N)."""
+    nx, nu, nc, nct, nc0, nth, N = d7
+    return dict(xs=(B, N + 1, nx), us=(B, N, nu), vs=(B, N, nc), vsT=(B, nct), lam0=(B, nc0), lams=(B, N, nx))
+
+
+def run_theta(raw, d7, lanes, chunk, dtheta=None, cot=None):
+    """Run the ab2_gar_theta_tangent program (dtheta [nrhs][B][nth] given) or the ab2_gar_theta_adjoint program (cot:
+    dict of [nrhs][B][...] cotangents, missing = zero) on the factors `raw` of an emulated parametric sweep
+    (emulate('parametric', ...), device layouts), `chunk` directions per item on `lanes` emulated lanes.  -> dict of
+    the solution's fields [nrhs][B][...], or theta_bar [nrhs][B][nth]."""
+    nx, nu, nc, nct, nc0, nth, N = d7
+    B = raw["xs"].shape[0]
+    adjoint = dtheta is None
+    nrhs = (next(v for v in cot.values() if v is not None).shape[0]) if adjoint else dtheta.shape[0]
+    ptr = lambda a: None if a is None or a.size == 0 else a.ctypes.data
+    keep = [np.ascontiguousarray(raw[k], dtype=np.float64) for k in ("fb", "fth", "fbT", "Vxx", "Vxt", "kkt0fth")]
+    if adjoint:
+        keep += [None if cot.get(k) is None else np.ascontiguousarray(cot[k], dtype=np.float64) for k in SOL]
+        out = {"theta_bar": np.full((nrhs, B, nth), np.nan)}
+    else:
+        keep.append(np.ascontiguousarray(dtheta, dtype=np.float64))
+        out = {k: np.full((nrhs,) + s, np.nan) for k, s in shapes(d7, B).items()}
+    ins = (C.c_void_p * 12)(*[ptr(a) for a in keep] + [None] * (12 - len(keep)))
+    outs = (C.c_void_p * 6)(*[ptr(a) for a in out.values()] + [None] * (6 - len(out)))
+    dims = np.array([B, N, nx, nu, nc, nct, nc0, nth, nrhs, chunk, lanes, int(adjoint)], dtype=np.int32)
+    lib().emu_theta(dims.ctypes.data, ins, outs)
     return out
 
 

@@ -137,12 +137,12 @@ def test_every_served_shape_fits_or_is_refused():
     it (ab2_gar_factor_adjoint compares the same item size with 227 KB); C1 to C5 fit."""
     from aligator_b200 import gar
     fn = C.CFUNCTYPE(C.c_int, C.c_int, C.c_int, C.c_int, C.c_int)(("ab2_gar_supported", gar.lib()))
-    bad = (C.c_int * 4)()
+    bad = (C.c_int * 6)()
     largest, accepted = C.c_long(), C.c_long()
     e = emu_harness.lib()
-    over = e.emu_factor_size_scan(e.emu_factor_adjoint_item_bytes, C.cast(fn, C.c_void_p), 130, bad,
+    over = e.emu_item_size_scan(e.emu_factor_adjoint_item_bytes, 0, C.cast(fn, C.c_void_p), 130, bad,
                                 C.byref(largest), C.byref(accepted))
     assert accepted.value > over >= 0
     assert 0 < largest.value <= 227 * 1024
     for nx, nu, nc in ((6, 3, 0), (12, 6, 0), (4, 2, 2), (14, 7, 0), (57, 28, 0)):
-        assert e.emu_factor_adjoint_item_bytes(nx, nu, nc) <= 227 * 1024, (nx, nu, nc)
+        assert e.emu_factor_adjoint_item_bytes(nx, nu, nc, 0, 0, 0, 1) <= 227 * 1024, (nx, nu, nc)

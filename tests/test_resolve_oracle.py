@@ -178,10 +178,11 @@ def test_every_served_shape_fits_shared_memory():
     right-hand side per warp within 227 KB of shared memory."""
     from aligator_b200 import gar
     fn = C.CFUNCTYPE(C.c_int, C.c_int, C.c_int, C.c_int, C.c_int)(("ab2_gar_supported", gar.lib()))
-    bad = (C.c_int * 4)()
-    largest = C.c_long()
+    bad = (C.c_int * 6)()
+    largest, accepted = C.c_long(), C.c_long()
     e = emu_harness.lib()
-    over = e.emu_resolve_size_scan(C.cast(fn, C.c_void_p), 130, bad, C.byref(largest))
+    over = e.emu_item_size_scan(e.emu_resolve_item_bytes, 0, C.cast(fn, C.c_void_p), 130, bad, C.byref(largest),
+                                C.byref(accepted))
     assert over == 0, (over, list(bad))
     assert 0 < largest.value <= 227 * 1024
 

@@ -14,8 +14,7 @@ import pytest
 import hp_reference as hp
 import lq_cases
 import lq_theta_ref as tref
-from emu_harness import emulate
-from theta_emu_harness import SOL as THETA_SOL, lib, run_theta, shapes as theta_shapes
+from emu_harness import SOL as THETA_SOL, emulate, lib, run_theta, shapes as theta_shapes
 from lq_cases import PARAM_CASES
 
 # nth in {1, nx, 33}, terminal Gv and constraints, N 0 and 1, nc0 in {0, 1, nx/2, nx}, mu 1e-3 and 1e-8
@@ -184,7 +183,8 @@ def test_every_served_shape_fits_or_is_refused():
     fn = C.CFUNCTYPE(C.c_int, C.c_int, C.c_int, C.c_int, C.c_int)(lambda nx, nu, nc, nc0: gar.supported(nx, nu, nc, nc0))
     bad = (C.c_int * 6)()
     largest, accepted = C.c_long(0), C.c_long(0)
-    over = e.emu_theta_size_scan(C.cast(fn, C.c_void_p), 80, bad, C.byref(largest), C.byref(accepted))
+    over = e.emu_item_size_scan(e.emu_theta_item_bytes, 1, C.cast(fn, C.c_void_p), 80, bad, C.byref(largest),
+                                C.byref(accepted))
     print("\naccepted %d, over 227 KB %d (first %s), largest fitting item %d bytes"
           % (accepted.value, over, list(bad), largest.value))
     assert accepted.value > 0 and 0 < largest.value <= 227 * 1024

@@ -4,9 +4,10 @@
 
 Each library runs in its own process (gar.py loads one library per process): on seeded problems at C2, C3 (with
 terminal constraints) and C5 shapes, with a scalar and a per-instance mu, after a cycle_append (nonzero ring head), it
-calls adjoint, tangent, adjoint_many and tangent_many (nrhs 1 and 8), resolve, refine, refine_many, factor_adjoint and
-factor_tangent, with some input and output fields left NULL, and saves every output, including the handle's trajectory
-after adjoint and tangent.  The outputs are then compared as uint64 views, so -0.0 and +0.0 differ.  A call a shape
+calls adjoint, tangent, adjoint_many and tangent_many (nrhs 1 and 8), resolve (nrhs 3 and 33), refine, refine_many,
+factor_adjoint and factor_tangent, with some input and output fields left NULL, and saves every output, including the
+handle's trajectory after adjoint and tangent.  On parametric handles at C2 and C3 shapes it calls theta_tangent and
+theta_adjoint at nrhs 1, 8 and 33 (33 spans two chunks of directions).  The outputs are then compared as uint64 views, so -0.0 and +0.0 differ.  A call a shape
 does not support is recorded as refused and must be refused by both.
 
 It also records a state transcript for each handle kind (warp kernel at C2, CTA kernel at C5, dense, parallel with two
@@ -27,6 +28,8 @@ RHS = ("q", "r", "d", "dN", "g0", "f")
 FAC = ("ff", "fb", "vxx", "vx", "fft", "fbt")
 # name, (nx, nu, nc, nct, nc0, N, batch)
 CASES = [("C2", (12, 6, 0, 0, 12, 20, 48)), ("C3", (4, 2, 2, 2, 4, 20, 96)), ("C5", (57, 28, 0, 0, 57, 5, 3))]
+# parametric handles for the theta calls: name, (nx, nu, nc, nct, nc0, nth, N, batch)
+THETA_CASES = [("C2_nth4", (12, 6, 0, 0, 12, 4, 20, 48)), ("C3_nth2", (4, 2, 2, 2, 4, 2, 20, 96))]
 # the state transcript's handle kinds: name, handle options, (nx, nu, N, batch) with nc = nct = 0 and nc0 = nx
 KINDS = [("warp_C2", {}, (12, 6, 6, 8)), ("cta_C5", {}, (57, 28, 3, 2)), ("dense", dict(dense=True), (12, 6, 6, 8)),
          ("legs2", dict(legs=2), (12, 6, 6, 8)), ("parametric", dict(nth=2), (12, 6, 6, 8))]
@@ -109,16 +112,29 @@ def dump(lib, path):
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import torch
     import gen
+    import lq_cases
     import aligator_b200.gar as gar
     gar.LIB_PATH = lib
     res = {}
+    dev = lambda a: torch.tensor(np.ascontiguousarray(a), device="cuda")
+    rand = lambda *shape: dev(rng.standard_normal(shape))
+    nan = lambda *shape: torch.full(shape, float("nan"), dtype=torch.float64, device="cuda")
+
+    def keep(key, f):
+        """f()'s outputs under tag/key/..., or tag/key/refused"""
+        try:
+            out = f()
+        except gar.GarError as e:
+            res[tag + key + "/refused"] = np.array([1.0])
+            return
+        torch.cuda.synchronize()
+        for k, v in out.items():
+            res[tag + key + "/" + k] = v.cpu().numpy() if torch.is_tensor(v) else np.asarray(v)
+
     for name, (nx, nu, nc, nct, nc0, N, B) in CASES:
         rng = np.random.default_rng(7)
         stage, term, G0, g0 = gar.pack_problems(gen.generate_batch(5, B, N, nx, nu, nc, nct))
         sol = dict(xs=(N + 1, nx), us=(N, nu), vs=(N, nc), vsT=(nct,), lam0=(nc0,), lams=(N, nx))
-        dev = lambda a: torch.tensor(np.ascontiguousarray(a), device="cuda")
-        rand = lambda *shape: dev(rng.standard_normal(shape))
-        nan = lambda *shape: torch.full(shape, float("nan"), dtype=torch.float64, device="cuda")
         for mname, mu in (("scalar", 1e-3), ("vector", rng.uniform(1e-4, 1e-2, B))):
             tag = "%s/%s/" % (name, mname)
             s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B)
@@ -126,16 +142,6 @@ def dump(lib, path):
             s.sweep(mu)
             s.cycle_append(rng.standard_normal((B, s.srec)) * 0.1 + stage[:, 0])
             rec = dict(stage=(N, s.srec), term=(s.trec,), G0=(nc0 * nx,), g0=(nc0,))
-
-            def keep(key, f):
-                try:
-                    out = f()
-                except gar.GarError as e:
-                    res[tag + key + "/refused"] = np.array([1.0])
-                    return
-                torch.cuda.synchronize()
-                for k, v in out.items():
-                    res[tag + key + "/" + k] = v.cpu().numpy() if torch.is_tensor(v) else np.asarray(v)
 
             def traj():
                 return {k: s.get(w) for k, w in zip(SOL, (gar.OUT_XS, gar.OUT_US, gar.OUT_VS, gar.OUT_VST,
@@ -174,9 +180,9 @@ def dump(lib, path):
                 keep("adjoint_many%d" % R, adjoint_many)
                 keep("tangent_many%d" % R, tangent_many)
 
-            def resolve():
-                o = {k: nan(3, B, *sol[k]) for k in SOL}
-                s.resolve({k: rand(3, B, *sol[x]) for k, x in zip(RHS, SOL) if k != "f"}, o, mu)
+            def resolve(R):
+                o = {k: nan(R, B, *sol[k]) for k in SOL}
+                s.resolve({k: rand(R, B, *sol[x]) for k, x in zip(RHS, SOL) if k != "f"}, o, mu)
                 return o
 
             def refine_many():
@@ -205,10 +211,34 @@ def dump(lib, path):
                 n = s.refine(mu, steps=2, norms=True)
                 return dict(traj(), norms=n)
 
-            for key, f in (("resolve", resolve), ("refine_many", refine_many), ("factor_adjoint", factor_adjoint),
+            for key, f in (("resolve", lambda: resolve(3)), ("resolve33", lambda: resolve(33)),
+                           ("refine_many", refine_many), ("factor_adjoint", factor_adjoint),
                            ("factor_tangent", factor_tangent), ("refine", refine)):
                 keep(key, f)
             s.close()
+    for name, (nx, nu, nc, nct, nc0, nth, N, B) in THETA_CASES:
+        rng = np.random.default_rng(9)
+        tag = name + "/"
+        sol = dict(xs=(N + 1, nx), us=(N, nu), vs=(N, nc), vsT=(nct,), lam0=(nc0,), lams=(N, nx))
+        s = gar.CudaRiccatiBatch(nx, nu, nc, nct, nc0, N, B, nth=nth)
+        s.set_problem(*gar.pack_problems([lq_cases.make_problem([5, b], N, nx, nu, nc, nct, nth, gv=True)
+                                          for b in range(B)]))
+        s.backward(1e-3)
+        s.forward(theta=rng.standard_normal((B, nth)))
+        for R in (1, 8, 33):
+            def theta_tangent():
+                o = {k: nan(R, B, *sol[k]) for k in SOL}
+                s.theta_tangent(rand(R, B, nth), o)
+                return o
+
+            def theta_adjoint():
+                tb = nan(R, B, nth)
+                s.theta_adjoint({k: rand(R, B, *sol[k]) for k in SOL if k != "us"}, tb)  # us: zero
+                return dict(theta_bar=tb)
+
+            keep("theta_tangent%d" % R, theta_tangent)
+            keep("theta_adjoint%d" % R, theta_adjoint)
+        s.close()
     for name, kw, dims in KINDS:
         res["transcript/" + name] = np.array(transcript(gar, torch, kw, dims))
     np.savez(path, **res)
